@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — mel-frames/sec of the E2-TTS flow-matching hot path on B200.
+"""bench.py — mel-frames/sec of the E2-TTS flow-matching hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|3|4|5] [--dropout P]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config 2|3|4|5] [--dropout P] [--dump-outputs DIR]
 
 Workloads (BASELINE.json `configs`):
   2 (default, the metric's config)  E2TTS(dim 512, depth 8, heads 8, 100 mels) forward + loss.backward(), per-GPU batch 16 x 1024 frames
-  3  E2TTS(dim 1024, depth 24, heads 16), per-GPU batch 8 x 2048 frames, forward + backward
+  3  E2TTS(dim 1024, depth 24, heads 16), per-GPU batch 4 x 2048 frames, forward + backward
   4  DurationPredictor(dim 512, depth 8), batch 32 x 1024 frames, forward + backward
   5  E2TTS(dim 1024, depth 24, heads 16).sample(): 32-step midpoint ODE with CFG/APG, batch 8, prompt 256 -> 2048 frames
 bf16 tensor-core compute, text conditioning on every step, synthetic data, random-init weights. One process per GPU (torchrun),
@@ -14,16 +14,23 @@ the CUDA-graph replay of forward + backward.
 One JSON line is printed by rank 0 (contract: see DESIGN.md §measurement):
   value     whole-job mel-frames/s with the batch already resident in HBM (device-timed, max over ranks)
   e2e       same metric through the public API with HOST (pinned) inputs: H2D of the inputs every step + D2H of the result
-  roofline  tcgen05 GEMM kernel family: algorithmic FLOPs of one step's GEMM launches / their device time (the recorded launches replayed
-            back to back as one CUDA graph, one CUDA-event pair around the replay) vs the measured bf16 peak (MEASURED_PEAKS.json)
+  roofline  wgmma GEMM kernel family: algorithmic FLOPs of one step's GEMM launches / their device time (the recorded launches replayed
+            back to back as one CUDA graph, one CUDA-event pair around the replay) vs the bf16 peak (MEASURED_PEAKS.json when present,
+            else the H100 SXM data-sheet figure, dense bf16)
   cpu_baseline  the oracle port (oracle/e2tts_oracle.py = the reference algorithm in fp32 PyTorch) on the host cores, on
                 BASELINE cfg1 exactly (B = 2 x 1024 frames, same d512 / depth-8 model): 2 warm-up + 5 timed steps, median
 `--impl reference` times that CPU path alone (the reference itself is pure Python + unvendored deps and cannot travel
 to the GPU box; see DESIGN.md).
+`--dump-outputs DIR` writes, after the timed steps, what the timed path computed in its last step as DIR/<name>.npy (float32): the
+loss and prediction of a training step and every parameter gradient (`grad.<parameter name>`), or the sampled mel of a sample() call.
+Inputs and weights are seeded, so two builds run with the same arguments can be compared output for output. An array of more than
+`per_array` elements is reduced to a fixed sample of its flattened elements (indices: the sorted first `per_array` of a randperm drawn
+from a generator seeded with 0), so that all files together stay within 64 MB.
 """
 import argparse
 import json
 import os
+import random
 import subprocess
 import sys
 import threading
@@ -34,12 +41,15 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+H100_BF16_DENSE_TFLOPS = 989.0   # NVIDIA H100 SXM data sheet, dense bf16 (a 700 W card)
+DUMP_BUDGET_BYTES = 64 << 20
+
 METRIC = 'mel-frames/sec E2TTS fwd+bwd (d512 depth8 L1024)'
 TEXT = ['Hello', 'Goodbye']
 CONFIGS = {
     1: dict(kind='train', dim=512, depth=8, heads=8, batch=2, seq=1024, name='cfg1: E2TTS d512 depth8 h8, B2 x N1024 x 100 mel, CPU fwd+bwd (README snippet)'),
     2: dict(kind='train', dim=512, depth=8, heads=8, batch=16, seq=1024, name='cfg2: E2TTS d512 depth8 h8, B16 x N1024 x 100 mel, fwd+bwd'),
-    3: dict(kind='train', dim=1024, depth=24, heads=16, batch=8, seq=2048, name='cfg3: E2TTS d1024 depth24 h16, B8 x N2048 per GPU, fwd+bwd'),
+    3: dict(kind='train', dim=1024, depth=24, heads=16, batch=4, seq=2048, name='cfg3: E2TTS d1024 depth24 h16, B4 x N2048 per GPU, fwd+bwd'),   # B8 does not fit 80 GB
     4: dict(kind='duration', dim=512, depth=8, heads=8, batch=32, seq=1024, name='cfg4: DurationPredictor d512 depth8, B32 x N1024, fwd+bwd'),
     5: dict(kind='sample', dim=1024, depth=24, heads=16, batch=8, seq=2048, prompt=256, ode_steps=32,
             name='cfg5: E2TTS d1024 depth24 h16 sample(), 32-step midpoint ODE + CFG/APG, B8, prompt 256 -> 2048 frames'),
@@ -80,6 +90,7 @@ def cpu_step_fn(cfg, threads):
     from oracle import e2tts_oracle as O
     torch.set_num_threads(threads)
     torch.manual_seed(0)
+    random.seed(0)   # the hyper-connections draw their initial stream with python's randrange
     batch, N = cfg['batch'], cfg['seq']
     model = pkg.E2TTS(transformer=dict(dim=cfg['dim'], depth=cfg['depth'], heads=cfg['heads'], dropout=0.), use_vocos=False)
     sd = {k: v.detach().clone().requires_grad_(v.is_floating_point()) for k, v in model.state_dict().items()}
@@ -180,14 +191,17 @@ class ClockSampler:
                     reasons=sorted(reasons), samples=len(self.samples))
 
 
-def gemm_traffic(config):
-    """DRAM bytes of the GEMM family per step from the committed ncu capture (profiles/r2_gemm_traffic.json, written by
-    tools/gemm_traffic.py from `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum`), or None."""
-    try:
-        t = json.load(open(os.path.join(ROOT, 'profiles', 'r2_gemm_traffic.json')))
-        return t.get(f'cfg{config}')
-    except Exception:
-        return None
+def dump_outputs(dirname, arrays):
+    """Write {name: tensor} as float32 .npy files; large arrays become a fixed seeded sample (see the module docstring)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    per_array = max(4096, DUMP_BUDGET_BYTES // 4 // max(1, len(arrays)))
+    for name, t in arrays.items():
+        v = t.detach().float().flatten().cpu()
+        if v.numel() > per_array:
+            idx = torch.randperm(v.numel(), generator=torch.Generator().manual_seed(0))[:per_array].sort().values
+            v = v[idx]
+        np.save(os.path.join(dirname, name + '.npy'), v.numpy().astype(np.float32))
 
 
 def run_gpu(args):
@@ -204,6 +218,7 @@ def run_gpu(args):
     if world > 1:
         dist.init_process_group('nccl', device_id=dev)
     torch.manual_seed(0)
+    random.seed(0)   # the hyper-connections draw their initial stream with python's randrange: same weights on every run
     tkw = dict(dim=cfg['dim'], depth=cfg['depth'], heads=cfg['heads'], dropout=args.dropout)
     B, N = cfg['batch'], cfg['seq']
     if kind == 'duration':
@@ -222,19 +237,43 @@ def run_gpu(args):
     text_dev = pkg.list_str_to_tensor(text).to(dev)
     d2h_bytes = 4
 
+    last = {}   # --dump-outputs: what the most recent step returned to its caller
+
+    def keep(out):
+        if not args.dump_outputs:
+            return
+        last.clear()
+        if kind == 'sample':
+            last['mel'] = out
+            return
+        # detached: an eager step's autograd graph must not outlive the step (it would pin the AccumulateGrad nodes to the default
+        # stream and break the CUDA-graph capture of the same model)
+        if torch.is_tensor(out):
+            last['loss'] = out.detach()
+        else:
+            last['loss'], last['pred'] = out.loss.detach(), out.pred_flow.detach()
+        for name, p in model.named_parameters():
+            if p.grad is not None:
+                last['grad.' + name] = p.grad.detach()
+
     if kind == 'sample':
         model.eval()
         d2h_bytes = B * N * 100 * 4
 
-        def step(mel, readback):
+        def step(mel, readback, record=True):
             out = model.sample(mel, text=text_dev, duration=N, steps=cfg['ode_steps'], cfg_strength=1.0, return_raw_output=True)
+            if record:
+                keep(out)
             return out.cpu() if readback else None
     else:
-        def step(mel, readback):
-            loss = model(mel, text=text_dev) if kind == 'duration' else model(mel, text=text_dev).loss
+        def step(mel, readback, record=True):
+            out = model(mel, text=text_dev)
+            loss = out if kind == 'duration' else out.loss
             loss.backward()
             if sync is not None:
                 sync()
+            if record:
+                keep(out)
             for p in model.parameters():
                 p.grad = None
             return loss.item() if readback else None
@@ -255,11 +294,10 @@ def run_gpu(args):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms) / steps
 
-    steps = args.steps if kind != 'sample' else max(1, min(args.steps, 3))   # one cfg5 step = 124 transformer forwards
-    warm = max(args.warmup, 3) if kind != 'sample' else 1
+    steps, warm = args.steps, args.warmup
     for _ in range(warm):
-        step(dev_mel, False)
-    # -- time of the tcgen05 GEMM family inside one real step (roofline numerator / denominator): every ops.gemm call of ONE step is
+        step(dev_mel, False, record=False)
+    # -- time of the wgmma GEMM family inside one real step (roofline numerator / denominator): every ops.gemm call of ONE step is
     #    recorded with its live operands, then the same calls are captured into one CUDA graph and replayed — the kernels run back to
     #    back exactly as launched in the step, and the whole list is bracketed by ONE event pair. (Bracketing each launch of an eager
     #    step with its own event pair also brackets the host's launch latency whenever the GPU waits for the host: h + max(kernel, h'),
@@ -314,7 +352,7 @@ def run_gpu(args):
                 model.cfg_transformer_with_pred_head(x, torch.zeros_like(x), times=torch.tensor(0.5, device=dev), text=text_dev,
                                                      mask=torch.ones(B, N, dtype=torch.bool, device=dev), cfg_strength=1.0)
         else:
-            step(dev_mel, False)
+            step(dev_mel, False, record=False)
         torch.cuda.synchronize()
         ops.gemm = orig_gemm
         gemm_ms = replay_gemms()
@@ -325,7 +363,7 @@ def run_gpu(args):
         #    all-reduce): identical kernels and work, no per-launch host cost. Falls back to the eager numbers if capture fails.
         if kind in ('train', 'duration') and not args.no_graph:
             try:
-                eager_loss = step(dev_mel, True)
+                eager_loss = step(dev_mel, True, record=False)
                 torch.cuda.empty_cache()      # the eager pool and the graph's private pool each hold a full set of activations
                 graphed = pkg.GraphedTrainStep(model, dev_mel, text=text_dev)
                 g_loss = float(graphed().item())
@@ -341,10 +379,14 @@ def run_gpu(args):
                 if float(ok) > 0:
                     eager_ms, step_mode = ms_dev, 'cuda_graph'
                     ms_dev, ms_e2e, launches = ms_g, ms_g_e2e, graphed.launches_per_step
+                    keep(graphed.out.loss if kind == 'duration' else graphed.out)   # the static outputs of the last replay
                 else:
                     graph_note = f'captured but not faster ({ms_g:.2f} ms)'
             except Exception as e:  # noqa: BLE001 - any capture problem: keep the eager measurement
                 graph_note = f'unavailable: {type(e).__name__}: {str(e)[:160]}'
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        dump_outputs(args.dump_outputs, last)
     if rank != 0:
         if world > 1:
             dist.destroy_process_group()
@@ -354,7 +396,7 @@ def run_gpu(args):
         peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
     except Exception:
         pass
-    peak_tf = peaks.get('bf16_tflops_sustained', 1400.0)
+    peak_tf = peaks.get('bf16_tflops_sustained', H100_BF16_DENSE_TFLOPS)
     achieved_tf = prof['flops'] / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
     frames = world * B * N
     fl = step_flops(cfg, B)
@@ -367,7 +409,7 @@ def run_gpu(args):
         'config': {'workload': cfg['name'], 'per_gpu_batch': B, 'seq_len': N, 'global_batch': world * B, 'parallelism': f'dp{world}',
                    'dropout': args.dropout if kind != 'sample' else 0.0, 'text_cond': 'on every step', 'weights': 'random init',
                    'optimizer_step': 'not part of the metric',
-                   'l2': 'per-step working set (GBs of activations) >> 126 MB L2, no flush needed',
+                   'l2': 'per-step working set (GBs of activations) >> 50 MB L2, no flush needed',
                    'grad_exchange': ('one flat fp32 ncclAllReduce per step after backward (e2_tts_pytorch_b200.GradSync)' if world > 1 and kind != 'sample' else 'none'),
                    'step': (what + ' replayed through e2_tts_pytorch_b200.GraphedTrainStep (one CUDA graph, same kernels)'
                             if step_mode == 'cuda_graph' else what + ', eager launches'),
@@ -378,11 +420,10 @@ def run_gpu(args):
                 'd2h_bytes_per_step': d2h_bytes},
         'gpu_launches': int(launches),
         'clocks': clk.summary(),
-        'roofline': {'kernel': 'gemm_tcgen05_kernel (all GEMMs of the step: fwd, dX, dW)' if kind != 'sample' else 'gemm_tcgen05_kernel (all GEMMs of one function evaluation)',
+        'roofline': {'kernel': 'gemm_wgmma_kernel (all GEMMs of the step: fwd, dX, dW)' if kind != 'sample' else 'gemm_wgmma_kernel (all GEMMs of one function evaluation)',
                      'bound': 'tensor', 'achieved': achieved_tf, 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': achieved_tf / peak_tf if peak_tf else None,
-                     'traffic': gemm_traffic(args.config),
                      'launches_per_step': n_gemm // max(nprof, 1), 'ms_per_step': gemm_ms / max(nprof, 1),
-                     'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained' if peaks else 'fallback 1.4 PF/s sustained',
+                     'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained' if peaks else 'H100 SXM data sheet, dense bf16 (not a measured rate)',
                      'step_flops': fl, 'step_tensor_frac': fl / (ms_dev * 1e-3) / 1e12 / peak_tf},
     }
     if world == 1 and not args.no_cpu:
@@ -402,6 +443,8 @@ def main():
     ap.add_argument('--dropout', type=float, default=0.1)
     ap.add_argument('--no-cpu', action='store_true')
     ap.add_argument('--no-graph', action='store_true', help='time the eager step only (skip the CUDA-graph replay of the same step)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the outputs of the last timed step as DIR/<name>.npy (float32)')
     ap.add_argument('--cpu-worker', action='store_true', help=argparse.SUPPRESS)
     ap.add_argument('--cpu-budget', type=float, default=150.0, help=argparse.SUPPRESS)
     args = ap.parse_args()

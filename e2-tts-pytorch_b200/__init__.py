@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of the e2-tts-pytorch flow-matching hot path.
+"""H100-native (sm_90a) implementation of the e2-tts-pytorch flow-matching hot path.
 
 Same public surface as the reference package (`/root/reference/e2_tts_pytorch/__init__.py:1-8` minus the
 trainer): `E2TTS`, `DurationPredictor`, `Transformer`, `MelSpec`, `E2TTSReturn`. Host code is Python/PyTorch

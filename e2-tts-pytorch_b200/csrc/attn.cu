@@ -7,9 +7,9 @@
 // m16n8k16 tensor-core tiles fed by cp.async double-buffered, XOR-swizzled shared memory.
 // Backward = recompute: a per-row prep kernel (dO = dOg*gate, delta = <dO,O>, d_gate), a dQ kernel
 // (query-stationary) and a dK/dV kernel (key-stationary), including the (1 - tanh^2) softclamp factor.
-// NOTE (DESIGN.md): these mma.sync kernels were the bring-up path. The product path is the tcgen05/TMEM kernels in attn_tc.cu;
+// NOTE (DESIGN.md): these mma.sync kernels were the bring-up path. The product path is the wgmma kernels in attn_tc.cu;
 // the entry points here are `*_legacy`: cross-checks for the tests, and the online-softmax fallback of b200_attn_fwd for
-// softclamp values > 64 (the tcgen05 forward exponentiates without a running maximum). attn_bwd_prep_kernel is shared.
+// softclamp values > 64 (the wgmma forward exponentiates without a running maximum). attn_bwd_prep_kernel is shared.
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -482,7 +482,7 @@ static int fill_common(AttnP& p, int B, int H, int Np, float scale, float clamp,
 
 using namespace b200;
 
-// mma.sync forward (round-1 bring-up kernel): kept as a cross-check for the tcgen05 forward in attn_tc.cu.
+// mma.sync forward (bring-up kernel): kept as a cross-check for the wgmma forward in attn_tc.cu.
 extern "C" int b200_attn_fwd_legacy(const b200_attn_fwd_args* a, b200_stream_t stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B200_REQUIRE(a && a->q && a->k && a->v && a->o && a->og && a->lse, "attn_fwd: null pointer");
@@ -508,7 +508,7 @@ int launch_attn_bwd_prep(const b200_attn_bwd_args* a, cudaStream_t st) {
 }
 }  // namespace b200
 
-// mma.sync backward (round-1 bring-up kernels, dq/dk/dv all bf16): kept as a cross-check for the tcgen05 backward.
+// mma.sync backward (bring-up kernels, dq/dk/dv all bf16): kept as a cross-check for the wgmma backward.
 extern "C" int b200_attn_bwd_legacy(const b200_attn_bwd_args* a, b200_stream_t stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B200_REQUIRE(a && a->q && a->k && a->v && a->o && a->d_og && a->lse && a->ws_dO && a->ws_delta && a->dq && a->dk && a->dv, "attn_bwd: null pointer");

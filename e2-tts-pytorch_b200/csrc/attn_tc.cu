@@ -1,16 +1,14 @@
-// tcgen05 / TMEM / TMA flash attention for the softclamped, key-masked, head-gated attention of the E2-TTS multistream block
-// (x-transformers Attend as configured by the reference: SURVEY A.4 steps 4-5) — forward and backward.
+// wgmma / TMA flash attention for the softclamped, key-masked, head-gated attention of the E2-TTS multistream block
+// (x-transformers Attend as configured by the reference: SURVEY A.4 steps 4-5) — forward and backward, sm_90a.
 //
-// Forward: one CTA per (128-query tile, head, batch) on 64-key tiles, 320 threads, two CTAs per SM (see attn_fwd_tc64_kernel):
-//   warp 0 lane 0 : TMA producer  — Q once, then K_j / V_j tiles (64 keys x 64) into a 3-stage smem ring
-//   warp 1 lane 0 : MMA issuer    — S_j = Q K_j^T  (tcgen05.mma 128x64x16 x4, both operands K-major) into TMEM S[j%2]
-//                                   O_j = P_j V_j  (tcgen05.mma 128x64x16 x4, A = P from smem (K-major), B = V MN-major)
-//                                   accumulating into TMEM O; S_{j+1} is issued before O_j so the tensor pipe never waits on softmax
-//   warps 2..9    : softmax       — thread = (query row, key half): 32 of the 64 scores of its row (tcgen05.ld 32x32b: lane == row).
-//                                   The softclamp bounds the logits to [-clamp, clamp], so exp() needs no running maximum: one pass
-//                                   softclamp (tanh) + exp2 + dropout, P_j written as bf16 into 128B-swizzled smem (the A operand of
-//                                   the PV MMA); P V accumulates in ONE TMEM accumulator over all key tiles and is read back once.
-// mbarrier pipelines: q_full, k_full/v_full/kv_empty[3], s_full/s_empty[2], p_full/p_empty[2], o_full.
+// Forward: one CTA per (128-query tile, head, batch) on 64-key tiles, 384 threads:
+//   warpgroup 0, one thread : TMA producer — Q once, then K_j / V_j tiles (64 keys x 64) into a 3-stage smem ring
+//   warpgroups 1, 2         : 64 query rows each — S_j = Q K_j^T (wgmma m64n64k16 x4, both operands K-major from smem) into
+//                             registers; softclamp (tanh) + exp2 + mask + dropout on the fragments; O += P_j V_j with P_j as the
+//                             REGISTER A operand (wgmma m64n64k16, B = V MN-major) — P never touches shared memory.
+//                             The softclamp bounds the logits to [-clamp, clamp], so exp() needs no running maximum: O accumulates
+//                             over all key tiles and is normalised once by the row sum.
+// mbarrier pipelines: q_full, kv_full/kv_empty[3].
 #include <type_traits>
 
 #include "common.cuh"
@@ -19,8 +17,8 @@
 namespace b200 {
 
 constexpr int TQ = 128, TKV = 128, DH = 64;
-constexpr int TILE16 = 128 * 64 * 2;          // 16 KB: Q, K or V tile
-constexpr int PTILE = 128 * 128 * 2;          // 32 KB: P tile (two 64-key swizzle atoms)
+constexpr int TILE16 = 128 * 64 * 2;          // 16 KB: 128 rows x 64 bf16
+constexpr int TILE8 = 64 * 64 * 2;            // 8 KB: 64 rows x 64 bf16
 constexpr float LOG2E_F = 1.4426950408889634f;
 
 struct AttnTcP {
@@ -44,15 +42,15 @@ __device__ __forceinline__ float tanh_approx(float x) {
 }
 // tanh of a pair on the FMA pipe: odd degree-9 Taylor polynomial, |error| < 5e-6 for |x| <= 0.5 (tanh.approx is ~5e-4). The clamp
 // argument score * scale / clamp is small in practice, so the callers take this path whenever a warp's whole tile fits the range and
-// keep MUFU.TANH for outliers: the softmax threads are MUFU/MIO-bound with two MUFU ops per score (ncu r3: xu 47 %, mio_throttle).
+// keep MUFU.TANH for outliers: with two MUFU operations per score the softmax math is otherwise bound by the MUFU pipe.
 constexpr float TANH_POLY_MAX = 0.5f;
 __device__ __forceinline__ float2 tanh_poly2(float2 x) {
-    const float2 x2 = __fmul2_rn(x, x);
-    float2 q = __ffma2_rn(x2, make_float2(62.f / 2835.f, 62.f / 2835.f), make_float2(-17.f / 315.f, -17.f / 315.f));
-    q = __ffma2_rn(q, x2, make_float2(2.f / 15.f, 2.f / 15.f));
-    q = __ffma2_rn(q, x2, make_float2(-1.f / 3.f, -1.f / 3.f));
-    q = __ffma2_rn(q, x2, make_float2(1.f, 1.f));
-    return __fmul2_rn(x, q);
+    const float2 x2 = fmul2(x, x);
+    float2 q = ffma2(x2, make_float2(62.f / 2835.f, 62.f / 2835.f), make_float2(-17.f / 315.f, -17.f / 315.f));
+    q = ffma2(q, x2, make_float2(2.f / 15.f, 2.f / 15.f));
+    q = ffma2(q, x2, make_float2(-1.f / 3.f, -1.f / 3.f));
+    q = ffma2(q, x2, make_float2(1.f, 1.f));
+    return fmul2(x, q);
 }
 __device__ __forceinline__ float ex2_approx(float x) {
     float y;
@@ -74,65 +72,40 @@ __global__ void attn_maskbits_kernel(const unsigned char* mask, unsigned int* bi
     bits[w] = v;
 }
 
-// ------------------------------------------------------------------------------------------------ forward, two CTAs per SM
-// 64-key tiles and a CTA sized at HALF an SM — 320 threads (TMA producer, MMA issuer, 8 softmax warps: thread = query row x key half,
-// 32 scores per thread and tile), 96 KB of shared memory, 256 TMEM columns (S[2] x 64 + O 64) — so that two CTAs share an SM. (Rounds 1-2
-// ran 128-key tiles with 16 softmax warps and one CTA per SM: 152.6 us at cfg2 against 121.9 us, profiles/r2s_attn_bench.txt.) The softmax of this attention flavour is bound by the CUDA-core pipes (tanh polynomial on FMA, exp on MUFU,
-// dropout hash on ALU), and inside one CTA its phases run in lockstep on all softmax warps; two independent CTAs interleave their
-// phases on the schedulers, overlap one CTA's prologue / epilogue with the other's main loop, and give the SM two MMA issuers.
-// 64-key tiles also waste less of the ragged last tile (17 x 64 = 1088 keys for N' = 1056 instead of 9 x 128 = 1152).
-constexpr int TKV2 = 64, KV2_STAGES = 3;
-constexpr int TILE8 = 64 * 64 * 2;            // 8 KB: K or V tile of 64 keys
+// ------------------------------------------------------------------------------------------------ forward
+constexpr int KV_STAGES = 3;
 
-__global__ void __launch_bounds__(320, 2)
-attn_fwd_tc64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                     const AttnTcP p) {
+__global__ void __launch_bounds__(384, 1)
+attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                      const AttnTcP p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sQ = smem;                         // 16 KB
     uint8_t* sK = sQ + TILE16;                  // [3] x 8 KB
-    uint8_t* sV = sK + KV2_STAGES * TILE8;      // [3] x 8 KB
-    uint8_t* sP = sV + KV2_STAGES * TILE8;      // [2] x 16 KB (128 rows x 64 keys bf16 = one 128-byte swizzle atom per row)
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * TILE16);
+    uint8_t* sV = sK + KV_STAGES * TILE8;       // [3] x 8 KB
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * TILE8);
     uint64_t* q_full = bars;                    // 1
-    uint64_t* k_full = bars + 1;                // 3
-    uint64_t* v_full = bars + 4;                // 3
-    uint64_t* kv_empty = bars + 7;              // 3
-    uint64_t* s_full = bars + 10;               // 2
-    uint64_t* s_empty = bars + 12;              // 2
-    uint64_t* p_full = bars + 14;               // 2
-    uint64_t* p_empty = bars + 16;              // 2
-    uint64_t* o_full = bars + 18;               // 1
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 19);
-    float* s_xch = reinterpret_cast<float*>(bars + 20);   // [2 halves][128 rows] row sums
+    uint64_t* kv_full = bars + 1;               // 3
+    uint64_t* kv_empty = bars + 4;              // 3 (one arrival per consumer warpgroup)
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int qt = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
     const int bh = b * p.H + hh;
     const int q0 = qt * TQ;
-    const int nkv = (p.Np + TKV2 - 1) / TKV2;
+    const int nkv = (p.Np + 63) / 64;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV);
         mbar_init(q_full, 1);
-        mbar_init(o_full, 1);
-        for (int i = 0; i < KV2_STAGES; ++i) { mbar_init(&k_full[i], 1); mbar_init(&v_full[i], 1); mbar_init(&kv_empty[i], 1); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 8);
-            mbar_init(&p_full[i], 8); mbar_init(&p_empty[i], 1);
-        }
+        for (int i = 0; i < KV_STAGES; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 256);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tS = tmem_base, tO = tmem_base + 128;   // S[2] at +0 / +64, O at +128 (64 columns)
     pdl_wait();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        regs_dealloc<40>();
+        if (threadIdx.x == 0) {
             // ---------------------------------------------------------------- TMA producer
             const int row_base = bh * p.Np;
             mbar_arrive_expect_tx(q_full, TILE16);
@@ -141,201 +114,167 @@ attn_fwd_tc64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
             uint32_t ph = 0;
             for (int j = 0; j < nkv; ++j) {
                 mbar_wait(&kv_empty[st], ph ^ 1);
-                mbar_arrive_expect_tx(&k_full[st], TILE8);
-                tma_load_2d(sK + st * TILE8, &tmK, &k_full[st], 0, row_base + j * TKV2);
-                mbar_arrive_expect_tx(&v_full[st], TILE8);
-                tma_load_2d(sV + st * TILE8, &tmV, &v_full[st], 0, row_base + j * TKV2);
-                if (++st == KV2_STAGES) { st = 0; ph ^= 1; }
+                mbar_arrive_expect_tx(&kv_full[st], 2 * TILE8);
+                tma_load_2d(sK + st * TILE8, &tmK, &kv_full[st], 0, row_base + j * 64);
+                tma_load_2d(sV + st * TILE8, &tmV, &kv_full[st], 0, row_base + j * 64);
+                if (++st == KV_STAGES) { st = 0; ph ^= 1; }
             }
             pdl_launch_dependents();
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // ---------------------------------------------------------------- MMA issuer
-            constexpr uint32_t idesc_s = make_idesc_bf16(128, 64, 0, 0);
-            constexpr uint32_t idesc_o = make_idesc_bf16(128, 64, 0, 1);
-            mbar_wait(q_full, 0);
-            const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ), 0, 1024);
-            int kst = 0; uint32_t kph = 0;       // K ring position of S_j
-            int vst = 0; uint32_t vph = 0;       // V ring position of O_{j-1}
-            for (int j = 0; j <= nkv; ++j) {
-                if (j < nkv) {
-                    const int ss = j & 1;
-                    mbar_wait(&k_full[kst], kph);
-                    mbar_wait(&s_empty[ss], ((j >> 1) & 1) ^ 1);
-                    tc_fence_after();
-                    const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + kst * TILE8), 0, 1024);
-#pragma unroll
-                    for (int k = 0; k < DH / 16; ++k) umma_f16(tS + ss * 64, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), idesc_s, k > 0 ? 1u : 0u);
-                    umma_commit(&s_full[ss]);
-                    if (++kst == KV2_STAGES) { kst = 0; kph ^= 1; }
-                }
-                if (j >= 1) {
-                    const int jj = j - 1, ps = jj & 1;
-                    mbar_wait(&p_full[ps], (jj >> 1) & 1);
-                    mbar_wait(&v_full[vst], vph);
-                    tc_fence_after();
-                    const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + vst * TILE8), 128 * 128, 1024);
-                    const uint32_t pbase = smem_u32(sP + ps * TILE16);
-#pragma unroll
-                    for (int k = 0; k < TKV2 / 16; ++k) {
-                        const uint64_t pdesc = make_smem_desc_sw128(pbase + k * 32, 0, 1024);
-                        umma_f16(tO, pdesc, vdesc + (uint64_t)(k * 128), idesc_o, (jj > 0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(&kv_empty[vst]);     // K_jj was consumed by S_jj earlier: the slot is free once O_jj has read V_jj
-                    umma_commit(&p_empty[ps]);
-                    if (jj == nkv - 1) umma_commit(o_full);
-                    if (++vst == KV2_STAGES) { vst = 0; vph ^= 1; }
-                }
-            }
-        }
-    } else {
-        // -------------------------------------------------------------------- softmax warps: thread = (row, key half)
-        const int qd = warp & 3, half = (warp - 2) >> 2;
-        const int row = qd * 32 + lane;
-        const int qi = q0 + row;
-        const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-        const unsigned int* mb = p.maskbits + (size_t)b * p.mask_words + half;
-        const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
-        const unsigned long long drop_row = ((unsigned long long)bh * p.Np + (unsigned long long)qi) * (unsigned long long)p.drop_stride;
-        const float2 soc2 = make_float2(p.scale_over_clamp, p.scale_over_clamp);
-        const float2 cl2 = make_float2(p.clamp * LOG2E_F, p.clamp * LOG2E_F);
-        const float soc = p.scale_over_clamp, soc2s = soc * soc;
-        const float k1 = soc * p.clamp * LOG2E_F, k3 = k1 * soc2s * (-1.f / 3.f), k5 = k1 * soc2s * soc2s * (2.f / 15.f),
-                    k7 = k1 * soc2s * soc2s * soc2s * (-17.f / 315.f), k9 = k1 * soc2s * soc2s * soc2s * soc2s * (62.f / 2835.f);
-        const float lim5 = 0.15f / fabsf(soc), lim9 = TANH_POLY_MAX / fabsf(soc);
-        const uint32_t thr32 = drop_thresh32(p.drop_thresh);
-        float2 l2 = make_float2(0.f, 0.f);
-
-        for (int j = 0; j < nkv; ++j) {
-            const int st = j & 1;
-            const uint32_t ph = (j >> 1) & 1;
-            const unsigned int mbits = mb[j * 2];
-            mbar_wait(&s_full[st], ph);
-            tc_fence_after();
-            uint32_t r[32];
-            tmem_ld32(tS + st * 64 + half * 32 + lane_off, r);
-            tmem_ld_wait();
-            tc_fence_before();          // the scores are in registers: hand the S buffer back before doing the math
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_empty[st]);
-            float pv[32];
-            float amax = 0.f;
-#pragma unroll
-            for (int i = 0; i < 32; ++i) { pv[i] = __uint_as_float(r[i]); amax = fmaxf(amax, fabsf(pv[i])); }
-            // clamp * log2(e) * tanh(u), u = s * scale / clamp, evaluated as an odd polynomial in the RAW score s with the constants folded
-            // in: s * (k1 + s^2 (k3 + s^2 (k5 + ...))) — 4 (degree 5, |u| <= 0.15: exact to 1e-7) or 6 (degree 9, |u| <= 0.5) packed
-            // instructions per key pair; MUFU.TANH only when a warp's tile leaves that range
-            if (__all_sync(0xffffffffu, amax <= lim5)) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float2 s = make_float2(pv[i], pv[i + 1]);
-                    const float2 s2 = __fmul2_rn(s, s);
-                    float2 q = __ffma2_rn(s2, make_float2(k5, k5), make_float2(k3, k3));
-                    q = __ffma2_rn(q, s2, make_float2(k1, k1));
-                    const float2 y = __fmul2_rn(s, q);
-                    pv[i] = ex2_approx(y.x);
-                    pv[i + 1] = ex2_approx(y.y);
-                }
-            } else if (__all_sync(0xffffffffu, amax <= lim9)) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float2 s = make_float2(pv[i], pv[i + 1]);
-                    const float2 s2 = __fmul2_rn(s, s);
-                    float2 q = __ffma2_rn(s2, make_float2(k9, k9), make_float2(k7, k7));
-                    q = __ffma2_rn(q, s2, make_float2(k5, k5));
-                    q = __ffma2_rn(q, s2, make_float2(k3, k3));
-                    q = __ffma2_rn(q, s2, make_float2(k1, k1));
-                    const float2 y = __fmul2_rn(s, q);
-                    pv[i] = ex2_approx(y.x);
-                    pv[i + 1] = ex2_approx(y.y);
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const float2 x = __fmul2_rn(make_float2(pv[i], pv[i + 1]), soc2);
-                    const float2 y = __fmul2_rn(make_float2(tanh_approx(x.x), tanh_approx(x.y)), cl2);
-                    pv[i] = ex2_approx(y.x);
-                    pv[i + 1] = ex2_approx(y.y);
-                }
-            }
-            if (mbits != 0xffffffffu) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) pv[i] = ((mbits >> i) & 1u) ? pv[i] : 0.f;
-            }
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) l2 = __fadd2_rn(l2, make_float2(pv[i], pv[i + 1]));
-            if (p.dropout_p > 0.f) {   // the 1/(1-p) factor is applied once, to the normalised output
-                const uint32_t pbase = (uint32_t)((drop_row + (unsigned long long)(j * TKV2 + half * 32)) >> 1);
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    const DropWords h = drop_words(seedmix, pbase + (i >> 1));
-                    pv[i] = (h.a >= thr32) ? pv[i] : 0.f;
-                    pv[i + 1] = (h.b >= thr32) ? pv[i + 1] : 0.f;
-                }
-            }
-            mbar_wait(&p_empty[st], ph ^ 1);     // the P buffer was last read by the PV MMA of tile j-2
-            uint8_t* pdst = sP + st * TILE16 + row * 128;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                const int chunk = half * 4 + g;
-                *reinterpret_cast<uint4*>(pdst + ((chunk ^ (row & 7)) << 4)) =
-                    make_uint4(pack_bf16(pv[g * 8], pv[g * 8 + 1]), pack_bf16(pv[g * 8 + 2], pv[g * 8 + 3]),
-                               pack_bf16(pv[g * 8 + 4], pv[g * 8 + 5]), pack_bf16(pv[g * 8 + 6], pv[g * 8 + 7]));
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&p_full[st]);
-        }
-        // ---- epilogue: row sum over the two halves, normalise, write O (ungated), Og (gated, head-merged) and LSE
-        s_xch[half * 128 + row] = l2.x + l2.y;
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        const float l_tot = s_xch[row] + s_xch[128 + row];
-        mbar_wait(o_full, 0);
-        tc_fence_after();
-        uint32_t ro[32];
-        tmem_ld32(tO + half * 32 + lane_off, ro);
-        tmem_ld_wait();
-        if (qi < p.Np) {
-            const float inv = l_tot > 0.f ? p.keep_scale / l_tot : 0.f;
-            const float gt = p.gate ? p.gate[((size_t)b * p.Np + qi) * p.H + hh] : 1.f;
-            __nv_bfloat16* orow = p.o + ((size_t)bh * p.Np + qi) * DH + half * 32;
-            __nv_bfloat16* grow = p.og + ((size_t)b * p.Np + qi) * (size_t)(p.H * DH) + hh * DH + half * 32;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                float v[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(ro[g * 8 + i]) * inv;
-                const uint4 u = make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
-                *reinterpret_cast<uint4*>(orow + g * 8) = u;
-                // gate the bf16-rounded output (what the backward pass sees) for consistency
-                *reinterpret_cast<uint4*>(grow + g * 8) =
-                    make_uint4(pack_bf16(bf16_lo(u.x) * gt, bf16_hi(u.x) * gt), pack_bf16(bf16_lo(u.y) * gt, bf16_hi(u.y) * gt),
-                               pack_bf16(bf16_lo(u.z) * gt, bf16_hi(u.z) * gt), pack_bf16(bf16_lo(u.w) * gt, bf16_hi(u.w) * gt));
-            }
-            if (half == 0) p.lse[(size_t)bh * p.Np + qi] = logf(l_tot);
-        }
+        return;
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 256);
+
+    // -------------------------------------------------------------------- consumer warpgroups: 64 query rows each
+    regs_alloc<232>();
+    const int cw = wg - 1, t = threadIdx.x & 127, lane = t & 31, wq = t >> 5;
+    const int cq = 2 * (lane & 3);
+    // fragment rows of this thread: r0 and r0 + 8 of the warpgroup's 64; columns 8 j + cq + {0, 1}
+    const int r0 = cw * 64 + wq * 16 + (lane >> 2);
+    const unsigned int* mb = p.maskbits + (size_t)b * p.mask_words;
+    const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
+    unsigned long long drop_row[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) drop_row[i] = ((unsigned long long)bh * p.Np + (unsigned long long)(q0 + r0 + 8 * i)) * (unsigned long long)p.drop_stride;
+    const float2 soc2 = make_float2(p.scale_over_clamp, p.scale_over_clamp);
+    const float2 cl2 = make_float2(p.clamp * LOG2E_F, p.clamp * LOG2E_F);
+    const float soc = p.scale_over_clamp, soc2s = soc * soc;
+    const float k1 = soc * p.clamp * LOG2E_F, k3 = k1 * soc2s * (-1.f / 3.f), k5 = k1 * soc2s * soc2s * (2.f / 15.f),
+                k7 = k1 * soc2s * soc2s * soc2s * (-17.f / 315.f), k9 = k1 * soc2s * soc2s * soc2s * soc2s * (62.f / 2835.f);
+    const float lim5 = 0.15f / fabsf(soc), lim9 = TANH_POLY_MAX / fabsf(soc);
+    const uint32_t thr32 = drop_thresh32(p.drop_thresh);
+    float l[2] = {0.f, 0.f};
+    float o[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+
+    mbar_wait(q_full, 0);
+    const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + cw * TILE8), 16, 1024);
+    int st = 0;
+    uint32_t ph = 0;
+    for (int j = 0; j < nkv; ++j) {
+        mbar_wait(&kv_full[st], ph);
+        float s[32];
+        fence_regs(s);
+        wgmma_fence();
+        const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + st * TILE8), 16, 1024);
+#pragma unroll
+        for (int k = 0; k < DH / 16; ++k) wgmma_ss_n64<0, 0>(s, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+        float amax = 0.f;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) amax = fmaxf(amax, fabsf(s[i]));
+        // clamp * log2(e) * tanh(u), u = s * scale / clamp, evaluated as an odd polynomial in the RAW score s with the constants folded
+        // in: s * (k1 + s^2 (k3 + s^2 (k5 + ...))) — degree 5 for |u| <= 0.15 (exact to 1e-7), degree 9 for |u| <= 0.5; tanh.approx
+        // only when a warp's tile leaves that range
+        if (__all_sync(0xffffffffu, amax <= lim5)) {
+#pragma unroll
+            for (int i = 0; i < 32; i += 2) {
+                const float2 x = make_float2(s[i], s[i + 1]);
+                const float2 x2 = fmul2(x, x);
+                float2 q = ffma2(x2, make_float2(k5, k5), make_float2(k3, k3));
+                q = ffma2(q, x2, make_float2(k1, k1));
+                const float2 y = fmul2(x, q);
+                s[i] = ex2_approx(y.x);
+                s[i + 1] = ex2_approx(y.y);
+            }
+        } else if (__all_sync(0xffffffffu, amax <= lim9)) {
+#pragma unroll
+            for (int i = 0; i < 32; i += 2) {
+                const float2 x = make_float2(s[i], s[i + 1]);
+                const float2 x2 = fmul2(x, x);
+                float2 q = ffma2(x2, make_float2(k9, k9), make_float2(k7, k7));
+                q = ffma2(q, x2, make_float2(k5, k5));
+                q = ffma2(q, x2, make_float2(k3, k3));
+                q = ffma2(q, x2, make_float2(k1, k1));
+                const float2 y = fmul2(x, q);
+                s[i] = ex2_approx(y.x);
+                s[i + 1] = ex2_approx(y.y);
+            }
+        } else {   // mixed tile: the polynomial wherever it is in range, tanh.approx only for the outliers themselves
+#pragma unroll
+            for (int i = 0; i < 32; ++i) {
+                const float x = s[i], x2 = x * x;
+                const float yp = x * __fmaf_rn(__fmaf_rn(__fmaf_rn(__fmaf_rn(k9, x2, k7), x2, k5), x2, k3), x2, k1);
+                const float y = fabsf(x) <= lim9 ? yp : tanh_approx(x * soc) * cl2.x;
+                s[i] = ex2_approx(y);
+            }
+        }
+        const unsigned int mw0 = mb[2 * j], mw1 = mb[2 * j + 1];   // keys 64 j .. 64 j + 31, 64 j + 32 .. 64 j + 63
+        if ((mw0 & mw1) != 0xffffffffu) {
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+                const unsigned int w = g < 4 ? mw0 : mw1;
+                const int bit = (8 * g + cq) & 31;
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    if (!((w >> bit) & 1u)) s[4 * g + 2 * i] = 0.f;
+                    if (!((w >> (bit + 1)) & 1u)) s[4 * g + 2 * i + 1] = 0.f;
+                }
+            }
+        }
+#pragma unroll
+        for (int g = 0; g < 8; ++g)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) l[i] += s[4 * g + 2 * i] + s[4 * g + 2 * i + 1];
+        if (p.dropout_p > 0.f) {   // the 1/(1-p) factor is applied once, to the normalised output
+#pragma unroll
+            for (int g = 0; g < 8; ++g)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const DropWords h = drop_words(seedmix, (uint32_t)((drop_row[i] + (unsigned long long)(j * 64 + 8 * g + cq)) >> 1));
+                    s[4 * g + 2 * i] = (h.a >= thr32) ? s[4 * g + 2 * i] : 0.f;
+                    s[4 * g + 2 * i + 1] = (h.b >= thr32) ? s[4 * g + 2 * i + 1] : 0.f;
+                }
+        }
+        // O += P V: the accumulator fragment of S is, 16 keys at a time, the register A fragment of the next MMA
+        fence_regs(o);
+        wgmma_fence();
+        const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + st * TILE8), 64 * 128, 1024);
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t a[4] = {pack_bf16(s[8 * kk], s[8 * kk + 1]), pack_bf16(s[8 * kk + 2], s[8 * kk + 3]),
+                                   pack_bf16(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16(s[8 * kk + 6], s[8 * kk + 7])};
+            wgmma_rs_n64<1>(o, a, vdesc + (uint64_t)(kk * 128), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o);
+        if (t == 0) mbar_arrive(&kv_empty[st]);
+        if (++st == KV_STAGES) { st = 0; ph ^= 1; }
+    }
+    // ---- epilogue: row sums over the quad, normalise, write O (ungated), Og (gated, head-merged) and LSE
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        float lt = l[i];
+        lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+        lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+        const int qi = q0 + r0 + 8 * i;
+        if (qi >= p.Np) continue;
+        const float inv = lt > 0.f ? p.keep_scale / lt : 0.f;
+        const float gt = p.gate ? p.gate[((size_t)b * p.Np + qi) * p.H + hh] : 1.f;
+        __nv_bfloat16* orow = p.o + ((size_t)bh * p.Np + qi) * DH;
+        __nv_bfloat16* grow = p.og + ((size_t)b * p.Np + qi) * (size_t)(p.H * DH) + hh * DH;
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+            const uint32_t u = pack_bf16(o[4 * g + 2 * i] * inv, o[4 * g + 2 * i + 1] * inv);
+            *reinterpret_cast<uint32_t*>(orow + 8 * g + cq) = u;
+            // gate the bf16-rounded output (what the backward pass sees) for consistency
+            *reinterpret_cast<uint32_t*>(grow + 8 * g + cq) = pack_bf16(bf16_lo(u) * gt, bf16_hi(u) * gt);
+        }
+        if ((lane & 3) == 0) p.lse[(size_t)bh * p.Np + qi] = logf(lt);
     }
 }
 
 // ================================================================================================ backward
-// One CTA per (128-key tile, head, batch), 576 threads:
-//   warp 0 lane 0 : TMA producer — K, V once; Q_i / dO_i tiles (128 queries) through a 2-stage ring
-//   warp 1 lane 0 : MMA issuer   — per query tile i:  S = Q_i K^T, dP = dO_i V^T           (128x128x16 x4 each, K-major operands)
-//                                   then, once the math warps have written P and dS (bf16) to swizzled smem:
-//                                   dV += P^T dO_i, dK += dS^T Q_i (A MN-major from the P / dS tiles, B MN-major)
-//                                   dQ_i = dS K                    (A K-major dS tile, B = K tile MN-major)
-//   warps 2..17   : math         — row r = 32*(warp%4)+lane, key quarter = (warp-2)/4 (4 warps per scheduler hide the MUFU /
-//                                   TMEM latencies): recompute softclamp + softmax from the saved LSE,
-//                                   dS = P (dP - delta)(1 - tanh^2) scale, write P_drop / dS tiles; warps 2..9 also flush dQ_i
-//                                   from TMEM with coalesced fp32 atomics and finally store dK, dV.
-// TMEM columns: S [0,128) dP [128,256) dV [256,320) dK [320,384) dQ [384,448).
+// One CTA per (128-key tile, head, batch), 384 threads:
+//   warpgroup 0, one thread : TMA producer — K, V once; Q_i / dO_i tiles (64 queries) through a 3-stage ring
+//   warpgroups 1, 2         : 64 keys each, per query tile i (all operands from smem, accumulators in registers):
+//                             S^T = K Q_i^T, dP^T = V dO_i^T                 (wgmma m64n64k16, K-major operands)
+//                             recompute softclamp + softmax from the saved LSE, dS^T = P^T (dP^T - delta)(1 - tanh^2) scale
+//                             dV += P^T dO_i, dK += dS^T Q_i                 (register A operands, B MN-major)
+//                             dQ_i += dS K_w through a swizzled smem copy of dS^T (A MN-major), flushed with fp32 vector atomics.
 struct AttnBwdTcP {
     const unsigned int* maskbits; int mask_words;
     const float *lse, *delta;
@@ -347,272 +286,217 @@ struct AttnBwdTcP {
     unsigned long long seed;
     const unsigned long long* seed_dev;   // optional device addend of the seed (CUDA-graph replays)
 };
+constexpr int QDO_STAGES = 3, TQB = 64;
 
-__global__ void __launch_bounds__(576, 1)
-attn_bwd_tc_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                   const __grid_constant__ CUtensorMap tmDO, const AttnBwdTcP p) {
+// P^T / dS^T of one query tile from the S^T / dP^T fragments (rows = keys kr, kr + 8; columns = queries qt0 + 8 g + cq + {0, 1})
+template <bool POLY, bool DROP>
+__device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float (&s)[32], const float (&dp)[32], int bh, int qt0, int cq,
+                                               const bool (&kok)[2], const int (&key)[2], uint32_t seedmix, uint32_t (&ppk)[16], uint32_t (&dpk)[16]) {
+    const uint32_t thr32 = drop_thresh32(p.drop_thresh);
+    const float clog = p.clamp * LOG2E_F;
+#pragma unroll
+    for (int g = 0; g < 8; ++g) {
+        float pe[2][2], dsv[2][2];
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+            const int qi = qt0 + 8 * g + cq + c;
+            const bool qok = qi < p.Np;
+            const float nlse2 = qok ? -__ldg(p.lse + (size_t)bh * p.Np + qi) * LOG2E_F : 0.f;
+            const float dl = qok ? __ldg(p.delta + (size_t)bh * p.Np + qi) : 0.f;
+            const unsigned long long qbase = ((unsigned long long)bh * p.Np + (unsigned long long)qi) * (unsigned long long)p.drop_stride;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int e = 4 * g + 2 * i + c;
+                const float x = s[e] * p.scale_over_clamp;
+                float th;
+                if constexpr (POLY) th = tanh_poly2(make_float2(x, 0.f)).x;
+                else th = fabsf(x) <= TANH_POLY_MAX ? tanh_poly2(make_float2(x, 0.f)).x : tanh_approx(x);   // outliers only
+                float pv = ex2_approx(__fmaf_rn(th, clog, nlse2));
+                pv = (qok && kok[i]) ? pv : 0.f;
+                const float dsc = __fmaf_rn(th * -p.scale, th, p.scale);   // (1 - tanh^2) * scale = d(clamped logit)/d(raw score)
+                float tt, pd;
+                if constexpr (DROP) {
+                    const DropWords h = drop_words(seedmix, (uint32_t)((qbase + (unsigned long long)key[i]) >> 1));
+                    const bool keep = ((key[i] & 1) ? h.b : h.a) >= thr32;
+                    tt = __fmaf_rn(keep ? dp[e] : 0.f, p.keep_scale, -dl);
+                    pd = keep ? pv : 0.f;   // dV uses the dropped probabilities, dS the un-dropped ones
+                } else {
+                    tt = dp[e] - dl;
+                    pd = pv;
+                }
+                pe[i][c] = pd;
+                dsv[i][c] = (pv * tt) * dsc;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            ppk[2 * g + i] = pack_bf16(pe[i][0], pe[i][1]);
+            dpk[2 * g + i] = pack_bf16(dsv[i][0], dsv[i][1]);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(384, 1)
+attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                      const __grid_constant__ CUtensorMap tmDO, const AttnBwdTcP p) {
     extern __shared__ uint8_t smem_raw[];
-    // 1024-byte alignment by OFFSET, not by integer round-trip: the pointer keeps its shared-memory provenance, so tile / staging
-    // accesses compile to LDS / STS instead of generic LD / ST (+ a full MEMBAR before the async-proxy fence)
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* sK = smem;
-    uint8_t* sV = sK + TILE16;
-    uint8_t* sQ = sV + TILE16;           // [2]
-    uint8_t* sDO = sQ + 2 * TILE16;      // [2]
-    uint8_t* sP = sDO + 2 * TILE16;      // 32 KB
-    uint8_t* sDS = sP + PTILE;           // 32 KB
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + PTILE);
-    uint64_t* kv_full = bars;            // 1
-    uint64_t* qdo_full = bars + 1;       // 2
-    uint64_t* qdo_empty = bars + 3;      // 2
-    uint64_t* sdp_full = bars + 5;       // 1
-    uint64_t* sdp_empty = bars + 6;      // 1 (8 arrivals)
-    uint64_t* pds_full = bars + 7;       // 1 (8 arrivals)
-    uint64_t* mma3_done = bars + 8;      // 1
-    uint64_t* dq_empty = bars + 9;       // 1 (8 arrivals)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
+    uint8_t* sK = smem;                          // 16 KB (128 keys)
+    uint8_t* sV = sK + TILE16;                   // 16 KB
+    uint8_t* sQ = sV + TILE16;                   // [3] x 8 KB (64 queries)
+    uint8_t* sDO = sQ + QDO_STAGES * TILE8;      // [3] x 8 KB
+    uint8_t* sDS = sDO + QDO_STAGES * TILE8;     // [2 warpgroups] x 8 KB: dS^T (64 keys x 64 queries), 128B-swizzled
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 2 * TILE8);
+    uint64_t* kv_full = bars;                    // 1
+    uint64_t* qdo_full = bars + 1;               // 3
+    uint64_t* qdo_empty = bars + 4;              // 3 (one arrival per consumer warpgroup)
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
     const int kt = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
     const int bh = b * p.H + hh;
     const int k0 = kt * TKV;
     const int nq = p.nq;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
         mbar_init(kv_full, 1);
-        for (int i = 0; i < 2; ++i) { mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 1); }
-        mbar_init(sdp_full, 1); mbar_init(sdp_empty, 16); mbar_init(pds_full, 16); mbar_init(mma3_done, 1); mbar_init(dq_empty, 8);
+        for (int i = 0; i < QDO_STAGES; ++i) { mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tS = tmem_base, tDP = tmem_base + 128, tDV = tmem_base + 256, tDK = tmem_base + 320, tDQ = tmem_base + 384;
-    pdl_wait();   // prologue above overlaps the previous kernel's tail (ptx.cuh)
+    pdl_wait();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        regs_dealloc<40>();
+        if (threadIdx.x == 0) {
             const int row_base = bh * p.Np;
             mbar_arrive_expect_tx(kv_full, 2 * TILE16);
             tma_load_2d(sK, &tmK, kv_full, 0, row_base + k0);
             tma_load_2d(sV, &tmV, kv_full, 0, row_base + k0);
+            int st = 0;
+            uint32_t ph = 0;
             for (int i = 0; i < nq; ++i) {
-                const int st = i & 1;
-                mbar_wait(&qdo_empty[st], (((i >> 1) & 1) ^ 1));
-                mbar_arrive_expect_tx(&qdo_full[st], 2 * TILE16);
+                mbar_wait(&qdo_empty[st], ph ^ 1);
+                mbar_arrive_expect_tx(&qdo_full[st], 2 * TILE8);
                 const int qt_i = (i + kt) % nq;   // staggered query-tile order: the key-tile CTAs of one head never flush the same dQ rows together
-                tma_load_2d(sQ + st * TILE16, &tmQ, &qdo_full[st], 0, row_base + qt_i * TQ);
-                tma_load_2d(sDO + st * TILE16, &tmDO, &qdo_full[st], 0, row_base + qt_i * TQ);
+                tma_load_2d(sQ + st * TILE8, &tmQ, &qdo_full[st], 0, row_base + qt_i * TQB);
+                tma_load_2d(sDO + st * TILE8, &tmDO, &qdo_full[st], 0, row_base + qt_i * TQB);
+                if (++st == QDO_STAGES) { st = 0; ph ^= 1; }
             }
             pdl_launch_dependents();
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            constexpr uint32_t id_s = make_idesc_bf16(128, 128, 0, 0);   // S, dP
-            constexpr uint32_t id_t = make_idesc_bf16(128, 64, 1, 1);    // dV, dK (A^T from smem, B MN-major)
-            constexpr uint32_t id_q = make_idesc_bf16(128, 64, 0, 1);    // dQ
-            mbar_wait(kv_full, 0);
-            const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK), 0, 1024);             // K-major (B of S)
-            const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV), 0, 1024);             // K-major (B of dP)
-            const uint64_t kmn = make_smem_desc_sw128(smem_u32(sK), 128 * 128, 1024);        // MN-major (B of dQ)
-            const uint64_t pT = make_smem_desc_sw128(smem_u32(sP), 128 * 128, 1024);         // MN-major A (P^T)
-            const uint64_t dsT = make_smem_desc_sw128(smem_u32(sDS), 128 * 128, 1024);       // MN-major A (dS^T)
-            // S_t = Q_t K^T and dP_t = dO_t V^T. They are issued one query tile AHEAD of the dV/dK/dQ MMAs: the math warps copy
-            // S/dP to registers first thing (sdp_empty), so tile t+1's scores are ready the moment they finish tile t and the three
-            // accumulation MMAs of tile t run under the math of tile t+1 (issued in tile order the two groups serialised: ncu r3).
-            auto issue_sdp = [&](int t) {
-                const int st = t & 1;
-                mbar_wait(&qdo_full[st], (t >> 1) & 1);
-                mbar_wait(sdp_empty, (uint32_t)(t & 1) ^ 1u);
-                tc_fence_after();
-                const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + st * TILE16), 0, 1024);
-                const uint64_t dodesc = make_smem_desc_sw128(smem_u32(sDO + st * TILE16), 0, 1024);
+        return;
+    }
+
+    regs_alloc<232>();
+    const int cw = wg - 1, t = threadIdx.x & 127, lane = t & 31, wq = t >> 5;
+    const int cq = 2 * (lane & 3);
+    const int kr0 = cw * 64 + wq * 16 + (lane >> 2);   // fragment rows (keys) kr0, kr0 + 8 of the CTA's 128
+    int key[2];
+    bool kok[2];
 #pragma unroll
-                for (int k = 0; k < 4; ++k) umma_f16(tS, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), id_s, k > 0 ? 1u : 0u);
+    for (int i = 0; i < 2; ++i) {
+        key[i] = k0 + kr0 + 8 * i;
+        kok[i] = key[i] < p.Np && ((p.maskbits[(size_t)b * p.mask_words + (key[i] >> 5)] >> (key[i] & 31)) & 1u);
+    }
+    const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
+    const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + cw * TILE8), 16, 1024);        // K-major A of S^T
+    const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + cw * TILE8), 16, 1024);        // K-major A of dP^T
+    const uint64_t kmn = make_smem_desc_sw128(smem_u32(sK + cw * TILE8), 64 * 128, 1024);    // MN-major B of dQ
+    uint8_t* ds_tile = sDS + cw * TILE8;
+    const uint64_t dsdesc = make_smem_desc_sw128(smem_u32(ds_tile), 64 * 128, 1024);         // MN-major A of dQ (dS^T stored)
+    float dv[32], dk[32];
 #pragma unroll
-                for (int k = 0; k < 4; ++k) umma_f16(tDP, dodesc + (uint64_t)(k * 2), vdesc + (uint64_t)(k * 2), id_s, k > 0 ? 1u : 0u);
-                umma_commit(sdp_full);
-            };
-            issue_sdp(0);
-            for (int i = 0; i < nq; ++i) {
-                const int st = i & 1;
-                const uint32_t ph = i & 1;
-                if (i + 1 < nq) issue_sdp(i + 1);
-                mbar_wait(pds_full, ph);
-                mbar_wait(dq_empty, ph ^ 1);
-                tc_fence_after();
-                const uint64_t qmn = make_smem_desc_sw128(smem_u32(sQ + st * TILE16), 128 * 128, 1024);
-                const uint64_t domn = make_smem_desc_sw128(smem_u32(sDO + st * TILE16), 128 * 128, 1024);
+    for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+
+    mbar_wait(kv_full, 0);
+    int st = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < nq; ++it) {
+        const int qt0 = ((it + kt) % nq) * TQB;
+        mbar_wait(&qdo_full[st], ph);
+        const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + st * TILE8), 16, 1024);
+        const uint64_t dodesc = make_smem_desc_sw128(smem_u32(sDO + st * TILE8), 16, 1024);
+        uint32_t ppk[16], dpk[16];   // bf16-packed P_drop^T and dS^T fragments
+        {
+            float s[32], dp[32];
+            fence_regs(s); fence_regs(dp);
+            wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < 8; ++k) umma_f16(tDV, pT + (uint64_t)(k * 128), domn + (uint64_t)(k * 128), id_t, (i > 0 || k > 0) ? 1u : 0u);
+            for (int k = 0; k < 4; ++k) wgmma_ss_n64<0, 0>(s, kdesc + (uint64_t)(k * 2), qdesc + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
 #pragma unroll
-                for (int k = 0; k < 8; ++k) umma_f16(tDK, dsT + (uint64_t)(k * 128), qmn + (uint64_t)(k * 128), id_t, (i > 0 || k > 0) ? 1u : 0u);
+            for (int k = 0; k < 4; ++k) wgmma_ss_n64<0, 0>(dp, vdesc + (uint64_t)(k * 2), dodesc + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(s); fence_regs(dp);
+            float amax = 0.f;
 #pragma unroll
-                for (int k = 0; k < 8; ++k) {
-                    const uint64_t dsk = make_smem_desc_sw128(smem_u32(sDS) + (k >> 2) * TILE16 + (k & 3) * 32, 0, 1024);
-                    umma_f16(tDQ, dsk, kmn + (uint64_t)(k * 128), id_q, k > 0 ? 1u : 0u);
-                }
-                umma_commit(mma3_done);
-                umma_commit(&qdo_empty[st]);
+            for (int e = 0; e < 32; ++e) amax = fmaxf(amax, fabsf(s[e]));
+            const bool small = __all_sync(0xffffffffu, amax * fabsf(p.scale_over_clamp) <= TANH_POLY_MAX);   // same rule as the forward
+            const bool drop = p.dropout_p > 0.f;
+            if (small) {
+                if (drop) bwd_score_math<true, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                else bwd_score_math<true, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+            } else {
+                if (drop) bwd_score_math<false, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                else bwd_score_math<false, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
             }
         }
-    } else {
-        // -------------------------------------------------------------------- math warps
-        const int mw = warp - 2;
-        const int qd = warp & 3, part = mw >> 2;   // part: which 32 of the tile's 128 keys
-        const int half = part & 1;                 // dQ / dK / dV column half handled by warps with part < 2
-        const bool flusher = part < 2;
-        const int row = qd * 32 + lane;
-        const uint32_t lane_off = (uint32_t)(qd * 32) << 16;
-        const unsigned int mbits1 = p.maskbits[(size_t)b * p.mask_words + kt * 4 + part];
-        const bool all_valid = mbits1 == 0xffffffffu;
-        const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
-        const float keep_scale = p.keep_scale;
-
-        float* dq_stg = reinterpret_cast<float*>(sDS + PTILE + 256) + (mw & 7) * (32 * 33);
-        auto flush_dq = [&](int i) {   // dQ_i (TMEM) -> fp32 global atomics; this warp owns 32 rows x 32 of the 64 columns
-            uint32_t r[32];
-            tmem_ld32(tDQ + half * 32 + lane_off, r);
-            tmem_ld_wait();
-            tc_fence_before();
-            float v[32];
+        // dS^T into the warpgroup's swizzled smem tile (row = key, 64 queries = one 128-byte swizzle atom per row)
 #pragma unroll
-            for (int c = 0; c < 32; ++c) v[c] = __uint_as_float(r[c]);
-            const int q0r = ((i + kt) % nq) * TQ + qd * 32;
-            warp_red_rows_f32(dq_stg, v, p.dq_acc + (size_t)bh * p.Np * DH + half * 32, DH, q0r, p.Np, 32, lane);
-            if (lane == 0) mbar_arrive(dq_empty);
-        };
-
-        for (int i = 0; i < nq; ++i) {
-            const uint32_t ph = i & 1;
-            const int qi = ((i + kt) % nq) * TQ + row;
-            const bool rvalid = qi < p.Np;
-            const float lse = rvalid ? p.lse[(size_t)bh * p.Np + qi] : 0.f;
-            const float dl = rvalid ? p.delta[(size_t)bh * p.Np + qi] : 0.f;
-            const float lse2 = lse * LOG2E_F;
-            mbar_wait(sdp_full, ph);
-            tc_fence_after();
-            uint32_t ppk[16], dpk[16];   // bf16-packed P_drop and dS of this thread's 32 keys
-            {
-                uint32_t rs[32], rd[32];
-                tmem_ld32(tS + part * 32 + lane_off, rs);
-                tmem_ld32(tDP + part * 32 + lane_off, rd);
-                tmem_ld_wait();
-                uint32_t pbase = 0;
-                if (p.dropout_p > 0.f) {
-                    const unsigned long long kbase = ((unsigned long long)bh * p.Np + (unsigned long long)qi) * (unsigned long long)p.drop_stride +
-                                                     (unsigned long long)(k0 + part * 32);
-                    pbase = (uint32_t)(kbase >> 1);
-                }
-                // warp-uniform: no key of this quarter is masked and every query row of the tile exists
-                const bool no_mask = all_valid && (((i + kt) % nq) * TQ + TQ <= p.Np);
-                const float2 soc2 = make_float2(p.scale_over_clamp, p.scale_over_clamp), cl2 = make_float2(p.clamp * LOG2E_F, p.clamp * LOG2E_F);
-                const float2 nlse2 = make_float2(-lse2, -lse2), sc2 = make_float2(p.scale, p.scale), nsc2 = make_float2(-p.scale, -p.scale);
-                const float2 ks2 = make_float2(keep_scale, keep_scale), ndl2 = make_float2(-dl, -dl);
-                const uint32_t thr32 = drop_thresh32(p.drop_thresh);
-                float amax = 0.f;
+        for (int g = 0; g < 8; ++g)
 #pragma unroll
-                for (int e = 0; e < 32; ++e) amax = fmaxf(amax, fabsf(__uint_as_float(rs[e])));
-                const bool small = __all_sync(0xffffffffu, amax * fabsf(p.scale_over_clamp) <= TANH_POLY_MAX);   // same rule as the forward
-                // one straight-line variant per (tanh path, masking, dropout) combination — all three are warp-uniform, and a
-                // runtime test inside the unrolled loop costs predicate juggling and stack traffic on every key pair (ncu r5)
-                auto score_math = [&](auto use_poly, auto masked, auto dropped) {
-#pragma unroll
-                for (int e = 0; e < 32; e += 2) {
-                    // packed fp32x2 math on the key pair (e, e+1); the 1/(1-p) of the dropped probabilities that feed dV is applied
-                    // once to the dV accumulator in the epilogue
-                    const float2 x = __fmul2_rn(make_float2(__uint_as_float(rs[e]), __uint_as_float(rs[e + 1])), soc2);
-                    float2 th;
-                    if constexpr (decltype(use_poly)::value) th = tanh_poly2(x);
-                    else th = make_float2(tanh_approx(x.x), tanh_approx(x.y));
-                    const float2 y = __ffma2_rn(th, cl2, nlse2);
-                    float pex = ex2_approx(y.x), pey = ex2_approx(y.y);
-                    if constexpr (decltype(masked)::value) {
-                        pex = (rvalid && ((mbits1 >> e) & 1u)) ? pex : 0.f;
-                        pey = (rvalid && ((mbits1 >> (e + 1)) & 1u)) ? pey : 0.f;
-                    }
-                    const float2 ds = __ffma2_rn(__fmul2_rn(th, nsc2), th, sc2);   // (1 - tanh^2) * scale = d(clamped logit)/d(raw score)
-                    const float dpx = __uint_as_float(rd[e]), dpy = __uint_as_float(rd[e + 1]);
-                    float2 t;
-                    if constexpr (decltype(dropped)::value) {
-                        const DropWords h = drop_words(seedmix, pbase + (e >> 1));
-                        const bool k0_ = h.a >= thr32, k1_ = h.b >= thr32;
-                        t = __ffma2_rn(make_float2(k0_ ? dpx : 0.f, k1_ ? dpy : 0.f), ks2, ndl2);
-                        ppk[e >> 1] = pack_bf16(k0_ ? pex : 0.f, k1_ ? pey : 0.f);   // dV uses the dropped probabilities, dS the un-dropped ones
-                    } else {
-                        t = __fadd2_rn(make_float2(dpx, dpy), ndl2);
-                        ppk[e >> 1] = pack_bf16(pex, pey);
-                    }
-                    const float2 dsv = __fmul2_rn(__fmul2_rn(make_float2(pex, pey), t), ds);
-                    dpk[e >> 1] = pack_bf16(dsv.x, dsv.y);
-                }
-                };
-                using T_ = std::true_type;
-                using F_ = std::false_type;
-                const bool drop = p.dropout_p > 0.f;
-                if (small) {
-                    if (no_mask) { if (drop) score_math(T_{}, F_{}, T_{}); else score_math(T_{}, F_{}, F_{}); }
-                    else { if (drop) score_math(T_{}, T_{}, T_{}); else score_math(T_{}, T_{}, F_{}); }
-                } else {
-                    if (no_mask) { if (drop) score_math(F_{}, F_{}, T_{}); else score_math(F_{}, F_{}, F_{}); }
-                    else { if (drop) score_math(F_{}, T_{}, T_{}); else score_math(F_{}, T_{}, F_{}); }
-                }
+            for (int i = 0; i < 2; ++i) {
+                const int r = wq * 16 + (lane >> 2) + 8 * i;
+                *reinterpret_cast<uint32_t*>(ds_tile + r * 128 + ((g ^ (r & 7)) << 4) + cq * 2) = dpk[2 * g + i];
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(sdp_empty);
-            // P / dS smem tiles and the dQ accumulator of the previous query tile must have been consumed by its MMAs
-            if (i > 0) {
-                mbar_wait(mma3_done, (i - 1) & 1);
-                tc_fence_after();
-                if (flusher) flush_dq(i - 1);
-            }
-            uint8_t* prow = sP + (part >> 1) * TILE16 + row * 128;
-            uint8_t* drow = sDS + (part >> 1) * TILE16 + row * 128;
+        fence_proxy_async();
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+        // dV += P^T dO_i, dK += dS^T Q_i (register A: 16 queries per MMA), dQ_i = dS K_w
+        const uint64_t domn = make_smem_desc_sw128(smem_u32(sDO + st * TILE8), 64 * 128, 1024);
+        const uint64_t qmn = make_smem_desc_sw128(smem_u32(sQ + st * TILE8), 64 * 128, 1024);
+        float dq[32];
+        fence_regs(dv); fence_regs(dk); fence_regs(dq);
+        wgmma_fence();
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                const int off = (((part & 1) * 4 + g) ^ (row & 7)) << 4;
-                *reinterpret_cast<uint4*>(prow + off) = make_uint4(ppk[g * 4], ppk[g * 4 + 1], ppk[g * 4 + 2], ppk[g * 4 + 3]);
-                *reinterpret_cast<uint4*>(drow + off) = make_uint4(dpk[g * 4], dpk[g * 4 + 1], dpk[g * 4 + 2], dpk[g * 4 + 3]);
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(pds_full);
+        for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t ap[4] = {ppk[4 * kk], ppk[4 * kk + 1], ppk[4 * kk + 2], ppk[4 * kk + 3]};
+            wgmma_rs_n64<1>(dv, ap, domn + (uint64_t)(kk * 128), 1u);
         }
-        mbar_wait(mma3_done, (nq - 1) & 1);
-        tc_fence_after();
-        if (flusher) flush_dq(nq - 1);
-        // ---- dV, dK (TMEM lanes = keys): a flusher thread stores 32 of the 64 columns of key row `row`
-        const int key = k0 + row;
-        if (flusher) {
-            uint32_t rv[32], rk[32];
-            tmem_ld32(tDV + half * 32 + lane_off, rv);
-            tmem_ld32(tDK + half * 32 + lane_off, rk);
-            tmem_ld_wait();
-            if (key < p.Np) {
-                __nv_bfloat16* dvp = p.dv + ((size_t)bh * p.Np + key) * DH + half * 32;
-                __nv_bfloat16* dkp = p.dk + ((size_t)bh * p.Np + key) * DH + half * 32;
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    const float ks = keep_scale;   // deferred 1/(1-p) of the dropped probabilities
-                    *reinterpret_cast<uint4*>(dvp + g * 8) =
-                        make_uint4(pack_bf16(__uint_as_float(rv[g * 8]) * ks, __uint_as_float(rv[g * 8 + 1]) * ks), pack_bf16(__uint_as_float(rv[g * 8 + 2]) * ks, __uint_as_float(rv[g * 8 + 3]) * ks),
-                                   pack_bf16(__uint_as_float(rv[g * 8 + 4]) * ks, __uint_as_float(rv[g * 8 + 5]) * ks), pack_bf16(__uint_as_float(rv[g * 8 + 6]) * ks, __uint_as_float(rv[g * 8 + 7]) * ks));
-                    *reinterpret_cast<uint4*>(dkp + g * 8) =
-                        make_uint4(pack_bf16(__uint_as_float(rk[g * 8]), __uint_as_float(rk[g * 8 + 1])), pack_bf16(__uint_as_float(rk[g * 8 + 2]), __uint_as_float(rk[g * 8 + 3])),
-                                   pack_bf16(__uint_as_float(rk[g * 8 + 4]), __uint_as_float(rk[g * 8 + 5])), pack_bf16(__uint_as_float(rk[g * 8 + 6]), __uint_as_float(rk[g * 8 + 7])));
-                }
-            }
+        for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t ad[4] = {dpk[4 * kk], dpk[4 * kk + 1], dpk[4 * kk + 2], dpk[4 * kk + 3]};
+            wgmma_rs_n64<1>(dk, ad, qmn + (uint64_t)(kk * 128), 1u);
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_ss_n64<1, 1>(dq, dsdesc + (uint64_t)(k * 128), kmn + (uint64_t)(k * 128), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dv); fence_regs(dk); fence_regs(dq);
+        if (t == 0) mbar_arrive(&qdo_empty[st]);
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");   // every thread's MMAs have read the dS tile before it is rewritten
+        if (++st == QDO_STAGES) { st = 0; ph ^= 1; }
+        // dQ_i partial of this warpgroup's 64 keys: rows = queries, columns = head dims
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int qi = qt0 + wq * 16 + (lane >> 2) + 8 * i;
+            if (qi >= p.Np) continue;
+            float* dqr = p.dq_acc + ((size_t)bh * p.Np + qi) * DH;
+#pragma unroll
+            for (int g = 0; g < 8; ++g) atomicAdd(reinterpret_cast<float2*>(dqr + 8 * g + cq), make_float2(dq[4 * g + 2 * i], dq[4 * g + 2 * i + 1]));
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
+    // ---- dV (with the deferred 1/(1-p) of the dropped probabilities), dK: rows = keys
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        if (key[i] >= p.Np) continue;
+        __nv_bfloat16* dvp = p.dv + ((size_t)bh * p.Np + key[i]) * DH;
+        __nv_bfloat16* dkp = p.dk + ((size_t)bh * p.Np + key[i]) * DH;
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+            *reinterpret_cast<uint32_t*>(dvp + 8 * g + cq) = pack_bf16(dv[4 * g + 2 * i] * p.keep_scale, dv[4 * g + 2 * i + 1] * p.keep_scale);
+            *reinterpret_cast<uint32_t*>(dkp + 8 * g + cq) = pack_bf16(dk[4 * g + 2 * i], dk[4 * g + 2 * i + 1]);
+        }
     }
 }
 
@@ -665,7 +549,7 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_fwd: bad shape");
     B200_REQUIRE(a->softclamp > 0.f, "attn_fwd: softclamp value must be > 0 (the reference always clamps, e2_tts.py:548-551)");
     B200_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_fwd: dropout must be in [0,1)");
-    // the tcgen05 kernel exponentiates the clamped logits without a running maximum: exp(+-64) is well inside fp32 / bf16 range,
+    // the wgmma kernel exponentiates the clamped logits without a running maximum: exp(+-64) is well inside fp32 / bf16 range,
     // a looser clamp (the reference default is 50, e2_tts.py:548-551) goes through the online-softmax mma.sync kernel instead
     if (a->softclamp > 64.f) return b200_attn_fwd_legacy(a, stream);
     AttnTcP p{};
@@ -687,14 +571,14 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     p.drop_stride = (a->Np + 1) & ~1;
     CUtensorMap tq, tk, tv;
     const long long rows = (long long)a->B * a->H * a->Np;
-    if (make_head_map(&tq, a->q, rows) || make_head_map(&tk, a->k, rows, TKV2) || make_head_map(&tv, a->v, rows, TKV2)) return -1;
-    const int smem = TILE16 + 2 * KV2_STAGES * TILE8 + 2 * TILE16 + 160 + 1024 + 1024;   // Q, K/V rings, P[2], barriers, row sums, alignment slack
+    if (make_head_map(&tq, a->q, rows) || make_head_map(&tk, a->k, rows, 64) || make_head_map(&tv, a->v, rows, 64)) return -1;
+    const int smem = TILE16 + 2 * KV_STAGES * TILE8 + 128 + 1024;   // Q, K/V rings, barriers, alignment slack
     static DeviceOnce once;
-    cudaError_t e = set_max_smem_once(once, attn_fwd_tc64_kernel, smem);
+    cudaError_t e = set_max_smem_once(once, attn_fwd_wgmma_kernel, smem);
     B200_REQUIRE(e == cudaSuccess, "attn_fwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     dim3 grid((a->Np + TQ - 1) / TQ, a->H, a->B);
-    B200_LAUNCH(attn_fwd_tc64_kernel, grid, 320, smem, st, tq, tk, tv, p);
-    return check_launch("attn_fwd_tc64_kernel");
+    B200_LAUNCH(attn_fwd_wgmma_kernel, grid, 384, smem, st, tq, tk, tv, p);
+    return check_launch("attn_fwd_wgmma_kernel");
 }
 
 // dO = dOg * gate, delta = <dO, O>, d_gate — defined in attn.cu
@@ -709,8 +593,8 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     B200_REQUIRE(a->softclamp > 0.f && a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_bwd: bad softclamp / dropout");
     if (int rc = launch_attn_bwd_prep(a, st)) return rc;
     AttnBwdTcP p{};
-    p.nq = (a->Np + TQ - 1) / TQ;
-    p.mask_words = p.nq * 4;
+    p.nq = (a->Np + TQB - 1) / TQB;
+    p.mask_words = ((a->Np + TKV - 1) / TKV) * 4;
     p.maskbits = reinterpret_cast<const unsigned int*>(a->ws_maskbits);
     if (!a->maskbits_ready) {
         const int total = a->B * p.mask_words;
@@ -731,12 +615,12 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     p.seed = a->seed; p.seed_dev = reinterpret_cast<const unsigned long long*>(a->seed_dev);
     CUtensorMap tq, tk, tv, tdo;
     const long long rows = (long long)a->B * a->H * a->Np;
-    if (make_head_map(&tq, a->q, rows) || make_head_map(&tk, a->k, rows) || make_head_map(&tv, a->v, rows) || make_head_map(&tdo, a->ws_dO, rows)) return -1;
-    const int smem = 6 * TILE16 + 2 * PTILE + 256 + 8 * 32 * 33 * 4 + 1024;
+    if (make_head_map(&tq, a->q, rows, TQB) || make_head_map(&tk, a->k, rows) || make_head_map(&tv, a->v, rows) || make_head_map(&tdo, a->ws_dO, rows, TQB)) return -1;
+    const int smem = 2 * TILE16 + 2 * QDO_STAGES * TILE8 + 2 * TILE8 + 128 + 1024;   // K, V, Q/dO rings, dS^T tiles, barriers, slack
     static DeviceOnce once;
-    cudaError_t e2 = set_max_smem_once(once, attn_bwd_tc_kernel, smem);
+    cudaError_t e2 = set_max_smem_once(once, attn_bwd_wgmma_kernel, smem);
     B200_REQUIRE(e2 == cudaSuccess, "attn_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
-    dim3 grid(p.nq, a->H, a->B);
-    B200_LAUNCH(attn_bwd_tc_kernel, grid, 576, smem, st, tq, tk, tv, tdo, p);
-    return check_launch("attn_bwd_tc_kernel");
+    dim3 grid((a->Np + TKV - 1) / TKV, a->H, a->B);
+    B200_LAUNCH(attn_bwd_wgmma_kernel, grid, 384, smem, st, tq, tk, tv, tdo, p);
+    return check_launch("attn_bwd_wgmma_kernel");
 }

@@ -79,7 +79,7 @@ inline int num_sms() {
     int n = cache[dev].load(std::memory_order_relaxed);
     if (!n) {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;   // H100 SXM
         cache[dev].store(n, std::memory_order_relaxed);
     }
     return n;

@@ -1,16 +1,13 @@
-// tcgen05 / TMEM / TMA GEMM for sm_100a — the tensor-core core of the E2-TTS hot path.
+// wgmma / TMA GEMM for sm_90a — the tensor-core core of the E2-TTS hot path.
 //
-//   D[M,N] = epilogue( sum_k A[m,k] * B[n,k] ),  bf16 operands, fp32 accumulation in tensor memory.
+//   D[M,N] = epilogue( sum_k A[m,k] * B[n,k] ),  bf16 operands, fp32 accumulation in registers.
 //
-// Structure (one persistent CTA per SM, 320 threads, warp-specialised):
-//   warp 0 lane 0 : TMA producer   — cp.async.bulk.tensor 2-D tiles (128B swizzle) into a kStages smem ring
-//   warp 1 lane 0 : MMA issuer     — tcgen05.mma.cta_group::1.kind::f16, 128 x BN x 16 per instruction,
-//                                    accumulators double-buffered in TMEM (2 x BN columns)
-//   warps 2..9    : epilogue       — tcgen05.ld 32x32b.x32 (one accumulator row per thread; two warps share a lane quadrant and
-//                                    split the tile columns), fused bias / AdaLN gate / row mask / residual / GEGLU(+dropout);
-//                                    bf16 tiles leave through swizzled smem staging + TMA tile stores, fp32 split-K partials through
-//                                    vector reductions (red.global.add.v4.f32)
-// Three mbarrier pipelines: smem full/empty (TMA<->MMA), TMEM full/empty (MMA<->epilogue), static tile loop.
+// Structure (one persistent CTA per SM, 384 threads, warp-specialised):
+//   warpgroup 0, one thread : TMA producer — cp.async.bulk.tensor 2-D tiles (128B swizzle) into a kStages smem ring
+//   warpgroups 1, 2         : MMA + epilogue — each owns 64 * MH rows of the CTA tile: wgmma.m64nBNk16 from the smem ring into
+//                             register accumulators, then the fused epilogue (bias / AdaLN gate / row mask / residual / GEGLU(+dropout))
+//                             straight from the accumulator fragments; fp32 split-K partials leave through vector atomics.
+// While a consumer warpgroup runs its epilogue the producer is already filling the ring with the next tile's operands.
 // Operands may be K-major or MN-major (transposed storage) so that the backward contractions
 // dX = dY*W and dW = dY^T*X read activations exactly as they lie in HBM — no transposes are materialised.
 #include <stdlib.h>
@@ -21,8 +18,8 @@
 namespace b200 {
 
 constexpr int BM = 128;
-constexpr int BK = 64;          // 64 bf16 = one 128-byte swizzle atom
-constexpr int kGemmThreads = 320;   // warp 0 TMA, warp 1 TMEM alloc + MMA issue, warps 2..9 epilogue (two per TMEM lane quadrant)
+constexpr int BK = 64;              // 64 bf16 = one 128-byte swizzle atom
+constexpr int kGemmThreads = 384;   // warpgroup 0 TMA, warpgroups 1..2 MMA + epilogue
 constexpr int A_STAGE_BYTES = BM * BK * 2;
 
 struct GemmParams {
@@ -40,450 +37,266 @@ struct GemmParams {
     int atomic_out;
 };
 
-// MH = number of 128-row halves of the CTA tile: MH == 2 gives a 256 x BN tile (two MMAs per k-step share one B tile), which
-// cuts the L2 -> smem bytes per FLOP by 25% — with 128 x 128 tiles the kernel is L2-bandwidth bound (profiles/r1_gemm_shapes).
-// CG = 2 pairs two CTAs (a 2-CTA cluster on neighbouring SMs) on one tcgen05.mma.cta_group::2 of M = 256: each CTA stages its own
-// 128 A rows and HALF of the B tile (BN/2 rows), so a 256 x 256 pair tile costs 32 KB of L2 -> smem traffic per CTA per k-block
-// for 2*128*256*64 FLOP — 128 FLOP/B against 87 FLOP/B for the single-CTA 256 x 128 tile.
-template <int BN, int MH, int CG>
+// Tiles: (BM * MH) x BN. MH == 2 gives each consumer warpgroup 128 rows (two m64 MMAs per k-step share one B tile); BN == 256 gives it
+// one m64n256 MMA per k-step. Both halve the smem -> tensor-core bytes per FLOP of the 128 x 128 tile; 128 fp32 accumulators per thread.
+template <int BN, int MH>
 struct GemmSmem {
     static constexpr int A_BYTES = MH * A_STAGE_BYTES;
-    static constexpr int B_STAGE_BYTES = (BN / CG) * BK * 2;
+    static constexpr int B_STAGE_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
     static constexpr int kStages = (STAGE_BYTES <= 32768) ? 6 : 4;
     static constexpr int TILE_BYTES = kStages * STAGE_BYTES;
-    static constexpr int BAR_BYTES = 160;
-    static constexpr int STG_WARP = 4096;        // per epilogue warp: 32 x 128 B bf16 TMA-store staging tile (1024-B aligned: the 128B swizzle
-                                                 // pattern is a function of the smem address), or 32 x 32 fp32 for split-K reductions
-    static constexpr int STG_BYTES = 8 * STG_WARP;
-    static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + 1024;  // + slack for manual 1024B alignment
+    static constexpr int BAR_BYTES = 128;
+    static constexpr int TOTAL = TILE_BYTES + BAR_BYTES + 1024;  // + slack for manual 1024B alignment
 };
-
-// Epilogue store of bf16 tiles: every lane holds NCH 16-byte pieces of ITS row (a tcgen05.ld 32x32b chunk is row-per-lane). The warp
-// writes them into its staging tile in the TMA swizzle pattern (NCH == 8: 128-byte rows / SWIZZLE_128B, NCH == 4: 64-byte rows /
-// SWIZZLE_64B — both bank-conflict free for row-per-lane 16-byte writes) and one lane issues a TMA tile store: the copy to global
-// memory, its address arithmetic and the clipping of rows >= M / columns >= N are the copy engine's work. (Round 1 read the tile back
-// with LDS and wrote it with predicated 16-byte STG: that store line alone was 16 % of the GEGLU kernel's stall samples and 11 % of
-// its instructions, and the serial STS -> LDS -> STG chain of 8 epilogue warps bounded every K <= 1024 problem: ncu r2l.)
-// `pending` = how many earlier store groups of this warp may still be reading OTHER staging buffers.
-template <int NCH, int PENDING>
-__device__ __forceinline__ void warp_store_tma(uint8_t* stg, const uint4 (&vals)[NCH], const CUtensorMap* map, int col, int row0, int lane) {
-    constexpr int ROWB = NCH * 16;
-    if (lane == 0) bulk_wait_group_read<PENDING>();   // the buffer's previous tile has been read out
-    __syncwarp();
-#pragma unroll
-    for (int c = 0; c < NCH; ++c) {
-        const int sw = (NCH == 8) ? (c ^ (lane & 7)) : (c ^ ((lane >> 1) & 3));
-        *reinterpret_cast<uint4*>(stg + lane * ROWB + sw * 16) = vals[c];
-    }
-    fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) {
-        tma_store_2d(map, stg, col, row0);
-        bulk_commit_group();
-    }
-}
 
 // Exact (erf) GELU of x-transformers' GLU (A.2) for a PAIR of pre-activations:  gelu(x) = x Phi(x) = relu(x) - |x| Phi(-|x|), with the
 // Gaussian tail written as Phi(-a) = 2^(-h(a)) and h a degree-7 polynomial (Chebyshev fit on [0, 6]; beyond, h keeps growing and
 // a 2^-h < 6e-9): |error| < 5e-7 absolute on the GELU value in fp32 Horner arithmetic, 0.5 % of a bf16 half-ulp of the result.
-// 7 FFMA2 + 2 MUFU.EX2 + ~5 more per PAIR; the Abramowitz-Stegun form it replaces cost 2 MUFU + ~13 scalar FMA-pipe instructions per
-// element, and this epilogue is what bounds the GEGLU GEMM (ncu r2l: 46 instructions per hidden unit, issue-active 48 %, tensor 34 %).
+// 7 paired FMAs + 2 MUFU.EX2 + ~5 more per PAIR; the Abramowitz-Stegun form it replaces cost 2 MUFU + ~13 scalar FMA-pipe instructions
+// per element, and the GEGLU GEMM is bounded by its epilogue.
 __device__ __forceinline__ float2 gelu_erf2(float2 x) {
     const float2 a = make_float2(fabsf(x.x), fabsf(x.y));
-    float2 t = __ffma2_rn(a, make_float2(-1.9449223600531695e-06f, -1.9449223600531695e-06f), make_float2(6.386057066265494e-05f, 6.386057066265494e-05f));
-    t = __ffma2_rn(t, a, make_float2(-0.0009488713694736362f, -0.0009488713694736362f));
-    t = __ffma2_rn(t, a, make_float2(0.008582375012338161f, 0.008582375012338161f));
-    t = __ffma2_rn(t, a, make_float2(-0.0541183240711689f, -0.0541183240711689f));
-    t = __ffma2_rn(t, a, make_float2(-0.4582974314689636f, -0.4582974314689636f));
-    t = __ffma2_rn(t, a, make_float2(-1.1513246297836304f, -1.1513246297836304f));
-    t = __ffma2_rn(t, a, make_float2(-0.9999869465827942f, -0.9999869465827942f));   // -h(a)
+    float2 t = ffma2(a, make_float2(-1.9449223600531695e-06f, -1.9449223600531695e-06f), make_float2(6.386057066265494e-05f, 6.386057066265494e-05f));
+    t = ffma2(t, a, make_float2(-0.0009488713694736362f, -0.0009488713694736362f));
+    t = ffma2(t, a, make_float2(0.008582375012338161f, 0.008582375012338161f));
+    t = ffma2(t, a, make_float2(-0.0541183240711689f, -0.0541183240711689f));
+    t = ffma2(t, a, make_float2(-0.4582974314689636f, -0.4582974314689636f));
+    t = ffma2(t, a, make_float2(-1.1513246297836304f, -1.1513246297836304f));
+    t = ffma2(t, a, make_float2(-0.9999869465827942f, -0.9999869465827942f));   // -h(a)
     float ex, ey;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(t.x));
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ey) : "f"(t.y));
-    return __ffma2_rn(make_float2(-a.x, -a.y), make_float2(ex, ey), make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f)));
+    return ffma2(make_float2(-a.x, -a.y), make_float2(ex, ey), make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f)));
 }
 
-template <int BN, bool A_MN, bool B_MN, int MH, int CG>
+
+// One bf16 pair / fp32 pair of the output: columns (col, col + 1) of `row`; col is even.
+__device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col, float v0, float v1) {
+    const bool two = col + 1 < p.N;
+    if (p.d_fp32) {
+        float* dp = reinterpret_cast<float*>(p.D) + (long long)row * p.ldd + col;
+        const bool vec = two && (reinterpret_cast<uintptr_t>(dp) & 7) == 0;
+        if (p.atomic_out) {
+            if (vec) atomicAdd(reinterpret_cast<float2*>(dp), make_float2(v0, v1));
+            else { atomicAdd(dp, v0); if (two) atomicAdd(dp + 1, v1); }
+        } else {
+            if (vec) *reinterpret_cast<float2*>(dp) = make_float2(v0, v1);
+            else { dp[0] = v0; if (two) dp[1] = v1; }
+        }
+    } else {
+        __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + col;
+        if (two) *reinterpret_cast<uint32_t*>(dp) = pack_bf16(v0, v1);   // ldd % 8 == 0 and col even: 4-byte aligned
+        else dp[0] = __float2bfloat16_rn(v0);
+    }
+}
+
+template <int BN, bool A_MN, bool B_MN, int MH>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                    const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
-                    const __grid_constant__ CUtensorMap tmD2, const GemmParams p) {
-    using S = GemmSmem<BN, MH, CG>;
-    static_assert(CG == 1 || (CG == 2 && MH == 1 && BN == 256), "pair kernel: 2 x (128 x 256) tile");
-    static_assert(2 * MH * BN <= 512, "accumulators must fit TMEM");
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
+                  const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+    using S = GemmSmem<BN, MH>;
     constexpr int kStages = S::kStages;
     constexpr int BMT = BM * MH;   // rows of the CTA tile
-    constexpr int BNL = BN / CG;   // B rows this CTA stages
-    // work items are tiles of (CG * BMT) x BN; with CG == 2 the two CTAs of a cluster walk the same list and own 128 rows each
-    const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;
-    const int w_first = blockIdx.x / CG, w_step = gridDim.x / CG;
+    constexpr int NACC = BN / 2;   // accumulators per thread and m64 block
     extern __shared__ uint8_t smem_raw[];
-    // 1024-byte alignment by OFFSET, not by integer round-trip: the pointer keeps its shared-memory provenance, so tile / staging
-    // accesses compile to LDS / STS instead of generic LD / ST (+ a full MEMBAR before the async-proxy fence)
+    // 1024-byte alignment by OFFSET, not by integer round-trip: the pointer keeps its shared-memory provenance
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* smA = smem;
     uint8_t* smB = smem + kStages * S::A_BYTES;
-    uint8_t* stg_base = smem + S::TILE_BYTES;     // 1024-byte aligned (TILE_BYTES is a multiple of 1024)
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES + S::STG_BYTES);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES);
     uint64_t* empty_bar = full_bar + kStages;
-    uint64_t* tfull_bar = empty_bar + kStages;
-    uint64_t* tempty_bar = tfull_bar + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmA2);
         tma_prefetch_desc(&tmB);
-        tma_prefetch_desc(&tmD);
-        tma_prefetch_desc(&tmD2);
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < kStages; ++i) {
-            mbar_init(&full_bar[i], CG);        // pair: the leader's barrier takes one arrival per producer (+ both CTAs' TMA bytes)
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull_bar[i], 1);
-            mbar_init(&tempty_bar[i], 8 * CG);  // pair: both CTAs' epilogue warps release the accumulator at the leader
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 2);   // one arrival per consumer warpgroup
         }
         fence_barrier_init();
     }
-    if (warp == 1) {
-        if constexpr (CG == 2) tmem_alloc_cg2(tmem_slot, 2 * MH * BN);
-        else tmem_alloc(tmem_slot, 2 * MH * BN);
-    }
-    tc_fence_before();
-    if constexpr (CG == 2) cluster_sync_all();   // peer barriers initialised before any remote arrive / multicast commit
-    else __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    pdl_wait();   // everything above (barriers, TMEM, descriptor prefetch) may overlap the tail of the previous kernel (ptx.cuh)
+    __syncthreads();
+    pdl_wait();   // barrier set-up and descriptor prefetch may overlap the tail of the previous kernel (ptx.cuh)
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        regs_dealloc<40>();
+        if (threadIdx.x == 0) {
             // ------------------------------------------------------------ TMA producer
             int stage = 0;
             uint32_t phase = 0;
-            auto load = [&](void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-                if constexpr (CG == 2) tma_load_2d_cg2(dst, m, bar, c0, c1);   // bytes are credited to the leader CTA's barrier
-                else tma_load_2d(dst, m, bar, c0, c1);
-            };
-            for (int w = w_first; w < p.num_work; w += w_step) {
+            for (int w = blockIdx.x; w < p.num_work; w += gridDim.x) {
                 const int tm = w % p.tiles_m;
                 const int rest = w / p.tiles_m;
                 const int tn = rest % p.tiles_n;
                 const int sp = rest / p.tiles_n;
                 const int kb0 = sp * p.kb_per_split;
                 const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-                const int arow = (tm * CG + (int)rank) * BMT;      // first A row of this CTA
-                const int brow = tn * BN + (int)rank * BNL;        // first B row (output column) this CTA stages
+                const int arow = tm * BMT;
+                const int brow = tn * BN;
                 for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
-                    if constexpr (CG == 2) {
-                        if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * S::STAGE_BYTES);
-                        else mbar_arrive_cluster(&full_bar[stage], 0);
-                    } else {
-                        mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
-                    }
+                    mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
                     uint8_t* a_dst = smA + stage * S::A_BYTES;
                     uint8_t* b_dst = smB + stage * S::B_STAGE_BYTES;
+                    const CUtensorMap* ma = kb < p.kb_a1 ? &tmA : &tmA2;
+                    const int ka = kb < p.kb_a1 ? kb * BK : (kb - p.kb_a1) * BK;
                     if constexpr (!A_MN) {
 #pragma unroll
-                        for (int h = 0; h < MH; ++h) {
-                            if (kb < p.kb_a1) load(a_dst + h * A_STAGE_BYTES, &tmA, &full_bar[stage], kb * BK, arow + h * BM);
-                            else load(a_dst + h * A_STAGE_BYTES, &tmA2, &full_bar[stage], (kb - p.kb_a1) * BK, arow + h * BM);
-                        }
+                        for (int h = 0; h < MH; ++h) tma_load_2d(a_dst + h * A_STAGE_BYTES, ma, &full_bar[stage], ka, arow + h * BM);
                     } else {
 #pragma unroll
-                        for (int i = 0; i < BMT / 64; ++i) {
-                            if (kb < p.kb_a1) load(a_dst + i * (BK * 128), &tmA, &full_bar[stage], arow + i * 64, kb * BK);
-                            else load(a_dst + i * (BK * 128), &tmA2, &full_bar[stage], arow + i * 64, (kb - p.kb_a1) * BK);
-                        }
+                        for (int i = 0; i < BMT / 64; ++i) tma_load_2d(a_dst + i * (BK * 128), ma, &full_bar[stage], arow + i * 64, ka);
                     }
                     if constexpr (!B_MN) {
-                        load(b_dst, &tmB, &full_bar[stage], kb * BK, brow);
+#pragma unroll
+                        for (int h = 0; h < BN / 128; ++h) tma_load_2d(b_dst + h * (128 * BK * 2), &tmB, &full_bar[stage], kb * BK, brow + h * 128);
                     } else {
 #pragma unroll
-                        for (int i = 0; i < BNL / 64; ++i)
-                            load(b_dst + i * (BK * 128), &tmB, &full_bar[stage], brow + i * 64, kb * BK);
+                        for (int i = 0; i < BN / 64; ++i) tma_load_2d(b_dst + i * (BK * 128), &tmB, &full_bar[stage], brow + i * 64, kb * BK);
                     }
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
             }
             pdl_launch_dependents();   // all operand loads are issued: the next kernel's CTAs may start their prologue
-            if constexpr (CG == 2) {
-                // the leader's commits multicast into this CTA's empty barriers: let the last ones land before the CTA may exit
-                for (int i = 0; i < kStages; ++i) {
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-            }
         }
-    } else if (warp == 1) {
-        if (lane == 0 && rank == 0) {
-            // ------------------------------------------------------------ MMA issuer (pair: the leader CTA issues for both)
-            constexpr uint32_t idesc = make_idesc_bf16(BM * CG, BN, A_MN ? 1u : 0u, B_MN ? 1u : 0u);
-            // K-major: 8-row groups 1024 B apart, one swizzle atom along K; MN-major: 64-element MN atoms
-            // BK*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO).
-            constexpr uint32_t a_lbo = A_MN ? BK * 128 : 0, b_lbo = B_MN ? BK * 128 : 0;
-            constexpr uint32_t a_adv = A_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;  // per UMMA_K=16 step, in 16-B units
-            constexpr uint32_t b_adv = B_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
-            int stage = 0;
-            uint32_t phase = 0;
-            int iter = 0;
-            for (int w = w_first; w < p.num_work; w += w_step, ++iter) {
-                const int sp = (w / p.tiles_m) / p.tiles_n;
-                const int kb0 = sp * p.kb_per_split;
-                const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-                const int as = iter & 1;
-                const uint32_t aphase = (iter >> 1) & 1;
-                mbar_wait(&tempty_bar[as], aphase ^ 1);
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + as * (MH * BN);
-                for (int kb = kb0; kb < kb1; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smB + stage * S::B_STAGE_BYTES), b_lbo, 1024);
-#pragma unroll
-                    for (int h = 0; h < MH; ++h) {
-                        const uint64_t adesc = make_smem_desc_sw128(smem_u32(smA + stage * S::A_BYTES + h * A_STAGE_BYTES), a_lbo, 1024);
-#pragma unroll
-                        for (int k = 0; k < BK / 16; ++k) {
-                            if constexpr (CG == 2)
-                                umma_f16_cg2(tmem_d + h * BN, adesc + (uint64_t)(k * a_adv), bdesc + (uint64_t)(k * b_adv), idesc,
-                                             (kb > kb0 || k > 0) ? 1u : 0u);
-                            else
-                                umma_f16(tmem_d + h * BN, adesc + (uint64_t)(k * a_adv), bdesc + (uint64_t)(k * b_adv), idesc,
-                                         (kb > kb0 || k > 0) ? 1u : 0u);
-                        }
-                    }
-                    if constexpr (CG == 2) {
-                        umma_commit_cg2(&empty_bar[stage], 3);                      // frees the slot in both CTAs
-                        if (kb == kb1 - 1) umma_commit_cg2(&tfull_bar[as], 3);      // both CTAs' accumulators complete
-                    } else {
-                        umma_commit(&empty_bar[stage]);            // smem slot is free once these MMAs retire
-                        if (kb == kb1 - 1) umma_commit(&tfull_bar[as]);  // accumulator complete
-                    }
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-            }
-        }
-    } else if (warp >= 2) {
-        // ---------------------------------------------------------------- epilogue (warps 2..9)
-        const int q = warp & 3;            // TMEM lane quadrant this warp may access
-        const int chalf = (warp - 2) >> 2; // which half of the tile columns (two 32-column chunks) this warp drains
-        const int ew = warp - 2;           // epilogue warp index -> private staging tile
-        uint32_t nstore = 0;               // GEGLU path: TMA stores issued by this warp (selects the staging half)
-        int iter = 0;
-        for (int w = w_first; w < p.num_work; w += w_step, ++iter) {
-            const int tm = (w % p.tiles_m) * CG + (int)rank;   // 128*MH-row tile index of this CTA
-            const int tn = (w / p.tiles_m) % p.tiles_n;
-            const int as = iter & 1;
-            const uint32_t aphase = (iter >> 1) & 1;
-            // bias / gate slices of this warp's column half (BN/2 fp32 = up to 4 lines each): pulled into L1 while the accumulator is
-            // still being produced, so the broadcast loads behind the TMEM read hit
-            {
-                const int colh = tn * BN + chalf * (BN / 2) + lane * 32;
-                if (lane < BN / 64 && colh < p.N) {
-                    if (p.bias) prefetch_l1(p.bias + colh);
-                    if (p.bias && p.geglu) prefetch_l1(p.bias + min(colh + BN / 2, p.N - 1));   // GEGLU warps read u and gate columns of both halves
-                    if (p.colscale) {
-#pragma unroll
-                        for (int mh = 0; mh < MH; ++mh) {
-                            const int rf = tm * BMT + mh * BM + q * 32;
-                            if (rf < p.M) prefetch_l1(p.colscale + (long long)(rf / p.rows_per_batch) * p.N + colh);
-                        }
-                    }
-                }
-            }
-            mbar_wait(&tfull_bar[as], aphase);
-            tc_fence_after();
-#pragma unroll 1
-            for (int mh = 0; mh < MH; ++mh) {
-            const int row0 = tm * BMT + mh * BM + q * 32;   // first of the warp's 32 rows
-            const int row = row0 + lane;
-            const bool row_ok = row < p.M;
-            const uint32_t taddr = tmem_base + as * (MH * BN) + mh * BN + ((uint32_t)(q * 32) << 16);
-            const bool masked = p.rowmask && row_ok && (p.rowmask[row] == 0);
-            // AdaLN gate row: per batch element. When the warp's 32 rows lie in one batch element (the usual case) the gate row is
-            // warp-uniform and is fetched with broadcast vector loads; a warp that straddles two elements loads per lane.
-            const float* cs = (p.colscale && row_ok) ? p.colscale + (long long)(row / p.rows_per_batch) * p.N : nullptr;
-            const int rlast = min(row0 + 31, p.M - 1);
-            const float* csu = (p.colscale && row0 < p.M && row0 / p.rows_per_batch == rlast / p.rows_per_batch)
-                                   ? p.colscale + (long long)(row0 / p.rows_per_batch) * p.N : nullptr;
-            uint8_t* stg = stg_base + ew * S::STG_WARP;
-
-            if (!p.geglu) {
-#pragma unroll 1
-                for (int cpair = chalf * (BN / 128); cpair < (chalf + 1) * (BN / 128); ++cpair) {   // 64 output columns = one 128-byte bf16 row segment
-                    if (tn * BN + cpair * 64 >= p.N) continue;       // warp-uniform
-                    uint4 held[8];
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        const int c = cpair * 2 + hh;
-                        const int col0 = tn * BN + c * 32;
-                        if (col0 >= p.N) {                           // warp-uniform: the TMA store clips these columns anyway
-#pragma unroll
-                            for (int g = 0; g < 4; ++g) held[hh * 4 + g] = make_uint4(0u, 0u, 0u, 0u);
-                            continue;
-                        }
-                        uint32_t r[32];
-                        __syncwarp();  // tcgen05.ld is .sync.aligned: reconverge after the predicated tails of the previous chunk
-                        tmem_ld32(taddr + c * 32, r);
-                        tmem_ld_wait();
-                        const int nvalid = min(32, p.N - col0);
-                        float v[32];
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-                        // bias / gate vectors: warp-uniform addresses -> one broadcast sector per 16-byte load (the shuffle broadcast
-                        // of round 1 was 20 % of the instructions of the gated out-projection GEMMs)
-                        if (p.bias) {
-                            if (nvalid == 32 && (reinterpret_cast<uintptr_t>(p.bias + col0) & 15) == 0) {
-#pragma unroll
-                                for (int g = 0; g < 8; ++g) {
-                                    const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + col0) + g);
-                                    v[4 * g] += b4.x; v[4 * g + 1] += b4.y; v[4 * g + 2] += b4.z; v[4 * g + 3] += b4.w;
-                                }
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) if (j < nvalid) v[j] += __ldg(p.bias + col0 + j);
-                            }
-                        }
-                        if (p.colscale) {
-                            if (csu && nvalid == 32 && (reinterpret_cast<uintptr_t>(csu + col0) & 15) == 0) {
-#pragma unroll
-                                for (int g = 0; g < 8; ++g) {
-                                    const float4 c4 = __ldg(reinterpret_cast<const float4*>(csu + col0) + g);
-                                    v[4 * g] *= c4.x; v[4 * g + 1] *= c4.y; v[4 * g + 2] *= c4.z; v[4 * g + 3] *= c4.w;
-                                }
-                            } else if (cs) {   // per-lane gate rows
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) if (j < nvalid) v[j] *= __ldg(cs + col0 + j);
-                            }
-                        }
-                        if (masked) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) v[j] = 0.f;
-                        }
-                        if (p.resid && row_ok) {
-                            const __nv_bfloat16* rp = reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr + col0;
-                            if (nvalid == 32) {
-#pragma unroll
-                                for (int g = 0; g < 4; ++g) {
-                                    const uint4 u = *reinterpret_cast<const uint4*>(rp + g * 8);
-                                    v[g * 8 + 0] += bf16_lo(u.x); v[g * 8 + 1] += bf16_hi(u.x);
-                                    v[g * 8 + 2] += bf16_lo(u.y); v[g * 8 + 3] += bf16_hi(u.y);
-                                    v[g * 8 + 4] += bf16_lo(u.z); v[g * 8 + 5] += bf16_hi(u.z);
-                                    v[g * 8 + 6] += bf16_lo(u.w); v[g * 8 + 7] += bf16_hi(u.w);
-                                }
-                            } else {   // (unrolled + predicated: a runtime trip count would index v[] dynamically and push it to local memory)
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) if (j < nvalid) v[j] += __bfloat162float(rp[j]);
-                            }
-                        }
-                        if (p.d_fp32 && p.atomic_out) {
-                            warp_red_rows_f32(reinterpret_cast<float*>(stg), v, reinterpret_cast<float*>(p.D) + col0, p.ldd, row0, p.M, nvalid, lane);
-                        } else if (p.d_fp32) {
-                            float* dp = reinterpret_cast<float*>(p.D) + (long long)row * p.ldd + col0;
-                            if (!row_ok) {
-                            } else if (nvalid == 32 && (p.ldd & 3) == 0) {
-#pragma unroll
-                                for (int g = 0; g < 8; ++g)
-                                    *reinterpret_cast<float4*>(dp + g * 4) = make_float4(v[g * 4], v[g * 4 + 1], v[g * 4 + 2], v[g * 4 + 3]);
-                            } else {
-#pragma unroll
-                                for (int j = 0; j < 32; ++j) if (j < nvalid) dp[j] = v[j];
-                            }
-                        } else {
-#pragma unroll
-                            for (int g = 0; g < 4; ++g)
-                                held[hh * 4 + g] = make_uint4(pack_bf16(v[g * 8], v[g * 8 + 1]), pack_bf16(v[g * 8 + 2], v[g * 8 + 3]),
-                                                              pack_bf16(v[g * 8 + 4], v[g * 8 + 5]), pack_bf16(v[g * 8 + 6], v[g * 8 + 7]));
-                        }
-                    }
-                    if (!p.d_fp32) warp_store_tma<8, 0>(stg, held, &tmD, tn * BN + cpair * 64, row0, lane);
-                }
-            } else {
-                // GEGLU: every 128 packed columns hold [0,64) = u, [64,128) = gate of the same 64 hidden units
-                const bool do_drop = p.dropout_p > 0.f;
-                const float keep_scale = do_drop ? 65536.f / (65536.f - (float)(uint32_t)(p.dropout_p * 65536.f)) : 1.f;
-                const uint32_t seedmix = do_drop ? seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull)) : 0u;
-                const uint32_t thr32 = drop_thresh32((uint32_t)(p.dropout_p * 65536.f));
-#pragma unroll 1
-                for (int sub = 0; sub < BN / 128; ++sub) {
-                    const int c = chalf;
-                    if (tn * BN + sub * 128 >= p.N) continue;   // warp-uniform (N % 128 == 0: a 128-column group is all in or all out)
-                    uint32_t ru[32], rg[32];
-                    const int colp = tn * BN + sub * 128 + c * 32;         // packed column of u
-                    __syncwarp();
-                    tmem_ld32(taddr + sub * 128 + c * 32, ru);
-                    tmem_ld32(taddr + sub * 128 + 64 + c * 32, rg);
-                    tmem_ld_wait();
-                    // packed bias of this warp's 32 u / 32 gate columns (N % 128 == 0, base 16-byte aligned): warp-uniform addresses, one
-                    // broadcast sector per load (the shuffle broadcast of round 1 cost 64 SHFL + selects per 32 hidden units)
-                    const float4* pbu = reinterpret_cast<const float4*>(p.bias + (p.bias ? colp : 0));
-                    const int hcol0 = tn * (BN / 2) + sub * 64 + c * 32;   // hidden-unit column
-                    // everything below works on column PAIRS (2k, 2k+1): packed fp32x2 adds / FMAs, one bf16x2 conversion per pair
-                    uint4 pu[4], pg[4], ph[4];
-                    uint32_t* wu = reinterpret_cast<uint32_t*>(pu);
-                    uint32_t* wg = reinterpret_cast<uint32_t*>(pg);
-                    uint32_t* wh = reinterpret_cast<uint32_t*>(ph);
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        float4 bu = make_float4(0.f, 0.f, 0.f, 0.f), bg = bu;
-                        if (p.bias) { bu = __ldg(pbu + i); bg = __ldg(pbu + 16 + i); }
-                        const float2 ua = __fadd2_rn(make_float2(__uint_as_float(ru[4 * i]), __uint_as_float(ru[4 * i + 1])), make_float2(bu.x, bu.y));
-                        const float2 ub = __fadd2_rn(make_float2(__uint_as_float(ru[4 * i + 2]), __uint_as_float(ru[4 * i + 3])), make_float2(bu.z, bu.w));
-                        const float2 ga = __fadd2_rn(make_float2(__uint_as_float(rg[4 * i]), __uint_as_float(rg[4 * i + 1])), make_float2(bg.x, bg.y));
-                        const float2 gb = __fadd2_rn(make_float2(__uint_as_float(rg[4 * i + 2]), __uint_as_float(rg[4 * i + 3])), make_float2(bg.z, bg.w));
-                        wu[2 * i] = pack_bf16(ua.x, ua.y); wu[2 * i + 1] = pack_bf16(ub.x, ub.y);
-                        wg[2 * i] = pack_bf16(ga.x, ga.y); wg[2 * i + 1] = pack_bf16(gb.x, gb.y);
-                    }
-                    // 2 KB tiles (32 rows x 64 B) alternate between the two halves of the staging buffer: before a half is rewritten, at
-                    // most ONE later store group may still be pending
-                    if (p.D2) {
-                        warp_store_tma<4, 1>(stg + (nstore++ & 1) * 2048, pu, &tmD2, colp, row0, lane);
-                        warp_store_tma<4, 1>(stg + (nstore++ & 1) * 2048, pg, &tmD2, colp + 64, row0, lane);
-                    }
-                    // hidden-unit pairs (2k, 2k+1) of one row share a 32-bit hash; N/2 is even, so (row * N/2 + hcol) >> 1 pairs them
-                    const uint32_t pbase = (uint32_t)(((unsigned long long)row * (unsigned long long)(p.N / 2) + hcol0) >> 1);
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        // the backward pass recomputes from the bf16-rounded pre-activations: use them here too
-                        const float2 ub = make_float2(bf16_lo(wu[j]), bf16_hi(wu[j]));
-                        const float2 gb = make_float2(bf16_lo(wg[j]), bf16_hi(wg[j]));
-                        float2 h2 = __fmul2_rn(ub, gelu_erf2(gb));
-                        if (do_drop) {
-                            const DropWords hsh = drop_words(seedmix, pbase + j);
-                            h2 = __fmul2_rn(h2, make_float2(hsh.a >= thr32 ? keep_scale : 0.f, hsh.b >= thr32 ? keep_scale : 0.f));
-                        }
-                        wh[j] = pack_bf16(h2.x, h2.y);
-                    }
-                    warp_store_tma<4, 1>(stg + (nstore++ & 1) * 2048, ph, &tmD, hcol0, row0, lane);
-                }
-            }
-            }  // mh
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-                if constexpr (CG == 2) mbar_arrive_cluster(&tempty_bar[as], 0);
-                else mbar_arrive(&tempty_bar[as]);
-            }
-        }
-        if (lane == 0) bulk_wait_group_read<0>();   // the staging tiles must stay valid until the copy engine has read them
+        return;
     }
 
-    tc_fence_before();
-    if constexpr (CG == 2) cluster_sync_all();   // neither CTA may retire while its peer can still touch its smem / TMEM
-    else __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        if constexpr (CG == 2) tmem_dealloc_cg2(tmem_base, 2 * MH * BN);
-        else tmem_dealloc(tmem_base, 2 * MH * BN);
+    // -------------------------------------------------------------------- consumer warpgroups: MMA, then epilogue
+    regs_alloc<232>();
+    const int cw = wg - 1;                     // which 64 * MH rows of the CTA tile
+    const int t = threadIdx.x & 127;
+    const int lane = t & 31, wq = t >> 5;      // warp within the warpgroup: accumulator rows 16 * wq ..
+    // K-major: 8-row groups 1024 B apart; MN-major: 64-element MN atoms BK*128 B apart (LBO), 8-k-row groups 1024 B apart (SBO).
+    constexpr uint32_t a_lbo = A_MN ? BK * 128 : 16, b_lbo = B_MN ? BK * 128 : 16;
+    constexpr uint32_t a_adv = A_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;   // per k16 step, in 16-B units
+    constexpr uint32_t b_adv = B_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
+    float acc[MH][NACC];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int w = blockIdx.x; w < p.num_work; w += gridDim.x) {
+        const int tm = w % p.tiles_m;
+        const int rest = w / p.tiles_m;
+        const int tn = rest % p.tiles_n;
+        const int sp = rest / p.tiles_n;
+        const int kb0 = sp * p.kb_per_split;
+        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+#pragma unroll
+            for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
+            wgmma_fence();
+            const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smB + stage * S::B_STAGE_BYTES), b_lbo, 1024);
+#pragma unroll
+            for (int h = 0; h < MH; ++h) {
+                // the warpgroup's m64 block (cw * MH + h) lies 64 rows = 8 KB into the A tile in both layouts
+                const uint64_t adesc = make_smem_desc_sw128(smem_u32(smA + stage * S::A_BYTES + (cw * MH + h) * 8192), a_lbo, 1024);
+#pragma unroll
+                for (int k = 0; k < BK / 16; ++k) {
+                    const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
+                    if constexpr (BN == 256) wgmma_ss_n256<A_MN, B_MN>(acc[h], adesc + (uint64_t)(k * a_adv), bdesc + (uint64_t)(k * b_adv), accum);
+                    else wgmma_ss_n128<A_MN, B_MN>(acc[h], adesc + (uint64_t)(k * a_adv), bdesc + (uint64_t)(k * b_adv), accum);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();   // the MMAs of the previous k-block have retired: its smem slot may be refilled
+#pragma unroll
+            for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
+            if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
+            prev = stage;
+            if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+#pragma unroll
+        for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
+        if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
+
+        // ---------------------------------------------------------------- epilogue from the accumulator fragments
+        // Fragment of an m64nBN accumulator: thread (wq, lane) holds rows 16 wq + lane / 4 (+ 8) and, for every 8-column group j,
+        // columns 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 i + c] = (row + 8 i, column + c).
+        const int cq = 2 * (lane & 3);
+        if (!p.geglu) {
+#pragma unroll
+            for (int h = 0; h < MH; ++h) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
+                    if (row >= p.M) continue;
+                    const bool masked = p.rowmask && p.rowmask[row] == 0;
+                    const float* cs = p.colscale ? p.colscale + (long long)(row / p.rows_per_batch) * p.N : nullptr;
+                    const __nv_bfloat16* rp = p.resid ? reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr : nullptr;
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j) {
+                        const int col = tn * BN + 8 * j + cq;
+                        if (col >= p.N) continue;
+                        const bool two = col + 1 < p.N;
+                        float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
+                        if (p.bias) { v0 += __ldg(p.bias + col); if (two) v1 += __ldg(p.bias + col + 1); }
+                        if (cs) { v0 *= __ldg(cs + col); if (two) v1 *= __ldg(cs + col + 1); }
+                        if (masked) { v0 = 0.f; v1 = 0.f; }
+                        if (rp) {
+                            if (two) {
+                                const uint32_t u = *reinterpret_cast<const uint32_t*>(rp + col);
+                                v0 += bf16_lo(u); v1 += bf16_hi(u);
+                            } else {
+                                v0 += __bfloat162float(rp[col]);
+                            }
+                        }
+                        store_pair(p, row, col, v0, v1);
+                    }
+                }
+            }
+        } else {
+            // GEGLU: every 128 packed columns hold [0,64) = u, [64,128) = gate of the same 64 hidden units, so a thread holds both
+            // halves of each of its hidden units (fragment groups j and j + 8 of the 128-column group)
+            const bool do_drop = p.dropout_p > 0.f;
+            const float keep_scale = do_drop ? 65536.f / (65536.f - (float)(uint32_t)(p.dropout_p * 65536.f)) : 1.f;
+            const uint32_t seedmix = do_drop ? seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull)) : 0u;
+            const uint32_t thr32 = drop_thresh32((uint32_t)(p.dropout_p * 65536.f));
+#pragma unroll
+            for (int h = 0; h < MH; ++h) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
+                    if (row >= p.M) continue;
+#pragma unroll
+                    for (int sub = 0; sub < BN / 128; ++sub) {
+                        const int colg = tn * BN + sub * 128;   // first packed column of the group (N % 128 == 0)
+                        if (colg >= p.N) continue;
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const int cu = colg + 8 * j + cq;           // packed column of u; the gate is 64 further
+                            const int hcol = colg / 2 + 8 * j + cq;     // hidden-unit column
+                            float2 u = make_float2(acc[h][4 * (sub * 16 + j) + 2 * i], acc[h][4 * (sub * 16 + j) + 2 * i + 1]);
+                            float2 g = make_float2(acc[h][4 * (sub * 16 + 8 + j) + 2 * i], acc[h][4 * (sub * 16 + 8 + j) + 2 * i + 1]);
+                            if (p.bias) {
+                                u = fadd2(u, make_float2(__ldg(p.bias + cu), __ldg(p.bias + cu + 1)));
+                                g = fadd2(g, make_float2(__ldg(p.bias + cu + 64), __ldg(p.bias + cu + 65)));
+                            }
+                            const uint32_t wu = pack_bf16(u.x, u.y), wgt = pack_bf16(g.x, g.y);
+                            if (p.D2) {
+                                __nv_bfloat16* d2 = reinterpret_cast<__nv_bfloat16*>(p.D2) + (long long)row * p.ldd2 + cu;
+                                *reinterpret_cast<uint32_t*>(d2) = wu;
+                                *reinterpret_cast<uint32_t*>(d2 + 64) = wgt;
+                            }
+                            // the backward pass recomputes from the bf16-rounded pre-activations: use them here too
+                            float2 h2 = fmul2(make_float2(bf16_lo(wu), bf16_hi(wu)), gelu_erf2(make_float2(bf16_lo(wgt), bf16_hi(wgt))));
+                            if (do_drop) {
+                                // hidden-unit pairs (2k, 2k+1) of one row share a 32-bit hash; N/2 is even, so (row * N/2 + hcol) >> 1 pairs them
+                                const DropWords hsh = drop_words(seedmix, (uint32_t)(((unsigned long long)row * (unsigned long long)(p.N / 2) + hcol) >> 1));
+                                h2 = fmul2(h2, make_float2(hsh.a >= thr32 ? keep_scale : 0.f, hsh.b >= thr32 ? keep_scale : 0.f));
+                            }
+                            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + hcol) = pack_bf16(h2.x, h2.y);
+                        }
+                    }
+                }
+            }
+        }
     }
 }
 
@@ -545,43 +358,18 @@ static int make_map_uncached(CUtensorMap* m, const void* ptr, int64_t inner, int
     return 0;
 }
 
-template <int BN, bool A_MN, bool B_MN, int MH, int CG = 1>
-static int launch_gemm(const CUtensorMap (&tm)[5], const GemmParams& p, cudaStream_t st) {
-    const CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2], &tD = tm[3], &tD2 = tm[4];
-    using S = GemmSmem<BN, MH, CG>;
-    auto kern = gemm_tcgen05_kernel<BN, A_MN, B_MN, MH, CG>;
+template <int BN, bool A_MN, bool B_MN, int MH>
+static int launch_gemm(const CUtensorMap (&tm)[3], const GemmParams& p, cudaStream_t st) {
+    using S = GemmSmem<BN, MH>;
+    auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, MH>;
     static DeviceOnce once;   // one flag per template instantiation and device
     {
         cudaError_t e = set_max_smem_once(once, kern, S::TOTAL);
         B200_REQUIRE(e == cudaSuccess, "gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
-    if constexpr (CG == 2) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.blockDim = dim3(kGemmThreads); cfg.dynamicSmemBytes = S::TOTAL; cfg.stream = st;
-        cudaLaunchAttribute attr[2];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // only counted when B200_PDL=1 (common.cuh)
-        attr[1].val.programmaticStreamSerializationAllowed = 1;
-        cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-        static std::atomic<int> pairs_cache[kMaxDevices];   // co-resident 2-CTA clusters (one CTA per SM): the persistent grid, per device
-        int pairs = pairs_cache[current_device()].load(std::memory_order_relaxed);
-        if (!pairs) {
-            cfg.gridDim = dim3(2 * (num_sms() / 2));
-            int n = 0;
-            cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
-            B200_REQUIRE(e == cudaSuccess && n > 0, "gemm: cudaOccupancyMaxActiveClusters: %s (%d)", cudaGetErrorString(e), n);
-            pairs = n < num_sms() / 2 ? n : num_sms() / 2;
-            pairs_cache[current_device()].store(pairs, std::memory_order_relaxed);
-        }
-        cfg.gridDim = dim3(2 * (p.num_work < pairs ? p.num_work : pairs));
-        cudaError_t e = cudaLaunchKernelEx(&cfg, kern, tA, tA2, tB, tD, tD2, p);
-        B200_REQUIRE(e == cudaSuccess, "gemm: cluster launch: %s", cudaGetErrorString(e));
-        return check_launch("gemm_tcgen05_kernel<pair>");
-    }
     const int grid = p.num_work < num_sms() ? p.num_work : num_sms();
-    B200_LAUNCH(kern, grid, kGemmThreads, S::TOTAL, st, tA, tA2, tB, tD, tD2, p);
-    return check_launch("gemm_tcgen05_kernel");
+    B200_LAUNCH(kern, grid, kGemmThreads, S::TOTAL, st, tm[0], tm[1], tm[2], p);
+    return check_launch("gemm_wgmma_kernel");
 }
 
 }  // namespace b200
@@ -596,12 +384,11 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     const bool a_mn = a->a_mn_major != 0, b_mn = a->b_mn_major != 0;
     GemmParams p{};
     p.M = (int)a->M; p.N = (int)a->N; p.K = (int)a->K;
-    // force_tile: 0 auto, 1 = 128x128, 2 = 256x128, 3 = CTA-pair 2x(128x256)
-    static const int pair_env = getenv("B200_GEMM_PAIR") ? atoi(getenv("B200_GEMM_PAIR")) : 1;   // developer A/B switch, default on
-    const bool pair = a->force_tile == 3 || (a->force_tile == 0 && pair_env && p.M >= 512 && p.N >= 256);
-    const int BN = pair ? 256 : 128;
-    const int MH = pair ? 1 : (a->force_tile == 1) ? 1 : ((a->force_tile == 2 || p.M >= 256) ? 2 : 1);   // 256-row CTA tiles for tall problems
-    const int tile_rows = pair ? 2 * BM : BM * MH;
+    // force_tile: 0 auto, 1 = 128x128, 2 = 256x128, 3 = 128x256 (auto: 128x256 for M >= 512, N >= 256; 256x128 for other M >= 256)
+    const bool wide = a->force_tile == 3 || (a->force_tile == 0 && p.M >= 512 && p.N >= 256);
+    const int BN = wide ? 256 : 128;
+    const int MH = wide ? 1 : (a->force_tile == 1) ? 1 : ((a->force_tile == 2 || p.M >= 256) ? 2 : 1);
+    const int tile_rows = BM * MH;
     p.tiles_m = (p.M + tile_rows - 1) / tile_rows;
     p.tiles_n = (p.N + BN - 1) / BN;
     p.kb_total = (p.K + BK - 1) / BK;
@@ -612,11 +399,9 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     }
     int split = a->split_k > 1 ? a->split_k : 1;
     if (a->split_k < 0) {
-        // auto (weight gradients: few output tiles, very long K): fill the machine once — one work item per CTA pair (or CTA) —
+        // auto (weight gradients: few output tiles, very long K): fill the machine once — one work item per CTA —
         // while every split keeps >= 8 k-blocks so that the pipeline fill and the fp32 reduction of its partial tile stay amortised.
-        // (The Python-side heuristic of round 1 counted 128 x 128 tiles whatever tile the kernel chose and left 35-50 % of the SMs idle
-        // on the dW problems, profiles/r2f_gemm_breakdown_by_shape.txt.)
-        const int units = pair ? num_sms() / 2 : num_sms();
+        const int units = num_sms();
         const int tiles = p.tiles_m * p.tiles_n;
         int s_fill = (units + tiles / 2) / tiles;                 // nearest number of splits that fills the units once
         while (s_fill > 1 && tiles * s_fill > units) --s_fill;     // never spill into a second, mostly empty round
@@ -649,8 +434,8 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     if (!a->d_fp32) B200_REQUIRE((a->ldd % 8) == 0, "gemm: bf16 output pitch must be a multiple of 8");
     if (a->resid) B200_REQUIRE((a->ldr % 8) == 0, "gemm: residual pitch must be a multiple of 8");
 
-    CUtensorMap tm[5];
-    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2], &tD = tm[3], &tD2 = tm[4];
+    CUtensorMap tm[3];
+    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2];
     int rc;
     const int64_t KA = a->A2 ? a->K1 : a->K;
     if (!a_mn) rc = make_map(&tA, a->A, KA, a->M, a->lda, BM);
@@ -663,32 +448,24 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     } else {
         tA2 = tA;
     }
-    if (!b_mn) rc = make_map(&tB, a->B, a->K, a->N, a->ldb, 128);   // 128 B rows per CTA for both the 128-wide tile and the pair's half of 256
+    if (!b_mn) rc = make_map(&tB, a->B, a->K, a->N, a->ldb, 128);   // 128-row boxes: one per 128 output columns of the tile
     else rc = make_map(&tB, a->B, a->N, a->K, a->ldb, BK);
     if (rc) return rc;
-    // bf16 outputs leave through TMA tile stores of 32 rows: [M, N] in 64-column pieces, GEGLU [M, N/2] (+ pre-activations [M, N]) in 32-column pieces
-    tD = tA; tD2 = tA;   // (placeholders when the fp32 paths write the output)
-    if (!a->d_fp32) {
-        if (a->geglu) rc = make_map(&tD, a->D, a->N / 2, a->M, a->ldd, 32, 32);
-        else rc = make_map(&tD, a->D, a->N, a->M, a->ldd, 32, 64);
-        if (rc) return rc;
-        if (a->geglu && a->D2) {
-            B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D2) & 15) == 0, "gemm: GEGLU pre-activation buffer must be 16-byte aligned");
-            if ((rc = make_map(&tD2, a->D2, a->N, a->M, a->ldd2, 32, 32))) return rc;
-        }
-    }
+    if (!a->d_fp32) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D) & 3) == 0, "gemm: bf16 output must be 4-byte aligned");
+    if (a->geglu && a->D2) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D2) & 3) == 0, "gemm: GEGLU pre-activation buffer must be 4-byte aligned");
+    if (a->resid) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->resid) & 3) == 0, "gemm: residual must be 4-byte aligned");
 
     {
-        static const bool trace = getenv("B200_GEMM_TRACE") != nullptr;   // developer aid: correlate ncu launch lists with problem shapes
+        static const bool trace = getenv("B200_GEMM_TRACE") != nullptr;   // developer aid: log every problem shape
         if (trace)
             fprintf(stderr, "GEMMTRACE %d %d %d amn=%d bmn=%d split=%d geglu=%d two=%d mh=%d epi=%d%d%d%d\n", p.M, p.N, p.K, (int)a_mn, (int)b_mn, split,
-                    p.geglu, a->A2 != nullptr, pair ? 3 : MH, p.bias != nullptr, p.colscale != nullptr, p.rowmask != nullptr, p.resid != nullptr);
+                    p.geglu, a->A2 != nullptr, wide ? 3 : MH, p.bias != nullptr, p.colscale != nullptr, p.rowmask != nullptr, p.resid != nullptr);
     }
-    if (pair) {
-        if (!a_mn && !b_mn) return launch_gemm<256, false, false, 1, 2>(tm, p, st);
-        if (!a_mn && b_mn) return launch_gemm<256, false, true, 1, 2>(tm, p, st);
-        if (a_mn && !b_mn) return launch_gemm<256, true, false, 1, 2>(tm, p, st);
-        return launch_gemm<256, true, true, 1, 2>(tm, p, st);
+    if (wide) {
+        if (!a_mn && !b_mn) return launch_gemm<256, false, false, 1>(tm, p, st);
+        if (!a_mn && b_mn) return launch_gemm<256, false, true, 1>(tm, p, st);
+        if (a_mn && !b_mn) return launch_gemm<256, true, false, 1>(tm, p, st);
+        return launch_gemm<256, true, true, 1>(tm, p, st);
     }
     if (MH == 2) {
         if (!a_mn && !b_mn) return launch_gemm<128, false, false, 2>(tm, p, st);

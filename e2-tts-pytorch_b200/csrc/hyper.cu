@@ -76,12 +76,8 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
     return make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
 }
 
-// Packed fp32x2 arithmetic: one FFMA2 issues two FMAs per lane. With three register operands a scalar FFMA issues every other
-// cycle per scheduler, so these FMA-heavy per-token kernels are FMA-pipe bound unless the math is paired (elements 2i, 2i+1 of a
-// bf16x2 word make the natural pair).
+// fp32x2 pairs (elements 2i, 2i+1 of a bf16x2 word); ffma2 / fmul2 are in ptx.cuh.
 typedef float2 f2;
-__device__ __forceinline__ f2 ffma2(f2 a, f2 b, f2 c) { return __ffma2_rn(a, b, c); }
-__device__ __forceinline__ f2 fmul2(f2 a, f2 b) { return __fmul2_rn(a, b); }
 __device__ __forceinline__ f2 splat(float a) { return make_float2(a, a); }
 __device__ __forceinline__ float hsum(f2 a) { return a.x + a.y; }
 __device__ __forceinline__ void unpack8p(const uint4& u, f2 (&f)[4]) {
@@ -118,7 +114,7 @@ __device__ __forceinline__ LaneConst lane_const(const HcP& p, int lane) {
 // Stage the per-feature parameters once per block, (gamma+1) folded in, as element PAIRS: for pair j of chunk c
 //   part 0 = { A0[e0], A0[e1], A1[e0], A1[e1] },  part 1 = { A2.., A3.. },  part 2 = { A4[e0], A4[e1], b[e0], b[e1] }
 // at sp[(j*3 + part) * nchunk + c]: the 32 lanes of a warp (consecutive chunks, same j/part) read 32 consecutive float4 —
-// bank-conflict free (a naive per-feature layout was an 8-way conflict, ncu r1). 12 * nchunk float4 = 24 * D bytes.
+// bank-conflict free (a naive per-feature layout is an 8-way conflict). 12 * nchunk float4 = 24 * D bytes.
 __device__ __forceinline__ int sp_idx(int nchunk, int chunk, int j, int part) { return (j * 3 + part) * nchunk + chunk; }
 __host__ __device__ inline size_t hc_param_smem(int D) { return (size_t)(D / 8) * 12 * sizeof(float4); }
 __device__ __forceinline__ void stage_params(const HcP& p, float4* sp) {
@@ -234,7 +230,7 @@ __device__ __forceinline__ void load_gain8(const float* g, f2 (&o)[4]) {   // 8 
 
 // PF: every warp prefetches its NEXT token's 4 streams into a private shared-memory double buffer with one bulk (TMA) copy while
 // it works on the current one. Without it the kernel alternates load and math phases with ~8 warps per SM and sits on
-// long-scoreboard stalls (profiles/r1g_ncu_full_hc_width_*).
+// long-scoreboard stalls.
 template <int VPT, bool PF, bool FUSED>
 __global__ void __launch_bounds__(256, (VPT <= 2) ? 2 : 1) hc_width_fwd_kernel(const HcP p) {
     pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
@@ -341,11 +337,11 @@ __global__ void __launch_bounds__(256, (VPT <= 2) ? 2 : 1) hc_width_fwd_kernel(c
 //   (1) token kernel   : one warp per token — recompute the forward scalars, produce d_xres, the scalar parameter grads, d(norm gain)
 //                        (register partial sums, one atomicAdd per column per block) and one bf16 row per (token, stream) of the
 //                        coefficient matrix C = inv * d(tanh argument);
-//   (2) tcgen05 GEMM   : G = R^T C over all (token, stream) rows (split-K), then hc_param_finalize_kernel turns G into
+//   (2) wgmma GEMM     : G = R^T C over all (token, stream) rows (split-K), then hc_param_finalize_kernel turns G into
 //                        d(dynamic_alpha_fn), d(dynamic_beta_fn), d(norm.gamma).
 // grid.y = batch element: a block never straddles two batch elements (adaptive-gain gradient is per batch).
 // Tokens per block are chosen by the host so that the whole grid is ONE wave of co-resident blocks (hc_tokens_per_block): with a fixed 64
-// the cfg2 grid was 272 blocks on 148 one-block SMs — a second round with 16 % of the machine idle.
+// a grid of just over one wave leaves most of the machine idle in its second round.
 // D <= 256 (VPT == 1) fits 128 registers, so two blocks (16 warps) share an SM: the per-token critical path (two warp-wide 32-value
 // reductions, tanh, ~70 shuffles) is latency-bound, and at D = 256 the backward took 70 % of the D = 512 time for half the bytes.
 // FUSED (preceding depth connection folded in): the streams are recomputed as xres + beta_prev (x) y_prev, and the kernel also emits the
@@ -636,7 +632,7 @@ __global__ void __launch_bounds__(256, (VPT == 1) ? 2 : 1) hc_width_bwd_kernel(c
 }
 
 // Parameter gradients from G[col][k] = sum_{token, stream} r[token, stream, col] * C[(token, stream)][k]  (fp32 [D, 8], produced by the
-// tcgen05 GEMM  R^T C):  with n^ = r * inv * (gamma + 1) and C = inv * d(tanh argument),
+// wgmma GEMM  R^T C):  with n^ = r * inv * (gamma + 1) and C = inv * d(tanh argument),
 //   d dynamic_alpha_fn[col][t] = (gamma+1) G[col][t],  d dynamic_beta_fn[col] = (gamma+1) G[col][5],
 //   d norm.gamma[col]          = sum_t alpha_fn[col][t] G[col][t] + beta_fn[col] G[col][5].
 // (The first versions marched 128-token slabs per thread pair on the CUDA cores: 48 us per call against ~15 us for the GEMM.)

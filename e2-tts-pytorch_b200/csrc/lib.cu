@@ -22,5 +22,5 @@ extern "C" int b200_seed_advance(uint64_t* seed_dev, b200_stream_t stream) {
 }
 
 extern "C" const char* b200_last_error(void) { return b200::g_err; }
-extern "C" int b200_version(void) { return 100; }
+extern "C" int b200_version(void) { return 90; }   // the compute capability the library is built for (sm_90a)
 extern "C" uint64_t b200_launch_count(void) { return b200::g_launches.load(); }

@@ -216,7 +216,7 @@ __global__ void fourier_embed_kernel(const float* times, const float* w, float* 
 // y = m * silu(conv1d_depthwise(m * x) + bias)  on bf16 [B, Np, D]  (DepthwiseConv, e2_tts.py:295-328).
 // Tile = 64 tokens x 64 channels staged in shared memory as fp32 (+ 15 halo rows each side). A thread owns a channel PAIR and a
 // run of consecutive tokens: its 31 taps sit in registers as fp32x2 and every window element is read once (one LDS.64) and fed to
-// all the outputs it touches, so the inner loop is pure FFMA2 — two FMAs per lane and issue slot. (The scalar version of round 1
+// all the outputs it touches, so the inner loop is pure FMA on fp32 pairs. (The scalar version of round 1
 // issued one FMA per slot: 110 FFMA per element in backward, 94 us per call, FMA-pipe bound at half the fp32 peak.)
 // Forward also stores the bf16 pre-activation; backward reads it back instead of recomputing the convolution over tile + halo
 // (the same trade as the GEGLU pre-activations: +2 B per element of HBM traffic for 42 % fewer FMAs).
@@ -224,7 +224,7 @@ constexpr int CV_TN = 64, CV_TC = 64, CV_HALO = 15;
 constexpr int CV_R = CV_TN + 2 * CV_HALO;   // staged rows of a tile: token n0 - 15 + r
 
 typedef float2 cf2;
-__device__ __forceinline__ cf2 cv_ffma2(cf2 a, cf2 b, cf2 c) { return __ffma2_rn(a, b, c); }
+__device__ __forceinline__ cf2 cv_ffma2(cf2 a, cf2 b, cf2 c) { return ffma2(a, b, c); }
 
 __device__ __forceinline__ bool tok_ok(const unsigned char* mask, int b, int n, int Np) {
     return n >= 0 && n < Np && (!mask || mask[(size_t)b * Np + n]);
@@ -235,7 +235,7 @@ __device__ __forceinline__ void cv_unpack8(const uint4& u, float (&v)[8]) {
 }
 // the tile's taps, staged once per block as [31][CV_TC] so that channel pairs are adjacent (one conflict-free LDS.64 per tap and thread);
 // centred inside a 31-wide window (kernel sizes < 31 are zero-padded); flip = reversed taps. (Per-thread global loads of the 62 taps
-// cost more address arithmetic and load latency than the convolution itself: ncu r2m.)
+// cost more address arithmetic and load latency than the convolution itself.)
 __device__ __forceinline__ void cv_stage_taps(const b200_dwconv_args& a, int c0, bool flip, float (*sw)[CV_TC]) {
     const int shift = CV_HALO - a.ksize / 2;
     const int c = threadIdx.x & (CV_TC - 1);          // 256 threads = 64 channels x 4 tap phases (no integer division in the loop)
@@ -266,7 +266,7 @@ __device__ __forceinline__ void conv_rows2(const cf2 (&w)[31], const float (*src
 
 // 256 threads = 32 channel pairs x 8 groups of 8 tokens. A block marches CV_FWD_TILES consecutive token tiles: the taps are staged once,
 // and the global loads of tile t+1 (three 16-byte pieces + their validity per thread) are issued before the convolution of tile t, so
-// their latency hides behind the FFMA2 loop instead of stalling every warp of the block (ncu r2n: 30 % of the samples sat on them).
+// their latency hides behind the FMA loop instead of stalling every warp of the block.
 constexpr int CV_FWD_TILES = 2;
 __global__ void __launch_bounds__(256, 3) dwconv_fwd_kernel(const b200_dwconv_args a) {
     pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
@@ -341,7 +341,7 @@ constexpr int CV_TILES_PER_BLOCK = 4;   // n-tiles marched by one block: weight/
 
 // Backward. Staging turns dy into d(pre-activation) = dy * silu'(pre) on the fly (rows outside the sequence or masked: 0). Then the
 // block splits by warp: warps 0-3 compute dx = flipped conv of d_pre (taps in registers), warps 4-7 accumulate the tap gradients
-// dW[k] += d_pre[n] * x[n + k - 15] and d(bias) in registers across the block's tiles — both halves run 31 FFMA2 per element pair.
+// dW[k] += d_pre[n] * x[n + k - 15] and d(bias) in registers across the block's tiles — both halves run 31 paired FMAs per element pair.
 __global__ void __launch_bounds__(256, 2) dwconv_bwd_kernel(const b200_dwconv_args a) {
     pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ __align__(16) float sm[];
@@ -686,7 +686,7 @@ extern "C" int b200_masked_mean_bwd(const float* dout, const uint8_t* mask, void
 extern "C" int b200_axpy(const float* y, const float* f, float a, float* out, int64_t n, b200_stream_t stream) {
     B200_REQUIRE(y && f && out && n > 0, "axpy: bad arguments");
     const long long g = (n + 255) / 256;
-    B200_LAUNCH(axpy_kernel, (unsigned)(g > 148 * 16 ? 148 * 16 : g), 256, 0, reinterpret_cast<cudaStream_t>(stream), y, f, a, out, n);
+    B200_LAUNCH(axpy_kernel, (unsigned)(g > num_sms() * 16 ? num_sms() * 16 : g), 256, 0, reinterpret_cast<cudaStream_t>(stream), y, f, a, out, n);
     return check_launch("axpy_kernel");
 }
 extern "C" int b200_cfg_combine(const float* pred, const float* null_pred, double* ws_red, float* out, int32_t B, int64_t per_sample,

@@ -1,6 +1,6 @@
-// Standalone bring-up harness for the tcgen05 GEMM (not part of the library): compares b200_gemm against
+// Standalone bring-up harness for the wgmma GEMM (not part of the library): compares b200_gemm against
 // a naive fp32 kernel on the same bf16 inputs, over operand-major / tail / epilogue / split-K cases, then
-// times the cfg2 shapes.  Build: make test_gemm ; run on a B200: timeout 120 ./test_gemm
+// times the cfg2 shapes.  Build: make test_gemm ; run on an H100: timeout 120 ./test_gemm [wide]
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <math.h>
@@ -170,13 +170,13 @@ int main(int argc, char** argv) {
         {"geglu", 260, 512, 128, 0, 0, 0, 1, 0, 0, 0, 1, 1, 0},
     };
     int bad = 0;
-    if (argc > 1 && !strcmp(argv[1], "pair")) {   // CTA-pair (cta_group::2) kernel: own process, a pipeline bug traps the context
+    if (argc > 1 && !strcmp(argv[1], "wide")) {   // 128 x 256 tiles (force_tile 3)
         cases.push_back({"kmajor multi-wave", 2048 + 32, 768, 512, 0, 0, 0, 0, 0, 0, 0, 0, 1, 0});
         cases.push_back({"dW-like split", 512, 512, 4096, 1, 1, 0, 0, 0, 0, 0, 0, 4, 1});
         cases.push_back({"two-source wide", 1000, 512, 768, 0, 0, 512, 1, 0, 0, 1, 0, 1, 0});
         cases.push_back({"geglu wide", 1100, 1408, 256, 0, 0, 0, 1, 0, 0, 0, 1, 1, 0});
         for (auto c : cases) { c.tile = 3; bad += run_case(c); }
-        printf("pair correctness: %d failing case(s)\n", bad);
+        printf("wide-tile correctness: %d failing case(s)\n", bad);
         if (bad) return 1;
         for (int tile = 2; tile <= 3; ++tile) {
             bench("ff-in (geglu)", 16896, 4096, 512, 0, 0, 1, 0, 1, tile, 1);
@@ -210,9 +210,9 @@ int main(int argc, char** argv) {
             cudaEventRecord(e0);
             for (int i = 0; i < it; ++i) {
                 b200_gemm(&g, 0);
-                if (mode == 1) tiny_kernel<<<148, 256>>>(scratch);
-                if (mode == 2) tiny_smem_kernel<<<148, 256, 100 * 1024>>>(scratch);
-                if (mode == 3) { tiny_kernel<<<148, 256>>>(scratch); tiny_kernel<<<148, 256>>>(scratch); }
+                if (mode == 1) tiny_kernel<<<132, 256>>>(scratch);
+                if (mode == 2) tiny_smem_kernel<<<132, 256, 100 * 1024>>>(scratch);
+                if (mode == 3) { tiny_kernel<<<132, 256>>>(scratch); tiny_kernel<<<132, 256>>>(scratch); }
             }
             cudaEventRecord(e1);
             CK(cudaDeviceSynchronize());
@@ -220,7 +220,7 @@ int main(int argc, char** argv) {
             printf("latency mode %d (0 gemm only, 1 gemm+tiny, 2 gemm+tiny(100KB smem), 3 gemm+2 tiny): %.2f us per iteration\n", mode, ms * 1e3 / it);
         }
         cudaEventRecord(e0);
-        for (int i = 0; i < 200; ++i) tiny_kernel<<<148, 256>>>(scratch);
+        for (int i = 0; i < 200; ++i) tiny_kernel<<<132, 256>>>(scratch);
         cudaEventRecord(e1); CK(cudaDeviceSynchronize());
         float ms; cudaEventElapsedTime(&ms, e0, e1);
         printf("tiny kernel alone: %.2f us per launch\n", ms * 1e3 / 200);

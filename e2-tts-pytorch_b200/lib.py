@@ -81,7 +81,7 @@ def load():
     if _lib is None:
         if not os.path.isfile(LIB_PATH):
             raise RuntimeError(f'{LIB_PATH} is missing: build it with `python -c "import __graft_entry__ as g; g.build()"` '
-                               f'(there is no CPU fallback for the B200 hot path)')
+                               f'(there is no CPU fallback for the CUDA hot path)')
         lib = ctypes.CDLL(LIB_PATH)
         for name, (restype, argt) in FUNCTIONS.items():
             fn = getattr(lib, name)  # AttributeError if the library does not export a declared symbol

@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's model classes for the hot path: same constructor / forward surface and
 the same state_dict keys as /root/reference/e2_tts_pytorch/e2_tts.py (SURVEY Appendix B), with every forward
-routed through the sm_100a kernels of libb200e2tts.so (ops.py). The nn.Modules below only HOLD parameters in
+routed through the sm_90a kernels of libb200e2tts.so (ops.py). The nn.Modules below only HOLD parameters in
 the reference's layout; the arithmetic lives in the CUDA library.
 """
 from __future__ import annotations
@@ -67,7 +67,7 @@ def _on_module_device(fn):
 
 def _unsupported(name, value, ref):
     raise NotImplementedError(
-        f'{name}={value!r} is a non-default research switch of the reference ({ref}) for which no B200 kernel is built; '
+        f'{name}={value!r} is a non-default research switch of the reference ({ref}) for which no CUDA kernel is built; '
         f'there is no fallback path (SURVEY.md §2 row 8)')
 
 
@@ -295,7 +295,7 @@ class _PackTable:
 
 class LinearFourierEmbed(Module):
     """e2_tts.py:368-386 — parameter holder (`linear.weight`, reference state_dict key `layers.{i}.0.4.linear.weight`); the arithmetic is
-    ops.FourierLinear (tcgen05 GEMM + b200_fourier_feat_*)."""
+    ops.FourierLinear (wgmma GEMM + b200_fourier_feat_*)."""
 
     def __init__(self, dim, p=0.5):
         super().__init__()
@@ -648,7 +648,7 @@ class Transformer(Module):
     @_on_module_device
     def forward(self, x, times=None, mask=None, text_embed=None):
         """Reference signature (e2_tts.py:731-737): x (b, n, d) -> (b, n, d)."""
-        assert x.ndim == 3, '`has_freq_axis` is not supported by the B200 build'
+        assert x.ndim == 3, '`has_freq_axis` is not supported by this build'
         assert not (exists(times) ^ self.cond_on_time), '`times` must be passed in if `cond_on_time` is set to `True` and vice versa'
         B, N, d = x.shape
         if torch.is_grad_enabled():

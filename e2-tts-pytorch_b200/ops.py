@@ -30,7 +30,7 @@ def _c(t):
 class _ZeroPool:
     """One zero-filled fp32 slab per training step for the ~300 small gradient accumulators the backward kernels add into
     (hyper-connection parameter grads, conv weight/bias grads, bias column sums, gate grads, abs-pos grads): ONE memset per step
-    instead of 300 `torch.zeros` fill kernels (3.1 % of the round-1 step, profiles/r1h_launch_summary.txt). `begin()` is called by the
+    instead of 300 `torch.zeros` fill kernels. `begin()` is called by the
     model's forward when a backward will follow; a fresh slab is allocated every step (gradients handed to autograd alias it and
     must outlive the step), sized by the previous step's demand; anything that does not fit falls back to torch.zeros."""
 
@@ -65,7 +65,7 @@ def _zeros(shape, device):
 def gemm(A, B, M, N, K, *, lda=None, ldb=None, A2=None, lda2=0, K1=0, a_mn=False, b_mn=False, out=None, ldd=None,
          out_fp32=False, D2=None, ldd2=0, bias=None, colscale=None, rows_per_batch=0, rowmask=None, resid=None, ldr=0,
          geglu=False, dropout_p=0.0, seed=0, split_k=1, force_tile=0, seed_dev=None):
-    """D[M,N] = epilogue(sum_k A[m,k] B[n,k]) on the tcgen05 GEMM (include/b200_e2tts.h: b200_gemm)."""
+    """D[M,N] = epilogue(sum_k A[m,k] B[n,k]) on the wgmma GEMM (include/b200_e2tts.h: b200_gemm)."""
     dev = A.device
     n_out = N // 2 if geglu else N
     if ldd is None:
@@ -334,7 +334,7 @@ class AttnCore(Function):
         dropout_p, seed, softclamp, seed_dev = ctx.meta
         B, H, Np, dh = q.shape
         legacy = ATTN_BWD_ENTRY.endswith('legacy')
-        dq = torch.empty(q.shape, device=q.device, dtype=BF16 if legacy else F32)   # tcgen05 backward accumulates dq in fp32
+        dq = torch.empty(q.shape, device=q.device, dtype=BF16 if legacy else F32)   # the wgmma backward accumulates dq in fp32
         dk, dv, ws_dO = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
         ws_delta = torch.empty_like(lse)
         d_gate = torch.empty_like(gate)
@@ -348,7 +348,7 @@ class AttnCore(Function):
 
 class Attention(Function):
     """Fused attention stage: ONE GEMM for to_q/to_k/to_v (+ head-gate and value-residual-mix logits), rotary + value
-    residual + gate post-processing, tcgen05 flash attention (softclamp, key mask, dropout, head gate). Returns the gated
+    residual + gate post-processing, wgmma flash attention (softclamp, key mask, dropout, head gate). Returns the gated
     head-merged output (input of to_out) and this layer's values (the first layer's feed every later layer, e2_tts.py:878,916).
     One autograd node: q/k/v never enter the graph, and dq stays fp32 from the attention backward into the rotary inverse."""
 
@@ -695,7 +695,7 @@ class TextStem(Function):
 class InterpText(Function):
     """InterpolatedCharacterEmbed (e2_tts.py:414-482): te = mask * (interpolate(embed(valid chars), audio_len) + abs_pos_mlp(linspace(0, Lt, La))).
     b200_interp_text_fwd stretches the embeddings and evaluates Linear(1, d) + SiLU per token; Linear(d, d) + bias + the stretched
-    embeddings (residual) + the row mask are ONE tcgen05 GEMM with its fused epilogue. Returns bf16 [B*N, d]."""
+    embeddings (residual) + the row mask are ONE wgmma GEMM with its fused epilogue. Returns bf16 [B*N, d]."""
 
     @staticmethod
     def forward(ctx, ids_c, text_len, audio_len, mask_u8, emb, w1, b1, w2, b2, B, N):

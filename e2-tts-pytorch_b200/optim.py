@@ -1,6 +1,6 @@
 """The step around forward/backward: gradient exchange, clipping, optimiser and EMA (SURVEY §8e, §8f row 1).
 
-Reference call sites (/root/reference/e2_tts_pytorch/trainer.py): DDP gradient all-reduce :155-162/:270, `clip_grad_norm_` :272-273,
+Reference call sites (e2_tts_pytorch/trainer.py of the original project): DDP gradient all-reduce :155-162/:270, `clip_grad_norm_` :272-273,
 `Adopt(model.parameters(), lr=...)` :183 + `optimizer.step()` :275, `EMA(model, include_online_model=False)` :170-174 + `.update()`
 :279. Here they are three launches over flat fp32 buffers:
 
@@ -9,7 +9,7 @@ Reference call sites (/root/reference/e2_tts_pytorch/trainer.py): DDP gradient a
                     b200_adopt_step   clip + Adopt + EMA in one pass
 
 Parameters remain the model's ordinary fp32 nn.Parameters (state_dict compatible); gradient / m / v / EMA storage is flat and owned
-here. `Adopt` and `EMA` are third-party packages that are not vendored under /root/reference: their update rules are restated in
+here. `Adopt` and `EMA` are third-party packages that are not vendored with the original project: their update rules are restated in
 oracle/optim_oracle.py (test infrastructure) and this module is checked against that restatement.
 """
 from __future__ import annotations

@@ -1,9 +1,9 @@
 /*
- * b200_e2tts.h — C ABI of libb200e2tts.so: the sm_100a kernels behind the E2-TTS flow-matching hot path.
+ * b200_e2tts.h — C ABI of libb200e2tts.so: the sm_90a (H100) kernels behind the E2-TTS flow-matching hot path.
  *
  * This is the drop-in boundary described in SURVEY.md §8(b): plain pointers and sizes, no torch types.
  * Every entry point replaces an eager PyTorch op chain of the reference (file:line cited per function,
- * relative to /root/reference/e2_tts_pytorch/e2_tts.py; "A.n" = SURVEY.md Appendix A, the unvendored
+ * relative to e2_tts_pytorch/e2_tts.py of the original project; "A.n" = SURVEY.md Appendix A, the unvendored
  * x-transformers / hyper-connections leaves the reference composes).
  *
  * Conventions
@@ -33,7 +33,7 @@ int b200_version(void);
 uint64_t b200_launch_count(void);
 
 /* ------------------------------------------------------------------------------------------------
- * Tensor-core GEMM (tcgen05 + TMEM + TMA):  D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )
+ * Tensor-core GEMM (wgmma + TMA):  D[M,N] = epilogue( sum_k A[m,k] * B[n,k] )
  * Replaces every nn.Linear on the path: to_q/to_k/to_v/to_out (A.4), FeedForward GLU proj + out (A.2),
  * skip_proj :649/:895-896, TextAudioCrossCondition :503-513, proj_in/cond_proj_in :1267-1277, to_pred
  * :1296, and all of their backward contractions (dX = dY*W, dW = dY^T*X).
@@ -66,7 +66,7 @@ typedef struct {
     int32_t geglu; float dropout_p; uint64_t seed;
     int32_t split_k;
     int32_t force_tile;   /* 0 = auto, 1 = 128 x 128 CTA tiles, 2 = 256 x 128 CTA tiles (two MMAs per k-step share one B tile),
-                           * 3 = CTA pair (cta_group::2): 2 x (128 x 256), each CTA stages half of the B tile; auto picks it for M >= 512, N >= 256 */
+                           * 3 = 128 x 256 CTA tiles (one m64n256 MMA per warpgroup and k-step); auto picks 3 for M >= 512, N >= 256 */
     const uint64_t* seed_dev;   /* optional DEVICE word added to `seed` when the kernel runs (see "dropout seeds" below); NULL = none */
 } b200_gemm_args;
 int b200_gemm(const b200_gemm_args* a, b200_stream_t stream);
@@ -101,13 +101,13 @@ typedef struct {
                                    one key mask, so the model builds the bitmask once instead of once per attention call */
 } b200_attn_fwd_args;
 size_t b200_attn_workspace_bytes(int32_t B, int32_t Np);
-/* key-validity bitmask of `keymask` (u8 [B,Np], NULL = all valid) into ws_maskbits, in the layout the tcgen05 kernels read */
+/* key-validity bitmask of `keymask` (u8 [B,Np], NULL = all valid) into ws_maskbits, in the layout the wgmma kernels read */
 int b200_attn_maskbits(const uint8_t* keymask, void* ws_maskbits, int32_t B, int32_t Np, b200_stream_t stream);
-int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream);        /* tcgen05 / TMEM / TMA kernel */
+int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream);        /* wgmma / TMA kernel */
 int b200_attn_fwd_legacy(const b200_attn_fwd_args* a, b200_stream_t stream); /* mma.sync bring-up kernel, kept for cross-checks */
 
 /* backward: d_og bf16 [B*Np, H*64] -> dk,dv bf16 [B,H,Np,64], dq FP32 [B,H,Np,64] (accumulated with atomics across key
- * tiles by the tcgen05 kernel; the legacy kernel writes bf16 dq), d_gate fp32 [B*Np,H] (grad wrt the sigmoid gate VALUE;
+ * tiles by the wgmma kernel; the legacy kernel writes bf16 dq), d_gate fp32 [B*Np,H] (grad wrt the sigmoid gate VALUE;
  * may be NULL). ws_dO (bf16 [B,H,Np,64]), ws_delta (fp32 [B,H,Np]) and ws_maskbits are caller workspaces. */
 typedef struct {
     const void *q, *k, *v, *o, *d_og;
@@ -123,7 +123,7 @@ typedef struct {
     const uint64_t* seed_dev;   /* optional device addend of `seed` (must be the forward's) */
     int32_t maskbits_ready;     /* as in b200_attn_fwd_args */
 } b200_attn_bwd_args;
-int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream);         /* tcgen05 / TMEM / TMA kernel, dq fp32 */
+int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream);         /* wgmma / TMA kernel, dq fp32 */
 int b200_attn_bwd_legacy(const b200_attn_bwd_args* a, b200_stream_t stream);  /* mma.sync bring-up kernels, dq bf16 */
 
 /* ------------------------------------------------------------------------------------------------
@@ -227,7 +227,7 @@ typedef struct {
     const void* dv_extra;   /* optional bf16 [B,H,Np,64] added to dv (value-residual gradients of later layers into layer 0) */
     void *d_qkvg, *d_vfirst;
     int32_t B, H, Np, dim_head;
-    int32_t dq_fp32;   /* bwd: dq is fp32 (tcgen05 attention backward) instead of bf16 */
+    int32_t dq_fp32;   /* bwd: dq is fp32 (wgmma attention backward) instead of bf16 */
 } b200_qkv_post_args;
 int b200_qkv_post_fwd(const b200_qkv_post_args* a, b200_stream_t stream);
 int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stream);
@@ -370,7 +370,7 @@ int b200_sumsq(const float* x, int64_t n, float* out, b200_stream_t stream);
  *   ("first" is tracked per chunk in chunk_state (int32 [n_chunks], zeroed once by the caller): a parameter that received no
  *   gradient on the first steps — the text stream while the text is dropped — is initialised when its first gradient arrives)
  *   ema_mode 1: ema += ema_weight (w - ema)   (ema-pytorch lerp, ema_weight = 1 - current decay);  2: ema = w (copy phase);  0: none
- * Adopt = adam-atan2-pytorch's `Adopt` (pyproject.toml:26, call site trainer.py:183) — the package is not under /root/reference;
+ * Adopt = adam-atan2-pytorch's `Adopt` (pyproject.toml:26, call site trainer.py:183) — the package is not part of the original project;
  * restated from the ADOPT algorithm it implements (Taniguchi et al. 2024, Alg. 2 without clipping) and pinned by a PyTorch
  * restatement in oracle/optim_oracle.py. chunk.ptr = the parameter piece. */
 typedef struct {

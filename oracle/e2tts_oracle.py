@@ -3,7 +3,7 @@
 THIS FILE IS TEST INFRASTRUCTURE. Only `tests/`, `__graft_entry__.smoke()` and the `cpu_baseline` /
 `--impl reference` legs of `bench.py` may import it; the product package never does.
 
-What it restates (all citations relative to /root/reference/e2_tts_pytorch/e2_tts.py unless noted):
+What it restates (all citations relative to e2_tts_pytorch/e2_tts.py of the original project unless noted):
   * E2TTS.forward            :1468-1595   (flow-matching objective)
   * transformer_with_pred_head :1250-1301, cfg_transformer_with_pred_head :1303-1330, project :113-124
   * E2TTS.sample             :1332-1466   (fixed-grid midpoint ODE, torchdiffeq semantics, SURVEY A.7)

@@ -1,8 +1,7 @@
 """Load the reference's OWN e2_tts.py, unmodified, by file path (build container only).
 
-TEST INFRASTRUCTURE. `/root/reference` exists only in the build container, never on the GPU box, so
-this module is used exclusively by `oracle/make_golden.py` and by the CPU tests that pin
-`oracle/e2tts_oracle.py` against the reference (they skip when the reference tree is absent).
+TEST INFRASTRUCTURE. E2TTS_REFERENCE_FILE names the original project's e2_tts.py; this module is used only by
+`oracle/make_golden.py` and `oracle/make_reference_golden.py`, which store the original's outputs under tests/golden/.
 The reference's seven unvendored third-party imports resolve to `oracle/ref_leaves/` (restated
 semantics, SURVEY.md Appendix A) — `e2_tts_pytorch/__init__.py` is bypassed because it pulls in
 trainer.py -> matplotlib/accelerate which are not installed.
@@ -11,7 +10,7 @@ import importlib.util
 import os
 import sys
 
-REF_FILE = os.environ.get('E2TTS_REFERENCE_FILE', '/root/reference/e2_tts_pytorch/e2_tts.py')
+REF_FILE = os.environ.get('E2TTS_REFERENCE_FILE', '')
 _LEAVES = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'ref_leaves')
 _cached = None
 

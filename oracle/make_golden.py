@@ -1,7 +1,7 @@
-"""Mint the golden vectors under tests/golden/ by running the reference's OWN e2_tts.py (build
-container only: needs /root/reference). TEST INFRASTRUCTURE.
+"""Mint the golden vectors under tests/golden/ by running the reference's OWN e2_tts.py (needs a checkout of the
+original project). TEST INFRASTRUCTURE.
 
-    python oracle/make_golden.py
+    E2TTS_REFERENCE_FILE=<original>/e2_tts_pytorch/e2_tts.py python oracle/make_golden.py
 
 The reference draws its randomness internally (x0, times, span mask); oracle/load_reference.py records
 those draws so they can be replayed into the oracle and the CUDA path. dropout=0 because dropout masks

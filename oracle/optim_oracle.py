@@ -1,9 +1,9 @@
 """CPU restatement of the optimiser-side step of the reference trainer — TEST INFRASTRUCTURE (only tests/ may import it).
 
-What it restates (call sites in /root/reference/e2_tts_pytorch/trainer.py):
+What it restates (call sites in e2_tts_pytorch/trainer.py of the original project):
   * `clip_grad_norm_(model.parameters(), max_grad_norm)`  :272-273  (torch.nn.utils: total L2 norm, coef = max_norm / (norm + 1e-6), clamped to 1)
   * `Adopt(model.parameters(), lr=...)` :183 and `.step()` :275 — adam-atan2-pytorch (pyproject.toml:26), NOT vendored under
-    /root/reference. PARITY UNPINNED: restated from the ADOPT algorithm (Taniguchi et al. 2024, "ADOPT: Modified Adam Can Converge
+    the original project. PARITY UNPINNED: restated from the ADOPT algorithm (Taniguchi et al. 2024, "ADOPT: Modified Adam Can Converge
     with Any beta2 with the Optimal Rate", Algorithm 2 without the optional update clipping) as lucidrains' `adopt.py` implements it:
         first call : v = g^2, m = 0, parameters untouched
         afterwards : m <- lerp(m, g / max(sqrt(v), eps), 1 - beta1);  p <- p - lr m;  v <- lerp(v, g^2, 1 - beta2)
