@@ -60,7 +60,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
 
 // key-validity bitmask: bit (n % 32) of word n / 32 is set iff key n participates (n < Np and mask[b, n] != 0)
 __global__ void attn_maskbits_kernel(const unsigned char* mask, unsigned int* bits, int B, int Np, int words) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= B * words) return;
     const int b = w / words, w0 = (w % words) * 32;
@@ -101,7 +100,6 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         fence_barrier_init();
     }
     __syncthreads();
-    pdl_wait();
 
     if (wg == 0) {
         regs_dealloc<40>();
@@ -119,7 +117,6 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
                 tma_load_2d(sV + st * TILE8, &tmV, &kv_full[st], 0, row_base + j * 64);
                 if (++st == KV_STAGES) { st = 0; ph ^= 1; }
             }
-            pdl_launch_dependents();
         }
         return;
     }
@@ -288,6 +285,48 @@ struct AttnBwdTcP {
 };
 constexpr int QDO_STAGES = 3, TQB = 64;
 
+// Backward prep, one 8-lane group per (b, h, n): dO = dOg * gate, d_gate = <dOg, O>, delta = gate * d_gate = <dO, O>
+struct AttnPrepP {
+    const float* gate;              // [B*Np, H] or null
+    const __nv_bfloat16* o;
+    int B, H, Np;
+    const __nv_bfloat16* dog;
+    float* dgate;                   // or null
+    __nv_bfloat16* dO_out;
+    float* delta_out;
+};
+__global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnPrepP p) {
+    const long long gidx = (long long)blockIdx.x * 256 + threadIdx.x;
+    const long long rowid = gidx >> 3;
+    const int c = (int)(gidx & 7);
+    const long long total = (long long)p.B * p.H * p.Np;
+    const bool ok = rowid < total;
+    float dot = 0.f, gt = 1.f;
+    long long b = 0, hh = 0, n = 0;
+    if (ok) {
+        n = rowid % p.Np; hh = (rowid / p.Np) % p.H; b = rowid / ((long long)p.Np * p.H);
+        const uint4 dg = *reinterpret_cast<const uint4*>(p.dog + ((size_t)b * p.Np + n) * (size_t)(p.H * DH) + hh * DH + c * 8);
+        const uint4 ov = *reinterpret_cast<const uint4*>(p.o + (size_t)rowid * DH + c * 8);
+        gt = p.gate ? p.gate[((size_t)b * p.Np + n) * p.H + hh] : 1.f;
+        const uint32_t dgv[4] = {dg.x, dg.y, dg.z, dg.w}, ovv[4] = {ov.x, ov.y, ov.z, ov.w};
+        uint32_t w[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float a0 = bf16_lo(dgv[i]), a1 = bf16_hi(dgv[i]);
+            dot += a0 * bf16_lo(ovv[i]) + a1 * bf16_hi(ovv[i]);
+            w[i] = pack_bf16(a0 * gt, a1 * gt);
+        }
+        *reinterpret_cast<uint4*>(p.dO_out + (size_t)rowid * DH + c * 8) = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+    dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+    dot += __shfl_xor_sync(0xffffffffu, dot, 4);
+    if (ok && c == 0) {
+        p.delta_out[rowid] = dot * gt;
+        if (p.dgate) p.dgate[((size_t)b * p.Np + n) * p.H + hh] = dot;
+    }
+}
+
 // P^T / dS^T of one query tile from the S^T / dP^T fragments (rows = keys kr, kr + 8; columns = queries qt0 + 8 g + cq + {0, 1})
 template <bool POLY, bool DROP>
 __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float (&s)[32], const float (&dp)[32], int bh, int qt0, int cq,
@@ -364,7 +403,6 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         fence_barrier_init();
     }
     __syncthreads();
-    pdl_wait();
 
     if (wg == 0) {
         regs_dealloc<40>();
@@ -383,7 +421,6 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
                 tma_load_2d(sDO + st * TILE8, &tmDO, &qdo_full[st], 0, row_base + qt_i * TQB);
                 if (++st == QDO_STAGES) { st = 0; ph ^= 1; }
             }
-            pdl_launch_dependents();
         }
         return;
     }
@@ -537,8 +574,8 @@ extern "C" size_t b200_attn_workspace_bytes(int32_t B, int32_t Np) {
 extern "C" int b200_attn_maskbits(const uint8_t* keymask, void* ws_maskbits, int32_t B, int32_t Np, b200_stream_t stream) {
     B200_REQUIRE(ws_maskbits && B > 0 && Np > 0, "attn_maskbits: bad arguments");
     const int words = ((Np + TKV - 1) / TKV) * 4;
-    B200_LAUNCH(attn_maskbits_kernel, (B * words + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream), keymask,
-                reinterpret_cast<unsigned int*>(ws_maskbits), B, Np, words);
+    attn_maskbits_kernel<<<(B * words + 127) / 128, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        keymask, reinterpret_cast<unsigned int*>(ws_maskbits), B, Np, words);
     return check_launch("attn_maskbits_kernel");
 }
 
@@ -549,16 +586,15 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_fwd: bad shape");
     B200_REQUIRE(a->softclamp > 0.f, "attn_fwd: softclamp value must be > 0 (the reference always clamps, e2_tts.py:548-551)");
     B200_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_fwd: dropout must be in [0,1)");
-    // the wgmma kernel exponentiates the clamped logits without a running maximum: exp(+-64) is well inside fp32 / bf16 range,
-    // a looser clamp (the reference default is 50, e2_tts.py:548-551) goes through the online-softmax mma.sync kernel instead
-    if (a->softclamp > 64.f) return b200_attn_fwd_legacy(a, stream);
+    B200_REQUIRE(a->softclamp <= 64.f, "attn_fwd: softclamp %g > 64: the wgmma kernel exponentiates the clamped logits without a running "
+                 "maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
     AttnTcP p{};
     p.nkv = (a->Np + TKV - 1) / TKV;
     p.mask_words = p.nkv * 4;
     p.maskbits = reinterpret_cast<const unsigned int*>(a->ws_maskbits);
     if (!a->maskbits_ready) {
         const int total = a->B * p.mask_words;
-        B200_LAUNCH(attn_maskbits_kernel, (total + 127) / 128, 128, 0, st, a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits), a->B, a->Np, p.mask_words);
+        attn_maskbits_kernel<<<(total + 127) / 128, 128, 0, st>>>(a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits), a->B, a->Np, p.mask_words);
         if (int rc = check_launch("attn_maskbits_kernel")) return rc;
     }
     p.gate = a->gate; p.o = (__nv_bfloat16*)a->o; p.og = (__nv_bfloat16*)a->og; p.lse = a->lse;
@@ -577,12 +613,9 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     cudaError_t e = set_max_smem_once(once, attn_fwd_wgmma_kernel, smem);
     B200_REQUIRE(e == cudaSuccess, "attn_fwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     dim3 grid((a->Np + TQ - 1) / TQ, a->H, a->B);
-    B200_LAUNCH(attn_fwd_wgmma_kernel, grid, 384, smem, st, tq, tk, tv, p);
+    attn_fwd_wgmma_kernel<<<grid, 384, smem, st>>>(tq, tk, tv, p);
     return check_launch("attn_fwd_wgmma_kernel");
 }
-
-// dO = dOg * gate, delta = <dO, O>, d_gate — defined in attn.cu
-namespace b200 { int launch_attn_bwd_prep(const b200_attn_bwd_args* a, cudaStream_t st); }
 
 extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -591,14 +624,20 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     B200_REQUIRE(a->dim_head == 64, "attn_bwd: only dim_head 64 is built (got %d)", a->dim_head);
     B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_bwd: bad shape");
     B200_REQUIRE(a->softclamp > 0.f && a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_bwd: bad softclamp / dropout");
-    if (int rc = launch_attn_bwd_prep(a, st)) return rc;
+    B200_REQUIRE(a->softclamp <= 64.f, "attn_bwd: softclamp %g > 64: the wgmma kernel exponentiates the clamped logits without a running "
+                 "maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
+    const AttnPrepP pp{a->gate, (const __nv_bfloat16*)a->o, a->B, a->H, a->Np, (const __nv_bfloat16*)a->d_og, a->d_gate,
+                       (__nv_bfloat16*)a->ws_dO, a->ws_delta};
+    const long long prep_threads = (long long)a->B * a->H * a->Np * 8;
+    attn_bwd_prep_kernel<<<(unsigned)((prep_threads + 255) / 256), 256, 0, st>>>(pp);
+    if (int rc = check_launch("attn_bwd_prep_kernel")) return rc;
     AttnBwdTcP p{};
     p.nq = (a->Np + TQB - 1) / TQB;
     p.mask_words = ((a->Np + TKV - 1) / TKV) * 4;
     p.maskbits = reinterpret_cast<const unsigned int*>(a->ws_maskbits);
     if (!a->maskbits_ready) {
         const int total = a->B * p.mask_words;
-        B200_LAUNCH(attn_maskbits_kernel, (total + 127) / 128, 128, 0, st, a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits), a->B, a->Np, p.mask_words);
+        attn_maskbits_kernel<<<(total + 127) / 128, 128, 0, st>>>(a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits), a->B, a->Np, p.mask_words);
         if (int rc = check_launch("attn_maskbits_kernel")) return rc;
     }
     const size_t nelem = (size_t)a->B * a->H * a->Np * DH;
@@ -621,6 +660,6 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     cudaError_t e2 = set_max_smem_once(once, attn_bwd_wgmma_kernel, smem);
     B200_REQUIRE(e2 == cudaSuccess, "attn_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
     dim3 grid((a->Np + TKV - 1) / TKV, a->H, a->B);
-    B200_LAUNCH(attn_bwd_wgmma_kernel, grid, 384, smem, st, tq, tk, tv, tdo, p);
+    attn_bwd_wgmma_kernel<<<grid, 384, smem, st>>>(tq, tk, tv, tdo, p);
     return check_launch("attn_bwd_wgmma_kernel");
 }

@@ -3,7 +3,6 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
-#include <stdlib.h>
 
 #include <atomic>
 #include <mutex>
@@ -35,36 +34,6 @@ inline int check_launch(const char* what) {
     }
     return 0;
 }
-
-// Programmatic dependent launch needs a `make PDL=1` build AND B200_PDL=1 at run time: with it every library kernel is launched through
-// cudaLaunchKernelEx with cudaLaunchAttributeProgrammaticStreamSerialization, without it through the plain <<< >>> launch.
-#ifndef B200_PDL_BUILD
-#define B200_PDL_BUILD 0
-#endif
-inline bool pdl_enabled() {
-#if B200_PDL_BUILD
-    static const bool on = getenv("B200_PDL") && atoi(getenv("B200_PDL")) != 0;
-    return on;
-#else
-    return false;   // the kernels of this build do not execute griddepcontrol.wait: never launch them as programmatic dependents
-#endif
-}
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
-}
-// B200_LAUNCH((kernel<...>), grid, block, smem, stream, args...) — errors surface through check_launch() as before
-#define B200_LAUNCH(kern, grid, block, smem, st, ...)                                  \
-    do {                                                                               \
-        if (b200::pdl_enabled()) (void)b200::launch_pdl(kern, grid, block, smem, st, __VA_ARGS__); \
-        else kern<<<grid, block, smem, st>>>(__VA_ARGS__);                             \
-    } while (0)
 
 constexpr int kMaxDevices = 64;
 inline int current_device() {

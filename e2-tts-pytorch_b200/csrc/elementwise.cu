@@ -30,7 +30,6 @@ __device__ __forceinline__ int pack_row(const b200_pack_desc& d, int r) {
     return r < inner ? (r >> 6) * 128 + (r & 63) : ((r - inner) >> 6) * 128 + 64 + ((r - inner) & 63);
 }
 __global__ void __launch_bounds__(256) pack_weights_kernel(const b200_pack_desc* descs) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const b200_pack_desc d = descs[blockIdx.y];
     if ((d.cols & 3) || (d.col_off & 3) || (d.ld_dst & 3)) {  // scalar path (1-D biases, odd widths)
         const long long total = (long long)d.rows * d.cols;
@@ -65,7 +64,6 @@ struct StemP {
     int concat;   // != 0: columns [0, C) = cond, [C, 2C) = x  (cat(cond, x), e2_tts.py:1265)
 };
 __global__ void __launch_bounds__(256) stem_prepare_kernel(const StemP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const long long total = (long long)p.B * p.N * p.Cp * 2;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
         const int col = (int)(i % (2 * p.Cp));
@@ -109,7 +107,6 @@ struct AsmP {
     float *d_tok, *d_abs_pos, *d_registers;
 };
 __global__ void __launch_bounds__(256) assemble_fwd_kernel(const AsmP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int nchunk = p.D >> 3;
     const long long total = (long long)p.B * (p.R + p.N) * nchunk;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -144,7 +141,6 @@ __global__ void __launch_bounds__(256) assemble_fwd_kernel(const AsmP p) {
 }
 // thread per (position, chunk): loops over batch; sums the S stream gradients
 __global__ void __launch_bounds__(256) assemble_bwd_kernel(const AsmP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int nchunk = p.D >> 3;
     const long long total = (long long)(p.R + p.N) * nchunk;
     const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -181,7 +177,6 @@ __global__ void __launch_bounds__(256) assemble_bwd_kernel(const AsmP p) {
 // embedding gradient: grid (vocab row, token slab); a block scans its slab for its id and adds its partial row
 // (the hot filler id 0 is spread over all slabs instead of one serial block). d_emb is zeroed by the host wrapper.
 __global__ void __launch_bounds__(256) embed_bwd_kernel(const float* d_tok, const int* ids, float* d_emb, int ntok, int D, int slab) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int v = blockIdx.x;
     const int t0 = blockIdx.y * slab, t1 = min(ntok, t0 + slab);
     __shared__ int hits[256];
@@ -204,7 +199,6 @@ __global__ void __launch_bounds__(256) embed_bwd_kernel(const float* d_tok, cons
 
 // ------------------------------------------------------------------------------------------------ rotary table
 __global__ void rotary_table_kernel(float* cs, float* sn, int Np, int half) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= Np * half) return;
     const int n = i / half, j = i % half;
@@ -231,7 +225,6 @@ struct QkvP {
     int dq_fp32;
 };
 __global__ void __launch_bounds__(256) qkv_post_fwd_kernel(const QkvP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const long long total = (long long)p.B * p.Np * p.H * 8;
     const int I = p.H * 64;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -266,7 +259,6 @@ __global__ void __launch_bounds__(256) qkv_post_fwd_kernel(const QkvP p) {
     }
 }
 __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const long long total = (long long)p.B * p.Np * p.H * 8;
     const int I = p.H * 64;
     const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
@@ -340,7 +332,6 @@ __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
 constexpr int GB_ROWS = 256;   // rows per block (8 row lanes x 32)
 __global__ void __launch_bounds__(256) geglu_bwd_kernel(const __nv_bfloat16* dh, const __nv_bfloat16* ug, __nv_bfloat16* dug, float* db, long long T,
                                                          int inner, float dropout_p, unsigned long long seed, const unsigned long long* seed_dev) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     __shared__ float red[8][32][17];
     const int nchunk = inner >> 3;
     const int cl = threadIdx.x & 31, rl = threadIdx.x >> 5;
@@ -409,7 +400,6 @@ __global__ void __launch_bounds__(256) geglu_bwd_kernel(const __nv_bfloat16* dh,
 template <int CL>
 __global__ void __launch_bounds__(256) colsum_kernel(const __nv_bfloat16* __restrict__ X, long long T, int ncols, int ld,
                                                      float* __restrict__ out, int rows_per_block) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     constexpr int RL = 256 / CL;
     __shared__ float red[8][CL * 8];
     const int cg = threadIdx.x % CL, rl = threadIdx.x / CL;
@@ -469,7 +459,6 @@ struct FnP {
 };
 template <int VPT>
 __global__ void __launch_bounds__(256) final_norm_fwd_kernel(const FnP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int lane = threadIdx.x & 31, nchunk = p.D >> 3;
     const long long ntok = (long long)p.B * p.N;
     for (long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5); row < ntok; row += (long long)gridDim.x * 8) {
@@ -508,7 +497,6 @@ __global__ void __launch_bounds__(256) final_norm_fwd_kernel(const FnP p) {
 }
 template <int VPT>
 __global__ void __launch_bounds__(256) final_norm_bwd_kernel(const FnP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ float sg[];  // [D]
     for (int i = threadIdx.x; i < p.D; i += 256) sg[i] = 0.f;
     __syncthreads();
@@ -575,7 +563,6 @@ struct LossP {
     const float* vel_target; float vel_weight; float* loss_parts;   // velocity-consistency term (e2_tts.py:1556-1576), optional
 };
 __global__ void __launch_bounds__(256) flow_loss_fwd_kernel(const LossP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     float acc = 0.f, cnt = 0.f, accv = 0.f;
     const long long total = p.rows * p.C;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -606,14 +593,12 @@ __global__ void __launch_bounds__(256) flow_loss_fwd_kernel(const LossP p) {
 }
 // loss = flow + vel_weight * velocity (e2_tts.py:1586-1589); loss_parts (optional) = {flow, velocity} for the LossBreakdown
 __global__ void flow_loss_finalize_kernel(const float* sums, float* loss, int C, int has_vel, float vel_weight, float* loss_parts) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const float den = sums[1] * (float)C;
     const float flow = sums[0] / den, vel = has_vel ? sums[2] / den : 0.f;
     *loss = flow + vel_weight * vel;
     if (loss_parts) { loss_parts[0] = flow; loss_parts[1] = vel; }
 }
 __global__ void __launch_bounds__(256) flow_loss_bwd_kernel(const LossP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const float scale = 2.f * (*p.dloss) / (p.sums[1] * (float)p.C);
     const long long total = p.rows * p.ldp;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -639,7 +624,6 @@ __global__ void __launch_bounds__(256) rowgate_bwd_kernel(const __nv_bfloat16* _
                                                            const float* __restrict__ cs, const unsigned char* __restrict__ mask,
                                                            __nv_bfloat16* __restrict__ dz, float* __restrict__ d_cs,
                                                            float* __restrict__ d_bias, int rows_per_batch, int D, int rows_per_block) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ float sacc[];  // [D] gate sums, then [D] bias sums
     float* sbias = sacc + D;
     const int b = blockIdx.y;
@@ -705,7 +689,6 @@ __global__ void __launch_bounds__(256) rowgate_bwd_kernel(const __nv_bfloat16* _
 
 // fp32 -> bf16 cast with row pitch (used for small host-provided matrices)
 __global__ void cast_rows_kernel(const float* src, __nv_bfloat16* dst, long long rows, int cols, int ld) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const long long total = rows * ld;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
         const int c = (int)(i % ld);
@@ -725,7 +708,7 @@ using namespace b200;
 
 extern "C" int b200_pack_weights(const b200_pack_desc* descs_dev, int32_t n, b200_stream_t stream) {
     B200_REQUIRE(descs_dev && n > 0, "pack_weights: empty table");
-    B200_LAUNCH(pack_weights_kernel, dim3(32, n), 256, 0, reinterpret_cast<cudaStream_t>(stream), descs_dev);
+    pack_weights_kernel<<<dim3(32, n), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(descs_dev);
     return check_launch("pack_weights_kernel");
 }
 
@@ -733,7 +716,7 @@ extern "C" int b200_stem_prepare(const b200_stem_args* a, b200_stream_t stream) 
     B200_REQUIRE(a && a->A && ((a->x1 && a->x0 && a->times && a->span) || (a->x_in && a->cond_in)), "stem_prepare: null pointer");
     B200_REQUIRE(a->C > 0 && a->Cp >= a->C && (a->Cp % 64) == 0, "stem_prepare: Cp must be a multiple of 64 >= C");
     StemP p{a->x1, a->x0, a->times, a->x_in, a->cond_in, a->span, (__nv_bfloat16*)a->A, a->cond_out, a->B, a->N, a->C, a->Cp, a->concat_cond};
-    B200_LAUNCH(stem_prepare_kernel, grid_for((long long)a->B * a->N * a->Cp * 2), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+    stem_prepare_kernel<<<grid_for((long long)a->B * a->N * a->Cp * 2), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("stem_prepare_kernel");
 }
 
@@ -749,7 +732,7 @@ extern "C" int b200_assemble_fwd(const b200_assemble_args* a, b200_stream_t stre
     if (fill_asm(p, a)) return -1;
     B200_REQUIRE(a->out, "assemble_fwd: null output");
     p.out = (__nv_bfloat16*)a->out;
-    B200_LAUNCH(assemble_fwd_kernel, grid_for((long long)a->B * (a->R + a->N) * (a->D / 8)), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+    assemble_fwd_kernel<<<grid_for((long long)a->B * (a->R + a->N) * (a->D / 8)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("assemble_fwd_kernel");
 }
 extern "C" int b200_assemble_bwd(const b200_assemble_args* a, b200_stream_t stream) {
@@ -758,7 +741,7 @@ extern "C" int b200_assemble_bwd(const b200_assemble_args* a, b200_stream_t stre
     B200_REQUIRE(a->d_out, "assemble_bwd: null d_out");
     p.d_out = (const __nv_bfloat16*)a->d_out; p.d_h = (__nv_bfloat16*)a->d_h; p.d_tok = a->d_tok; p.d_abs_pos = a->d_abs_pos; p.d_registers = a->d_registers;
     const long long total = (long long)(a->R + a->N) * (a->D / 8);
-    B200_LAUNCH(assemble_bwd_kernel, (unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+    assemble_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("assemble_bwd_kernel");
 }
 extern "C" int b200_embed_bwd(const float* d_tok, const int32_t* ids, float* d_emb, int32_t ntok, int32_t D, int32_t vocab, b200_stream_t stream) {
@@ -767,12 +750,12 @@ extern "C" int b200_embed_bwd(const float* d_tok, const int32_t* ids, float* d_e
     cudaError_t e = cudaMemsetAsync(d_emb, 0, (size_t)vocab * D * sizeof(float), st);
     B200_REQUIRE(e == cudaSuccess, "embed_bwd: memset: %s", cudaGetErrorString(e));
     const int slab = 1024;
-    B200_LAUNCH(embed_bwd_kernel, dim3(vocab, (ntok + slab - 1) / slab), 256, 0, st, d_tok, ids, d_emb, ntok, D, slab);
+    embed_bwd_kernel<<<dim3(vocab, (ntok + slab - 1) / slab), 256, 0, st>>>(d_tok, ids, d_emb, ntok, D, slab);
     return check_launch("embed_bwd_kernel");
 }
 extern "C" int b200_rotary_table(float* cos_out, float* sin_out, int32_t Np, int32_t dim_head, b200_stream_t stream) {
     B200_REQUIRE(cos_out && sin_out && Np > 0 && dim_head == 64, "rotary_table: only dim_head 64 is built");
-    B200_LAUNCH(rotary_table_kernel, (Np * 32 + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream), cos_out, sin_out, Np, 32);
+    rotary_table_kernel<<<(Np * 32 + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(cos_out, sin_out, Np, 32);
     return check_launch("rotary_table_kernel");
 }
 
@@ -790,7 +773,7 @@ extern "C" int b200_qkv_post_fwd(const b200_qkv_post_args* a, b200_stream_t stre
     if (fill_qkv(p, a)) return -1;
     B200_REQUIRE(a->q && a->k && a->v, "qkv_post_fwd: null output");
     p.q = (__nv_bfloat16*)a->q; p.k = (__nv_bfloat16*)a->k; p.v = (__nv_bfloat16*)a->v;
-    B200_LAUNCH(qkv_post_fwd_kernel, grid_for((long long)a->B * a->Np * a->H * 8), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+    qkv_post_fwd_kernel<<<grid_for((long long)a->B * a->Np * a->H * 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("qkv_post_fwd_kernel");
 }
 extern "C" int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stream) {
@@ -800,7 +783,7 @@ extern "C" int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stre
     p.dq = (const __nv_bfloat16*)a->dq; p.dk = (const __nv_bfloat16*)a->dk; p.dv = (const __nv_bfloat16*)a->dv; p.d_gate = a->d_gate;
     p.d_qkvg = (__nv_bfloat16*)a->d_qkvg; p.d_vfirst = (__nv_bfloat16*)a->d_vfirst; p.dq_fp32 = a->dq_fp32; p.dv_extra = (const __nv_bfloat16*)a->dv_extra;
     const long long total = (long long)a->B * a->Np * a->H * 8;
-    B200_LAUNCH(qkv_post_bwd_kernel, (unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+    qkv_post_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("qkv_post_bwd_kernel");
 }
 
@@ -808,7 +791,7 @@ extern "C" int b200_geglu_bwd(const void* dh, const void* ug, void* dug, float* 
                               const uint64_t* seed_dev, b200_stream_t stream) {
     B200_REQUIRE(dh && ug && dug && T > 0 && inner > 0 && (inner % 64) == 0, "geglu_bwd: inner must be a multiple of 64");
     dim3 grid((inner / 8 + 31) / 32, (unsigned)((T + GB_ROWS - 1) / GB_ROWS));
-    B200_LAUNCH(geglu_bwd_kernel, grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), 
+    geglu_bwd_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
         (const __nv_bfloat16*)dh, (const __nv_bfloat16*)ug, (__nv_bfloat16*)dug, db_packed, T, inner, dropout_p, seed, reinterpret_cast<const unsigned long long*>(seed_dev));
     return check_launch("geglu_bwd_kernel");
 }
@@ -829,11 +812,11 @@ extern "C" int b200_colsum(const void* X, int64_t T, int32_t ncols, int32_t ld, 
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const __nv_bfloat16* x = (const __nv_bfloat16*)X;
     switch (cl) {
-        case 32: B200_LAUNCH(colsum_kernel<32>, grid, 256, 0, st, x, T, ncols, ld, out, (int)rows_per_block); break;
-        case 16: B200_LAUNCH(colsum_kernel<16>, grid, 256, 0, st, x, T, ncols, ld, out, (int)rows_per_block); break;
-        case 8: B200_LAUNCH(colsum_kernel<8>, grid, 256, 0, st, x, T, ncols, ld, out, (int)rows_per_block); break;
-        case 4: B200_LAUNCH(colsum_kernel<4>, grid, 256, 0, st, x, T, ncols, ld, out, (int)rows_per_block); break;
-        default: B200_LAUNCH(colsum_kernel<2>, grid, 256, 0, st, x, T, ncols, ld, out, (int)rows_per_block); break;
+        case 32: colsum_kernel<32><<<grid, 256, 0, st>>>(x, T, ncols, ld, out, (int)rows_per_block); break;
+        case 16: colsum_kernel<16><<<grid, 256, 0, st>>>(x, T, ncols, ld, out, (int)rows_per_block); break;
+        case 8: colsum_kernel<8><<<grid, 256, 0, st>>>(x, T, ncols, ld, out, (int)rows_per_block); break;
+        case 4: colsum_kernel<4><<<grid, 256, 0, st>>>(x, T, ncols, ld, out, (int)rows_per_block); break;
+        default: colsum_kernel<2><<<grid, 256, 0, st>>>(x, T, ncols, ld, out, (int)rows_per_block); break;
     }
     return check_launch("colsum_kernel");
 }
@@ -844,9 +827,9 @@ extern "C" int b200_final_norm_fwd(const b200_final_norm_args* a, b200_stream_t 
     FnP p{(const __nv_bfloat16*)a->xres, a->g, (__nv_bfloat16*)a->y, a->B, a->N, a->R, a->D, a->S, nullptr, nullptr, nullptr};
     const int grid = (int)min(((long long)a->B * a->N + 7) / 8, (long long)num_sms() * 8);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (a->D <= 256) B200_LAUNCH(final_norm_fwd_kernel<1>, grid, 256, 0, st, p);
-    else if (a->D <= 512) B200_LAUNCH(final_norm_fwd_kernel<2>, grid, 256, 0, st, p);
-    else B200_LAUNCH(final_norm_fwd_kernel<4>, grid, 256, 0, st, p);
+    if (a->D <= 256) final_norm_fwd_kernel<1><<<grid, 256, 0, st>>>(p);
+    else if (a->D <= 512) final_norm_fwd_kernel<2><<<grid, 256, 0, st>>>(p);
+    else final_norm_fwd_kernel<4><<<grid, 256, 0, st>>>(p);
     return check_launch("final_norm_fwd_kernel");
 }
 extern "C" int b200_final_norm_bwd(const b200_final_norm_args* a, b200_stream_t stream) {
@@ -856,9 +839,9 @@ extern "C" int b200_final_norm_bwd(const b200_final_norm_args* a, b200_stream_t 
     const int grid = (int)min(((long long)a->B * (a->N + a->R) + 7) / 8, (long long)num_sms() * 4);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const size_t smem = (size_t)a->D * 4;
-    if (a->D <= 256) B200_LAUNCH(final_norm_bwd_kernel<1>, grid, 256, smem, st, p);
-    else if (a->D <= 512) B200_LAUNCH(final_norm_bwd_kernel<2>, grid, 256, smem, st, p);
-    else B200_LAUNCH(final_norm_bwd_kernel<4>, grid, 256, smem, st, p);
+    if (a->D <= 256) final_norm_bwd_kernel<1><<<grid, 256, smem, st>>>(p);
+    else if (a->D <= 512) final_norm_bwd_kernel<2><<<grid, 256, smem, st>>>(p);
+    else final_norm_bwd_kernel<4><<<grid, 256, smem, st>>>(p);
     return check_launch("final_norm_bwd_kernel");
 }
 
@@ -868,15 +851,15 @@ extern "C" int b200_flow_loss_fwd(const b200_flow_loss_args* a, b200_stream_t st
     cudaError_t e = cudaMemsetAsync(a->sums, 0, 4 * sizeof(float), st);
     B200_REQUIRE(e == cudaSuccess, "flow_loss_fwd: memset: %s", cudaGetErrorString(e));
     LossP p{a->pred, a->x1, a->x0, a->span, a->sums, a->pred_data, a->rows, a->C, nullptr, nullptr, 0, a->vel_target, a->vel_weight, a->loss_parts};
-    B200_LAUNCH(flow_loss_fwd_kernel, grid_for(a->rows * a->C), 256, 0, st, p);
+    flow_loss_fwd_kernel<<<grid_for(a->rows * a->C), 256, 0, st>>>(p);
     if (int rc = check_launch("flow_loss_fwd_kernel")) return rc;
-    B200_LAUNCH(flow_loss_finalize_kernel, 1, 1, 0, st, a->sums, a->loss, a->C, a->vel_target != nullptr, a->vel_weight, a->loss_parts);
+    flow_loss_finalize_kernel<<<1, 1, 0, st>>>(a->sums, a->loss, a->C, a->vel_target != nullptr, a->vel_weight, a->loss_parts);
     return check_launch("flow_loss_finalize_kernel");
 }
 extern "C" int b200_flow_loss_bwd(const b200_flow_loss_args* a, b200_stream_t stream) {
     B200_REQUIRE(a && a->pred && a->x1 && a->x0 && a->span && a->sums && a->dloss && a->dpred && a->ldp >= a->C && (a->ldp % 8) == 0, "flow_loss_bwd: bad arguments");
     LossP p{a->pred, a->x1, a->x0, a->span, a->sums, nullptr, a->rows, a->C, a->dloss, (__nv_bfloat16*)a->dpred, a->ldp, a->vel_target, a->vel_weight, nullptr};
-    B200_LAUNCH(flow_loss_bwd_kernel, grid_for(a->rows * a->ldp), 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+    flow_loss_bwd_kernel<<<grid_for(a->rows * a->ldp), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("flow_loss_bwd_kernel");
 }
 
@@ -886,7 +869,7 @@ extern "C" int b200_rowgate_bwd(const void* dy, const void* y, const float* cs, 
     B200_REQUIRE(!cs || (y && d_cs), "rowgate_bwd: gate backward needs y and d_cs");
     const int rpb = 64;
     dim3 grid((rows_per_batch + rpb - 1) / rpb, B);
-    B200_LAUNCH(rowgate_bwd_kernel, grid, 256, (size_t)D * 8, reinterpret_cast<cudaStream_t>(stream), 
+    rowgate_bwd_kernel<<<grid, 256, (size_t)D * 8, reinterpret_cast<cudaStream_t>(stream)>>>(
         (const __nv_bfloat16*)dy, (const __nv_bfloat16*)y, cs, mask, (__nv_bfloat16*)dz, d_cs, d_bias, rows_per_batch, D, rpb);
     return check_launch("rowgate_bwd_kernel");
 }
@@ -897,7 +880,6 @@ extern "C" int b200_rowgate_bwd(const void* dy, const void* y, const float* cs, 
 namespace b200 {
 __global__ void __launch_bounds__(256) fourier_feat_fwd_kernel(const __nv_bfloat16* __restrict__ z, long long ldz, __nv_bfloat16* __restrict__ out,
                                                                long long T, int df, int dr) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int dout = 2 * df + dr;
     const long long total = T * dout;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -914,7 +896,6 @@ __global__ void __launch_bounds__(256) fourier_feat_fwd_kernel(const __nv_bfloat
 // dz[:, :df] = d_out[:, :df] * cos(z) - d_out[:, df:2df] * sin(z);  dz[:, df:] = d_out[:, 2df:]
 __global__ void __launch_bounds__(256) fourier_feat_bwd_kernel(const __nv_bfloat16* __restrict__ d_out, const __nv_bfloat16* __restrict__ z,
                                                                long long ldz, __nv_bfloat16* __restrict__ dz, long long T, int df, int dr) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int dout = 2 * df + dr, dz_cols = df + dr;
     const long long total = T * ldz;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
@@ -936,13 +917,13 @@ __global__ void __launch_bounds__(256) fourier_feat_bwd_kernel(const __nv_bfloat
 
 extern "C" int b200_fourier_feat_fwd(const void* z, int64_t ldz, void* out, int64_t T, int32_t df, int32_t dr, b200_stream_t stream) {
     B200_REQUIRE(z && out && T > 0 && df >= 0 && dr >= 0 && df + dr > 0 && ldz >= df + dr, "fourier_feat_fwd: bad arguments");
-    B200_LAUNCH(fourier_feat_fwd_kernel, grid_for(T * (2 * df + dr)), 256, 0, reinterpret_cast<cudaStream_t>(stream), (const __nv_bfloat16*)z,
+    fourier_feat_fwd_kernel<<<grid_for(T * (2 * df + dr)), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>((const __nv_bfloat16*)z,
                 (long long)ldz, (__nv_bfloat16*)out, (long long)T, df, dr);
     return check_launch("fourier_feat_fwd_kernel");
 }
 extern "C" int b200_fourier_feat_bwd(const void* d_out, const void* z, int64_t ldz, void* dz, int64_t T, int32_t df, int32_t dr, b200_stream_t stream) {
     B200_REQUIRE(d_out && z && dz && T > 0 && df >= 0 && dr >= 0 && df + dr > 0 && ldz >= df + dr, "fourier_feat_bwd: bad arguments");
-    B200_LAUNCH(fourier_feat_bwd_kernel, grid_for(T * ldz), 256, 0, reinterpret_cast<cudaStream_t>(stream), (const __nv_bfloat16*)d_out,
+    fourier_feat_bwd_kernel<<<grid_for(T * ldz), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>((const __nv_bfloat16*)d_out,
                 (const __nv_bfloat16*)z, (long long)ldz, (__nv_bfloat16*)dz, (long long)T, df, dr);
     return check_launch("fourier_feat_bwd_kernel");
 }
@@ -971,7 +952,6 @@ __device__ __forceinline__ void interp_coords(int n, int Lt, int La, int& i0, in
     pos = (n < La / 2 || La == 1) ? (float)n * step : (float)Lt - (float)(La - 1 - n) * step;
 }
 __global__ void __launch_bounds__(256) interp_text_fwd_kernel(const InterpP p, __nv_bfloat16* __restrict__ lerp, __nv_bfloat16* __restrict__ h1) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const long long total = (long long)p.B * p.N * p.D;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
         const int c = (int)(i % p.D);
@@ -995,7 +975,6 @@ __global__ void __launch_bounds__(256) interp_text_fwd_kernel(const InterpP p, _
 constexpr int INTERP_ROWS = 64;
 __global__ void __launch_bounds__(256) interp_text_bwd_kernel(const InterpP p, const __nv_bfloat16* __restrict__ d_lerp, const __nv_bfloat16* __restrict__ d_h1,
                                                               float* __restrict__ d_emb, float* __restrict__ dw1, float* __restrict__ db1) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int c = blockIdx.x * 256 + threadIdx.x;
     if (c >= p.D) return;
     const long long r0 = (long long)blockIdx.y * INTERP_ROWS, r1 = min((long long)p.B * p.N, r0 + INTERP_ROWS);
@@ -1035,7 +1014,7 @@ extern "C" int b200_interp_text_fwd(const b200_interp_text_args* a, b200_stream_
     InterpP p{};
     if (fill_interp(p, a)) return -1;
     B200_REQUIRE(a->lerp && a->h1, "interp_text_fwd: null output");
-    B200_LAUNCH(interp_text_fwd_kernel, grid_for((long long)a->B * a->N * a->D), 256, 0, reinterpret_cast<cudaStream_t>(stream), p,
+    interp_text_fwd_kernel<<<grid_for((long long)a->B * a->N * a->D), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p,
                 (__nv_bfloat16*)a->lerp, (__nv_bfloat16*)a->h1);
     return check_launch("interp_text_fwd_kernel");
 }
@@ -1045,13 +1024,13 @@ extern "C" int b200_interp_text_bwd(const b200_interp_text_args* a, b200_stream_
     B200_REQUIRE(a->d_lerp && a->d_h1 && a->d_emb && a->d_w1 && a->d_b1, "interp_text_bwd: null pointer");
     const long long rows = (long long)a->B * a->N;
     dim3 grid((a->D + 255) / 256, (unsigned)((rows + INTERP_ROWS - 1) / INTERP_ROWS));
-    B200_LAUNCH(interp_text_bwd_kernel, grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), p, (const __nv_bfloat16*)a->d_lerp,
+    interp_text_bwd_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p, (const __nv_bfloat16*)a->d_lerp,
                 (const __nv_bfloat16*)a->d_h1, a->d_emb, a->d_w1, a->d_b1);
     return check_launch("interp_text_bwd_kernel");
 }
 
 extern "C" int b200_cast_rows(const float* src, void* dst, int64_t rows, int32_t cols, int32_t ld, b200_stream_t stream) {
     B200_REQUIRE(src && dst && rows > 0 && cols > 0 && ld >= cols, "cast_rows: bad arguments");
-    B200_LAUNCH(cast_rows_kernel, grid_for(rows * ld), 256, 0, reinterpret_cast<cudaStream_t>(stream), src, (__nv_bfloat16*)dst, rows, cols, ld);
+    cast_rows_kernel<<<grid_for(rows * ld), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(src, (__nv_bfloat16*)dst, rows, cols, ld);
     return check_launch("cast_rows_kernel");
 }

@@ -120,7 +120,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         fence_barrier_init();
     }
     __syncthreads();
-    pdl_wait();   // barrier set-up and descriptor prefetch may overlap the tail of the previous kernel (ptx.cuh)
 
     if (wg == 0) {
         regs_dealloc<40>();
@@ -161,7 +160,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
             }
-            pdl_launch_dependents();   // all operand loads are issued: the next kernel's CTAs may start their prologue
         }
         return;
     }
@@ -368,7 +366,7 @@ static int launch_gemm(const CUtensorMap (&tm)[3], const GemmParams& p, cudaStre
         B200_REQUIRE(e == cudaSuccess, "gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
     const int grid = p.num_work < num_sms() ? p.num_work : num_sms();
-    B200_LAUNCH(kern, grid, kGemmThreads, S::TOTAL, st, tm[0], tm[1], tm[2], p);
+    kern<<<grid, kGemmThreads, S::TOTAL, st>>>(tm[0], tm[1], tm[2], p);
     return check_launch("gemm_wgmma_kernel");
 }
 

@@ -9,8 +9,6 @@
 // HBM layout: residual streams are (token, stream, d) bf16 so the 4 streams of a token are adjacent (the
 // reference's '(b s) n d' puts them N'*d apart). One warp owns one token; all reductions are warp shuffles.
 // These kernels are HBM-bound: width reads S*d and writes (S+1)*d bf16 per token (algorithmic minimum).
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -233,7 +231,6 @@ __device__ __forceinline__ void load_gain8(const float* g, f2 (&o)[4]) {   // 8 
 // long-scoreboard stalls.
 template <int VPT, bool PF, bool FUSED>
 __global__ void __launch_bounds__(256, (VPT <= 2) ? 2 : 1) hc_width_fwd_kernel(const HcP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ float4 sp[];
     __shared__ uint64_t bars[8][2];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -350,7 +347,6 @@ __global__ void __launch_bounds__(256, (VPT <= 2) ? 2 : 1) hc_width_fwd_kernel(c
 // R^T C = xres^T C + y_prev^T C' needs no materialised R.
 template <int VPT, bool PF, bool FUSED>
 __global__ void __launch_bounds__(256, (VPT == 1) ? 2 : 1) hc_width_bwd_kernel(const HcP p, __nv_bfloat16* __restrict__ cmat, int tok_per_block) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ float4 sp[];
     __shared__ float s_scal[32];
     __shared__ float s_gng[VPT * 256];   // d(norm gain) partial sums of this block (one batch element), VPT*256 >= D
@@ -637,7 +633,6 @@ __global__ void __launch_bounds__(256, (VPT == 1) ? 2 : 1) hc_width_bwd_kernel(c
 //   d norm.gamma[col]          = sum_t alpha_fn[col][t] G[col][t] + beta_fn[col] G[col][5].
 // (The first versions marched 128-token slabs per thread pair on the CUDA cores: 48 us per call against ~15 us for the GEMM.)
 __global__ void __launch_bounds__(256) hc_param_finalize_kernel(const HcP p, const float* __restrict__ G) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int col = blockIdx.x * 256 + threadIdx.x;
     if (col >= p.D) return;
     const float4 g0 = *reinterpret_cast<const float4*>(G + (size_t)col * 8), g1v = *reinterpret_cast<const float4*>(G + (size_t)col * 8 + 4);
@@ -666,7 +661,6 @@ struct HdP {
 
 // out[t,s,:] = res[t,s,:] + beta[t,s] * y[t,:]     (one 16-byte chunk of y per thread, all 4 streams)
 __global__ void __launch_bounds__(256) hc_depth_fwd_kernel(const HdP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int nchunk = p.D >> 3;
     const long long total = (long long)p.T * nchunk;
     for (long long idx = (long long)blockIdx.x * 256 + threadIdx.x; idx < total; idx += (long long)gridDim.x * 256) {
@@ -690,7 +684,6 @@ __global__ void __launch_bounds__(256) hc_depth_fwd_kernel(const HdP p) {
 
 // d_y[t,:] = sum_s beta[t,s] d_out[t,s,:];  d_beta[t,s] = <d_out[t,s,:], y[t,:]>   (one warp per token)
 __global__ void __launch_bounds__(256) hc_depth_bwd_kernel(const HdP p) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int lane = threadIdx.x & 31;
     const int nchunk = p.D >> 3;
     const long long nwarps = (long long)gridDim.x * 8;
@@ -718,10 +711,6 @@ __global__ void __launch_bounds__(256) hc_depth_bwd_kernel(const HdP p) {
     }
 }
 
-static bool hc_prefetch_enabled() {
-    static const bool on = !(getenv("B200_HC_PREFETCH") && atoi(getenv("B200_HC_PREFETCH")) == 0);   // developer A/B switch, default on
-    return on;
-}
 // the dynamic shared-memory ceiling of a token kernel depends on D, which a process may vary between calls (text / audio streams):
 // raise it once per (kernel instantiation, device) to the kernel's maximum instead of per call (SURVEY §8b: once_flag-guarded init)
 template <auto kern>          // the kernel is a template VALUE: instantiations that share a function type still get their own flag
@@ -759,24 +748,24 @@ using namespace b200;
 template <bool FUSED>
 static int launch_hc_fwd(const HcP& p, const b200_hc_width_args* a, cudaStream_t st) {
     const size_t smem_par = hc_param_smem(a->D);
-    if (a->D <= 512 && hc_prefetch_enabled()) {
+    if (a->D <= 512) {
         // prefetching variant: 2 blocks per SM, each warp owns a double buffer of one token {4 streams (+ y_prev, beta_prev)}
         const size_t tok = (size_t)HS * a->D * 2 + (FUSED ? (size_t)a->D * 2 + 16 : 0);
         const size_t smem = smem_par + 8 * 2 * tok;
         const int grid = (int)min((long long)(a->T + 7) / 8, (long long)num_sms() * 2);
         if (a->D <= 256) {
             if (int rc = set_smem<hc_width_fwd_kernel<1, true, FUSED>>(smem)) return rc;
-            B200_LAUNCH((hc_width_fwd_kernel<1, true, FUSED>), grid, 256, smem, st, p);
+            hc_width_fwd_kernel<1, true, FUSED><<<grid, 256, smem, st>>>(p);
         } else {
             if (int rc = set_smem<hc_width_fwd_kernel<2, true, FUSED>>(smem)) return rc;
-            B200_LAUNCH((hc_width_fwd_kernel<2, true, FUSED>), grid, 256, smem, st, p);
+            hc_width_fwd_kernel<2, true, FUSED><<<grid, 256, smem, st>>>(p);
         }
         return check_launch("hc_width_fwd_kernel");
     }
     const int grid = (int)min((long long)(a->T + 7) / 8, (long long)num_sms() * 8);
-    if (a->D <= 256) B200_LAUNCH((hc_width_fwd_kernel<1, false, FUSED>), grid, 256, smem_par, st, p);
-    else if (a->D <= 512) B200_LAUNCH((hc_width_fwd_kernel<2, false, FUSED>), grid, 256, smem_par, st, p);
-    else B200_LAUNCH((hc_width_fwd_kernel<4, false, FUSED>), grid, 256, smem_par, st, p);
+    if (a->D <= 256) hc_width_fwd_kernel<1, false, FUSED><<<grid, 256, smem_par, st>>>(p);
+    else if (a->D <= 512) hc_width_fwd_kernel<2, false, FUSED><<<grid, 256, smem_par, st>>>(p);
+    else hc_width_fwd_kernel<4, false, FUSED><<<grid, 256, smem_par, st>>>(p);
     return check_launch("hc_width_fwd_kernel");
 }
 
@@ -801,19 +790,19 @@ static int launch_hc_bwd(const HcP& p, const b200_hc_width_args* a, __nv_bfloat1
     if (tpb < 32) tpb = 32;                     // amortise the per-block parameter staging
     dim3 grid((a->rows_per_batch + tpb - 1) / tpb, nbatch);
     const size_t smem_par = hc_param_smem(a->D);
-    if (a->D <= 512 && hc_prefetch_enabled()) {
+    if (a->D <= 512) {
         // + per-warp {r, d_res, d_branch (, y_prev, beta_prev)} double buffers
         const size_t smem = smem_par + (size_t)8 * 2 * ((2 * HS + 1 + (FUSED ? 1 : 0)) * a->D * 2 + (FUSED ? 16 : 0));
         if (a->D <= 256) {
             if (int rc = set_smem<hc_width_bwd_kernel<1, true, FUSED>>(smem)) return rc;
-            B200_LAUNCH((hc_width_bwd_kernel<1, true, FUSED>), grid, 256, smem, st, p, cmat, tpb);
+            hc_width_bwd_kernel<1, true, FUSED><<<grid, 256, smem, st>>>(p, cmat, tpb);
         } else {
             if (int rc = set_smem<hc_width_bwd_kernel<2, true, FUSED>>(smem)) return rc;
-            B200_LAUNCH((hc_width_bwd_kernel<2, true, FUSED>), grid, 256, smem, st, p, cmat, tpb);
+            hc_width_bwd_kernel<2, true, FUSED><<<grid, 256, smem, st>>>(p, cmat, tpb);
         }
-    } else if (a->D <= 256) B200_LAUNCH((hc_width_bwd_kernel<1, false, FUSED>), grid, 256, smem_par, st, p, cmat, tpb);
-    else if (a->D <= 512) B200_LAUNCH((hc_width_bwd_kernel<2, false, FUSED>), grid, 256, smem_par, st, p, cmat, tpb);
-    else B200_LAUNCH((hc_width_bwd_kernel<4, false, FUSED>), grid, 256, smem_par, st, p, cmat, tpb);
+    } else if (a->D <= 256) hc_width_bwd_kernel<1, false, FUSED><<<grid, 256, smem_par, st>>>(p, cmat, tpb);
+    else if (a->D <= 512) hc_width_bwd_kernel<2, false, FUSED><<<grid, 256, smem_par, st>>>(p, cmat, tpb);
+    else hc_width_bwd_kernel<4, false, FUSED><<<grid, 256, smem_par, st>>>(p, cmat, tpb);
     return check_launch("hc_width_bwd_kernel");
 }
 
@@ -853,7 +842,7 @@ extern "C" int b200_hc_width_bwd(const b200_hc_width_args* a, b200_stream_t stre
     const int tiles = (a->D + 255) / 256;
     g.split_k = num_sms() / tiles > 1 ? num_sms() / tiles : 2;   // >= 2: the split-K path zeroes and accumulates G
     if (int rc = b200_gemm(&g, stream)) return rc;
-    B200_LAUNCH(hc_param_finalize_kernel, (a->D + 255) / 256, 256, 0, st, p, G);
+    hc_param_finalize_kernel<<<(a->D + 255) / 256, 256, 0, st>>>(p, G);
     return check_launch("hc_param_finalize_kernel");
 }
 
@@ -865,7 +854,7 @@ extern "C" int b200_hc_depth_fwd(const b200_hc_depth_args* a, b200_stream_t stre
     p.res = (const __nv_bfloat16*)a->res; p.y = (const __nv_bfloat16*)a->y; p.beta = a->beta; p.out = (__nv_bfloat16*)a->out; p.T = a->T; p.D = a->D;
     const long long total = (long long)a->T * (a->D / 8);
     const int grid = (int)min((total + 255) / 256, (long long)num_sms() * 16);
-    B200_LAUNCH(hc_depth_fwd_kernel, grid, 256, 0, st, p);
+    hc_depth_fwd_kernel<<<grid, 256, 0, st>>>(p);
     return check_launch("hc_depth_fwd_kernel");
 }
 
@@ -877,6 +866,6 @@ extern "C" int b200_hc_depth_bwd(const b200_hc_depth_args* a, b200_stream_t stre
     p.y = (const __nv_bfloat16*)a->y; p.beta = a->beta; p.T = a->T; p.D = a->D;
     p.d_out = (const __nv_bfloat16*)a->d_out; p.d_y = (__nv_bfloat16*)a->d_y; p.d_beta = a->d_beta;
     const int grid = (int)min((long long)(a->T + 7) / 8, (long long)num_sms() * 8);
-    B200_LAUNCH(hc_depth_bwd_kernel, grid, 256, 0, st, p);
+    hc_depth_bwd_kernel<<<grid, 256, 0, st>>>(p);
     return check_launch("hc_depth_bwd_kernel");
 }

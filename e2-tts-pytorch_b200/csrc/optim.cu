@@ -13,7 +13,6 @@ namespace b200 {
 
 __global__ void __launch_bounds__(256) flat_gather_kernel(const b200_chunk* __restrict__ chunks, float* __restrict__ flat, float scale,
                                                           float* __restrict__ used) {
-    pdl_wait();
     const b200_chunk c = chunks[blockIdx.x];
     const float* __restrict__ src = reinterpret_cast<const float*>(c.ptr);
     float* __restrict__ dst = flat + c.flat_offset;
@@ -33,7 +32,6 @@ __global__ void __launch_bounds__(256) flat_gather_kernel(const b200_chunk* __re
 }
 
 __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x, long long n, float* __restrict__ out) {
-    pdl_wait();
     float acc = 0.f;
     const long long n4 = ((reinterpret_cast<uintptr_t>(x) & 15) == 0) ? (n >> 2) : 0;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)gridDim.x * 256) {
@@ -83,7 +81,6 @@ __device__ __forceinline__ void adopt_elem(const AdoptP& p, float g, float& w, f
 }
 
 __global__ void __launch_bounds__(256) adopt_step_kernel(const AdoptP p) {
-    pdl_wait();
     const b200_chunk c = p.chunks[blockIdx.x];
     float* __restrict__ w = reinterpret_cast<float*>(c.ptr);
     const long long off = c.flat_offset;
@@ -121,7 +118,6 @@ __global__ void __launch_bounds__(256) adopt_step_kernel(const AdoptP p) {
 
 // scatter: param_ptr[i] = flat[flat_offset + i] (EMA weights back into a module's parameters, e.g. for sampling with the EMA model)
 __global__ void __launch_bounds__(256) flat_scatter_kernel(const b200_chunk* __restrict__ chunks, const float* __restrict__ flat) {
-    pdl_wait();
     const b200_chunk c = chunks[blockIdx.x];
     float* __restrict__ dst = reinterpret_cast<float*>(c.ptr);
     const float* __restrict__ src = flat + c.flat_offset;
@@ -134,13 +130,13 @@ using namespace b200;
 
 extern "C" int b200_flat_gather(const b200_chunk* chunks_dev, int32_t n_chunks, float* flat, float scale, float* used, b200_stream_t stream) {
     B200_REQUIRE(chunks_dev && flat && n_chunks > 0, "flat_gather: null pointer / empty table");
-    B200_LAUNCH(flat_gather_kernel, n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream), chunks_dev, flat, scale, used);
+    flat_gather_kernel<<<n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(chunks_dev, flat, scale, used);
     return check_launch("flat_gather_kernel");
 }
 
 extern "C" int b200_flat_scatter(const b200_chunk* chunks_dev, int32_t n_chunks, const float* flat, b200_stream_t stream) {
     B200_REQUIRE(chunks_dev && flat && n_chunks > 0, "flat_scatter: null pointer / empty table");
-    B200_LAUNCH(flat_scatter_kernel, n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream), chunks_dev, flat);
+    flat_scatter_kernel<<<n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(chunks_dev, flat);
     return check_launch("flat_scatter_kernel");
 }
 
@@ -151,7 +147,7 @@ extern "C" int b200_sumsq(const float* x, int64_t n, float* out, b200_stream_t s
     B200_REQUIRE(e == cudaSuccess, "sumsq: memset: %s", cudaGetErrorString(e));
     const long long blocks = (n / 4 + 255) / 256;
     const int grid = (int)(blocks < 1 ? 1 : (blocks > (long long)num_sms() * 8 ? (long long)num_sms() * 8 : blocks));
-    B200_LAUNCH(sumsq_kernel, grid, 256, 0, st, x, (long long)n, out);
+    sumsq_kernel<<<grid, 256, 0, st>>>(x, (long long)n, out);
     return check_launch("sumsq_kernel");
 }
 
@@ -164,6 +160,6 @@ extern "C" int b200_adopt_step(const b200_adopt_args* a, b200_stream_t stream) {
     p.gradnorm_sq = a->gradnorm_sq; p.max_grad_norm = a->max_grad_norm; p.used = a->used;
     p.lr = a->lr; p.beta1 = a->beta1; p.beta2 = a->beta2; p.eps = a->eps; p.weight_decay = a->weight_decay;
     p.chunk_state = a->chunk_state; p.ema_mode = a->ema_mode; p.ema_weight = a->ema_weight;
-    B200_LAUNCH(adopt_step_kernel, a->n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream), p);
+    adopt_step_kernel<<<a->n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("adopt_step_kernel");
 }

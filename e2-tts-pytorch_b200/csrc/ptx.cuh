@@ -99,24 +99,6 @@ __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bul
 template <int N>
 __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 
-// ---------------------------------------------------------------- programmatic dependent launch
-// Programmatic dependent launch (PDL). Every kernel of the library executes pdl_wait() before its first global-memory access: when
-// the kernel was launched with the programmatic-stream-serialisation attribute (B200_PDL=1, common.cuh) its CTAs may become resident
-// and run their prologue while the previous kernel in the stream is still draining, and pdl_wait() blocks until that kernel has
-// completed and flushed; launched normally, the instruction returns immediately. pdl_launch_dependents() lets the NEXT kernel start
-// that early once every CTA of this grid has issued it (or exited) — placed after the main loop of the long persistent kernels.
-// Compiled in only with `make PDL=1` (-DB200_PDL_BUILD=1) and enabled at run time with B200_PDL=1; the default build carries neither.
-#ifndef B200_PDL_BUILD
-#define B200_PDL_BUILD 0
-#endif
-#if B200_PDL_BUILD
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-#else
-__device__ __forceinline__ void pdl_wait() {}
-__device__ __forceinline__ void pdl_launch_dependents() {}
-#endif
-
 // 1-D bulk copy global -> shared (TMA engine, no tensor map): `bytes` a multiple of 16, both addresses 16-byte aligned
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"

@@ -56,7 +56,6 @@ __device__ __forceinline__ void sl_halve16(float (&v)[16], int lane) {   // on r
 }
 
 __global__ void __launch_bounds__(256) small_linear_fwd_kernel(const b200_small_linear_args a, int n_per_warp, int x_in_smem) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ __align__(16) float xs[];
     const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
     if (x_in_smem) {
@@ -105,7 +104,6 @@ __global__ void __launch_bounds__(256) small_linear_fwd_kernel(const b200_small_
 }
 // one warp per output feature n: dZ[:,n], dbias[n], dW[n,:]
 __global__ void __launch_bounds__(256) small_linear_bwd_w_kernel(const b200_small_linear_args a) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     __shared__ float sdz[8][SL_MAXB];
     const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
     const int n = blockIdx.x * 8 + wl;
@@ -133,7 +131,6 @@ __global__ void __launch_bounds__(256) small_linear_bwd_w_kernel(const b200_smal
 // consecutive k (16-byte W loads, 16-byte vector reductions into dX) and one of two 128-row halves of the slab.
 constexpr int SL_SLAB = 256;   // largest slab of output features per block (a multiple of 8; smaller slabs when N is small)
 __global__ void __launch_bounds__(256) small_linear_bwd_x_kernel(const b200_small_linear_args a, int slab) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ __align__(16) float sdz[];   // [B][slab]
     const int n0 = blockIdx.x * slab, n1 = min(a.N, n0 + slab);
     for (int i = threadIdx.x; i < a.B * slab; i += 256) {
@@ -198,7 +195,6 @@ __global__ void __launch_bounds__(256) small_linear_bwd_x_kernel(const b200_smal
 }
 
 __global__ void fourier_embed_kernel(const float* times, const float* w, float* out, int B, int half) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= B * half) return;
     const int b = i / half, j = i % half;
@@ -269,7 +265,6 @@ __device__ __forceinline__ void conv_rows2(const cf2 (&w)[31], const float (*src
 // their latency hides behind the FMA loop instead of stalling every warp of the block.
 constexpr int CV_FWD_TILES = 2;
 __global__ void __launch_bounds__(256, 3) dwconv_fwd_kernel(const b200_dwconv_args a) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     __shared__ __align__(16) float xs[CV_R][CV_TC];
     __shared__ __align__(16) float sw[31][CV_TC];
     __shared__ unsigned char sok[CV_R];
@@ -343,7 +338,6 @@ constexpr int CV_TILES_PER_BLOCK = 4;   // n-tiles marched by one block: weight/
 // block splits by warp: warps 0-3 compute dx = flipped conv of d_pre (taps in registers), warps 4-7 accumulate the tap gradients
 // dW[k] += d_pre[n] * x[n + k - 15] and d(bias) in registers across the block's tiles — both halves run 31 paired FMAs per element pair.
 __global__ void __launch_bounds__(256, 2) dwconv_bwd_kernel(const b200_dwconv_args a) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ __align__(16) float sm[];
     float (*xs)[CV_TC] = reinterpret_cast<float (*)[CV_TC]>(sm);                          // [CV_R] masked x
     float (*dps)[CV_TC] = reinterpret_cast<float (*)[CV_TC]>(sm + CV_R * CV_TC);           // [CV_R] d_pre
@@ -448,7 +442,6 @@ __global__ void __launch_bounds__(256, 2) dwconv_bwd_kernel(const b200_dwconv_ar
 
 // ------------------------------------------------------------------------------------------------ masked mean
 __global__ void __launch_bounds__(256) masked_mean_fwd_kernel(const __nv_bfloat16* x, const unsigned char* mask, float* out, int N, int D) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int b = blockIdx.y, d = blockIdx.x * 256 + threadIdx.x;
     if (d >= D) return;
     float acc = 0.f, den = 0.f;
@@ -459,7 +452,6 @@ __global__ void __launch_bounds__(256) masked_mean_fwd_kernel(const __nv_bfloat1
     out[(size_t)b * D + d] = acc / fmaxf(den, 1.f);
 }
 __global__ void __launch_bounds__(256) masked_mean_bwd_kernel(const float* dout, const unsigned char* mask, __nv_bfloat16* dx, int N, int D) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     __shared__ float sden;
     const int b = blockIdx.y;
     if (threadIdx.x == 0) {
@@ -480,12 +472,10 @@ __global__ void __launch_bounds__(256) masked_mean_bwd_kernel(const float* dout,
 // ------------------------------------------------------------------------------------------------ ODE / CFG helpers
 // out = y + a * f  (fixed-grid midpoint / Euler update, torchdiffeq semantics A.7)
 __global__ void __launch_bounds__(256) axpy_kernel(const float* y, const float* f, float a, float* out, long long n) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) out[i] = y[i] + a * f[i];
 }
 // per-sample fp64 reductions for the APG projection (e2_tts.py:113-124): red[b] = (<pred - null, pred>, <pred, pred>)
 __global__ void __launch_bounds__(256) cfg_reduce_kernel(const float* pred, const float* null_pred, double* red, long long per) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int b = blockIdx.y;
     const float* p = pred + (size_t)b * per;
     const float* q = null_pred + (size_t)b * per;
@@ -509,7 +499,6 @@ __global__ void __launch_bounds__(256) cfg_reduce_kernel(const float* pred, cons
 // out = pred + (orth + par * keep) * strength, par = (<upd, unit>) unit, unit = pred / max(||pred||, 1e-12)
 __global__ void __launch_bounds__(256) cfg_apply_kernel(const float* pred, const float* null_pred, const double* red, float* out, long long per,
                                                          float strength, int remove_parallel, float keep) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     const int b = blockIdx.y;
     const double nrm = fmax(sqrt(red[2 * b + 1]), 1e-12);
     const double coef = red[2 * b] / (nrm * nrm);   // <upd, unit> / ||pred||
@@ -534,7 +523,6 @@ __global__ void __launch_bounds__(256) cfg_apply_kernel(const float* pred, const
 // non-zero; the bands are found once per call by mel_bands_kernel), log. Output [B, n_mels, frames] like the reference.
 // (Round 1 used a direct O(n^2) DFT and the dense filterbank: ~1 M serial FMAs per frame.)
 __global__ void mel_bands_kernel(const float* __restrict__ fb, int nbins, int n_mels, int2* __restrict__ bands) {
-    pdl_wait();
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= n_mels) return;
     int lo = nbins, hi = 0;
@@ -546,7 +534,6 @@ __global__ void mel_bands_kernel(const float* __restrict__ fb, int nbins, int n_
 __global__ void __launch_bounds__(256) melspec_kernel(const float* __restrict__ wave, const float* __restrict__ window, const float* __restrict__ fb,
                                                        const int2* __restrict__ bands, float* __restrict__ out, int nw_max, int n_fft, int log2n,
                                                        int hop, int n_mels, int frames, const int* __restrict__ wave_lens, int out_bnd) {
-    pdl_wait();   // no global access before the previous kernel of the stream has completed (ptx.cuh)
     extern __shared__ float2 zsm[];
     float2* z = zsm;                 // [n_fft] in-place FFT buffer
     float2* tw = z + n_fft;          // [n_fft/2] twiddles e^{-2 pi i k / n_fft}
@@ -615,7 +602,7 @@ extern "C" int b200_small_linear_fwd(const b200_small_linear_args* a, b200_strea
         int npw = 1;
         while (npw < 8 && (a->N + 8 * (npw * 2) - 1) / (8 * (npw * 2)) >= 2 * num_sms()) npw *= 2;
         const int per_block = 8 * npw;
-        B200_LAUNCH(small_linear_fwd_kernel, (a->N + per_block - 1) / per_block, 256, smem, reinterpret_cast<cudaStream_t>(stream), *a, npw, x_in_smem);
+        small_linear_fwd_kernel<<<(a->N + per_block - 1) / per_block, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(*a, npw, x_in_smem);
     }
     return check_launch("small_linear_fwd_kernel");
 }
@@ -623,7 +610,7 @@ extern "C" int b200_small_linear_bwd(const b200_small_linear_args* a, b200_strea
     B200_REQUIRE(a && a->X && a->W && a->Z && a->dY && a->dZ && a->dW, "small_linear_bwd: null pointer");
     B200_REQUIRE(a->B > 0 && a->B <= SL_MAXB && a->N > 0 && a->K > 0, "small_linear: batch must be 1..%d", SL_MAXB);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    B200_LAUNCH(small_linear_bwd_w_kernel, (a->N + 7) / 8, 256, 0, st, *a);
+    small_linear_bwd_w_kernel<<<(a->N + 7) / 8, 256, 0, st>>>(*a);
     if (int rc = check_launch("small_linear_bwd_w_kernel")) return rc;
     if (a->dX) {
         cudaError_t e = cudaMemsetAsync(a->dX, 0, (size_t)a->B * a->K * sizeof(float), st);
@@ -634,14 +621,14 @@ extern "C" int b200_small_linear_bwd(const b200_small_linear_args* a, b200_strea
         static DeviceOnce once;
         cudaError_t e2 = set_max_smem_once(once, small_linear_bwd_x_kernel, SL_MAXB * SL_SLAB * (int)sizeof(float));
         B200_REQUIRE(e2 == cudaSuccess, "small_linear_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
-        B200_LAUNCH(small_linear_bwd_x_kernel, (a->N + slab - 1) / slab, 256, smem, st, *a, slab);
+        small_linear_bwd_x_kernel<<<(a->N + slab - 1) / slab, 256, smem, st>>>(*a, slab);
         return check_launch("small_linear_bwd_x_kernel");
     }
     return 0;
 }
 extern "C" int b200_fourier_embed(const float* times, const float* weights, float* out, int32_t B, int32_t half, b200_stream_t stream) {
     B200_REQUIRE(times && weights && out && B > 0 && half > 0, "fourier_embed: bad arguments");
-    B200_LAUNCH(fourier_embed_kernel, (B * half + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream), times, weights, out, B, half);
+    fourier_embed_kernel<<<(B * half + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(times, weights, out, B, half);
     return check_launch("fourier_embed_kernel");
 }
 
@@ -656,7 +643,7 @@ extern "C" int b200_dwconv_fwd(const b200_dwconv_args* a, b200_stream_t stream) 
     B200_REQUIRE(a->y, "dwconv_fwd: null output");
     const int ntiles = (a->Np + CV_TN - 1) / CV_TN;
     dim3 grid((ntiles + CV_FWD_TILES - 1) / CV_FWD_TILES, (a->D + CV_TC - 1) / CV_TC, a->B);
-    B200_LAUNCH(dwconv_fwd_kernel, grid, 256, 0, reinterpret_cast<cudaStream_t>(stream), *a);
+    dwconv_fwd_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
     return check_launch("dwconv_fwd_kernel");
 }
 extern "C" int b200_dwconv_bwd(const b200_dwconv_args* a, b200_stream_t stream) {
@@ -668,25 +655,25 @@ extern "C" int b200_dwconv_bwd(const b200_dwconv_args* a, b200_stream_t stream) 
     B200_REQUIRE(set_max_smem_once(once, dwconv_bwd_kernel, (int)smem) == cudaSuccess, "dwconv_bwd: cudaFuncSetAttribute failed");
     const int ntiles = (a->Np + CV_TN - 1) / CV_TN;
     dim3 grid((ntiles + CV_TILES_PER_BLOCK - 1) / CV_TILES_PER_BLOCK, (a->D + CV_TC - 1) / CV_TC, a->B);
-    B200_LAUNCH(dwconv_bwd_kernel, grid, 256, smem, reinterpret_cast<cudaStream_t>(stream), *a);
+    dwconv_bwd_kernel<<<grid, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
     return check_launch("dwconv_bwd_kernel");
 }
 
 extern "C" int b200_masked_mean_fwd(const void* x, const uint8_t* mask, float* out, int32_t B, int32_t N, int32_t D, b200_stream_t stream) {
     B200_REQUIRE(x && out && B > 0 && N > 0 && D > 0, "masked_mean_fwd: bad arguments");
-    B200_LAUNCH(masked_mean_fwd_kernel, dim3((D + 255) / 256, B), 256, 0, reinterpret_cast<cudaStream_t>(stream), (const __nv_bfloat16*)x, mask, out, N, D);
+    masked_mean_fwd_kernel<<<dim3((D + 255) / 256, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>((const __nv_bfloat16*)x, mask, out, N, D);
     return check_launch("masked_mean_fwd_kernel");
 }
 extern "C" int b200_masked_mean_bwd(const float* dout, const uint8_t* mask, void* dx, int32_t B, int32_t N, int32_t D, b200_stream_t stream) {
     B200_REQUIRE(dout && dx && B > 0 && N > 0 && D > 0, "masked_mean_bwd: bad arguments");
-    B200_LAUNCH(masked_mean_bwd_kernel, dim3(64, B), 256, 0, reinterpret_cast<cudaStream_t>(stream), dout, mask, (__nv_bfloat16*)dx, N, D);
+    masked_mean_bwd_kernel<<<dim3(64, B), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(dout, mask, (__nv_bfloat16*)dx, N, D);
     return check_launch("masked_mean_bwd_kernel");
 }
 
 extern "C" int b200_axpy(const float* y, const float* f, float a, float* out, int64_t n, b200_stream_t stream) {
     B200_REQUIRE(y && f && out && n > 0, "axpy: bad arguments");
     const long long g = (n + 255) / 256;
-    B200_LAUNCH(axpy_kernel, (unsigned)(g > num_sms() * 16 ? num_sms() * 16 : g), 256, 0, reinterpret_cast<cudaStream_t>(stream), y, f, a, out, n);
+    axpy_kernel<<<(unsigned)(g > num_sms() * 16 ? num_sms() * 16 : g), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(y, f, a, out, n);
     return check_launch("axpy_kernel");
 }
 extern "C" int b200_cfg_combine(const float* pred, const float* null_pred, double* ws_red, float* out, int32_t B, int64_t per_sample,
@@ -696,9 +683,9 @@ extern "C" int b200_cfg_combine(const float* pred, const float* null_pred, doubl
     cudaError_t e = cudaMemsetAsync(ws_red, 0, (size_t)B * 2 * sizeof(double), st);
     B200_REQUIRE(e == cudaSuccess, "cfg_combine: memset: %s", cudaGetErrorString(e));
     const int gx = (int)((per_sample + 256 * 8 - 1) / (256 * 8));
-    B200_LAUNCH(cfg_reduce_kernel, dim3(gx < 1 ? 1 : gx, B), 256, 0, st, pred, null_pred, ws_red, per_sample);
+    cfg_reduce_kernel<<<dim3(gx < 1 ? 1 : gx, B), 256, 0, st>>>(pred, null_pred, ws_red, per_sample);
     if (int rc = check_launch("cfg_reduce_kernel")) return rc;
-    B200_LAUNCH(cfg_apply_kernel, dim3(gx < 1 ? 1 : gx, B), 256, 0, st, pred, null_pred, ws_red, out, per_sample, cfg_strength, remove_parallel, keep_parallel_frac);
+    cfg_apply_kernel<<<dim3(gx < 1 ? 1 : gx, B), 256, 0, st>>>(pred, null_pred, ws_red, out, per_sample, cfg_strength, remove_parallel, keep_parallel_frac);
     return check_launch("cfg_apply_kernel");
 }
 extern "C" int b200_melspec(const float* wave, const float* window, const float* fb, float* out, int32_t B, int32_t nw, int32_t n_fft,
@@ -711,11 +698,11 @@ extern "C" int b200_melspec(const float* wave, const float* window, const float*
     int log2n = 0;
     while ((1 << log2n) < n_fft) ++log2n;
     int2* bands = reinterpret_cast<int2*>(ws_bands);
-    B200_LAUNCH(mel_bands_kernel, (n_mels + 127) / 128, 128, 0, st, fb, n_fft / 2 + 1, n_mels, bands);
+    mel_bands_kernel<<<(n_mels + 127) / 128, 128, 0, st>>>(fb, n_fft / 2 + 1, n_mels, bands);
     if (int rc = check_launch("mel_bands_kernel")) return rc;
     const size_t smem = (size_t)n_fft * 8 + (size_t)(n_fft / 2) * 8 + (size_t)(n_fft / 2 + 1) * 4;
     static DeviceOnce once;
     B200_REQUIRE(set_max_smem_once(once, melspec_kernel, 64 * 1024) == cudaSuccess, "melspec: cudaFuncSetAttribute failed");
-    B200_LAUNCH(melspec_kernel, dim3(frames, B), 256, smem, st, wave, window, fb, bands, out, nw, n_fft, log2n, hop, n_mels, frames, wave_lens, out_bnd);
+    melspec_kernel<<<dim3(frames, B), 256, smem, st>>>(wave, window, fb, bands, out, nw, n_fft, log2n, hop, n_mels, frames, wave_lens, out_bnd);
     return check_launch("melspec_kernel");
 }

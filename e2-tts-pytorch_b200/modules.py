@@ -29,8 +29,6 @@ SOFTCLAMP = 50.0  # x-transformers logit_softclamp_value default (A.4)
 # B200_TWO_STREAM=0 serialises them on the current stream (developer A/B switch)
 import os as _os
 TWO_STREAM = _os.environ.get('B200_TWO_STREAM', '1') != '0'
-# depth connection of a sub-block fused into the next sub-block's width connection (ops.HcDepthWidth); B200_FUSE_HC=0: separate kernels
-FUSE_HC = _os.environ.get('B200_FUSE_HC', '1') != '0'
 _SIDE_STREAMS = {}
 
 
@@ -545,7 +543,7 @@ class Transformer(Module):
         # Hyper-connection plumbing of one stream: a sub-block returns its depth connection PENDING — (residual', branch_out, beta) — and
         # the next sub-block's width connection consumes it in one fused kernel (ops.HcDepthWidth); `close` materialises the streams
         # where something else reads them (cross-conditioning, skip path, final norm).
-        fuse = FUSE_HC and ops.hc_can_fuse(xs.shape[0], xs.shape[1])
+        fuse = ops.hc_can_fuse(xs.shape[0], xs.shape[1])
 
         def width(res, hcm, gain, mode):
             if isinstance(res, tuple):

@@ -15,8 +15,6 @@ from torch.autograd.function import once_differentiable
 from . import lib
 
 BF16, F32 = torch.bfloat16, torch.float32
-ATTN_FWD_ENTRY = 'b200_attn_fwd'   # tests may point these at the '*_legacy' (mma.sync) entry points to cross-check the kernels
-ATTN_BWD_ENTRY = 'b200_attn_bwd'
 
 
 def _stream():
@@ -265,64 +263,48 @@ class DwConv(Function):
 
 
 # ---------------------------------------------------------------------------------------------------- attention
-class QkvProj(Function):
-    """to_q/to_k/to_v (+ to_v_head_gate, to_value_residual_mix logits) as ONE GEMM, then rotary on q,k, value-residual
-    lerp on v and sigmoid head gate (A.3, A.4 steps 1-3/5; ctor e2_tts.py:641,689)."""
+def _maskbits_ws(B, Np, device):
+    return torch.empty(((Np + 127) // 128) * 4 * B, device=device, dtype=torch.int32)   # b200_attn_workspace_bytes(B, Np)
 
-    @staticmethod
-    def forward(ctx, xn, wq, wk, wv, wg, bg, wm, bm, v_first, wpack, cs, sn, B, Np, H):
-        T, Din = xn.shape
-        I = H * 64
-        ncat = 3 * I + (2 if wm is not None else 1) * H
-        ld = (ncat + 7) // 8 * 8
-        qkvg = gemm(xn, wpack, T, ncat, Din, ldd=ld)
-        q = torch.empty((B, H, Np, 64), device=xn.device, dtype=BF16)
-        k, v = torch.empty_like(q), torch.empty_like(q)
-        gate = torch.empty((T, H), device=xn.device, dtype=F32)
-        a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
-                          q=q, k=k, v=v, gate=gate, B=B, H=H, Np=Np, dim_head=64)
-        lib.call('b200_qkv_post_fwd', a, _stream())
-        ctx.save_for_backward(xn, qkvg, gate, v_first, wpack, cs, sn, bg, bm)
-        ctx.meta = (B, Np, H, ncat, ld, wm is not None)
-        return q, k, v, gate
 
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, dq, dk, dv, dgate):
-        xn, qkvg, gate, v_first, wpack, cs, sn, bg, bm = ctx.saved_tensors
-        B, Np, H, ncat, ld, has_mix = ctx.meta
-        T, Din = xn.shape
-        I = H * 64
-        dev = xn.device
-        if dgate is None:
-            dgate = torch.zeros_like(gate)
-        d_qkvg = torch.empty((T, ld), device=dev, dtype=BF16)
-        d_vfirst = torch.empty_like(v_first) if v_first is not None else None
-        a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
-                          gate=gate, dq=_c(dq), dk=_c(dk), dv=_c(dv), d_gate=_c(dgate), d_qkvg=d_qkvg, d_vfirst=d_vfirst,
-                          B=B, H=H, Np=Np, dim_head=64, dq_fp32=int(dq.dtype == F32))
-        lib.call('b200_qkv_post_bwd', a, _stream())
-        dx = gemm(d_qkvg, wpack, T, Din, ncat, lda=ld, ldb=Din, b_mn=True)
-        dW = grad_weight(d_qkvg, xn, T, ncat, Din, ldy=ld)
-        db = colsum(d_qkvg, T, ncat, ld)
-        return (dx, dW[:I], dW[I:2 * I], dW[2 * I:3 * I], dW[3 * I:3 * I + H], db[3 * I:3 * I + H],
-                dW[3 * I + H:3 * I + 2 * H] if has_mix else None, db[3 * I + H:3 * I + 2 * H] if has_mix else None,
-                d_vfirst, None, None, None, None, None, None)
+def _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits=None):
+    """b200_attn_fwd on q, k, v bf16 [B, H, Np, 64] -> og (gated, head-merged bf16 [B*Np, H*64]), o (bf16 [B, H, Np, 64]), lse (fp32
+    [B, H, Np]). `maskbits` is attn_maskbits(mask), shared by every layer of a step; without it the call builds its own."""
+    B, H, Np, dh = q.shape
+    o = torch.empty_like(q)
+    og = torch.empty((B * Np, H * dh), device=q.device, dtype=BF16)
+    lse = torch.empty((B, H, Np), device=q.device, dtype=F32)
+    a = lib.make_args('b200_attn_fwd_args', q=q, k=k, v=v, keymask=mask, gate=gate, o=o, og=og, lse=lse, B=B, H=H, Np=Np, dim_head=dh,
+                      scale=dh ** -0.5, softclamp=softclamp, dropout_p=dropout_p, seed=seed,
+                      ws_maskbits=maskbits if maskbits is not None else _maskbits_ws(B, Np, q.device), seed_dev=seed_dev,
+                      maskbits_ready=int(maskbits is not None))
+    lib.call('b200_attn_fwd', a, _stream())
+    return og, o, lse
+
+
+def _attn_core_bwd(d_og, q, k, v, o, lse, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits=None):
+    """b200_attn_bwd -> dq (fp32: accumulated across key tiles with atomics), dk, dv (bf16 [B, H, Np, 64]), d_gate (fp32 [B*Np, H])."""
+    B, H, Np, dh = q.shape
+    dq = torch.empty(q.shape, device=q.device, dtype=F32)
+    dk, dv, ws_dO = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+    ws_delta = torch.empty_like(lse)
+    d_gate = torch.empty_like(gate)
+    a = lib.make_args('b200_attn_bwd_args', q=q, k=k, v=v, o=o, d_og=_c(d_og), keymask=mask, gate=gate, lse=lse, ws_dO=ws_dO,
+                      ws_delta=ws_delta, d_gate=d_gate, dq=dq, dk=dk, dv=dv, B=B, H=H, Np=Np, dim_head=dh, scale=dh ** -0.5,
+                      softclamp=softclamp, dropout_p=dropout_p, seed=seed,
+                      ws_maskbits=maskbits if maskbits is not None else _maskbits_ws(B, Np, q.device), seed_dev=seed_dev,
+                      maskbits_ready=int(maskbits is not None))
+    lib.call('b200_attn_bwd', a, _stream())
+    return dq, dk, dv, d_gate
 
 
 class AttnCore(Function):
-    """Softclamped, key-masked, head-gated flash attention (A.4 steps 4-5). Returns the gated, head-merged output."""
+    """Softclamped, key-masked, head-gated flash attention (A.4 steps 4-5) on given q, k, v. Returns the gated, head-merged output.
+    The model runs the same kernels inside Attention; this node serves the attention-core tests and benchmarks."""
 
     @staticmethod
     def forward(ctx, q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev):
-        B, H, Np, dh = q.shape
-        o = torch.empty_like(q)
-        og = torch.empty((B * Np, H * dh), device=q.device, dtype=BF16)
-        lse = torch.empty((B, H, Np), device=q.device, dtype=F32)
-        ws = torch.empty(((Np + 127) // 128) * 4 * B, device=q.device, dtype=torch.int32)
-        a = lib.make_args('b200_attn_fwd_args', q=q, k=k, v=v, keymask=mask, gate=gate, o=o, og=og, lse=lse, B=B, H=H, Np=Np,
-                          dim_head=dh, scale=dh ** -0.5, softclamp=softclamp, dropout_p=dropout_p, seed=seed, ws_maskbits=ws, seed_dev=seed_dev)
-        lib.call(ATTN_FWD_ENTRY, a, _stream())
+        og, o, lse = _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev)
         ctx.save_for_backward(q, k, v, gate, mask, o, lse)
         ctx.meta = (dropout_p, seed, softclamp, seed_dev)
         return og
@@ -331,18 +313,7 @@ class AttnCore(Function):
     @once_differentiable
     def backward(ctx, d_og):
         q, k, v, gate, mask, o, lse = ctx.saved_tensors
-        dropout_p, seed, softclamp, seed_dev = ctx.meta
-        B, H, Np, dh = q.shape
-        legacy = ATTN_BWD_ENTRY.endswith('legacy')
-        dq = torch.empty(q.shape, device=q.device, dtype=BF16 if legacy else F32)   # the wgmma backward accumulates dq in fp32
-        dk, dv, ws_dO = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-        ws_delta = torch.empty_like(lse)
-        d_gate = torch.empty_like(gate)
-        ws = torch.empty(((Np + 127) // 128) * 4 * B, device=q.device, dtype=torch.int32)
-        a = lib.make_args('b200_attn_bwd_args', q=q, k=k, v=v, o=o, d_og=_c(d_og), keymask=mask, gate=gate, lse=lse, ws_dO=ws_dO,
-                          ws_delta=ws_delta, d_gate=d_gate, dq=dq, dk=dk, dv=dv, B=B, H=H, Np=Np, dim_head=dh, scale=dh ** -0.5,
-                          softclamp=softclamp, dropout_p=dropout_p, seed=seed, ws_maskbits=ws, seed_dev=seed_dev)
-        lib.call(ATTN_BWD_ENTRY, a, _stream())
+        dq, dk, dv, d_gate = _attn_core_bwd(d_og, q, k, v, o, lse, gate, mask, *ctx.meta)
         return dq, dk, dv, d_gate, None, None, None, None, None
 
 
@@ -363,18 +334,12 @@ class Attention(Function):
         ld = (ncat + 7) // 8 * 8
         qkvg = gemm(xn, wpack, T, ncat, Din, ldd=ld)
         q = torch.empty((B, H, Np, 64), device=dev, dtype=BF16)
-        k, v, o = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+        k, v = torch.empty_like(q), torch.empty_like(q)
         gate = torch.empty((T, H), device=dev, dtype=F32)
         a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
                           q=q, k=k, v=v, gate=gate, B=B, H=H, Np=Np, dim_head=64)
         lib.call('b200_qkv_post_fwd', a, _stream())
-        og = torch.empty((T, I), device=dev, dtype=BF16)
-        lse = torch.empty((B, H, Np), device=dev, dtype=F32)
-        ws = maskbits if maskbits is not None else torch.empty(((Np + 127) // 128) * 4 * B, device=dev, dtype=torch.int32)
-        a = lib.make_args('b200_attn_fwd_args', q=q, k=k, v=v, keymask=mask, gate=gate, o=o, og=og, lse=lse, B=B, H=H, Np=Np,
-                          dim_head=64, scale=0.125, softclamp=softclamp, dropout_p=dropout_p, seed=seed, ws_maskbits=ws, seed_dev=seed_dev,
-                          maskbits_ready=int(maskbits is not None))
-        lib.call(ATTN_FWD_ENTRY, a, _stream())
+        og, o, lse = _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits)
         ctx.maskbits = maskbits
         ctx.save_for_backward(xn, qkvg, gate, v_first, wpack, cs, sn, bg, bm, q, k, v, o, lse, mask)
         ctx.meta = (B, Np, H, ncat, ld, has_mix, dropout_p, seed, softclamp, seed_dev)
@@ -390,22 +355,12 @@ class Attention(Function):
         T, Din = xn.shape
         I = H * 64
         dev = xn.device
-        legacy = ATTN_BWD_ENTRY.endswith('legacy')
-        dq = torch.empty(q.shape, device=dev, dtype=BF16 if legacy else F32)
-        dk, dv, ws_dO = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
-        ws_delta = torch.empty_like(lse)
-        d_gate = torch.empty_like(gate)
-        ws = ctx.maskbits if ctx.maskbits is not None else torch.empty(((Np + 127) // 128) * 4 * B, device=dev, dtype=torch.int32)
-        a = lib.make_args('b200_attn_bwd_args', q=q, k=k, v=v, o=o, d_og=_c(d_og), keymask=mask, gate=gate, lse=lse, ws_dO=ws_dO,
-                          ws_delta=ws_delta, d_gate=d_gate, dq=dq, dk=dk, dv=dv, B=B, H=H, Np=Np, dim_head=64, scale=0.125,
-                          softclamp=softclamp, dropout_p=dropout_p, seed=seed, ws_maskbits=ws, seed_dev=seed_dev,
-                          maskbits_ready=int(ctx.maskbits is not None))
-        lib.call(ATTN_BWD_ENTRY, a, _stream())
+        dq, dk, dv, d_gate = _attn_core_bwd(d_og, q, k, v, o, lse, gate, mask, dropout_p, seed, softclamp, seed_dev, ctx.maskbits)
         d_qkvg = torch.empty((T, ld), device=dev, dtype=BF16)
         d_vfirst = torch.empty_like(v_first) if v_first is not None else None
         a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
                           gate=gate, dq=dq, dk=dk, dv=dv, dv_extra=_c(d_v_extra), d_gate=d_gate, d_qkvg=d_qkvg, d_vfirst=d_vfirst,
-                          B=B, H=H, Np=Np, dim_head=64, dq_fp32=int(dq.dtype == F32))
+                          B=B, H=H, Np=Np, dim_head=64, dq_fp32=1)
         lib.call('b200_qkv_post_bwd', a, _stream())
         dx = gemm(d_qkvg, wpack, T, Din, ncat, lda=ld, ldb=Din, b_mn=True)
         dW = grad_weight(d_qkvg, xn, T, ncat, Din, ldy=ld)
@@ -417,7 +372,7 @@ class Attention(Function):
 
 def attn_maskbits(mask_u8, B, Np, device):
     """Key-validity bitmask shared by every attention call of one forward/backward (all layers see the same key mask)."""
-    ws = torch.empty(((Np + 127) // 128) * 4 * B, device=device, dtype=torch.int32)
+    ws = _maskbits_ws(B, Np, device)
     lib.call('b200_attn_maskbits', mask_u8, ws, B, Np, _stream())
     return ws
 

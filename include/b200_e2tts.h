@@ -103,11 +103,11 @@ typedef struct {
 size_t b200_attn_workspace_bytes(int32_t B, int32_t Np);
 /* key-validity bitmask of `keymask` (u8 [B,Np], NULL = all valid) into ws_maskbits, in the layout the wgmma kernels read */
 int b200_attn_maskbits(const uint8_t* keymask, void* ws_maskbits, int32_t B, int32_t Np, b200_stream_t stream);
-int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream);        /* wgmma / TMA kernel */
-int b200_attn_fwd_legacy(const b200_attn_fwd_args* a, b200_stream_t stream); /* mma.sync bring-up kernel, kept for cross-checks */
+/* wgmma / TMA kernel; softclamp must be in (0, 64] (the softmax is exponentiated without a running maximum) */
+int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream);
 
 /* backward: d_og bf16 [B*Np, H*64] -> dk,dv bf16 [B,H,Np,64], dq FP32 [B,H,Np,64] (accumulated with atomics across key
- * tiles by the wgmma kernel; the legacy kernel writes bf16 dq), d_gate fp32 [B*Np,H] (grad wrt the sigmoid gate VALUE;
+ * tiles), d_gate fp32 [B*Np,H] (grad wrt the sigmoid gate VALUE;
  * may be NULL). ws_dO (bf16 [B,H,Np,64]), ws_delta (fp32 [B,H,Np]) and ws_maskbits are caller workspaces. */
 typedef struct {
     const void *q, *k, *v, *o, *d_og;
@@ -123,8 +123,7 @@ typedef struct {
     const uint64_t* seed_dev;   /* optional device addend of `seed` (must be the forward's) */
     int32_t maskbits_ready;     /* as in b200_attn_fwd_args */
 } b200_attn_bwd_args;
-int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream);         /* wgmma / TMA kernel, dq fp32 */
-int b200_attn_bwd_legacy(const b200_attn_bwd_args* a, b200_stream_t stream);  /* mma.sync bring-up kernels, dq bf16 */
+int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream);         /* wgmma / TMA kernel, dq fp32; softclamp as in fwd */
 
 /* ------------------------------------------------------------------------------------------------
  * Hyper-connections (A.5; e2_tts.py:607, 673-678, 709-713, 870-882, 900-939), S = 4 residual streams held

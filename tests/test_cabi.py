@@ -42,6 +42,15 @@ def test_argument_validation_without_gpu(pkg):
     a = pkg.lib.make_args('b200_hc_width_args', num_streams=3)
     with pytest.raises(RuntimeError):
         pkg.lib.call('b200_hc_width_fwd', a, None)
+    # the wgmma attention exponentiates without a running maximum: a softclamp above 64 is refused (placeholder pointers, never read)
+    ptrs = dict.fromkeys(('q', 'k', 'v', 'o', 'lse', 'ws_maskbits'), 256)
+    shape = dict(B=1, H=1, Np=64, dim_head=64, scale=0.125, softclamp=100.0)
+    a = pkg.lib.make_args('b200_attn_fwd_args', og=256, **ptrs, **shape)
+    with pytest.raises(RuntimeError, match='softclamp'):
+        pkg.lib.call('b200_attn_fwd', a, None)
+    a = pkg.lib.make_args('b200_attn_bwd_args', d_og=256, ws_dO=256, ws_delta=256, dq=256, dk=256, dv=256, **ptrs, **shape)
+    with pytest.raises(RuntimeError, match='softclamp'):
+        pkg.lib.call('b200_attn_bwd', a, None)
 
 
 def test_state_dict_is_reference_compatible(pkg):

@@ -178,21 +178,49 @@ def test_hyper_depth_width_fused(pkg, D):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# (d) wgmma attention core at the benchmark's sequence length against an fp32 softmax written here (x-transformers Attend as the
-#     reference configures it, SURVEY A.4 steps 4-5: scale, tanh soft clamp 50, key-padding mask, fp32 softmax, per-head gate)
-def _attn_core_ref(q, k, v, gate, mask, clamp=50.0):
+# (d) wgmma attention core against an fp32 softmax written here (x-transformers Attend as the reference configures it, SURVEY A.4
+#     steps 4-5: scale, tanh soft clamp 50, key-padding mask, fp32 softmax, dropout, per-head gate), at the benchmark's sequence length
+#     and at short, unmasked and dropout cases
+def _mul32(x, c):
+    """(x * c) mod 2^32 for int64 tensors x < 2^32 and a 32-bit constant c, without overflowing int64."""
+    return (x * (c & 0xFFFF) + ((x * (c >> 16)) & 0xFFFF) * 65536) & 0xFFFFFFFF
+
+
+def _dropout_keep(seed, B, H, Np, p):
+    """The kernels' attention-dropout mask (ptx.cuh: seed_mix32, drop_words) for element ((b*H + h)*Np + i)*stride + j, as bool
+    [B, H, Np, Np]: keep iff the 32-bit word of the element >= thresh16 << 16, thresh16 = int(p * 65536)."""
+    stride = (Np + 1) & ~1
+    seedmix = (seed & 0xFFFFFFFF) ^ (((seed >> 32) * 0x85EBCA77) & 0xFFFFFFFF)
+    row = torch.arange(B * H * Np, dtype=torch.int64).view(B, H, Np, 1)
+    idx = row * stride + torch.arange(Np, dtype=torch.int64)
+    x = (_mul32((idx >> 1) & 0xFFFFFFFF, 0x9E3779B1) + seedmix) & 0xFFFFFFFF
+    x = x ^ (x >> 15)
+    word = torch.where((idx & 1) == 1, _mul32(x, 0xC2B2AE35), _mul32(x, 0x85EBCA6B))
+    return word >= (int(p * 65536) << 16)
+
+
+def _attn_core_ref(q, k, v, gate, mask, clamp=50.0, dropout=0.0, seed=0):
+    """-> og [B*Np, H*dh] (gated, head-merged), o [B, H, Np, dh], lse [B, H, Np] (log-sum-exp of the clamped, masked logits). With
+    dropout the kept probabilities are scaled by 65536 / (65536 - thresh16), the kernels' exact 1 / (1 - p)."""
     B, H, Np, dh = q.shape
     sim = torch.einsum('bhid,bhjd->bhij', q, k) * dh ** -0.5
     sim = torch.tanh(sim / clamp) * clamp
     if mask is not None:
         sim = sim.masked_fill(~mask[:, None, None, :], -torch.finfo(sim.dtype).max)
-    out = torch.einsum('bhij,bhjd->bhid', torch.softmax(sim, dim=-1), v)
-    out = out * gate.view(B, Np, H).permute(0, 2, 1)[..., None]
-    return out.permute(0, 2, 1, 3).reshape(B * Np, H * dh)
+    attn = torch.softmax(sim, dim=-1)
+    if dropout > 0:
+        thresh16 = int(dropout * 65536)
+        attn = attn * _dropout_keep(seed, B, H, Np, dropout) * (65536 / (65536 - thresh16))
+    o = torch.einsum('bhij,bhjd->bhid', attn, v)
+    og = o * gate.view(B, Np, H).permute(0, 2, 1)[..., None]
+    return og.permute(0, 2, 1, 3).reshape(B * Np, H * dh), o, torch.logsumexp(sim, dim=-1)
 
 
-@pytest.mark.parametrize('Np,H,big_logits', [(1056, 8, False), (1056, 8, True), (2080, 16, False), (331, 3, True)])
-def test_attention_core_vs_fp32_softmax(pkg, Np, H, big_logits):
+@pytest.mark.parametrize('Np,H,big_logits,masked,dropout', [
+    (1056, 8, False, True, 0.0), (1056, 8, True, True, 0.0), (2080, 16, False, True, 0.0), (331, 3, True, True, 0.0),
+    (128, 3, False, False, 0.0), (300, 3, False, True, 0.0), (1056, 3, False, True, 0.1)],
+    ids=['1056-8-False', '1056-8-True', '2080-16-False', '331-3-True', '128-3-unmasked', '300-3-masked', '1056-3-masked-dropout'])
+def test_attention_core_vs_fp32_softmax(pkg, Np, H, big_logits, masked, dropout):
     torch.manual_seed(30 + Np + H)
     ops = pkg.ops
     B = 2 if Np < 2000 else 1
@@ -200,16 +228,24 @@ def test_attention_core_vs_fp32_softmax(pkg, Np, H, big_logits):
     q, k, v = (bf(torch.randn(B, H, Np, 64, device=dev()) * (s if i < 2 else 1.0)) for i in range(3))
     gate = torch.rand(B * Np, H, device=dev())
     m = torch.ones(B, Np, dtype=torch.bool, device=dev())
-    m[0, Np // 3: Np // 3 + 40] = False
-    m[B - 1, Np - 29:] = False
+    if masked:
+        m[0, Np // 3: Np // 3 + 40] = False
+        m[B - 1, Np - 29:] = False
+    mask = m.to(torch.uint8).contiguous() if masked else None
+    seed = 4242
+    og, o, lse = ops._attn_core_fwd(q, k, v, gate, mask, dropout, seed, 50.0, None)
     leaves = [t.clone().requires_grad_() for t in (q, k, v)] + [gate.clone().requires_grad_()]
-    og = ops.AttnCore.apply(*leaves, m.to(torch.uint8).contiguous(), 0.0, 0, 50.0, None)
+    og_g = ops.AttnCore.apply(*leaves, mask, dropout, seed, 50.0, None)
     w = bf(torch.randn(B * Np, H * 64, device=dev()))
-    grads = torch.autograd.grad(og, leaves, w)
+    grads = torch.autograd.grad(og_g, leaves, w)
     rl = [t.detach().float().cpu().requires_grad_() for t in leaves]
-    ref = _attn_core_ref(*rl, m.cpu())
-    rgrads = torch.autograd.grad(ref, rl, w.float().cpu())
-    check('attention out', og, ref, 1e-2)
+    ref_og, ref_o, ref_lse = _attn_core_ref(*rl, m.cpu(), dropout=dropout, seed=seed)
+    rgrads = torch.autograd.grad(ref_og, rl, w.float().cpu())
+    check('attention out', og, ref_og, 1e-2)
+    assert torch.equal(og_g, og)
+    check('attention o', o, ref_o, 1e-2)
+    lse_err = float((lse.cpu() - ref_lse.detach()).abs().max())
+    assert lse_err < 2e-2, f'attention lse: max abs error {lse_err:.4g}'
     for nm, a, b in zip(['dq', 'dk', 'dv', 'dgate'], grads, rgrads):
         check(f'attention {nm}', a, b, 2e-2)
 
