@@ -721,7 +721,7 @@ extern "C" int b200_stem_prepare(const b200_stem_args* a, b200_stream_t stream) 
 }
 
 static int fill_asm(AsmP& p, const b200_assemble_args* a) {
-    B200_REQUIRE(a && (a->h || (a->ids && a->emb)) && a->registers, "assemble: null pointer");
+    B200_REQUIRE(a && (a->h || (a->ids && a->emb)) && (a->registers || a->R == 0), "assemble: null pointer");   // R = 0: no register rows to read
     B200_REQUIRE(a->D % 8 == 0 && a->S >= 1 && a->B > 0 && a->N > 0 && a->R >= 0, "assemble: unsupported shape");
     p.h = (const __nv_bfloat16*)a->h; p.ids = a->ids; p.emb = a->emb; p.abs_pos = a->abs_pos; p.registers = a->registers;
     p.B = a->B; p.N = a->N; p.R = a->R; p.D = a->D; p.S = a->S;

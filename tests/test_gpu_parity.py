@@ -113,9 +113,10 @@ def test_hyper_width_depth(pkg):
             check(f'{nm} m{mode}', a.reshape(-1), b.reshape(-1), 3e-2)
 
 
-@pytest.mark.parametrize('D,ks,Np', [(128, 31, 100), (64, 7, 100), (512, 31, 333), (264, 31, 70)])
+@pytest.mark.parametrize('D,ks,Np', [(128, 31, 100), (64, 7, 100), (512, 31, 333), (264, 31, 70), (128, 31, 40)])
 def test_dwconv(pkg, D, ks, Np):
-    """fwd + (dx, dw, db) vs the oracle; Np = 333 spans two blocks of four 64-token tiles, D = 264 leaves a partial channel tile."""
+    """fwd + (dx, dw, db) vs the oracle; Np = 333 spans two blocks of four 64-token tiles, D = 264 leaves a partial channel tile,
+    Np = 40 is shorter than one tile, so the 15-row halo runs past both ends of the sequence."""
     torch.manual_seed(2)
     ops = pkg.ops
     B = 2

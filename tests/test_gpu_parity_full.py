@@ -218,8 +218,9 @@ def _attn_core_ref(q, k, v, gate, mask, clamp=50.0, dropout=0.0, seed=0):
 
 @pytest.mark.parametrize('Np,H,big_logits,masked,dropout', [
     (1056, 8, False, True, 0.0), (1056, 8, True, True, 0.0), (2080, 16, False, True, 0.0), (331, 3, True, True, 0.0),
-    (128, 3, False, False, 0.0), (300, 3, False, True, 0.0), (1056, 3, False, True, 0.1)],
-    ids=['1056-8-False', '1056-8-True', '2080-16-False', '331-3-True', '128-3-unmasked', '300-3-masked', '1056-3-masked-dropout'])
+    (128, 3, False, False, 0.0), (300, 3, False, True, 0.0), (1056, 3, False, True, 0.1), (40, 3, False, True, 0.0), (65, 2, False, False, 0.0)],
+    ids=['1056-8-False', '1056-8-True', '2080-16-False', '331-3-True', '128-3-unmasked', '300-3-masked', '1056-3-masked-dropout', '40-3-masked',
+         '65-2-unmasked'])
 def test_attention_core_vs_fp32_softmax(pkg, Np, H, big_logits, masked, dropout):
     torch.manual_seed(30 + Np + H)
     ops = pkg.ops
