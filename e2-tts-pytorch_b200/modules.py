@@ -5,6 +5,8 @@ the reference's layout; the arithmetic lives in the CUDA library.
 """
 from __future__ import annotations
 
+import contextlib
+import copy
 import ctypes
 import math
 import random as pyrandom
@@ -242,8 +244,9 @@ class InterpolatedCharacterEmbed(Module):  # e2_tts.py:414-482 (E2TTS(interpolat
         ids_c = torch.gather(text.clamp(min=0), 1, order).to(torch.int32).contiguous()
         return ids_c, valid.sum(dim=1).to(torch.int32)
 
-    def embed_bf16(self, text, max_seq_len, mask=None):
-        """text (b, nt) int64 with -1 padding, mask (b, n) bool | None -> bf16 [b * n, dim] (rows of masked frames are zero)."""
+    def embed_bf16(self, text, max_seq_len, mask, w2_packed):
+        """text (b, nt) int64 with -1 padding, mask (b, n) bool | None, w2_packed: the bf16 copy of abs_pos_mlp[3].weight
+        -> bf16 [b * n, dim] (rows of masked frames are zero)."""
         B = text.shape[0]
         ids_c, text_len = self.compact(text)
         if exists(mask):
@@ -253,19 +256,29 @@ class InterpolatedCharacterEmbed(Module):  # e2_tts.py:414-482 (E2TTS(interpolat
             audio_len = torch.full((B,), max_seq_len, device=text.device, dtype=torch.int32)
             mask_u8 = None
         lin1, lin2 = self.abs_pos_mlp[1], self.abs_pos_mlp[3]
-        return ops.InterpText.apply(ids_c, text_len, audio_len, mask_u8, self.embed.weight, lin1.weight, lin1.bias, lin2.weight, lin2.bias,
-                                    B, max_seq_len)
+        return ops.InterpText.apply(ids_c, text_len, audio_len, mask_u8, self.embed.weight, lin1.weight, lin1.bias, lin2.weight, w2_packed,
+                                    lin2.bias, B, max_seq_len)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
 # weight packing: one kernel launch per forward refreshes every bf16 GEMM operand from the fp32 parameters
 
 
-class _PackTable:
-    def __init__(self):
+class WeightPack:
+    """The GEMM operands of one model: bf16 (or fp32) copies of its parameters in the layouts the kernels read, all written by
+    ONE b200_pack_weights launch. The module whose forward the user calls (E2TTS, DurationPredictor, or a Transformer called
+    directly) owns one pack and runs it at the start of every forward, so the operands always match the current parameters."""
+
+    def __init__(self, device):
+        self.device = device
         self.entries = []  # (param, dst, rows, cols, ld_dst, row_off, col_off, mode, out_fp32)
         self.dev_table = None
         self.ptrs = None
+        self.frozen = False
+
+    def buffer(self, *shape, dtype=BF16):
+        """A zero-filled destination on the pack's device (padding that no entry writes stays 0)."""
+        return torch.zeros(shape, device=self.device, dtype=dtype)
 
     def add(self, param, dst, *, ld=None, row_off=0, col_off=0, mode=0):
         p2 = param if param.dim() != 3 else param.reshape(param.shape[0], -1)
@@ -275,17 +288,67 @@ class _PackTable:
         self.entries.append((param, dst, rows, cols, ld, row_off, col_off, mode, int(dst.dtype == F32)))
 
     def run(self):
+        if self.frozen:
+            return
         ptrs = tuple(e[0].data_ptr() for e in self.entries)
-        if self.dev_table is None or ptrs != self.ptrs:
+        if ptrs != self.ptrs:   # rebuilt only when a parameter gets new storage: a CUDA-graph capture never copies host to device
             Desc = lib.STRUCTS['b200_pack_desc']
             arr = (Desc * len(self.entries))()
             for i, (p, dst, rows, cols, ld, ro, co, mode, f32) in enumerate(self.entries):
                 arr[i].src, arr[i].dst = p.data_ptr(), dst.data_ptr()
                 arr[i].rows, arr[i].cols, arr[i].ld_dst, arr[i].row_off, arr[i].col_off, arr[i].mode, arr[i].out_fp32 = rows, cols, ld, ro, co, mode, f32
             raw = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8)
-            self.dev_table = raw.to(self.entries[0][1].device)
+            self.dev_table = raw.to(self.device)
             self.ptrs = ptrs
         ops.pack_weights(self.dev_table, len(self.entries))
+
+    @contextlib.contextmanager
+    def freeze(self):
+        """Pack now, then skip every run() inside the block: for a block in which the weights cannot change (sample()'s ODE solve)."""
+        self.run()
+        was, self.frozen = self.frozen, True
+        try:
+            yield
+        finally:
+            self.frozen = was
+
+
+class _PackOwner(Module):
+    """A module that can own a WeightPack. `_add_weights(pack)` lays out its operands and returns their handles. The pack and the
+    rotary tables are derived device state: `_apply` (.to(), .cuda(), .float(), ...) drops them, and a deep copy (EMA(model))
+    starts without them and without any attribute listed in `_NOT_COPIED`, so the copy never holds buffers that the original
+    packs into."""
+    _NOT_COPIED = ('_derived',)
+
+    def __init__(self):
+        super().__init__()
+        self._derived = {}
+
+    def _apply(self, fn, *a, **k):
+        out = super()._apply(fn, *a, **k)
+        self._derived = {}
+        return out
+
+    def __deepcopy__(self, memo):
+        new = self.__class__.__new__(self.__class__)
+        memo[id(self)] = new
+        for k, v in self.__dict__.items():
+            new.__dict__[k] = None if k in self._NOT_COPIED else copy.deepcopy(v, memo)
+        new._derived = {}
+        return new
+
+    def _pack(self):
+        """-> (this module's WeightPack, the handles `_add_weights` returned), built on first use."""
+        if 'pack' not in self._derived:
+            pack = WeightPack(next(self.parameters()).device)
+            self._derived['pack'] = pack, self._add_weights(pack)
+        return self._derived['pack']
+
+    def _packed_weights(self):
+        """Refresh the pack from the current parameters (one launch, none while frozen) and return its handles."""
+        pack, handles = self._pack()
+        pack.run()
+        return handles
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -304,9 +367,10 @@ class LinearFourierEmbed(Module):
         self.split_dims = (dim_fourier, dim_rest)
 
 
-class Transformer(Module):
+class Transformer(_PackOwner):
     """Multistream flow-matching backbone — constructor and forward signature of the reference's Transformer
     (e2_tts.py:518-952). Non-default research switches raise (no kernels, no fallback)."""
+    _NOT_COPIED = ('_derived', '_seed_dev')   # the copy gets no GraphedTrainStep seed word of its own
 
     def __init__(
         self, *, dim, dim_text=None, depth=8, heads=8, dim_head=64, ff_mult=4, text_depth=None, text_heads=None, text_dim_head=None,
@@ -393,40 +457,17 @@ class Transformer(Module):
         self.hyper_conns = ModuleList(hyper_conns)
         self.final_norm = RMSNorm(dim)
 
-        self._pack = None
-        self._packed = None
-        self._rot = {}
         # optional int64 device word added to every dropout seed when the kernels RUN (include/b200_e2tts.h "dropout seeds"):
         # set by GraphedTrainStep, whose captured graph would otherwise replay the same dropout masks on every step
         self._seed_dev = None
-        self._frozen = False   # True inside E2TTS.sample(): the bf16 operands were packed once for the whole ODE solve (weights cannot change)
 
     # ------------------------------------------------------------------ packed operands
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self._pack, self._packed, self._rot = None, None, {}
-        return out
-
-    def __deepcopy__(self, memo):  # EMA(model) deep-copies the module (trainer.py:170-174): caches are per instance
-        pack, packed, rot, seed_dev = self._pack, self._packed, self._rot, self._seed_dev
-        self._pack, self._packed, self._rot, self._seed_dev, self._frozen = None, None, {}, None, False
-        try:
-            cls = self.__class__
-            new = cls.__new__(cls)
-            memo[id(self)] = new
-            import copy
-            for k, v in self.__dict__.items():
-                new.__dict__[k] = copy.deepcopy(v, memo)
-        finally:
-            self._pack, self._packed, self._rot, self._seed_dev = pack, packed, rot, seed_dev
-        return new
-
-    def _build_pack(self):
-        dev = self.registers.device
+    def _add_weights(self, pack):
+        """Add every per-layer GEMM operand and the stacked to_gamma weights to `pack`; -> dict(layers=[per-layer handles], cond=...)."""
         d, dt, H = self.dim, self.dim_text, self.heads
         I = H * 64
-        tab, cond_tab, packed = _PackTable(), _PackTable(), []
-        e = lambda *s: torch.zeros(s, device=dev, dtype=BF16)
+        packed = []
+        e = pack.buffer
         cond_rows = []
         for i, (speech, text) in enumerate(self.layers):
             L = {}
@@ -438,32 +479,32 @@ class Transformer(Module):
                 has_mix = attn.to_value_residual_mix is not None
                 qkv = e(3 * I + (2 if has_mix else 1) * H, din)
                 for j, lin in enumerate((attn.to_q, attn.to_k, attn.to_v)):
-                    tab.add(lin.weight, qkv, row_off=j * I)
-                tab.add(attn.to_v_head_gate.weight, qkv, row_off=3 * I)
+                    pack.add(lin.weight, qkv, row_off=j * I)
+                pack.add(attn.to_v_head_gate.weight, qkv, row_off=3 * I)
                 if has_mix:
-                    tab.add(attn.to_value_residual_mix[0].weight, qkv, row_off=3 * I + H)
+                    pack.add(attn.to_value_residual_mix[0].weight, qkv, row_off=3 * I + H)
                 out_w = e(din, I)
-                tab.add(attn.to_out.weight, out_w)
+                pack.add(attn.to_out.weight, out_w)
                 inner = ff.ff[2].weight.shape[1]
-                w1, b1 = e(2 * inner, din), torch.zeros(2 * inner, device=dev, dtype=F32)
-                tab.add(ff.ff[0].proj.weight, w1, mode=1)
-                tab.add(ff.ff[0].proj.bias, b1, mode=1)
+                w1, b1 = e(2 * inner, din), e(2 * inner, dtype=F32)
+                pack.add(ff.ff[0].proj.weight, w1, mode=1)
+                pack.add(ff.ff[0].proj.bias, b1, mode=1)
                 w2 = e(din, inner)
-                tab.add(ff.ff[2].weight, w2)
+                pack.add(ff.ff[2].weight, w2)
                 L[pre] = dict(qkv=qkv, out=out_w, w1=w1, b1=b1, w2=w2)
             if isinstance(speech[4], LinearFourierEmbed):
                 lfe = e(*speech[4].linear.weight.shape)
-                tab.add(speech[4].linear.weight, lfe)
+                pack.add(speech[4].linear.weight, lfe)
                 L['a']['lfe'] = lfe
             if speech[0] is not None:
                 L['skip'] = e(d, 2 * d)
-                tab.add(speech[0].weight, L['skip'])
+                pack.add(speech[0].weight, L['skip'])
             if text is not None:
                 cc = text[5]
                 stack = e(d + (dt if cc.cond_audio_to_text else 0), d + dt)
-                tab.add(cc.text_to_audio.weight, stack)
+                pack.add(cc.text_to_audio.weight, stack)
                 if cc.cond_audio_to_text:
-                    tab.add(cc.audio_to_text.weight, stack, row_off=d)
+                    pack.add(cc.audio_to_text.weight, stack, row_off=d)
                 L['cross'] = stack
             if self.cond_on_time:
                 cond_rows += [speech[2].to_gamma, speech[5].to_gamma, speech[6].to_gamma, speech[8].to_gamma]
@@ -471,63 +512,39 @@ class Transformer(Module):
         cond = None
         if self.cond_on_time:
             n = len(cond_rows) * d
-            W_all = torch.zeros((n, d), device=dev, dtype=F32)
-            b_all = torch.zeros(n, device=dev, dtype=F32)
+            W_all, b_all = e(n, d, dtype=F32), e(n, dtype=F32)
             for j, lin in enumerate(cond_rows):
-                cond_tab.add(lin.weight, W_all, row_off=j * d)
+                pack.add(lin.weight, W_all, row_off=j * d)
                 if lin.bias is not None:
-                    cond_tab.add(lin.bias, b_all, row_off=j * d)
+                    pack.add(lin.bias, b_all, row_off=j * d)
             cond = dict(W=W_all, b=b_all, lins=cond_rows)
-        self._pack, self._packed = (tab, cond_tab), dict(layers=packed, cond=cond)
-
-    def refresh_packed(self):
-        """Re-pack the bf16 GEMM operands from the current fp32 parameters (one launch)."""
-        if self._frozen and self._pack is not None:
-            return
-        if self._pack is None:
-            self._build_pack()
-        self._pack[0].run()
-
-    def freeze_packed(self, on):
-        """sample() runs 124 forwards over frozen weights (e2_tts.py:1332 @torch.no_grad, :1351 eval): pack the tensor-core operands and the
-        batched to_gamma matrix ONCE instead of once per forward (SURVEY §7.8)."""
-        self._frozen = False
-        if on:
-            self.refresh_packed()
-            if self.cond_on_time:
-                self._pack[1].run()
-            self._frozen = True
+        return dict(layers=packed, cond=cond)
 
     def _rotary(self, Np, dev):
-        if Np not in self._rot:
-            self._rot[Np] = ops.rotary_table(Np, dev)
-        return self._rot[Np]
+        rot = self._derived.setdefault('rot', {})
+        if Np not in rot:
+            rot[Np] = ops.rotary_table(Np, dev)
+        return rot[Np]
 
     # ------------------------------------------------------------------ conditioning vectors
-    def _cond_gains(self, times, batch):
-        """time_cond_mlp (:621-625, 778-789) and every per-layer to_gamma projection in ONE batched launch.
-        Returns a list [4 * depth] of contiguous fp32 [B, d]: (1 + gamma) for the adaptive norms, sigmoid gates for AdaLNZero."""
+    def _cond_gains(self, times, batch, c):
+        """time_cond_mlp (:621-625, 778-789) and every per-layer to_gamma projection in ONE batched launch; `c` is the packed
+        to_gamma stack. Returns a list [4 * depth] of contiguous fp32 [B, d]: (1 + gamma) for the adaptive norms, sigmoid gates for AdaLNZero."""
         if times.ndim == 0:
             times = times.expand(batch)
         times = times.to(F32).contiguous()
         four = ops.fourier_embed(times, self.time_cond_mlp[0].weights)
         lin = self.time_cond_mlp[1]
         cond = ops.SmallLinear.apply(four, lin.weight, lin.bias, 1, self.dim, False)
-        c = self._packed['cond']
-        tab = self._pack[1]
         weights = [l.weight for l in c['lins']]
         biases = [l.bias for l in c['lins'] if l.bias is not None]  # AdaLNZero gates sit on the odd d-wide segments
-        if self._frozen:
-            W, b_full = c['W'], c['b']
-        else:
-            W, b_full = ops.CondPack.apply(tab.run, c['W'], c['b'], self.dim, len(weights), *weights, *biases)
+        W, b_full = ops.CondPack.apply(c['W'], c['b'], self.dim, len(weights), *weights, *biases)
         gains = ops.SmallLinear.apply(cond, W, b_full, 5, self.dim, True)
         return list(gains.unbind(0))
 
     # ------------------------------------------------------------------ the block stack
-    def _run_layers(self, xs, ts, gains, mask_u8, B, Np, seed):
-        """xs bf16 [T,S,d], ts bf16 [T,S,dt] | None -> final residual streams. Layer loop of e2_tts.py:825-939."""
-        P = self._packed['layers']
+    def _run_layers(self, P, xs, ts, gains, mask_u8, B, Np, seed):
+        """P: the per-layer packed operands; xs bf16 [T,S,d], ts bf16 [T,S,dt] | None -> final residual streams. Layer loop of e2_tts.py:825-939."""
         H = self.heads
         cs, sn = self._rotary(Np, xs.device)
         p_drop = self.dropout if self.training else 0.0
@@ -651,14 +668,14 @@ class Transformer(Module):
         B, N, d = x.shape
         if torch.is_grad_enabled():
             ops.zero_pool.begin(x.device)
+        w = self._packed_weights()
         h = ops.CastRows.apply(x.reshape(B * N, d))
         te = ops.CastRows.apply(text_embed.reshape(B * N, -1)) if exists(text_embed) else None
-        y = self._forward_from_h(h, B, N, times, mask, te_bf16=te)
+        y = self._forward_from_h(w, h, B, N, times, mask, te_bf16=te)
         return y.view(B, N, d).to(x.dtype)
 
-    def _forward_from_h(self, h, B, N, times, mask, text_ids=None, text_embed_module=None, te_bf16=None):
-        """h bf16 [B*N, d] (already projected) -> final-normed bf16 [B*N, d]."""
-        self.refresh_packed()
+    def _forward_from_h(self, w, h, B, N, times, mask, text_ids=None, text_embed_module=None, te_bf16=None):
+        """w: the handles of `_add_weights`, already packed; h bf16 [B*N, d] (already projected) -> final-normed bf16 [B*N, d]."""
         S, R = self.num_streams, self.num_registers
         Np, mask_u8 = self._prepare(B, N, mask)
         abs_w = self.abs_pos_emb.weight if exists(self.abs_pos_emb) else None
@@ -668,9 +685,9 @@ class Transformer(Module):
             ts = ops.TextStem.apply(text_ids, text_embed_module.embed.weight, self.text_registers, B, N, S)
         elif exists(te_bf16):
             ts = ops.Assemble.apply(te_bf16, None, self.text_registers, B, N, S)
-        gains = self._cond_gains(times, B) if self.cond_on_time else None
+        gains = self._cond_gains(times, B, w['cond']) if self.cond_on_time else None
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if (self.training and self.dropout > 0) else 0
-        xs = self._run_layers(xs, ts, gains, mask_u8, B, Np, seed)
+        xs = self._run_layers(w['layers'], xs, ts, gains, mask_u8, B, Np, seed)
         return ops.FinalNorm.apply(xs, self.final_norm.g, B, N, R)
 
 
@@ -777,7 +794,7 @@ def _resolve_tokenizer(tokenizer, text_num_embeds):
     raise ValueError(f'unknown tokenizer string {tokenizer}')
 
 
-class DurationPredictor(Module):
+class DurationPredictor(_PackOwner):
     """Reference surface: e2_tts.py:956-1113."""
 
     def __init__(self, transformer: dict | Transformer, num_channels=None, mel_spec_kwargs: dict = dict(), char_embed_kwargs: dict = dict(),
@@ -802,12 +819,11 @@ class DurationPredictor(Module):
         self.tokenizer, text_num_embeds = _resolve_tokenizer(tokenizer, text_num_embeds)
         self.embed_text = CharacterEmbed(transformer.dim_text, num_embeds=text_num_embeds, **char_embed_kwargs)
         self.hl_gauss_layer = _HLGaussRegression(self.dim)
-        self._wpack = None
 
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self._wpack = None
-        return out
+    def _add_weights(self, pack):
+        w = dict(tr=self.transformer._add_weights(pack), proj_in=pack.buffer(self.dim, (self.num_channels + 7) // 8 * 8))
+        pack.add(self.proj_in.weight, w['proj_in'])
+        return w
 
     @_on_module_device
     def forward(self, x, *, text=None, lens=None, return_loss=True):
@@ -818,15 +834,9 @@ class DurationPredictor(Module):
         dev = x.device
         if torch.is_grad_enabled() and return_loss:
             ops.zero_pool.begin(dev)
-        Cp = (C + 7) // 8 * 8
-        if self._wpack is None or self._wpack[0].device != dev:
-            w = torch.zeros((self.dim, Cp), device=dev, dtype=BF16)
-            tab = _PackTable()
-            tab.add(self.proj_in.weight, w)
-            self._wpack = (w, tab)
-        self._wpack[1].run()
-        A = ops.cast_rows(x.reshape(B * N, C), B * N, C, Cp)
-        h = ops.StemLinear.apply(A, self.proj_in.weight, self.proj_in.bias, None, None, self._wpack[0])
+        w = self._packed_weights()
+        A = ops.cast_rows(x.reshape(B * N, C), B * N, C, w['proj_in'].shape[1])
+        h = ops.StemLinear.apply(A, self.proj_in.weight, self.proj_in.bias, None, None, w['proj_in'])
         ids = None
         if exists(text):
             if isinstance(text, list):
@@ -841,7 +851,7 @@ class DurationPredictor(Module):
             rand_index = (rand_frac_index * lens).long()
             mask = mask & (torch.arange(N, device=dev)[None] < rand_index[:, None])
         tr = self.transformer
-        y = tr._forward_from_h(h, B, N, None, mask, text_ids=ids, text_embed_module=self.embed_text)
+        y = tr._forward_from_h(w['tr'], h, B, N, None, mask, text_ids=ids, text_embed_module=self.embed_text)
         pooled = ops.MaskedMean.apply(y, mask.to(torch.uint8).contiguous(), B, N)
         lin = self.hl_gauss_layer.to_pred[0]
         pred = ops.SmallLinear.apply(pooled, lin.weight, lin.bias, 4, 1, False).squeeze(-1)
@@ -877,7 +887,7 @@ class inject_randomness:
         _rng.values = None
 
 
-class E2TTS(Module):
+class E2TTS(_PackOwner):
     """Reference surface: e2_tts.py:1115-1595 (constructor, forward, sample, transformer_with_pred_head,
     cfg_transformer_with_pred_head, device)."""
 
@@ -926,60 +936,49 @@ class E2TTS(Module):
         # Vocos is a separate pretrained network fetched from the HF hub (e2_tts.py:1244): out of scope (SURVEY §2 row 10).
         self.vocos = None
         self._use_vocos_requested = use_vocos
-        self._wpack = None
 
     @property
     def device(self):
         return next(self.parameters()).device
 
-    def _apply(self, fn, *a, **k):
-        out = super()._apply(fn, *a, **k)
-        self._wpack = None
-        return out
+    def _add_weights(self, pack):
+        C, d = self.num_channels, self.dim
+        Cp = (C + 63) // 64 * 64
+        w = dict(tr=self.transformer._add_weights(pack), Cp=Cp, stem=pack.buffer(d, 2 * Cp), pred=pack.buffer(C, d))
+        pack.add(self.proj_in.weight, w['stem'])          # concat_cond: all 2C columns, matching stem_prepare's cat(cond, x) layout
+        if not self.concat_cond:
+            pack.add(self.cond_proj_in.weight, w['stem'], col_off=Cp)
+        pack.add(self.to_pred.weight, w['pred'])
+        if isinstance(self.embed_text, InterpolatedCharacterEmbed):
+            w2 = self.embed_text.abs_pos_mlp[3].weight
+            w['interp'] = pack.buffer(*w2.shape)
+            pack.add(w2, w['interp'])
+        return w
 
-    def _packed(self):
-        dev = self.device
-        if self.transformer._frozen and self._wpack is not None and self._wpack['stem'].device == dev:
-            return self._wpack
-        if self._wpack is None or self._wpack['stem'].device != dev:
-            C, d = self.num_channels, self.dim
-            Cp = (C + 63) // 64 * 64
-            stem = torch.zeros((d, 2 * Cp), device=dev, dtype=BF16)
-            pred = torch.zeros((C, d), device=dev, dtype=BF16)
-            tab = _PackTable()
-            tab.add(self.proj_in.weight, stem)          # concat_cond: all 2C columns, matching stem_prepare's cat(cond, x) layout
-            if not self.concat_cond:
-                tab.add(self.cond_proj_in.weight, stem, col_off=Cp)
-            tab.add(self.to_pred.weight, pred)
-            self._wpack = dict(stem=stem, pred=pred, tab=tab, Cp=Cp)
-        self._wpack['tab'].run()
-        return self._wpack
-
-    def _embed(self, A, B, N, times, mask, text, drop_text_cond, pk):
+    def _embed(self, w, A, B, N, times, mask, text, drop_text_cond):
         if self.concat_cond:
-            h = ops.StemLinear.apply(A, self.proj_in.weight, self.proj_in.bias, None, None, pk['stem'])
+            h = ops.StemLinear.apply(A, self.proj_in.weight, self.proj_in.bias, None, None, w['stem'])
         else:
-            h = ops.StemLinear.apply(A, self.proj_in.weight, self.proj_in.bias, self.cond_proj_in.weight, self.cond_proj_in.bias, pk['stem'])
+            h = ops.StemLinear.apply(A, self.proj_in.weight, self.proj_in.bias, self.cond_proj_in.weight, self.cond_proj_in.bias, w['stem'])
         ids, te = None, None
         if exists(text) and not drop_text_cond:
             if isinstance(self.embed_text, InterpolatedCharacterEmbed):
-                te = self.embed_text.embed_bf16(text, N, mask)      # :1283 embed_text(text, seq_len, mask = mask)
+                te = self.embed_text.embed_bf16(text, N, mask, w['interp'])      # :1283 embed_text(text, seq_len, mask = mask)
             else:
                 ids = self.embed_text.ids(text, N)
-        y = self.transformer._forward_from_h(h, B, N, times, mask, text_ids=ids, text_embed_module=self.embed_text, te_bf16=te)
-        return y, pk
+        return self.transformer._forward_from_h(w['tr'], h, B, N, times, mask, text_ids=ids, text_embed_module=self.embed_text, te_bf16=te)
 
     @_on_module_device
     def transformer_with_pred_head(self, x, cond, times, mask=None, text=None, drop_text_cond=None, return_drop_text_cond=False):
         """e2_tts.py:1250-1301."""
         B, N, C = x.shape
         drop_text_cond = default(drop_text_cond, self.training and pyrandom.random() < self.cond_drop_prob)
-        pk = self._packed()
-        A, _ = ops.stem_prepare(B, N, C, pk['Cp'], x_in=x.to(F32).contiguous(), cond_in=cond.to(F32).contiguous(), concat=self.concat_cond)
+        w = self._packed_weights()
+        A, _ = ops.stem_prepare(B, N, C, w['Cp'], x_in=x.to(F32).contiguous(), cond_in=cond.to(F32).contiguous(), concat=self.concat_cond)
         if not torch.is_tensor(times):
             times = torch.tensor(times, device=x.device)
-        y, pk = self._embed(A, B, N, times.to(x.device), mask, text, drop_text_cond, pk)
-        pred = ops.PredHead.apply(y, self.to_pred.weight, self.to_pred.bias, pk['pred']).view(B, N, C).to(x.dtype)
+        y = self._embed(w, A, B, N, times.to(x.device), mask, text, drop_text_cond)
+        pred = ops.PredHead.apply(y, self.to_pred.weight, self.to_pred.bias, w['pred']).view(B, N, C).to(x.dtype)
         if not return_drop_text_cond:
             return pred
         return pred, drop_text_cond
@@ -1039,13 +1038,9 @@ class E2TTS(Module):
         ts_host = torch.linspace(0, 1, steps)          # fixed grid (torchdiffeq semantics); step sizes stay host floats: no device sync per step
         ts = ts_host.to(dev)
         method = self.odeint_kwargs.get('method', 'midpoint')
-        frozen = [self.transformer] + ([cfg_null_model.transformer] if exists(cfg_null_model) else [])
-        try:
-            self._packed()               # weights are fixed for the whole solve: pack the bf16 operands once (fresh), not 124 times
-            if exists(cfg_null_model):
-                cfg_null_model._packed()
-            for tr in frozen:
-                tr.freeze_packed(True)
+        # weights are fixed for the whole solve: pack each model's operands once (fresh), not once per function evaluation
+        freeze_null = cfg_null_model._pack()[0].freeze() if exists(cfg_null_model) else contextlib.nullcontext()
+        with self._pack()[0].freeze(), freeze_null:
             fn_eval = fn   # (one function evaluation as a CUDA graph was measured: -1 % at cfg5, but re-capturing per call costs the e2e path 19 %)
             for i in range(steps - 1):
                 t0, dt = ts[i], float(ts_host[i + 1] - ts_host[i])
@@ -1055,9 +1050,6 @@ class E2TTS(Module):
                     half = 0.5 * dt
                     ymid = ops.axpy(y, fn_eval(t0, y), half)
                     y = ops.axpy(y, fn_eval(t0 + half, ymid), dt)
-        finally:
-            for tr in frozen:
-                tr.freeze_packed(False)
         out = torch.where(cond_mask, cond, y)
         if exists(return_raw_output) and return_raw_output:
             return out
@@ -1098,14 +1090,14 @@ class E2TTS(Module):
             vcm = velocity_consistency_model
             with torch.no_grad():
                 t_d = times + velocity_consistency_delta
-                vpk = vcm._packed()
-                A_d, _ = ops.stem_prepare(B, N, C, vpk['Cp'], x1=x1, x0=x0, times=t_d, span=span_u8, concat=velocity_consistency_model.concat_cond)
-                y_d, vpk = vcm._embed(A_d, B, N, t_d, mask, text, drop_text_cond, vpk)
-                vel_target = ops.PredHead.apply(y_d, vcm.to_pred.weight, vcm.to_pred.bias, vpk['pred'])
-        pk = self._packed()
-        A, cond = ops.stem_prepare(B, N, C, pk['Cp'], x1=x1, x0=x0, times=times, span=span_u8, want_cond=True, concat=self.concat_cond)
-        y, pk = self._embed(A, B, N, times, mask, text, drop_text_cond, pk)
-        loss, pred, pred_data, parts = ops.FlowLossHead.apply(y, self.to_pred.weight, self.to_pred.bias, pk['pred'], x1, x0, span_u8, vel_target,
+                vw = vcm._packed_weights()
+                A_d, _ = ops.stem_prepare(B, N, C, vw['Cp'], x1=x1, x0=x0, times=t_d, span=span_u8, concat=velocity_consistency_model.concat_cond)
+                y_d = vcm._embed(vw, A_d, B, N, t_d, mask, text, drop_text_cond)
+                vel_target = ops.PredHead.apply(y_d, vcm.to_pred.weight, vcm.to_pred.bias, vw['pred'])
+        w = self._packed_weights()
+        A, cond = ops.stem_prepare(B, N, C, w['Cp'], x1=x1, x0=x0, times=times, span=span_u8, want_cond=True, concat=self.concat_cond)
+        y = self._embed(w, A, B, N, times, mask, text, drop_text_cond)
+        loss, pred, pred_data, parts = ops.FlowLossHead.apply(y, self.to_pred.weight, self.to_pred.bias, w['pred'], x1, x0, span_u8, vel_target,
                                                               float(self.velocity_consistency_weight) if need_velocity_loss else 0.0)
         breakdown = LossBreakdown(parts[0], parts[1] if need_velocity_loss else self.zero)
         return E2TTSReturn(loss, cond, pred.view(B, N, C), pred_data.view(B, N, C), breakdown)

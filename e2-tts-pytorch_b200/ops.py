@@ -650,10 +650,11 @@ class TextStem(Function):
 class InterpText(Function):
     """InterpolatedCharacterEmbed (e2_tts.py:414-482): te = mask * (interpolate(embed(valid chars), audio_len) + abs_pos_mlp(linspace(0, Lt, La))).
     b200_interp_text_fwd stretches the embeddings and evaluates Linear(1, d) + SiLU per token; Linear(d, d) + bias + the stretched
-    embeddings (residual) + the row mask are ONE wgmma GEMM with its fused epilogue. Returns bf16 [B*N, d]."""
+    embeddings (residual) + the row mask are ONE wgmma GEMM with its fused epilogue, over w2p, the packed bf16 copy of w2.
+    Returns bf16 [B*N, d]."""
 
     @staticmethod
-    def forward(ctx, ids_c, text_len, audio_len, mask_u8, emb, w1, b1, w2, b2, B, N):
+    def forward(ctx, ids_c, text_len, audio_len, mask_u8, emb, w1, b1, w2, w2p, b2, B, N):
         V, D = emb.shape
         dev = emb.device
         nt = ids_c.shape[1]
@@ -662,7 +663,6 @@ class InterpText(Function):
         a = lib.make_args('b200_interp_text_args', ids=ids_c, text_len=text_len, audio_len=audio_len, emb=emb, w1=w1, b1=b1,
                           B=B, N=N, nt=nt, D=D, vocab=V, lerp=lerp, h1=h1)
         lib.call('b200_interp_text_fwd', a, _stream())
-        w2p = w2.detach().to(BF16).contiguous()          # a d x d operand, re-cast per call (non-default variant: not in the pack table)
         te = gemm(h1, w2p, B * N, D, D, bias=b2, rowmask=mask_u8, resid=lerp, ldr=D)
         ctx.save_for_backward(ids_c, text_len, audio_len, mask_u8, emb, w1, b1, w2p, h1)
         ctx.meta = (B, N)
@@ -683,7 +683,7 @@ class InterpText(Function):
         a = lib.make_args('b200_interp_text_args', ids=ids_c, text_len=text_len, audio_len=audio_len, emb=emb, w1=w1, b1=b1,
                           B=B, N=N, nt=ids_c.shape[1], D=D, vocab=V, d_lerp=dz, d_h1=d_h1, d_emb=d_emb, d_w1=dw1, d_b1=db1)
         lib.call('b200_interp_text_bwd', a, _stream())
-        return None, None, None, None, d_emb, dw1.view_as(w1), db1, dW2, db2, None, None
+        return None, None, None, None, d_emb, dw1.view_as(w1), db1, dW2, None, db2, None, None
 
 
 class FinalNorm(Function):
@@ -863,13 +863,12 @@ def stem_prepare(B, N, C, Cp, *, x1=None, x0=None, times=None, span=None, x_in=N
 
 
 class CondPack(Function):
-    """Pack every per-layer to_gamma weight (AdaptiveRMSNorm A.1, AdaLNZero e2_tts.py:341) into one fp32 [4L*d, d] matrix
-    and the AdaLNZero biases into the odd d-wide segments of one [4L*d] vector (one launch of the pack kernel);
-    backward hands each parameter its slice of the packed gradients."""
+    """The packed to_gamma stack as an autograd node: W_out, b_out hold every per-layer to_gamma weight (AdaptiveRMSNorm A.1,
+    AdaLNZero e2_tts.py:341) as one fp32 [4L*d, d] matrix and the AdaLNZero biases in the odd d-wide segments of one [4L*d]
+    vector, already written by the model's weight pack; backward hands each parameter its slice of the packed gradients."""
 
     @staticmethod
-    def forward(ctx, run_pack, W_out, b_out, d, n_w, *params):
-        run_pack()
+    def forward(ctx, W_out, b_out, d, n_w, *params):
         ctx.meta = (d, n_w, len(params) - n_w)
         return W_out, b_out
 
@@ -879,7 +878,7 @@ class CondPack(Function):
         d, n_w, n_b = ctx.meta
         gw = [dW[j * d:(j + 1) * d] if dW is not None else None for j in range(n_w)]
         gb = [db[(2 * m + 1) * d:(2 * m + 2) * d] if db is not None else None for m in range(n_b)]
-        return (None, None, None, None, None, *gw, *gb)
+        return (None, None, None, None, *gw, *gb)
 
 
 class CastRows(Function):

@@ -90,11 +90,6 @@ def broadcast_module(module, src=0, process_group=None):
     with torch.no_grad():
         for t in list(module.parameters()) + list(module.buffers()):
             dist.broadcast(t.data, src=src, group=process_group)
-    for m in module.modules():            # packed bf16 operand caches are derived from the parameters
-        if hasattr(m, '_pack'):
-            m._pack, m._packed = None, None
-        if hasattr(m, '_wpack'):
-            m._wpack = None
 
 
 class GradSync:

@@ -479,7 +479,7 @@ class _f64_default:
         torch.set_default_dtype(self.old)
 
 
-def test_interp_text(pkg):
+def test_interp_text_packed_operand(pkg):
     """ops.InterpText against O.interpolated_character_embed: downsampling (Lt 50 -> La 20), equal lengths, a single character,
     a single frame, upsampling; La < N, so every sample has padded rows, which must be exactly 0."""
     ops = pkg.ops
@@ -500,8 +500,9 @@ def test_interp_text(pkg):
     ids_c = torch.zeros(B, nt, dtype=torch.int32)
     ids_c[:, :] = text.clamp(min=0).to(torch.int32)          # the valid ids are already first
     params = [t.to(dev()).requires_grad_() for t in (emb, w1, b1, w2, b2)]
+    w2p = params[3].detach().to(BF16)        # the model passes its weight pack's copy: the same round to nearest even
     te = ops.InterpText.apply(ids_c.to(dev()), Lt.to(torch.int32).to(dev()), La.to(torch.int32).to(dev()), mask.to(torch.uint8).to(dev()),
-                              *params, B, N)
+                              *params[:4], w2p, params[4], B, N)
     d_te = bfr(torch.randn(B * N, D, generator=g))
     grads = torch.autograd.grad(te, params, d_te.to(dev()))
     names = ['embed.weight', 'abs_pos_mlp.1.weight', 'abs_pos_mlp.1.bias', 'abs_pos_mlp.3.weight', 'abs_pos_mlp.3.bias']
@@ -894,8 +895,8 @@ def test_cast_rows(pkg):
     check_zero('cast pad columns', out[:, cols:])
 
 
-def test_pack_weights(pkg):
-    """modules._PackTable / b200_pack_weights: mode 0 with row and column offsets, mode 1 (GEGLU interleave) for a weight and a 1-D
+def test_weight_pack(pkg):
+    """modules.WeightPack / b200_pack_weights: mode 0 with row and column offsets, mode 1 (GEGLU interleave) for a weight and a 1-D
     bias, fp32 output, the scalar path (cols % 4 != 0: 1-D biases, 3-D conv weights, odd column offsets). The destinations are filled
     with a sentinel first: every byte outside the described slots must be untouched."""
     mods = pkg.modules
@@ -911,7 +912,7 @@ def test_pack_weights(pkg):
     dst_conv = torch.full((30, 40), 3.0, dtype=BF16)
     D = {k: v.to(dev()) for k, v in dict(w_geglu=w_geglu, b_geglu=b_geglu, w_plain=w_plain, w_conv=w_conv, w_odd=w_odd,
                                          dst_bf=dst_bf, dst_f32=dst_f32, dst_conv=dst_conv).items()}
-    tab = mods._PackTable()
+    tab = mods.WeightPack(dev())
     tab.add(D['w_plain'], D['dst_bf'], row_off=7, col_off=64)
     tab.add(D['w_geglu'], D['dst_bf'], row_off=44, col_off=132, mode=1)
     tab.add(D['w_odd'], D['dst_bf'], row_off=290, col_off=3)
