@@ -6,7 +6,10 @@
 //   warpgroup 0, one thread : TMA producer — cp.async.bulk.tensor 2-D tiles (128B swizzle) into a kStages smem ring
 //   warpgroups 1, 2         : MMA + epilogue — each owns 64 * MH rows of the CTA tile: wgmma.m64nBNk16 from the smem ring into
 //                             register accumulators, then the fused epilogue (bias / AdaLN gate / row mask / residual / GEGLU(+dropout))
-//                             straight from the accumulator fragments; fp32 split-K partials leave through vector atomics.
+//                             on the accumulator fragments. Plain bf16 outputs are written 64 x 64 at a time into a 128B-swizzled smem
+//                             staging slice (two per warpgroup, alternating) and leave as TMA tile stores (bulk async groups), so the
+//                             warpgroup moves on to the next slice while the previous one drains; GEGLU outputs leave as bf16x2 stores
+//                             from the fragments, fp32 split-K partials through vector atomics.
 // While a consumer warpgroup runs its epilogue the producer is already filling the ring with the next tile's operands.
 // Operands may be K-major or MN-major (transposed storage) so that the backward contractions
 // dX = dY*W and dW = dY^T*X read activations exactly as they lie in HBM — no transposes are materialised.
@@ -35,6 +38,7 @@ struct GemmParams {
     int geglu; float dropout_p; unsigned long long seed;
     const unsigned long long* seed_dev;   // optional device addend of the seed (CUDA-graph replays)
     int atomic_out;
+    int tma_store;   // bf16 output through the smem staging slices and TMA stores (tmD)
 };
 
 // Tiles: (BM * MH) x BN. MH == 2 gives each consumer warpgroup 128 rows (two m64 MMAs per k-step share one B tile); BN == 256 gives it
@@ -46,8 +50,11 @@ struct GemmSmem {
     static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
     static constexpr int kStages = (STAGE_BYTES <= 32768) ? 6 : 4;
     static constexpr int TILE_BYTES = kStages * STAGE_BYTES;
+    static constexpr int SLICE_BYTES = 64 * 64 * 2;              // one 64 x 64 bf16 output slice, 128B-swizzled
+    static constexpr int STG_BYTES = 2 * 2 * SLICE_BYTES;        // two slices per consumer warpgroup: 32 KB
     static constexpr int BAR_BYTES = 128;
-    static constexpr int TOTAL = TILE_BYTES + BAR_BYTES + 1024;  // + slack for manual 1024B alignment
+    static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + 1024;  // + slack for manual 1024B alignment
+    static_assert(TOTAL <= 227 * 1024, "GEMM shared memory exceeds the 227 KB a block may use");
 };
 
 // Exact (erf) GELU of x-transformers' GLU (A.2) for a PAIR of pre-activations:  gelu(x) = x Phi(x) = relu(x) - |x| Phi(-|x|), with the
@@ -94,7 +101,7 @@ __device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col
 template <int BN, bool A_MN, bool B_MN, int MH>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                  const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+                  const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD, const GemmParams p) {
     using S = GemmSmem<BN, MH>;
     constexpr int kStages = S::kStages;
     constexpr int BMT = BM * MH;   // rows of the CTA tile
@@ -104,7 +111,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* smA = smem;
     uint8_t* smB = smem + kStages * S::A_BYTES;
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES);
+    uint8_t* stg = smem + S::TILE_BYTES;   // output staging slices: [warpgroup][2][64 x 128 B]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES + S::STG_BYTES);
     uint64_t* empty_bar = full_bar + kStages;
 
     const int wg = threadIdx.x >> 7;
@@ -113,6 +121,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         tma_prefetch_desc(&tmA);
         tma_prefetch_desc(&tmA2);
         tma_prefetch_desc(&tmB);
+        if (p.tma_store) tma_prefetch_desc(&tmD);
         for (int i = 0; i < kStages; ++i) {
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 2);   // one arrival per consumer warpgroup
@@ -174,6 +183,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     constexpr uint32_t a_adv = A_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;   // per k16 step, in 16-B units
     constexpr uint32_t b_adv = B_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
     float acc[MH][NACC];
+    uint8_t* my_stg = stg + cw * 2 * S::SLICE_BYTES;
+    uint32_t nslice = 0;                       // staging slices this warpgroup has filled so far (buffer = nslice & 1)
     int stage = 0;
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < p.num_work; w += gridDim.x) {
@@ -218,7 +229,74 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         // Fragment of an m64nBN accumulator: thread (wq, lane) holds rows 16 wq + lane / 4 (+ 8) and, for every 8-column group j,
         // columns 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 i + c] = (row + 8 i, column + c).
         const int cq = 2 * (lane & 3);
-        if (!p.geglu) {
+        if (p.tma_store) {
+            // first the element-wise epilogue in place on the fragments (rows >= M and columns >= N are left as they are: the TMA
+            // store clips them), then 64 x 64 slices: the thread's rows r, r + 8 and, per 8-column group jj of the slice, the 4 bytes
+            // at column 8 jj + cq, written to 16-byte chunk (jj ^ (r & 7)) of the row — the TMA's 128B swizzle, and conflict-free:
+            // the 8 rows of a warp store land in 8 different chunks. r & 7 == lane / 4 for both rows.
+            if (p.bias || p.colscale || p.rowmask || p.resid) {
+#pragma unroll
+                for (int h = 0; h < MH; ++h) {
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
+                        if (row >= p.M) continue;
+                        const bool masked = p.rowmask && p.rowmask[row] == 0;
+                        const float* cs = p.colscale ? p.colscale + (long long)(row / p.rows_per_batch) * p.N : nullptr;
+                        const __nv_bfloat16* rp = p.resid ? reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr : nullptr;
+#pragma unroll
+                        for (int j = 0; j < BN / 8; ++j) {
+                            const int col = tn * BN + 8 * j + cq;
+                            if (col >= p.N) continue;
+                            const bool two = col + 1 < p.N;
+                            float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
+                            if (p.bias) { v0 += __ldg(p.bias + col); if (two) v1 += __ldg(p.bias + col + 1); }
+                            if (cs) { v0 *= __ldg(cs + col); if (two) v1 *= __ldg(cs + col + 1); }
+                            if (masked) { v0 = 0.f; v1 = 0.f; }
+                            if (rp) {
+                                if (two) {
+                                    const uint32_t u = *reinterpret_cast<const uint32_t*>(rp + col);
+                                    v0 += bf16_lo(u); v1 += bf16_hi(u);
+                                } else {
+                                    v0 += __bfloat162float(rp[col]);
+                                }
+                            }
+                            acc[h][4 * j + 2 * i] = v0;
+                            acc[h][4 * j + 2 * i + 1] = v1;
+                        }
+                    }
+                }
+            }
+            const uint32_t swz = (uint32_t)(lane >> 2) << 4;
+            const uint32_t toff = (uint32_t)(wq * 16 + (lane >> 2)) * 128 + 2 * cq;
+#pragma unroll
+            for (int h = 0; h < MH; ++h) {
+                const int rowb = tm * BMT + (cw * MH + h) * 64;
+#pragma unroll
+                for (int s = 0; s < BN / 64; ++s) {
+                    const int colb = tn * BN + s * 64;
+                    if (colb >= p.N) break;                  // uniform across the warpgroup
+                    const uint32_t buf = smem_u32(my_stg + (nslice & 1) * S::SLICE_BYTES);
+                    if (t == 0) bulk_wait_group_read<1>();   // the store issued from this buffer two slices ago has read it
+                    named_bar_sync(1 + cw, 128);
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                        for (int jj = 0; jj < 8; ++jj) {
+                            const int j = s * 8 + jj;
+                            st_shared_u32(buf + toff + i * 8 * 128 + (((uint32_t)jj << 4) ^ swz), pack_bf16(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]));
+                        }
+                    }
+                    fence_proxy_async();                     // the generic-proxy smem writes, before the TMA (async proxy) reads them
+                    named_bar_sync(1 + cw, 128);
+                    if (t == 0) {
+                        tma_store_2d(&tmD, my_stg + (nslice & 1) * S::SLICE_BYTES, colb, rowb);   // rows >= M, columns >= N are clipped
+                        bulk_commit_group();
+                    }
+                    ++nslice;
+                }
+            }
+        } else if (!p.geglu) {
 #pragma unroll
             for (int h = 0; h < MH; ++h) {
 #pragma unroll
@@ -296,6 +374,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
         }
     }
+    if (t == 0) bulk_wait_group<0>();   // the staging slices stay valid until the last store has completed
 }
 
 // ---------------------------------------------------------------------------------------------- host
@@ -357,7 +436,7 @@ static int make_map_uncached(CUtensorMap* m, const void* ptr, int64_t inner, int
 }
 
 template <int BN, bool A_MN, bool B_MN, int MH>
-static int launch_gemm(const CUtensorMap (&tm)[3], const GemmParams& p, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap (&tm)[4], const GemmParams& p, cudaStream_t st) {
     using S = GemmSmem<BN, MH>;
     auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, MH>;
     static DeviceOnce once;   // one flag per template instantiation and device
@@ -366,7 +445,7 @@ static int launch_gemm(const CUtensorMap (&tm)[3], const GemmParams& p, cudaStre
         B200_REQUIRE(e == cudaSuccess, "gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
     const int grid = p.num_work < num_sms() ? p.num_work : num_sms();
-    kern<<<grid, kGemmThreads, S::TOTAL, st>>>(tm[0], tm[1], tm[2], p);
+    kern<<<grid, kGemmThreads, S::TOTAL, st>>>(tm[0], tm[1], tm[2], tm[3], p);
     return check_launch("gemm_wgmma_kernel");
 }
 
@@ -432,8 +511,8 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     if (!a->d_fp32) B200_REQUIRE((a->ldd % 8) == 0, "gemm: bf16 output pitch must be a multiple of 8");
     if (a->resid) B200_REQUIRE((a->ldr % 8) == 0, "gemm: residual pitch must be a multiple of 8");
 
-    CUtensorMap tm[3];
-    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2];
+    CUtensorMap tm[4];
+    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2], &tD = tm[3];
     int rc;
     const int64_t KA = a->A2 ? a->K1 : a->K;
     if (!a_mn) rc = make_map(&tA, a->A, KA, a->M, a->lda, BM);
@@ -450,6 +529,13 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     else rc = make_map(&tB, a->B, a->N, a->K, a->ldb, BK);
     if (rc) return rc;
     if (!a->d_fp32) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D) & 3) == 0, "gemm: bf16 output must be 4-byte aligned");
+    // TMA tile stores need a 16-byte aligned base (the pitch is a multiple of 16 bytes already); other bf16 outputs store from the fragments
+    p.tma_store = !a->d_fp32 && !a->geglu && (reinterpret_cast<uintptr_t>(a->D) & 15) == 0;
+    if (p.tma_store) {
+        if ((rc = make_map(&tD, a->D, a->N, a->M, a->ldd, 64))) return rc;
+    } else {
+        tD = tB;   // unused
+    }
     if (a->geglu && a->D2) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D2) & 3) == 0, "gemm: GEGLU pre-activation buffer must be 4-byte aligned");
     if (a->resid) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->resid) & 3) == 0, "gemm: residual must be 4-byte aligned");
 

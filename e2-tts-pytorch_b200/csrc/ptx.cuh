@@ -98,6 +98,11 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// named barriers (ids 1..15; __syncthreads owns id 0): bar.sync waits until `n` threads of the CTA have reached barrier `id`
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // 1-D bulk copy global -> shared (TMA engine, no tensor map): `bytes` a multiple of 16, both addresses 16-byte aligned
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
