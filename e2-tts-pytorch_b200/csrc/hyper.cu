@@ -825,11 +825,12 @@ extern "C" int b200_hc_width_bwd(const b200_hc_width_args* a, b200_stream_t stre
     p.g_bfn = a->g_dynamic_beta_fn; p.g_bscale = a->g_dynamic_beta_scale; p.g_sbeta = a->g_static_beta; p.g_ng = a->g_norm_gain;
     B200_REQUIRE(a->stats, "hc_width_bwd: the per-token reduction results saved by b200_hc_width_fwd (stats_out) are required");
     p.stats = a->stats;
-    B200_REQUIRE(a->ws_records, "hc_width_bwd: missing workspace (T * 40 floats)");
-    // workspace: coefficient matrix C bf16 [T*S (+ T fused rows), 8] (80 B per token), then G fp32 [D, 8]
+    // workspace: coefficient matrix C bf16 [T*S (+ T fused rows), 8] (80 B per token), then G fp32 [D, 8] at byte offset 80 T
+    // (16-byte aligned: finalize reads G as float4)
+    B200_REQUIRE(a->ws_records && (reinterpret_cast<uintptr_t>(a->ws_records) & 15) == 0,
+                 "hc_width_bwd: missing or misaligned workspace (T * 20 + D * 8 floats, 16-byte aligned)");
     __nv_bfloat16* cmat = reinterpret_cast<__nv_bfloat16*>(a->ws_records);
     float* G = a->ws_records + (size_t)a->T * 20;
-    B200_REQUIRE((size_t)a->T * 20 >= (size_t)a->D * 8, "hc_width_bwd: workspace too small for D=%d at T=%lld", a->D, (long long)a->T);
     if (int rc = fused ? launch_hc_bwd<true>(p, a, cmat, st) : launch_hc_bwd<false>(p, a, cmat, st)) return rc;
     // G = R^T C on the tensor cores: A = residual streams [T*S, D] read MN-major (fused: followed by y_prev [T, D] against the C' rows),
     // B = C [T*S (+ T), 8] MN-major, split-K over the tokens

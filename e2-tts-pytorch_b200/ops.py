@@ -148,7 +148,7 @@ def _hc_width_bwd(xres, y_prev, beta_prev, stats, params, norm_gain, norm_mode, 
                       d_branch=_c(d_branch), d_res=_c(d_res), d_beta=_c(d_beta), d_xres=d_xres,
                       g_norm_gamma=g_gamma, g_dynamic_alpha_fn=g_afn, g_dynamic_alpha_scale=g_as, g_static_alpha=g_sal,
                       g_dynamic_beta_fn=g_bfn, g_dynamic_beta_scale=g_bs, g_static_beta=g_sbe,
-                      g_norm_gain=g_gain if norm_mode else None, ws_records=torch.empty((T, 40), device=dev, dtype=F32),
+                      g_norm_gain=g_gain if norm_mode else None, ws_records=torch.empty(T * 20 + D * 8, device=dev, dtype=F32),
                       y_prev=y_prev, beta_prev=beta_prev, d_y_prev=d_y, d_beta_prev=d_bp, stats=stats)
     lib.call('b200_hc_width_bwd', a, _stream())
     pg = (g_gamma, g_afn.view(D, S + 1), g_as.view(()), g_sal.view(S, S + 1), g_bfn, g_bs.view(()), g_sbe,

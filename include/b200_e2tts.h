@@ -150,7 +150,8 @@ typedef struct {
     void* d_xres;
     float *g_norm_gamma, *g_dynamic_alpha_fn, *g_dynamic_alpha_scale, *g_static_alpha, *g_dynamic_beta_fn, *g_dynamic_beta_scale,
         *g_static_beta, *g_norm_gain;
-    float* ws_records;   /* bwd workspace: T * 40 floats (bf16 coefficient matrix [T*S (+T), 8] + fp32 [D, 8] result of the parameter GEMM) */
+    float* ws_records;   /* bwd workspace: T * 20 + D * 8 floats, 16-byte aligned: bf16 coefficient matrix [T*S (+T), 8] (T * 20 floats,
+                            the T fused C' rows included), then the fp32 [D, 8] result of the parameter GEMM at byte offset 80 T */
     float* stats_out;    /* fwd (optional): fp32 [T, 32] per-token reduction results; bwd REQUIRES them back in `stats` (caller-owned) */
     const float* stats;
     const void* y_prev; const float* beta_prev;              /* fused preceding depth connection (both or neither) */
