@@ -752,7 +752,9 @@ class MelSpec(Module):
         `rearrange(batch['mel'], 'b d n -> b n d')` (:253), as ONE kernel launch over the ragged batch.
         waves: list of 1-D fp32 tensors at `sampling_rate` (resampling is the dataset's job) or a zero-padded [B, nw_max] tensor with
         `lens` (samples per sequence). Returns dict(mel [B, n_frames_max, n_mels] fp32, mel_lengths [B] int64) — pass as
-        `model(batch['mel'], text=..., lens=batch['mel_lengths'])`."""
+        `model(batch['mel'], text=..., lens=batch['mel_lengths'])`. A length past the padded wave counts as the padded length;
+        an item of at most n_fft/2 samples is too short for the reflect padding (the reference's MelSpec raises on it): its
+        frames are zeros and its mel_lengths entry is 0."""
         if isinstance(waves, (list, tuple)):
             dev = self.dummy.device if self.dummy.device.type == 'cuda' else waves[0].device
             lens = torch.tensor([w.shape[-1] for w in waves], dtype=torch.int32)
@@ -769,7 +771,8 @@ class MelSpec(Module):
             self.to(waves.device)
         mel = ops.melspec(waves.to(F32).contiguous(), self.mel_stft.spectrogram.window, self.mel_stft.mel_scale.fb, self.n_fft, self.hop,
                           wave_lens=lens.contiguous(), out_bnd=True)
-        mel_lengths = 1 + lens.long() // self.hop
+        lens = lens.long().clamp(max=waves.shape[1])      # the kernel clamps the same way
+        mel_lengths = torch.where(lens > self.n_fft // 2, 1 + lens // self.hop, 0)
         n_max = int(1 + waves.shape[1] // self.hop)
         return dict(mel=mel[:, :n_max], mel_lengths=mel_lengths)
 

@@ -338,9 +338,11 @@ int b200_cfg_combine(const float* pred, const float* null_pred, double* ws_red, 
  * Shared-memory radix-2 FFT per frame + band-limited filterbank; ws_bands: caller workspace of 2 * n_mels int32 (8-byte aligned),
  * filled by the call with each filter's non-zero bin range.
  * On-device collate (trainer.py:61-82 collate_fn + :101-131 HFDataset.__getitem__, SURVEY §8f row 3): wave_lens (optional int32 [B]) =
- * samples per sequence of a zero-padded ragged batch — sequence b yields 1 + wave_lens[b]/hop frames (reflect-padded at its own end),
- * the remaining frames are the collate's zero padding; out_bnd != 0 writes [B, frames, n_mels] (the layout E2TTS.forward consumes,
- * trainer.py:253 rearrange 'b d n -> b n d') instead of the reference MelSpec's [B, n_mels, frames]. */
+ * samples per sequence of a zero-padded ragged batch (a length past nw counts as nw) — sequence b yields 1 + wave_lens[b]/hop frames
+ * (reflect-padded at its own end), the remaining frames are the collate's zero padding. A sequence of wave_lens[b] <= n_fft/2 samples
+ * is too short to reflect-pad (the reference's MelSpec raises on it): all its frames are written as zeros. out_bnd != 0 writes
+ * [B, frames, n_mels] (the layout E2TTS.forward consumes, trainer.py:253 rearrange 'b d n -> b n d') instead of the reference
+ * MelSpec's [B, n_mels, frames]. */
 int b200_melspec(const float* wave, const float* window, const float* fb, float* out, int32_t B, int32_t nw, int32_t n_fft,
                  int32_t hop, int32_t n_mels, int32_t* ws_bands, const int32_t* wave_lens, int32_t out_bnd, b200_stream_t stream);
 
