@@ -9,6 +9,12 @@
 //                             The softclamp bounds the logits to [-clamp, clamp], so exp() needs no running maximum: O accumulates
 //                             over all key tiles and is normalised once by the row sum.
 // mbarrier pipelines: q_full, kv_full/kv_empty[3].
+//
+// Unclamped mode (UNCLAMPED = true; x-transformers Attention without softclamp_logits): the same pipeline and fragment layout with an
+// online softmax. Per key tile, masked keys go to -inf, the row maximum m is reduced over the quad, O and the row sum are rescaled by
+// 2^((m_old - m_new) scale log2 e) and P = 2^(s scale log2 e - m_new scale log2 e); LSE = m scale + ln(l). The backward recomputes
+// P from that LSE with no tanh factor. A row whose keys are all masked gives o = og = 0, lse = -inf and zero gradients, as the clamped
+// kernels do.
 #include <type_traits>
 
 #include "common.cuh"
@@ -33,6 +39,7 @@ struct AttnTcP {
     int drop_stride;                // even row pitch of the dropout counter space
     unsigned long long seed;
     const unsigned long long* seed_dev;   // optional device addend of the seed (CUDA-graph replays)
+    float scale, scale_log2e;       // unclamped mode: the score scale, and scale * log2(e)
 };
 
 __device__ __forceinline__ float tanh_approx(float x) {
@@ -74,6 +81,7 @@ __global__ void attn_maskbits_kernel(const unsigned char* mask, unsigned int* bi
 // ------------------------------------------------------------------------------------------------ forward
 constexpr int KV_STAGES = 3;
 
+template <bool UNCLAMPED>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const AttnTcP p) {
@@ -140,6 +148,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const float lim5 = 0.15f / fabsf(soc), lim9 = TANH_POLY_MAX / fabsf(soc);
     const uint32_t thr32 = drop_thresh32(p.drop_thresh);
     float l[2] = {0.f, 0.f};
+    float m[2] = {-INFINITY, -INFINITY};   // unclamped mode: running row maximum of the raw scores
     float o[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) o[i] = 0.f;
@@ -159,62 +168,101 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(s);
-        float amax = 0.f;
+        if constexpr (UNCLAMPED) {
+            const unsigned int mw0 = mb[2 * j], mw1 = mb[2 * j + 1];
+            if ((mw0 & mw1) != 0xffffffffu) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) amax = fmaxf(amax, fabsf(s[i]));
-        // clamp * log2(e) * tanh(u), u = s * scale / clamp, evaluated as an odd polynomial in the RAW score s with the constants folded
-        // in: s * (k1 + s^2 (k3 + s^2 (k5 + ...))) — degree 5 for |u| <= 0.15 (exact to 1e-7), degree 9 for |u| <= 0.5; tanh.approx
-        // only when a warp's tile leaves that range
-        if (__all_sync(0xffffffffu, amax <= lim5)) {
+                for (int g = 0; g < 8; ++g) {
+                    const unsigned int w = g < 4 ? mw0 : mw1;
+                    const int bit = (8 * g + cq) & 31;
 #pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-                const float2 x = make_float2(s[i], s[i + 1]);
-                const float2 x2 = fmul2(x, x);
-                float2 q = ffma2(x2, make_float2(k5, k5), make_float2(k3, k3));
-                q = ffma2(q, x2, make_float2(k1, k1));
-                const float2 y = fmul2(x, q);
-                s[i] = ex2_approx(y.x);
-                s[i + 1] = ex2_approx(y.y);
-            }
-        } else if (__all_sync(0xffffffffu, amax <= lim9)) {
-#pragma unroll
-            for (int i = 0; i < 32; i += 2) {
-                const float2 x = make_float2(s[i], s[i + 1]);
-                const float2 x2 = fmul2(x, x);
-                float2 q = ffma2(x2, make_float2(k9, k9), make_float2(k7, k7));
-                q = ffma2(q, x2, make_float2(k5, k5));
-                q = ffma2(q, x2, make_float2(k3, k3));
-                q = ffma2(q, x2, make_float2(k1, k1));
-                const float2 y = fmul2(x, q);
-                s[i] = ex2_approx(y.x);
-                s[i + 1] = ex2_approx(y.y);
-            }
-        } else {   // mixed tile: the polynomial wherever it is in range, tanh.approx only for the outliers themselves
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                const float x = s[i], x2 = x * x;
-                const float yp = x * __fmaf_rn(__fmaf_rn(__fmaf_rn(__fmaf_rn(k9, x2, k7), x2, k5), x2, k3), x2, k1);
-                const float y = fabsf(x) <= lim9 ? yp : tanh_approx(x * soc) * cl2.x;
-                s[i] = ex2_approx(y);
-            }
-        }
-        const unsigned int mw0 = mb[2 * j], mw1 = mb[2 * j + 1];   // keys 64 j .. 64 j + 31, 64 j + 32 .. 64 j + 63
-        if ((mw0 & mw1) != 0xffffffffu) {
-#pragma unroll
-            for (int g = 0; g < 8; ++g) {
-                const unsigned int w = g < 4 ? mw0 : mw1;
-                const int bit = (8 * g + cq) & 31;
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    if (!((w >> bit) & 1u)) s[4 * g + 2 * i] = 0.f;
-                    if (!((w >> (bit + 1)) & 1u)) s[4 * g + 2 * i + 1] = 0.f;
+                    for (int i = 0; i < 2; ++i) {
+                        if (!((w >> bit) & 1u)) s[4 * g + 2 * i] = -INFINITY;
+                        if (!((w >> (bit + 1)) & 1u)) s[4 * g + 2 * i + 1] = -INFINITY;
+                    }
                 }
             }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                float tm = m[i];
+#pragma unroll
+                for (int g = 0; g < 8; ++g) tm = fmaxf(tm, fmaxf(s[4 * g + 2 * i], s[4 * g + 2 * i + 1]));
+                tm = fmaxf(tm, __shfl_xor_sync(0xffffffffu, tm, 1));
+                tm = fmaxf(tm, __shfl_xor_sync(0xffffffffu, tm, 2));
+                // every key this row has seen so far is masked: subtract 0 instead of -inf, so that P and the rescale factor are 0
+                const float mt = tm == -INFINITY ? 0.f : tm;
+                const float alpha = ex2_approx((m[i] - mt) * p.scale_log2e);
+                const float nm = -mt * p.scale_log2e;
+                m[i] = tm;
+                float ls = 0.f;
+#pragma unroll
+                for (int g = 0; g < 8; ++g) {
+                    o[4 * g + 2 * i] *= alpha;
+                    o[4 * g + 2 * i + 1] *= alpha;
+                    s[4 * g + 2 * i] = ex2_approx(__fmaf_rn(s[4 * g + 2 * i], p.scale_log2e, nm));
+                    s[4 * g + 2 * i + 1] = ex2_approx(__fmaf_rn(s[4 * g + 2 * i + 1], p.scale_log2e, nm));
+                    ls += s[4 * g + 2 * i] + s[4 * g + 2 * i + 1];
+                }
+                l[i] = __fmaf_rn(l[i], alpha, ls);
+            }
+        } else {
+            float amax = 0.f;
+#pragma unroll
+            for (int i = 0; i < 32; ++i) amax = fmaxf(amax, fabsf(s[i]));
+            // clamp * log2(e) * tanh(u), u = s * scale / clamp, evaluated as an odd polynomial in the RAW score s with the constants folded
+            // in: s * (k1 + s^2 (k3 + s^2 (k5 + ...))) — degree 5 for |u| <= 0.15 (exact to 1e-7), degree 9 for |u| <= 0.5; tanh.approx
+            // only when a warp's tile leaves that range
+            if (__all_sync(0xffffffffu, amax <= lim5)) {
+#pragma unroll
+                for (int i = 0; i < 32; i += 2) {
+                    const float2 x = make_float2(s[i], s[i + 1]);
+                    const float2 x2 = fmul2(x, x);
+                    float2 q = ffma2(x2, make_float2(k5, k5), make_float2(k3, k3));
+                    q = ffma2(q, x2, make_float2(k1, k1));
+                    const float2 y = fmul2(x, q);
+                    s[i] = ex2_approx(y.x);
+                    s[i + 1] = ex2_approx(y.y);
+                }
+            } else if (__all_sync(0xffffffffu, amax <= lim9)) {
+#pragma unroll
+                for (int i = 0; i < 32; i += 2) {
+                    const float2 x = make_float2(s[i], s[i + 1]);
+                    const float2 x2 = fmul2(x, x);
+                    float2 q = ffma2(x2, make_float2(k9, k9), make_float2(k7, k7));
+                    q = ffma2(q, x2, make_float2(k5, k5));
+                    q = ffma2(q, x2, make_float2(k3, k3));
+                    q = ffma2(q, x2, make_float2(k1, k1));
+                    const float2 y = fmul2(x, q);
+                    s[i] = ex2_approx(y.x);
+                    s[i + 1] = ex2_approx(y.y);
+                }
+            } else {   // mixed tile: the polynomial wherever it is in range, tanh.approx only for the outliers themselves
+#pragma unroll
+                for (int i = 0; i < 32; ++i) {
+                    const float x = s[i], x2 = x * x;
+                    const float yp = x * __fmaf_rn(__fmaf_rn(__fmaf_rn(__fmaf_rn(k9, x2, k7), x2, k5), x2, k3), x2, k1);
+                    const float y = fabsf(x) <= lim9 ? yp : tanh_approx(x * soc) * cl2.x;
+                    s[i] = ex2_approx(y);
+                }
+            }
+            const unsigned int mw0 = mb[2 * j], mw1 = mb[2 * j + 1];   // keys 64 j .. 64 j + 31, 64 j + 32 .. 64 j + 63
+            if ((mw0 & mw1) != 0xffffffffu) {
+#pragma unroll
+                for (int g = 0; g < 8; ++g) {
+                    const unsigned int w = g < 4 ? mw0 : mw1;
+                    const int bit = (8 * g + cq) & 31;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        if (!((w >> bit) & 1u)) s[4 * g + 2 * i] = 0.f;
+                        if (!((w >> (bit + 1)) & 1u)) s[4 * g + 2 * i + 1] = 0.f;
+                    }
+                }
+            }
+#pragma unroll
+            for (int g = 0; g < 8; ++g)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) l[i] += s[4 * g + 2 * i] + s[4 * g + 2 * i + 1];
         }
-#pragma unroll
-        for (int g = 0; g < 8; ++g)
-#pragma unroll
-            for (int i = 0; i < 2; ++i) l[i] += s[4 * g + 2 * i] + s[4 * g + 2 * i + 1];
         if (p.dropout_p > 0.f) {   // the 1/(1-p) factor is applied once, to the normalised output
 #pragma unroll
             for (int g = 0; g < 8; ++g)
@@ -260,7 +308,10 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
             // gate the bf16-rounded output (what the backward pass sees) for consistency
             *reinterpret_cast<uint32_t*>(grow + 8 * g + cq) = pack_bf16(bf16_lo(u) * gt, bf16_hi(u) * gt);
         }
-        if ((lane & 3) == 0) p.lse[(size_t)bh * p.Np + qi] = logf(lt);
+        if ((lane & 3) == 0) {
+            if constexpr (UNCLAMPED) p.lse[(size_t)bh * p.Np + qi] = __fmaf_rn(m[i], p.scale, logf(lt));
+            else p.lse[(size_t)bh * p.Np + qi] = logf(lt);
+        }
     }
 }
 
@@ -270,6 +321,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 //   warpgroups 1, 2         : 64 keys each, per query tile i (all operands from smem, accumulators in registers):
 //                             S^T = K Q_i^T, dP^T = V dO_i^T                 (wgmma m64n64k16, K-major operands)
 //                             recompute softclamp + softmax from the saved LSE, dS^T = P^T (dP^T - delta)(1 - tanh^2) scale
+//                             (unclamped mode: no tanh, dS^T = P^T (dP^T - delta) scale)
 //                             dV += P^T dO_i, dK += dS^T Q_i                 (register A operands, B MN-major)
 //                             dQ_i += dS K_w through a swizzled smem copy of dS^T (A MN-major), flushed with fp32 vector atomics.
 struct AttnBwdTcP {
@@ -282,6 +334,7 @@ struct AttnBwdTcP {
     unsigned int drop_thresh; int drop_stride;
     unsigned long long seed;
     const unsigned long long* seed_dev;   // optional device addend of the seed (CUDA-graph replays)
+    float scale_log2e;              // unclamped mode: scale * log2(e)
 };
 constexpr int QDO_STAGES = 3, TQB = 64;
 
@@ -327,8 +380,9 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnPrepP p) {
     }
 }
 
-// P^T / dS^T of one query tile from the S^T / dP^T fragments (rows = keys kr, kr + 8; columns = queries qt0 + 8 g + cq + {0, 1})
-template <bool POLY, bool DROP>
+// P^T / dS^T of one query tile from the S^T / dP^T fragments (rows = keys kr, kr + 8; columns = queries qt0 + 8 g + cq + {0, 1}).
+// UNCLAMPED: P = 2^(s scale log2 e - lse log2 e), dS = P (dP - delta) scale (POLY is then unused).
+template <bool UNCLAMPED, bool POLY, bool DROP>
 __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float (&s)[32], const float (&dp)[32], int bh, int qt0, int cq,
                                                const bool (&kok)[2], const int (&key)[2], uint32_t seedmix, uint32_t (&ppk)[16], uint32_t (&dpk)[16]) {
     const uint32_t thr32 = drop_thresh32(p.drop_thresh);
@@ -346,13 +400,20 @@ __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float 
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 const int e = 4 * g + 2 * i + c;
-                const float x = s[e] * p.scale_over_clamp;
-                float th;
-                if constexpr (POLY) th = tanh_poly2(make_float2(x, 0.f)).x;
-                else th = fabsf(x) <= TANH_POLY_MAX ? tanh_poly2(make_float2(x, 0.f)).x : tanh_approx(x);   // outliers only
-                float pv = ex2_approx(__fmaf_rn(th, clog, nlse2));
-                pv = (qok && kok[i]) ? pv : 0.f;
-                const float dsc = __fmaf_rn(th * -p.scale, th, p.scale);   // (1 - tanh^2) * scale = d(clamped logit)/d(raw score)
+                float pv, dsc;
+                if constexpr (UNCLAMPED) {
+                    pv = ex2_approx(__fmaf_rn(s[e], p.scale_log2e, nlse2));
+                    pv = (qok && kok[i]) ? pv : 0.f;
+                    dsc = p.scale;
+                } else {
+                    const float x = s[e] * p.scale_over_clamp;
+                    float th;
+                    if constexpr (POLY) th = tanh_poly2(make_float2(x, 0.f)).x;
+                    else th = fabsf(x) <= TANH_POLY_MAX ? tanh_poly2(make_float2(x, 0.f)).x : tanh_approx(x);   // outliers only
+                    pv = ex2_approx(__fmaf_rn(th, clog, nlse2));
+                    pv = (qok && kok[i]) ? pv : 0.f;
+                    dsc = __fmaf_rn(th * -p.scale, th, p.scale);   // (1 - tanh^2) * scale = d(clamped logit)/d(raw score)
+                }
                 float tt, pd;
                 if constexpr (DROP) {
                     const DropWords h = drop_words(seedmix, (uint32_t)((qbase + (unsigned long long)key[i]) >> 1));
@@ -375,6 +436,7 @@ __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float 
     }
 }
 
+template <bool UNCLAMPED>
 __global__ void __launch_bounds__(384, 1)
 attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const __grid_constant__ CUtensorMap tmDO, const AttnBwdTcP p) {
@@ -466,17 +528,22 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(s); fence_regs(dp);
-            float amax = 0.f;
-#pragma unroll
-            for (int e = 0; e < 32; ++e) amax = fmaxf(amax, fabsf(s[e]));
-            const bool small = __all_sync(0xffffffffu, amax * fabsf(p.scale_over_clamp) <= TANH_POLY_MAX);   // same rule as the forward
             const bool drop = p.dropout_p > 0.f;
-            if (small) {
-                if (drop) bwd_score_math<true, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
-                else bwd_score_math<true, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+            if constexpr (UNCLAMPED) {
+                if (drop) bwd_score_math<true, false, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                else bwd_score_math<true, false, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
             } else {
-                if (drop) bwd_score_math<false, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
-                else bwd_score_math<false, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                float amax = 0.f;
+#pragma unroll
+                for (int e = 0; e < 32; ++e) amax = fmaxf(amax, fabsf(s[e]));
+                const bool small = __all_sync(0xffffffffu, amax * fabsf(p.scale_over_clamp) <= TANH_POLY_MAX);   // same rule as the forward
+                if (small) {
+                    if (drop) bwd_score_math<false, true, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                    else bwd_score_math<false, true, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                } else {
+                    if (drop) bwd_score_math<false, false, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                    else bwd_score_math<false, false, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                }
             }
         }
         // dS^T into the warpgroup's swizzled smem tile (row = key, 64 queries = one 128-byte swizzle atom per row)
@@ -584,10 +651,14 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     B200_REQUIRE(a && a->q && a->k && a->v && a->o && a->og && a->lse && a->ws_maskbits, "attn_fwd: null pointer");
     B200_REQUIRE(a->dim_head == 64, "attn_fwd: only dim_head 64 is built (got %d)", a->dim_head);
     B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_fwd: bad shape");
-    B200_REQUIRE(a->softclamp > 0.f, "attn_fwd: softclamp value must be > 0 (the reference always clamps, e2_tts.py:548-551)");
+    if (a->unclamped) {
+        B200_REQUIRE(a->softclamp == 0.f, "attn_fwd: unclamped attention needs softclamp == 0 (got %g)", a->softclamp);
+    } else {
+        B200_REQUIRE(a->softclamp > 0.f, "attn_fwd: softclamp value must be > 0, or set unclamped for attention without the logit soft-clamp");
+    }
     B200_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_fwd: dropout must be in [0,1)");
-    B200_REQUIRE(a->softclamp <= 64.f, "attn_fwd: softclamp %g > 64: the wgmma kernel exponentiates the clamped logits without a running "
-                 "maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
+    B200_REQUIRE(a->softclamp <= 64.f, "attn_fwd: softclamp %g > 64: the clamped wgmma kernel exponentiates the clamped logits without a "
+                 "running maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
     AttnTcP p{};
     p.nkv = (a->Np + TKV - 1) / TKV;
     p.mask_words = p.nkv * 4;
@@ -599,7 +670,12 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     }
     p.gate = a->gate; p.o = (__nv_bfloat16*)a->o; p.og = (__nv_bfloat16*)a->og; p.lse = a->lse;
     p.B = a->B; p.H = a->H; p.Np = a->Np;
-    p.clamp = a->softclamp; p.scale_over_clamp = a->scale / a->softclamp;
+    if (a->unclamped) {
+        p.clamp = 0.f; p.scale_over_clamp = 0.f;
+    } else {
+        p.clamp = a->softclamp; p.scale_over_clamp = a->scale / a->softclamp;
+    }
+    p.scale = a->scale; p.scale_log2e = a->scale * LOG2E_F;
     p.dropout_p = a->dropout_p;
     p.drop_thresh = (unsigned int)(a->dropout_p * 65536.f);
     p.keep_scale = 65536.f / (65536.f - (float)p.drop_thresh);
@@ -609,11 +685,12 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     const long long rows = (long long)a->B * a->H * a->Np;
     if (make_head_map(&tq, a->q, rows) || make_head_map(&tk, a->k, rows, 64) || make_head_map(&tv, a->v, rows, 64)) return -1;
     const int smem = TILE16 + 2 * KV_STAGES * TILE8 + 128 + 1024;   // Q, K/V rings, barriers, alignment slack
-    static DeviceOnce once;
-    cudaError_t e = set_max_smem_once(once, attn_fwd_wgmma_kernel, smem);
+    static DeviceOnce once[2];
+    const auto kern = a->unclamped ? attn_fwd_wgmma_kernel<true> : attn_fwd_wgmma_kernel<false>;
+    cudaError_t e = set_max_smem_once(once[a->unclamped ? 1 : 0], kern, smem);
     B200_REQUIRE(e == cudaSuccess, "attn_fwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     dim3 grid((a->Np + TQ - 1) / TQ, a->H, a->B);
-    attn_fwd_wgmma_kernel<<<grid, 384, smem, st>>>(tq, tk, tv, p);
+    kern<<<grid, 384, smem, st>>>(tq, tk, tv, p);
     return check_launch("attn_fwd_wgmma_kernel");
 }
 
@@ -623,9 +700,12 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
                  "attn_bwd: null pointer");
     B200_REQUIRE(a->dim_head == 64, "attn_bwd: only dim_head 64 is built (got %d)", a->dim_head);
     B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_bwd: bad shape");
-    B200_REQUIRE(a->softclamp > 0.f && a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_bwd: bad softclamp / dropout");
-    B200_REQUIRE(a->softclamp <= 64.f, "attn_bwd: softclamp %g > 64: the wgmma kernel exponentiates the clamped logits without a running "
-                 "maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
+    if (a->unclamped) {
+        B200_REQUIRE(a->softclamp == 0.f, "attn_bwd: unclamped attention needs softclamp == 0 (got %g)", a->softclamp);
+    }
+    B200_REQUIRE((a->unclamped || a->softclamp > 0.f) && a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_bwd: bad softclamp / dropout");
+    B200_REQUIRE(a->softclamp <= 64.f, "attn_bwd: softclamp %g > 64: the clamped wgmma kernel exponentiates the clamped logits without a "
+                 "running maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
     const AttnPrepP pp{a->gate, (const __nv_bfloat16*)a->o, a->B, a->H, a->Np, (const __nv_bfloat16*)a->d_og, a->d_gate,
                        (__nv_bfloat16*)a->ws_dO, a->ws_delta};
     const long long prep_threads = (long long)a->B * a->H * a->Np * 8;
@@ -646,7 +726,12 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     p.lse = a->lse; p.delta = a->ws_delta; p.dq_acc = reinterpret_cast<float*>(a->dq);
     p.dk = (__nv_bfloat16*)a->dk; p.dv = (__nv_bfloat16*)a->dv;
     p.B = a->B; p.H = a->H; p.Np = a->Np;
-    p.scale = a->scale; p.clamp = a->softclamp; p.scale_over_clamp = a->scale / a->softclamp;
+    p.scale = a->scale; p.scale_log2e = a->scale * LOG2E_F;
+    if (a->unclamped) {
+        p.clamp = 0.f; p.scale_over_clamp = 0.f;
+    } else {
+        p.clamp = a->softclamp; p.scale_over_clamp = a->scale / a->softclamp;
+    }
     p.dropout_p = a->dropout_p;
     p.drop_thresh = (unsigned int)(a->dropout_p * 65536.f);
     p.keep_scale = 65536.f / (65536.f - (float)p.drop_thresh);
@@ -656,10 +741,11 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     const long long rows = (long long)a->B * a->H * a->Np;
     if (make_head_map(&tq, a->q, rows, TQB) || make_head_map(&tk, a->k, rows) || make_head_map(&tv, a->v, rows) || make_head_map(&tdo, a->ws_dO, rows, TQB)) return -1;
     const int smem = 2 * TILE16 + 2 * QDO_STAGES * TILE8 + 2 * TILE8 + 128 + 1024;   // K, V, Q/dO rings, dS^T tiles, barriers, slack
-    static DeviceOnce once;
-    cudaError_t e2 = set_max_smem_once(once, attn_bwd_wgmma_kernel, smem);
+    static DeviceOnce once[2];
+    const auto kern = a->unclamped ? attn_bwd_wgmma_kernel<true> : attn_bwd_wgmma_kernel<false>;
+    cudaError_t e2 = set_max_smem_once(once[a->unclamped ? 1 : 0], kern, smem);
     B200_REQUIRE(e2 == cudaSuccess, "attn_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
     dim3 grid((a->Np + TKV - 1) / TKV, a->H, a->B);
-    attn_bwd_wgmma_kernel<<<grid, 384, smem, st>>>(tq, tk, tv, tdo, p);
+    kern<<<grid, 384, smem, st>>>(tq, tk, tv, tdo, p);
     return check_launch("attn_bwd_wgmma_kernel");
 }

@@ -209,8 +209,8 @@ __global__ void rotary_table_kernel(float* cs, float* sn, int Np, int half) {
 }
 
 // ------------------------------------------------------------------------------------------------ qkv post
-// qkvg [T, ld] = [q(I) | k(I) | v(I) | gate(h) | mix(h)] (raw GEMM output). Produces rotated q,k and the
-// value-residual-mixed v in [B,H,Np,64] (A.3, A.4 steps 1-3), plus sigmoid(head gate) [T,H] fp32.
+// qkvg [T, ld] = [q(I) | k(I) | v(I) | gate(h) | mix(h)] (raw GEMM output), or [q | k | v | mix(h)] without the head gate
+// (no_gate). Produces rotated q,k and the value-residual-mixed v in [B,H,Np,64] (A.3, A.4 steps 1-3), plus sigmoid(head gate) [T,H] fp32.
 struct QkvP {
     const __nv_bfloat16* qkvg; int ld;
     const float *gate_b, *mix_b, *cs, *sn;
@@ -223,6 +223,7 @@ struct QkvP {
     const float* d_gate;
     __nv_bfloat16 *d_qkvg, *d_vfirst;
     int dq_fp32;
+    int no_gate;
 };
 __global__ void __launch_bounds__(256) qkv_post_fwd_kernel(const QkvP p) {
     const long long total = (long long)p.B * p.Np * p.H * 8;
@@ -248,14 +249,14 @@ __global__ void __launch_bounds__(256) qkv_post_fwd_kernel(const QkvP p) {
         *reinterpret_cast<uint4*>(p.k + dst) = pack8(y);
         unpack8(*reinterpret_cast<const uint4*>(row + 2 * I + hh * 64 + c * 8), x);
         if (p.v_first) {
-            const float mix = sigmoidf_(__bfloat162float(row[3 * I + p.H + hh]) + p.mix_b[hh]);
+            const float mix = sigmoidf_(__bfloat162float(row[3 * I + (p.no_gate ? 0 : p.H) + hh]) + p.mix_b[hh]);
             float vf[8];
             unpack8(*reinterpret_cast<const uint4*>(p.v_first + dst), vf);
 #pragma unroll
             for (int j = 0; j < 8; ++j) x[j] = x[j] * mix + vf[j] * (1.f - mix);
         }
         *reinterpret_cast<uint4*>(p.v + dst) = pack8(x);
-        if (c == 0) p.gate[(size_t)tok * p.H + hh] = sigmoidf_(__bfloat162float(row[3 * I + hh]) + p.gate_b[hh]);
+        if (c == 0 && !p.no_gate) p.gate[(size_t)tok * p.H + hh] = sigmoidf_(__bfloat162float(row[3 * I + hh]) + p.gate_b[hh]);
     }
 }
 __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
@@ -300,7 +301,7 @@ __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
             for (int j = 0; j < 8; ++j) x[j] += xe[j];
         }
         if (p.v_first) {
-            mix = sigmoidf_(__bfloat162float(row[3 * I + p.H + hh]) + p.mix_b[hh]);
+            mix = sigmoidf_(__bfloat162float(row[3 * I + (p.no_gate ? 0 : p.H) + hh]) + p.mix_b[hh]);
             float vr[8], vf[8], o[8];
             unpack8(*reinterpret_cast<const uint4*>(row + 2 * I + hh * 64 + c * 8), vr);
             unpack8(*reinterpret_cast<const uint4*>(p.v_first + src), vf);
@@ -315,12 +316,15 @@ __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
     dmix += __shfl_xor_sync(0xffffffffu, dmix, 4);
     if (ok && c == 0) {
         __nv_bfloat16* drow = p.d_qkvg + (size_t)tok * p.ld;
-        const float g = p.gate[(size_t)tok * p.H + hh];
-        drow[3 * I + hh] = __float2bfloat16(p.d_gate[(size_t)tok * p.H + hh] * g * (1.f - g));
-        if (p.v_first) drow[3 * I + p.H + hh] = __float2bfloat16(dmix * mix * (1.f - mix));
+        if (!p.no_gate) {
+            const float g = p.gate[(size_t)tok * p.H + hh];
+            drow[3 * I + hh] = __float2bfloat16(p.d_gate[(size_t)tok * p.H + hh] * g * (1.f - g));
+        }
+        const int mix_col = 3 * I + (p.no_gate ? 0 : p.H);
+        if (p.v_first) drow[mix_col + hh] = __float2bfloat16(dmix * mix * (1.f - mix));
         // zero the pad columns (ld may exceed 3I + 2H) so that dW / colsum of the packed matrix stay clean
         if (hh == 0) {
-            const int used = 3 * I + (p.v_first ? 2 : 1) * p.H;
+            const int used = mix_col + (p.v_first ? p.H : 0);
             for (int j = used; j < p.ld; ++j) drow[j] = __float2bfloat16(0.f);
         }
     }
@@ -760,12 +764,13 @@ extern "C" int b200_rotary_table(float* cos_out, float* sin_out, int32_t Np, int
 }
 
 static int fill_qkv(QkvP& p, const b200_qkv_post_args* a) {
-    B200_REQUIRE(a && a->qkvg && a->gate_bias && a->rot_cos && a->rot_sin && a->gate, "qkv_post: null pointer");
+    B200_REQUIRE(a && a->qkvg && a->rot_cos && a->rot_sin && (a->no_gate || (a->gate_bias && a->gate)), "qkv_post: null pointer");
     B200_REQUIRE(a->dim_head == 64, "qkv_post: only dim_head 64 is built");
-    B200_REQUIRE(a->ld % 8 == 0 && a->ld >= 3 * a->H * 64 + (a->v_first ? 2 : 1) * a->H, "qkv_post: bad row pitch %d", a->ld);
+    B200_REQUIRE(a->ld % 8 == 0 && a->ld >= 3 * a->H * 64 + ((a->no_gate ? 0 : 1) + (a->v_first ? 1 : 0)) * a->H, "qkv_post: bad row pitch %d", a->ld);
     B200_REQUIRE(!a->v_first || a->mix_bias, "qkv_post: value residual needs the mix bias");
     p.qkvg = (const __nv_bfloat16*)a->qkvg; p.ld = a->ld; p.gate_b = a->gate_bias; p.mix_b = a->mix_bias; p.cs = a->rot_cos; p.sn = a->rot_sin;
     p.v_first = (const __nv_bfloat16*)a->v_first; p.gate = a->gate; p.B = a->B; p.H = a->H; p.Np = a->Np;
+    p.no_gate = a->no_gate;
     return 0;
 }
 extern "C" int b200_qkv_post_fwd(const b200_qkv_post_args* a, b200_stream_t stream) {
@@ -779,7 +784,7 @@ extern "C" int b200_qkv_post_fwd(const b200_qkv_post_args* a, b200_stream_t stre
 extern "C" int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stream) {
     QkvP p{};
     if (fill_qkv(p, a)) return -1;
-    B200_REQUIRE(a->dq && a->dk && a->dv && a->d_gate && a->d_qkvg && (!a->v_first || a->d_vfirst), "qkv_post_bwd: null pointer");
+    B200_REQUIRE(a->dq && a->dk && a->dv && (a->no_gate || a->d_gate) && a->d_qkvg && (!a->v_first || a->d_vfirst), "qkv_post_bwd: null pointer");
     p.dq = (const __nv_bfloat16*)a->dq; p.dk = (const __nv_bfloat16*)a->dk; p.dv = (const __nv_bfloat16*)a->dv; p.d_gate = a->d_gate;
     p.d_qkvg = (__nv_bfloat16*)a->d_qkvg; p.d_vfirst = (__nv_bfloat16*)a->d_vfirst; p.dq_fp32 = a->dq_fp32; p.dv_extra = (const __nv_bfloat16*)a->dv_extra;
     const long long total = (long long)a->B * a->Np * a->H * 8;

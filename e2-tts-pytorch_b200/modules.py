@@ -27,6 +27,9 @@ E2TTSReturn = namedtuple('E2TTS', ['loss', 'cond', 'pred_flow', 'pred_data', 'lo
 
 BF16, F32 = torch.bfloat16, torch.float32
 SOFTCLAMP = 50.0  # x-transformers logit_softclamp_value default (A.4)
+SOFTCLAMP_MAX = 64.0  # largest clamp the clamped attention kernels take (include/b200_e2tts.h)
+# x-transformers Attention keywords the kernels implement, with x-transformers' own defaults for a missing key
+ATTN_KWARGS_DEFAULTS = dict(gate_value_heads=False, softclamp_logits=False, logit_softclamp_value=50.)
 # text sub-blocks of layer i+1 overlap the audio sub-blocks of layer i on a second CUDA stream (Transformer._run_layers);
 # B200_TWO_STREAM=0 serialises them on the current stream (developer A/B switch)
 import os as _os
@@ -135,16 +138,18 @@ class DepthwiseConv(Module):  # e2_tts.py:295-328
 
 
 class Attention(Module):  # A.4
-    def __init__(self, dim, heads, dim_head, learned_value_residual_mix):
+    def __init__(self, dim, heads, dim_head, learned_value_residual_mix, gate_value_heads=True):
         super().__init__()
         inner = heads * dim_head
         self.heads = heads
         self.to_q = nn.Linear(dim, inner, bias=False)
         self.to_k = nn.Linear(dim, inner, bias=False)
         self.to_v = nn.Linear(dim, inner, bias=False)
-        self.to_v_head_gate = nn.Linear(dim, heads)
-        nn.init.constant_(self.to_v_head_gate.weight, 0)
-        nn.init.constant_(self.to_v_head_gate.bias, 10)
+        self.to_v_head_gate = None
+        if gate_value_heads:
+            self.to_v_head_gate = nn.Linear(dim, heads)
+            nn.init.constant_(self.to_v_head_gate.weight, 0)
+            nn.init.constant_(self.to_v_head_gate.bias, 10)
         self.to_value_residual_mix = nn.Sequential(nn.Linear(dim, heads), nn.Sigmoid()) if learned_value_residual_mix else None
         self.to_out = nn.Linear(inner, dim, bias=False)
 
@@ -367,6 +372,23 @@ class LinearFourierEmbed(Module):
         self.split_dims = (dim_fourier, dim_rest)
 
 
+def _parse_attn_kwargs(attn_kwargs):
+    """x-transformers Attention keywords (e2_tts.py:548-551, passed to both the audio and the text attention) -> (gate_value_heads,
+    softclamp or None). A missing key takes x-transformers' default, so dict() is attention without head gate and without clamp."""
+    unknown = sorted(set(attn_kwargs) - set(ATTN_KWARGS_DEFAULTS))
+    if unknown:
+        _unsupported(f'attn_kwargs[{unknown[0]!r}]', attn_kwargs[unknown[0]], 'e2_tts.py:548-551')
+    kw = {**ATTN_KWARGS_DEFAULTS, **attn_kwargs}
+    if not kw['softclamp_logits']:
+        return bool(kw['gate_value_heads']), None
+    clamp = float(kw['logit_softclamp_value'])
+    if not 0. < clamp <= SOFTCLAMP_MAX:
+        raise NotImplementedError(
+            f'attn_kwargs logit_softclamp_value={clamp!r}: the clamped attention kernels take a clamp in (0, {SOFTCLAMP_MAX:g}], because they '
+            f'exponentiate the clamped logits without a running maximum; use softclamp_logits=False for attention without the clamp')
+    return bool(kw['gate_value_heads']), clamp
+
+
 class Transformer(_PackOwner):
     """Multistream flow-matching backbone — constructor and forward signature of the reference's Transformer
     (e2_tts.py:518-952). Non-default research switches raise (no kernels, no fallback)."""
@@ -385,8 +407,7 @@ class Transformer(_PackOwner):
             _unsupported('has_freq_axis', has_freq_axis, 'e2_tts.py:533')
         if attn_laser:
             _unsupported('attn_laser', attn_laser, 'e2_tts.py:543')
-        if dict(attn_kwargs) != dict(gate_value_heads=True, softclamp_logits=True):
-            _unsupported('attn_kwargs', attn_kwargs, 'e2_tts.py:548-551')
+        gate_value_heads, self.softclamp = _parse_attn_kwargs(attn_kwargs)
         if dict(ff_kwargs):
             _unsupported('ff_kwargs', ff_kwargs, 'e2_tts.py:552')
         if num_residual_streams != 4:
@@ -431,7 +452,7 @@ class Transformer(_PackOwner):
                 nn.Linear(dim * 2, dim, bias=False) if later_half else None,
                 DepthwiseConv(dim, kernel_size=kernel_size),
                 norm_klass(dim),
-                Attention(dim, heads, dim_head, not first),
+                Attention(dim, heads, dim_head, not first, gate_value_heads),
                 LinearFourierEmbed(dim, p=attn_fourier_embed_input_frac) if attn_fourier_embed_input else nn.Identity(),   # :639
                 post_klass(),
                 norm_klass(dim),
@@ -445,7 +466,7 @@ class Transformer(_PackOwner):
                 text = ModuleList([
                     DepthwiseConv(dim_text, kernel_size=kernel_size),
                     RMSNorm(dim_text),
-                    Attention(dim_text, text_heads, text_dim_head, not first),
+                    Attention(dim_text, text_heads, text_dim_head, not first, gate_value_heads),
                     RMSNorm(dim_text),
                     FeedForward(dim_text, text_ff_mult, dropout),
                     TextAudioCrossCondition(dim, dim_text, cond_audio_to_text=ind != text_depth - 1),
@@ -477,12 +498,14 @@ class Transformer(_PackOwner):
                 attn = mods[3] if pre == 'a' else mods[2]
                 ff = mods[7] if pre == 'a' else mods[4]
                 has_mix = attn.to_value_residual_mix is not None
-                qkv = e(3 * I + (2 if has_mix else 1) * H, din)
+                has_gate = attn.to_v_head_gate is not None
+                qkv = e(3 * I + (int(has_gate) + int(has_mix)) * H, din)   # rows [q | k | v | gate | mix], gate and mix optional
                 for j, lin in enumerate((attn.to_q, attn.to_k, attn.to_v)):
                     pack.add(lin.weight, qkv, row_off=j * I)
-                pack.add(attn.to_v_head_gate.weight, qkv, row_off=3 * I)
+                if has_gate:
+                    pack.add(attn.to_v_head_gate.weight, qkv, row_off=3 * I)
                 if has_mix:
-                    pack.add(attn.to_value_residual_mix[0].weight, qkv, row_off=3 * I + H)
+                    pack.add(attn.to_value_residual_mix[0].weight, qkv, row_off=3 * I + (H if has_gate else 0))
                 out_w = e(din, I)
                 pack.add(attn.to_out.weight, out_w)
                 inner = ff.ff[2].weight.shape[1]
@@ -582,11 +605,11 @@ class Transformer(_PackOwner):
             br, rest, beta = width(res, hcm, gain, mode)
             if lfe is not None:   # attn_input_fourier_embed (:909): between the attention norm (fused into the width kernel) and the attention
                 br = ops.FourierLinear.apply(br, lfe.linear.weight, pk['lfe'], *lfe.split_dims)
-            mix = attn.to_value_residual_mix
-            og, v = ops.Attention.apply(br, attn.to_q.weight, attn.to_k.weight, attn.to_v.weight, attn.to_v_head_gate.weight,
-                                        attn.to_v_head_gate.bias, mix[0].weight if mix is not None else None,
+            mix, gate = attn.to_value_residual_mix, attn.to_v_head_gate
+            og, v = ops.Attention.apply(br, attn.to_q.weight, attn.to_k.weight, attn.to_v.weight, gate.weight if gate is not None else None,
+                                        gate.bias if gate is not None else None, mix[0].weight if mix is not None else None,
                                         mix[0].bias if mix is not None else None, vf if mix is not None else None,
-                                        pk['qkv'], cs, sn, mask_u8, B, Np, H, p_drop, next_seed(), SOFTCLAMP, self._seed_dev, mbits)
+                                        pk['qkv'], cs, sn, mask_u8, B, Np, H, p_drop, next_seed(), self.softclamp, self._seed_dev, mbits)
             y = ops.OutProj.apply(og, attn.to_out.weight, pk['out'], colscale, mask_u8, B, Np)
             return depth(rest, y, beta), (v if vf is None else vf)
 

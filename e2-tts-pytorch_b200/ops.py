@@ -267,40 +267,48 @@ def _maskbits_ws(B, Np, device):
     return torch.empty(((Np + 127) // 128) * 4 * B, device=device, dtype=torch.int32)   # b200_attn_workspace_bytes(B, Np)
 
 
+def _clamp_args(softclamp):
+    """softclamp None: attention without the logit soft-clamp (the running-maximum kernels)"""
+    return dict(softclamp=0.0, unclamped=1) if softclamp is None else dict(softclamp=softclamp, unclamped=0)
+
+
 def _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits=None):
     """b200_attn_fwd on q, k, v bf16 [B, H, Np, 64] -> og (gated, head-merged bf16 [B*Np, H*64]), o (bf16 [B, H, Np, 64]), lse (fp32
-    [B, H, Np]). `maskbits` is attn_maskbits(mask), shared by every layer of a step; without it the call builds its own."""
+    [B, H, Np]). `maskbits` is attn_maskbits(mask), shared by every layer of a step; without it the call builds its own. `gate` may be
+    None (no head gate), `softclamp` None (no logit soft-clamp)."""
     B, H, Np, dh = q.shape
     o = torch.empty_like(q)
     og = torch.empty((B * Np, H * dh), device=q.device, dtype=BF16)
     lse = torch.empty((B, H, Np), device=q.device, dtype=F32)
     a = lib.make_args('b200_attn_fwd_args', q=q, k=k, v=v, keymask=mask, gate=gate, o=o, og=og, lse=lse, B=B, H=H, Np=Np, dim_head=dh,
-                      scale=dh ** -0.5, softclamp=softclamp, dropout_p=dropout_p, seed=seed,
+                      scale=dh ** -0.5, dropout_p=dropout_p, seed=seed,
                       ws_maskbits=maskbits if maskbits is not None else _maskbits_ws(B, Np, q.device), seed_dev=seed_dev,
-                      maskbits_ready=int(maskbits is not None))
+                      maskbits_ready=int(maskbits is not None), **_clamp_args(softclamp))
     lib.call('b200_attn_fwd', a, _stream())
     return og, o, lse
 
 
 def _attn_core_bwd(d_og, q, k, v, o, lse, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits=None):
-    """b200_attn_bwd -> dq (fp32: accumulated across key tiles with atomics), dk, dv (bf16 [B, H, Np, 64]), d_gate (fp32 [B*Np, H])."""
+    """b200_attn_bwd -> dq (fp32: accumulated across key tiles with atomics), dk, dv (bf16 [B, H, Np, 64]), d_gate (fp32 [B*Np, H],
+    None without a gate)."""
     B, H, Np, dh = q.shape
     dq = torch.empty(q.shape, device=q.device, dtype=F32)
     dk, dv, ws_dO = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
     ws_delta = torch.empty_like(lse)
-    d_gate = torch.empty_like(gate)
+    d_gate = torch.empty_like(gate) if gate is not None else None
     a = lib.make_args('b200_attn_bwd_args', q=q, k=k, v=v, o=o, d_og=_c(d_og), keymask=mask, gate=gate, lse=lse, ws_dO=ws_dO,
                       ws_delta=ws_delta, d_gate=d_gate, dq=dq, dk=dk, dv=dv, B=B, H=H, Np=Np, dim_head=dh, scale=dh ** -0.5,
-                      softclamp=softclamp, dropout_p=dropout_p, seed=seed,
+                      dropout_p=dropout_p, seed=seed,
                       ws_maskbits=maskbits if maskbits is not None else _maskbits_ws(B, Np, q.device), seed_dev=seed_dev,
-                      maskbits_ready=int(maskbits is not None))
+                      maskbits_ready=int(maskbits is not None), **_clamp_args(softclamp))
     lib.call('b200_attn_bwd', a, _stream())
     return dq, dk, dv, d_gate
 
 
 class AttnCore(Function):
     """Softclamped, key-masked, head-gated flash attention (A.4 steps 4-5) on given q, k, v. Returns the gated, head-merged output.
-    The model runs the same kernels inside Attention; this node serves the attention-core tests and benchmarks."""
+    The model runs the same kernels inside Attention; this node serves the attention-core tests and benchmarks. gate None: no head
+    gate; softclamp None: no logit soft-clamp."""
 
     @staticmethod
     def forward(ctx, q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev):
@@ -321,7 +329,8 @@ class Attention(Function):
     """Fused attention stage: ONE GEMM for to_q/to_k/to_v (+ head-gate and value-residual-mix logits), rotary + value
     residual + gate post-processing, wgmma flash attention (softclamp, key mask, dropout, head gate). Returns the gated
     head-merged output (input of to_out) and this layer's values (the first layer's feed every later layer, e2_tts.py:878,916).
-    One autograd node: q/k/v never enter the graph, and dq stays fp32 from the attention backward into the rotary inverse."""
+    One autograd node: q/k/v never enter the graph, and dq stays fp32 from the attention backward into the rotary inverse.
+    wg, bg None: no head gate (x-transformers gate_value_heads=False; packed rows [q|k|v|mix]); softclamp None: no logit soft-clamp."""
 
     @staticmethod
     def forward(ctx, xn, wq, wk, wv, wg, bg, wm, bm, v_first, wpack, cs, sn, mask, B, Np, H, dropout_p, seed, softclamp, seed_dev, maskbits=None):
@@ -330,19 +339,20 @@ class Attention(Function):
         I = H * 64
         dev = xn.device
         has_mix = wm is not None
-        ncat = 3 * I + (2 if has_mix else 1) * H
+        has_gate = wg is not None
+        ncat = 3 * I + (int(has_gate) + int(has_mix)) * H
         ld = (ncat + 7) // 8 * 8
         qkvg = gemm(xn, wpack, T, ncat, Din, ldd=ld)
         q = torch.empty((B, H, Np, 64), device=dev, dtype=BF16)
         k, v = torch.empty_like(q), torch.empty_like(q)
-        gate = torch.empty((T, H), device=dev, dtype=F32)
+        gate = torch.empty((T, H), device=dev, dtype=F32) if has_gate else None
         a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
-                          q=q, k=k, v=v, gate=gate, B=B, H=H, Np=Np, dim_head=64)
+                          q=q, k=k, v=v, gate=gate, B=B, H=H, Np=Np, dim_head=64, no_gate=int(not has_gate))
         lib.call('b200_qkv_post_fwd', a, _stream())
         og, o, lse = _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits)
         ctx.maskbits = maskbits
         ctx.save_for_backward(xn, qkvg, gate, v_first, wpack, cs, sn, bg, bm, q, k, v, o, lse, mask)
-        ctx.meta = (B, Np, H, ncat, ld, has_mix, dropout_p, seed, softclamp, seed_dev)
+        ctx.meta = (B, Np, H, ncat, ld, has_mix, dropout_p, seed, softclamp, seed_dev, has_gate)
         return og, v
 
     @staticmethod
@@ -351,7 +361,7 @@ class Attention(Function):
         xn, qkvg, gate, v_first, wpack, cs, sn, bg, bm, q, k, v, o, lse, mask = ctx.saved_tensors
         if d_og is None:   # (only the values were used: not a case the model produces, kept for completeness)
             d_og = torch.zeros((xn.shape[0], ctx.meta[2] * 64), device=xn.device, dtype=BF16)
-        B, Np, H, ncat, ld, has_mix, dropout_p, seed, softclamp, seed_dev = ctx.meta
+        B, Np, H, ncat, ld, has_mix, dropout_p, seed, softclamp, seed_dev, has_gate = ctx.meta
         T, Din = xn.shape
         I = H * 64
         dev = xn.device
@@ -360,13 +370,15 @@ class Attention(Function):
         d_vfirst = torch.empty_like(v_first) if v_first is not None else None
         a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
                           gate=gate, dq=dq, dk=dk, dv=dv, dv_extra=_c(d_v_extra), d_gate=d_gate, d_qkvg=d_qkvg, d_vfirst=d_vfirst,
-                          B=B, H=H, Np=Np, dim_head=64, dq_fp32=1)
+                          B=B, H=H, Np=Np, dim_head=64, dq_fp32=1, no_gate=int(not has_gate))
         lib.call('b200_qkv_post_bwd', a, _stream())
         dx = gemm(d_qkvg, wpack, T, Din, ncat, lda=ld, ldb=Din, b_mn=True)
         dW = grad_weight(d_qkvg, xn, T, ncat, Din, ldy=ld)
-        db = colsum(d_qkvg[:, 3 * I:], T, ld - 3 * I, ld)   # only the head-gate / value-residual-mix logits have biases
-        return (dx, dW[:I], dW[I:2 * I], dW[2 * I:3 * I], dW[3 * I:3 * I + H], db[:H],
-                dW[3 * I + H:3 * I + 2 * H] if has_mix else None, db[H:2 * H] if has_mix else None,
+        # only the head-gate / value-residual-mix logits have biases (none at all: the first layer without a head gate)
+        db = colsum(d_qkvg[:, 3 * I:], T, ld - 3 * I, ld) if ld > 3 * I else None
+        m0 = H if has_gate else 0                           # first mix column past 3 I
+        return (dx, dW[:I], dW[I:2 * I], dW[2 * I:3 * I], dW[3 * I:3 * I + H] if has_gate else None, db[:H] if has_gate else None,
+                dW[3 * I + m0:3 * I + m0 + H] if has_mix else None, db[m0:m0 + H] if has_mix else None,
                 d_vfirst, None, None, None, None, None, None, None, None, None, None, None, None)
 
 

@@ -85,6 +85,10 @@ int b200_seed_advance(uint64_t* seed_dev, b200_stream_t stream);   /* *seed_dev 
  * NULL; gate: fp32 [B*Np, H] = sigmoid(to_v_head_gate(x)) or NULL; og: bf16 [B*Np, H*64] gated, merged
  * heads (the input of to_out); lse: fp32 [B,H,Np] (natural log of the softmax denominator of the CLAMPED
  * logits). Dropout on P uses a counter-based hash of (seed, b,h,i,j) that backward recomputes.
+ * Logits: softclamp * tanh(scale q.k / softclamp) with softclamp in (0, 64] (x-transformers softclamp_logits), or, when
+ * `unclamped` != 0, plain scale q.k (an online softmax with a running row maximum; softclamp must then be 0, and lse is the
+ * log-sum-exp of the unclamped logits). A query row whose keys are all masked gives o = og = 0, lse = -inf and zero gradients in
+ * both modes (the model never produces one: its register keys are always valid).
  */
 typedef struct {
     const void *q, *k, *v;
@@ -99,11 +103,13 @@ typedef struct {
     const uint64_t* seed_dev;   /* optional device addend of `seed` (dropout seeds, above) */
     int32_t maskbits_ready;     /* != 0: ws_maskbits already holds b200_attn_maskbits(keymask) — every layer of a forward/backward shares
                                    one key mask, so the model builds the bitmask once instead of once per attention call */
+    int32_t unclamped;          /* != 0: no logit soft-clamp (softclamp must be 0); 0: clamped by softclamp */
 } b200_attn_fwd_args;
 size_t b200_attn_workspace_bytes(int32_t B, int32_t Np);
 /* key-validity bitmask of `keymask` (u8 [B,Np], NULL = all valid) into ws_maskbits, in the layout the wgmma kernels read */
 int b200_attn_maskbits(const uint8_t* keymask, void* ws_maskbits, int32_t B, int32_t Np, b200_stream_t stream);
-/* wgmma / TMA kernel; softclamp must be in (0, 64] (the softmax is exponentiated without a running maximum) */
+/* wgmma / TMA kernel; clamped: softclamp must be in (0, 64] (the clamped softmax is exponentiated without a running maximum);
+ * unclamped: softclamp must be 0 */
 int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream);
 
 /* backward: d_og bf16 [B*Np, H*64] -> dk,dv bf16 [B,H,Np,64], dq FP32 [B,H,Np,64] (accumulated with atomics across key
@@ -122,8 +128,9 @@ typedef struct {
     void* ws_maskbits;
     const uint64_t* seed_dev;   /* optional device addend of `seed` (must be the forward's) */
     int32_t maskbits_ready;     /* as in b200_attn_fwd_args */
+    int32_t unclamped;          /* as in b200_attn_fwd_args (must be the forward's) */
 } b200_attn_bwd_args;
-int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream);         /* wgmma / TMA kernel, dq fp32; softclamp as in fwd */
+int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream);   /* wgmma / TMA kernel, dq fp32; softclamp, unclamped as in fwd */
 
 /* ------------------------------------------------------------------------------------------------
  * Hyper-connections (A.5; e2_tts.py:607, 673-678, 709-713, 870-882, 900-939), S = 4 residual streams held
@@ -217,7 +224,9 @@ int b200_rotary_table(float* cos_out, float* sin_out, int32_t Np, int32_t dim_he
 
 /* Post-processing of the fused [q|k|v|gate|mix] projection (A.4 steps 1-3, 5): interleaved-pair rotary on
  * q,k; v = lerp(v_first, v, sigmoid(mix)) when v_first != NULL; gate = sigmoid(gate_logit + bias) fp32 [T,H];
- * q,k,v written as [B,H,Np,64]. bwd inverts all of it into d_qkvg (same packed layout) and d_vfirst. */
+ * q,k,v written as [B,H,Np,64]. bwd inverts all of it into d_qkvg (same packed layout) and d_vfirst.
+ * no_gate != 0 (x-transformers Attention without gate_value_heads): the layout is [q|k|v|mix], the mix logits at column 3I;
+ * gate, gate_bias and d_gate are then neither read nor written (may be NULL). */
 typedef struct {
     const void* qkvg; int32_t ld;
     const float *gate_bias, *mix_bias, *rot_cos, *rot_sin;
@@ -228,6 +237,7 @@ typedef struct {
     void *d_qkvg, *d_vfirst;
     int32_t B, H, Np, dim_head;
     int32_t dq_fp32;   /* bwd: dq is fp32 (wgmma attention backward) instead of bf16 */
+    int32_t no_gate;   /* != 0: no head-gate column (layout above) */
 } b200_qkv_post_args;
 int b200_qkv_post_fwd(const b200_qkv_post_args* a, b200_stream_t stream);
 int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stream);
