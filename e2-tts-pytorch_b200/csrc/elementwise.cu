@@ -460,9 +460,105 @@ struct FnP {
     const __nv_bfloat16* xres; const float* g; __nv_bfloat16* y;
     int B, N, R, D, S;
     const __nv_bfloat16* dy; __nv_bfloat16* d_xres; float* g_g;
+    int rpb, rows_per_block; const float* gains; float* d_gains; const __nv_bfloat16* d_res;   // branch-norm mode (BRANCH = true) only
 };
+
+// Branch-norm mode: y[r] = F.normalize(x[r]) * sqrt(D) * gain, x bf16 [rows, D] (S = 1, R = 0). Block (x, b) owns rows
+// [x * rows_per_block, (x + 1) * rows_per_block) of batch b, so the per-batch gain and its gradient are one row of [B, D] per block
+// (shared-memory sums, one atomic per column and block); one warp per row. gain = gains[b] or g.
 template <int VPT>
+__device__ __forceinline__ void branch_norm_fwd(const FnP& p) {
+    const int lane = threadIdx.x & 31, nchunk = p.D >> 3;
+    const long long base = (long long)blockIdx.y * p.rpb;
+    const float* gain = p.gains ? p.gains + (size_t)blockIdx.y * p.D : p.g;
+    const int r1 = min(p.rpb, ((int)blockIdx.x + 1) * p.rows_per_block);
+    for (int r = (int)blockIdx.x * p.rows_per_block + (threadIdx.x >> 5); r < r1; r += 8) {
+        const size_t row = (size_t)(base + r);
+        float x[VPT][8];
+        float ss = 0.f;
+#pragma unroll
+        for (int v = 0; v < VPT; ++v) {
+            const int c = lane + 32 * v;
+            if (c < nchunk) unpack8(*reinterpret_cast<const uint4*>(p.xres + row * p.D + c * 8), x[v]);
+            else {
+#pragma unroll
+                for (int e = 0; e < 8; ++e) x[v][e] = 0.f;
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) ss += x[v][e] * x[v][e];
+        }
+        const float cn = sqrtf((float)p.D) / fmaxf(sqrtf(warp_sum(ss)), 1e-12f);
+#pragma unroll
+        for (int v = 0; v < VPT; ++v) {
+            const int c = lane + 32 * v;
+            if (c < nchunk) {
+                float o[8];
+#pragma unroll
+                for (int e = 0; e < 8; ++e) o[e] = x[v][e] * cn * __ldg(gain + c * 8 + e);
+                *reinterpret_cast<uint4*>(p.y + row * p.D + c * 8) = pack8(o);
+            }
+        }
+    }
+}
+// dx = cn * (gain dy - x <gain dy, x> / |x|^2) with cn = sqrt(D) / max(|x|, 1e-12) (the second term vanishes where the clamp holds,
+// as in F.normalize's backward); d_gain += dy * x * cn
+template <int VPT>
+__device__ __forceinline__ void branch_norm_bwd(const FnP& p, float* sg) {
+    const int lane = threadIdx.x & 31, nchunk = p.D >> 3;
+    const long long base = (long long)blockIdx.y * p.rpb;
+    const float* gain = p.gains ? p.gains + (size_t)blockIdx.y * p.D : p.g;
+    const int r1 = min(p.rpb, ((int)blockIdx.x + 1) * p.rows_per_block);
+    for (int r = (int)blockIdx.x * p.rows_per_block + (threadIdx.x >> 5); r < r1; r += 8) {
+        const size_t row = (size_t)(base + r);
+        float x[VPT][8], dy[VPT][8];
+        float ss = 0.f, dot = 0.f;
+#pragma unroll
+        for (int v = 0; v < VPT; ++v) {
+            const int c = lane + 32 * v;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) { x[v][e] = 0.f; dy[v][e] = 0.f; }
+            if (c < nchunk) {
+                unpack8(*reinterpret_cast<const uint4*>(p.xres + row * p.D + c * 8), x[v]);
+                unpack8(*reinterpret_cast<const uint4*>(p.dy + row * p.D + c * 8), dy[v]);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                    dy[v][e] *= __ldg(gain + c * 8 + e);   // from here on: gain * dy (the gain gradient divides it back out below)
+                    dot += dy[v][e] * x[v][e];
+                }
+            }
+#pragma unroll
+            for (int e = 0; e < 8; ++e) ss += x[v][e] * x[v][e];
+        }
+        ss = warp_sum(ss);
+        const float nrm = sqrtf(ss);
+        const float cn = sqrtf((float)p.D) / fmaxf(nrm, 1e-12f);
+        dot = warp_sum(dot);
+        const float k = nrm > 1e-12f ? dot / ss : 0.f;
+#pragma unroll
+        for (int v = 0; v < VPT; ++v) {
+            const int c = lane + 32 * v;
+            if (c < nchunk) {
+                float o[8], dyr[8], dr[8];
+                unpack8(*reinterpret_cast<const uint4*>(p.dy + row * p.D + c * 8), dyr);   // L1-resident re-read: the raw dy for the gain
+                if (p.d_res) unpack8(*reinterpret_cast<const uint4*>(p.d_res + row * p.D + c * 8), dr);
+#pragma unroll
+                for (int e = 0; e < 8; ++e) {
+                    atomicAdd(&sg[c * 8 + e], dyr[e] * x[v][e] * cn);
+                    o[e] = cn * (dy[v][e] - x[v][e] * k);
+                    if (p.d_res) o[e] += dr[e];
+                }
+                *reinterpret_cast<uint4*>(p.d_xres + row * p.D + c * 8) = pack8(o);
+            }
+        }
+    }
+}
+
+template <int VPT, bool BRANCH = false>
 __global__ void __launch_bounds__(256) final_norm_fwd_kernel(const FnP p) {
+    if constexpr (BRANCH) {
+        branch_norm_fwd<VPT>(p);
+        return;
+    }
     const int lane = threadIdx.x & 31, nchunk = p.D >> 3;
     const long long ntok = (long long)p.B * p.N;
     for (long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5); row < ntok; row += (long long)gridDim.x * 8) {
@@ -499,11 +595,18 @@ __global__ void __launch_bounds__(256) final_norm_fwd_kernel(const FnP p) {
         }
     }
 }
-template <int VPT>
+template <int VPT, bool BRANCH = false>
 __global__ void __launch_bounds__(256) final_norm_bwd_kernel(const FnP p) {
     extern __shared__ float sg[];  // [D]
     for (int i = threadIdx.x; i < p.D; i += 256) sg[i] = 0.f;
     __syncthreads();
+    if constexpr (BRANCH) {
+        branch_norm_bwd<VPT>(p, sg);
+        __syncthreads();
+        float* out = p.gains ? p.d_gains + (size_t)blockIdx.y * p.D : p.g_g;
+        for (int i = threadIdx.x; i < p.D; i += 256) atomicAdd(out + i, sg[i]);
+        return;
+    }
     const int lane = threadIdx.x & 31, nchunk = p.D >> 3;
     const long long ntok = (long long)p.B * (p.R + p.N);
     const float invD = 1.f / (float)p.D;
@@ -624,10 +727,13 @@ __global__ void __launch_bounds__(256) flow_loss_bwd_kernel(const LossP p) {
 // Forward epilogue was y = mask * cs[b,:] * (x W^T + bias). Given dy and y: dz = dy * mask * cs, d_cs[b,:] += sum_rows dy * y / cs,
 // and (optionally) d_bias[:] += sum_rows dz — the bias gradient rides along so that no separate column-sum pass re-reads dz.
 // Each thread keeps ONE 8-column chunk and marches over rows, four rows (eight 16-byte loads) in flight.
+// RESID: the epilogue also added resid (y = gated + resid): the gated value is read back as y - resid.
+template <bool RESID = false>
 __global__ void __launch_bounds__(256) rowgate_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ y,
                                                            const float* __restrict__ cs, const unsigned char* __restrict__ mask,
                                                            __nv_bfloat16* __restrict__ dz, float* __restrict__ d_cs,
-                                                           float* __restrict__ d_bias, int rows_per_batch, int D, int rows_per_block) {
+                                                           float* __restrict__ d_bias, int rows_per_batch, int D, int rows_per_block,
+                                                           const __nv_bfloat16* __restrict__ resid = nullptr) {
     extern __shared__ float sacc[];  // [D] gate sums, then [D] bias sums
     float* sbias = sacc + D;
     const int b = blockIdx.y;
@@ -665,6 +771,14 @@ __global__ void __launch_bounds__(256) rowgate_bwd_kernel(const __nv_bfloat16* _
                 float g[8], yv[8], o[8];
                 unpack8(ug[k], g);
                 unpack8(uy[k], yv);
+                if constexpr (RESID) {
+                    if (cs) {
+                        float rv[8];
+                        unpack8(__ldg(reinterpret_cast<const uint4*>(resid + row * D + cc * 8)), rv);
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) yv[j] -= rv[j];
+                    }
+                }
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     o[j] = keep[k] ? g[j] * s8[j] : 0.f;
@@ -826,8 +940,40 @@ extern "C" int b200_colsum(const void* X, int64_t T, int32_t ncols, int32_t ld, 
     return check_launch("colsum_kernel");
 }
 
+// branch-norm mode (rows_per_batch > 0): validation shared by fwd / bwd, and the launch shape (block rows of one batch)
+static int check_branch_norm(const b200_final_norm_args* a, FnP& p, dim3& grid) {
+    B200_REQUIRE(a->D % 8 == 0 && a->D <= 1024, "final_norm: D must be a multiple of 8 and <= 1024");
+    B200_REQUIRE(a->S == 1 && a->R == 0, "final_norm: branch-norm mode (rows_per_batch > 0) takes S == 1 and R == 0 (got S=%d, R=%d)", a->S, a->R);
+    B200_REQUIRE(a->B > 0 && a->N > 0, "final_norm: unsupported shape");
+    const long long rows = (long long)a->B * a->N;
+    B200_REQUIRE(rows % a->rows_per_batch == 0 && rows / a->rows_per_batch <= 65535,
+                 "final_norm: B*N (%lld) must be a multiple of rows_per_batch (%d), at most 65535 batches", rows, a->rows_per_batch);
+    B200_REQUIRE(a->gains || a->g, "final_norm: branch-norm mode needs gains or g");
+    // about four blocks per SM over all batches, 8 to 128 rows (a multiple of the 8 warps) per block
+    const long long nb = rows / a->rows_per_batch;
+    long long rb = (rows + 4LL * num_sms() - 1) / (4LL * num_sms());
+    rb = min(128LL, max(8LL, (rb + 7) / 8 * 8));
+    p = FnP{(const __nv_bfloat16*)a->xres, a->g, (__nv_bfloat16*)a->y, a->B, a->N, a->R, a->D, a->S, (const __nv_bfloat16*)a->dy,
+            (__nv_bfloat16*)a->d_xres, a->g_g, a->rows_per_batch, (int)rb, a->gains, a->d_gains, (const __nv_bfloat16*)a->d_res};
+    grid = dim3((unsigned)((a->rows_per_batch + rb - 1) / rb), (unsigned)nb);
+    return 0;
+}
 extern "C" int b200_final_norm_fwd(const b200_final_norm_args* a, b200_stream_t stream) {
-    B200_REQUIRE(a && a->xres && a->g && a->y, "final_norm_fwd: null pointer");
+    B200_REQUIRE(a, "final_norm_fwd: null pointer");
+    B200_REQUIRE(a->rows_per_batch >= 0, "final_norm: rows_per_batch must be >= 0 (got %d)", a->rows_per_batch);
+    if (a->rows_per_batch > 0) {
+        B200_REQUIRE(a->xres && a->y, "final_norm_fwd: null pointer");
+        FnP p;
+        dim3 grid;
+        if (check_branch_norm(a, p, grid)) return -1;
+        cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+        if (a->D <= 256) final_norm_fwd_kernel<1, true><<<grid, 256, 0, st>>>(p);
+        else if (a->D <= 512) final_norm_fwd_kernel<2, true><<<grid, 256, 0, st>>>(p);
+        else final_norm_fwd_kernel<4, true><<<grid, 256, 0, st>>>(p);
+        return check_launch("final_norm_fwd_kernel");
+    }
+    B200_REQUIRE(!a->gains && !a->d_gains, "final_norm: gains / d_gains need rows_per_batch > 0 (branch-norm mode)");
+    B200_REQUIRE(a->xres && a->g && a->y, "final_norm_fwd: null pointer");
     B200_REQUIRE(a->D % 8 == 0 && a->D <= 1024 && a->S >= 1, "final_norm: D must be a multiple of 8 and <= 1024");
     FnP p{(const __nv_bfloat16*)a->xres, a->g, (__nv_bfloat16*)a->y, a->B, a->N, a->R, a->D, a->S, nullptr, nullptr, nullptr};
     const int grid = (int)min(((long long)a->B * a->N + 7) / 8, (long long)num_sms() * 8);
@@ -838,7 +984,23 @@ extern "C" int b200_final_norm_fwd(const b200_final_norm_args* a, b200_stream_t 
     return check_launch("final_norm_fwd_kernel");
 }
 extern "C" int b200_final_norm_bwd(const b200_final_norm_args* a, b200_stream_t stream) {
-    B200_REQUIRE(a && a->xres && a->g && a->dy && a->d_xres && a->g_g, "final_norm_bwd: null pointer");
+    B200_REQUIRE(a, "final_norm_bwd: null pointer");
+    B200_REQUIRE(a->rows_per_batch >= 0, "final_norm: rows_per_batch must be >= 0 (got %d)", a->rows_per_batch);
+    if (a->rows_per_batch > 0) {
+        B200_REQUIRE(a->xres && a->dy && a->d_xres, "final_norm_bwd: null pointer");
+        B200_REQUIRE(a->gains ? a->d_gains != nullptr : a->g_g != nullptr, "final_norm_bwd: gains need d_gains, g needs g_g");
+        FnP p;
+        dim3 grid;
+        if (check_branch_norm(a, p, grid)) return -1;
+        cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+        const size_t smem = (size_t)a->D * 4;
+        if (a->D <= 256) final_norm_bwd_kernel<1, true><<<grid, 256, smem, st>>>(p);
+        else if (a->D <= 512) final_norm_bwd_kernel<2, true><<<grid, 256, smem, st>>>(p);
+        else final_norm_bwd_kernel<4, true><<<grid, 256, smem, st>>>(p);
+        return check_launch("final_norm_bwd_kernel");
+    }
+    B200_REQUIRE(!a->gains && !a->d_gains && !a->d_res, "final_norm: gains / d_gains / d_res need rows_per_batch > 0 (branch-norm mode)");
+    B200_REQUIRE(a->xres && a->g && a->dy && a->d_xres && a->g_g, "final_norm_bwd: null pointer");
     B200_REQUIRE(a->D % 8 == 0 && a->D <= 1024 && a->S >= 1, "final_norm: D must be a multiple of 8 and <= 1024");
     FnP p{(const __nv_bfloat16*)a->xres, a->g, nullptr, a->B, a->N, a->R, a->D, a->S, (const __nv_bfloat16*)a->dy, (__nv_bfloat16*)a->d_xres, a->g_g};
     const int grid = (int)min(((long long)a->B * (a->N + a->R) + 7) / 8, (long long)num_sms() * 4);
@@ -876,6 +1038,18 @@ extern "C" int b200_rowgate_bwd(const void* dy, const void* y, const float* cs, 
     dim3 grid((rows_per_batch + rpb - 1) / rpb, B);
     rowgate_bwd_kernel<<<grid, 256, (size_t)D * 8, reinterpret_cast<cudaStream_t>(stream)>>>(
         (const __nv_bfloat16*)dy, (const __nv_bfloat16*)y, cs, mask, (__nv_bfloat16*)dz, d_cs, d_bias, rows_per_batch, D, rpb);
+    return check_launch("rowgate_bwd_kernel");
+}
+extern "C" int b200_rowgate_resid_bwd(const void* dy, const void* y, const void* resid, const float* cs, const uint8_t* mask, void* dz,
+                                      float* d_cs, float* d_bias, int32_t B, int32_t rows_per_batch, int32_t D, b200_stream_t stream) {
+    B200_REQUIRE(dy && dz && B > 0 && B <= 65535 && rows_per_batch > 0 && D % 8 == 0, "rowgate_bwd: bad arguments");
+    B200_REQUIRE(!cs || (y && d_cs), "rowgate_bwd: gate backward needs y and d_cs");
+    B200_REQUIRE(resid, "rowgate_resid_bwd: null resid");
+    const int rpb = 64;
+    dim3 grid((rows_per_batch + rpb - 1) / rpb, B);
+    rowgate_bwd_kernel<true><<<grid, 256, (size_t)D * 8, reinterpret_cast<cudaStream_t>(stream)>>>(
+        (const __nv_bfloat16*)dy, (const __nv_bfloat16*)y, cs, mask, (__nv_bfloat16*)dz, d_cs, d_bias, rows_per_batch, D, rpb,
+        (const __nv_bfloat16*)resid);
     return check_launch("rowgate_bwd_kernel");
 }
 

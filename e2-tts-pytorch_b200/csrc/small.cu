@@ -264,6 +264,8 @@ __device__ __forceinline__ void conv_rows2(const cf2 (&w)[31], const float (*src
 // and the global loads of tile t+1 (three 16-byte pieces + their validity per thread) are issued before the convolution of tile t, so
 // their latency hides behind the FMA loop instead of stalling every warp of the block.
 constexpr int CV_FWD_TILES = 2;
+// RESID: y = x + (the masked SiLU output), the add unmasked (b200_dwconv_args.residual)
+template <bool RESID = false>
 __global__ void __launch_bounds__(256, 3) dwconv_fwd_kernel(const b200_dwconv_args a) {
     __shared__ __align__(16) float xs[CV_R][CV_TC];
     __shared__ __align__(16) float sw[31][CV_TC];
@@ -324,7 +326,11 @@ __global__ void __launch_bounds__(256, 3) dwconv_fwd_kernel(const b200_dwconv_ar
             if (n < a.Np) {
                 const size_t off = ((size_t)b * a.Np + n) * a.D + ch;
                 const bool ok = sok[r + CV_HALO];
-                const float o0 = ok ? __fdividef(out[j].x, 1.f + __expf(-out[j].x)) : 0.f, o1 = ok ? __fdividef(out[j].y, 1.f + __expf(-out[j].y)) : 0.f;
+                float o0 = ok ? __fdividef(out[j].x, 1.f + __expf(-out[j].x)) : 0.f, o1 = ok ? __fdividef(out[j].y, 1.f + __expf(-out[j].y)) : 0.f;
+                if constexpr (RESID) {
+                    const uint32_t ux = *reinterpret_cast<const uint32_t*>(x + off);
+                    o0 += bf16_lo(ux); o1 += bf16_hi(ux);
+                }
                 *reinterpret_cast<uint32_t*>(y + off) = pack_bf16(o0, o1);
                 if (pre) *reinterpret_cast<uint32_t*>(pre + off) = pack_bf16(out[j].x, out[j].y);
             }
@@ -337,6 +343,8 @@ constexpr int CV_TILES_PER_BLOCK = 4;   // n-tiles marched by one block: weight/
 // Backward. Staging turns dy into d(pre-activation) = dy * silu'(pre) on the fly (rows outside the sequence or masked: 0). Then the
 // block splits by warp: warps 0-3 compute dx = flipped conv of d_pre (taps in registers), warps 4-7 accumulate the tap gradients
 // dW[k] += d_pre[n] * x[n + k - 15] and d(bias) in registers across the block's tiles — both halves run 31 paired FMAs per element pair.
+// RESID: dx = dy + the convolution's dx (b200_dwconv_args.residual)
+template <bool RESID = false>
 __global__ void __launch_bounds__(256, 2) dwconv_bwd_kernel(const b200_dwconv_args a) {
     extern __shared__ __align__(16) float sm[];
     float (*xs)[CV_TC] = reinterpret_cast<float (*)[CV_TC]>(sm);                          // [CV_R] masked x
@@ -402,7 +410,13 @@ __global__ void __launch_bounds__(256, 2) dwconv_bwd_kernel(const b200_dwconv_ar
                 const int r = rg * 16 + j, n = n0 + r;
                 if (n < a.Np) {
                     const bool ok = sok[r + CV_HALO];
-                    *reinterpret_cast<uint32_t*>(dx + ((size_t)b * a.Np + n) * a.D + ch) = pack_bf16(ok ? dxo[j].x : 0.f, ok ? dxo[j].y : 0.f);
+                    const size_t off = ((size_t)b * a.Np + n) * a.D + ch;
+                    float v0 = ok ? dxo[j].x : 0.f, v1 = ok ? dxo[j].y : 0.f;
+                    if constexpr (RESID) {
+                        const uint32_t ud = *reinterpret_cast<const uint32_t*>(dy + off);
+                        v0 += bf16_lo(ud); v1 += bf16_hi(ud);
+                    }
+                    *reinterpret_cast<uint32_t*>(dx + off) = pack_bf16(v0, v1);
                 }
             }
         } else {
@@ -636,14 +650,17 @@ static int check_conv(const b200_dwconv_args* a) {
     B200_REQUIRE(a && a->x && a->weight && a->bias, "dwconv: null pointer");
     B200_REQUIRE((a->ksize & 1) && a->ksize >= 1 && a->ksize <= 31, "dwconv: kernel_size must be odd and <= 31 (got %d)", a->ksize);
     B200_REQUIRE(a->D % 8 == 0 && a->B > 0 && a->B <= 65535 && a->Np > 0, "dwconv: unsupported shape");
+    B200_REQUIRE(a->residual == 0 || a->residual == 1, "dwconv: residual must be 0 or 1 (got %d)", a->residual);
     return 0;
 }
 extern "C" int b200_dwconv_fwd(const b200_dwconv_args* a, b200_stream_t stream) {
     if (check_conv(a)) return -1;
     B200_REQUIRE(a->y, "dwconv_fwd: null output");
+    B200_REQUIRE(!a->residual || a->y != a->x, "dwconv_fwd: with residual, y must not alias x (neighbouring tiles read x)");
     const int ntiles = (a->Np + CV_TN - 1) / CV_TN;
     dim3 grid((ntiles + CV_FWD_TILES - 1) / CV_FWD_TILES, (a->D + CV_TC - 1) / CV_TC, a->B);
-    dwconv_fwd_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
+    if (a->residual) dwconv_fwd_kernel<true><<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
+    else dwconv_fwd_kernel<false><<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
     return check_launch("dwconv_fwd_kernel");
 }
 extern "C" int b200_dwconv_bwd(const b200_dwconv_args* a, b200_stream_t stream) {
@@ -651,11 +668,17 @@ extern "C" int b200_dwconv_bwd(const b200_dwconv_args* a, b200_stream_t stream) 
     B200_REQUIRE(a->dy && a->dx && a->dweight && a->dbias, "dwconv_bwd: null pointer");
     B200_REQUIRE(a->pre, "dwconv_bwd: the pre-activation saved by b200_dwconv_fwd (args.pre) is required");
     const size_t smem = (size_t)(2 * CV_R + 32) * CV_TC * sizeof(float) + 128;
-    static DeviceOnce once;
-    B200_REQUIRE(set_max_smem_once(once, dwconv_bwd_kernel, (int)smem) == cudaSuccess, "dwconv_bwd: cudaFuncSetAttribute failed");
     const int ntiles = (a->Np + CV_TN - 1) / CV_TN;
     dim3 grid((ntiles + CV_TILES_PER_BLOCK - 1) / CV_TILES_PER_BLOCK, (a->D + CV_TC - 1) / CV_TC, a->B);
-    dwconv_bwd_kernel<<<grid, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
+    if (a->residual) {
+        static DeviceOnce once_r;
+        B200_REQUIRE(set_max_smem_once(once_r, dwconv_bwd_kernel<true>, (int)smem) == cudaSuccess, "dwconv_bwd: cudaFuncSetAttribute failed");
+        dwconv_bwd_kernel<true><<<grid, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
+    } else {
+        static DeviceOnce once;
+        B200_REQUIRE(set_max_smem_once(once, dwconv_bwd_kernel<false>, (int)smem) == cudaSuccess, "dwconv_bwd: cudaFuncSetAttribute failed");
+        dwconv_bwd_kernel<false><<<grid, 256, smem, reinterpret_cast<cudaStream_t>(stream)>>>(*a);
+    }
     return check_launch("dwconv_bwd_kernel");
 }
 

@@ -28,6 +28,7 @@ E2TTSReturn = namedtuple('E2TTS', ['loss', 'cond', 'pred_flow', 'pred_data', 'lo
 BF16, F32 = torch.bfloat16, torch.float32
 SOFTCLAMP = 50.0  # x-transformers logit_softclamp_value default (A.4)
 SOFTCLAMP_MAX = 64.0  # largest clamp the clamped attention kernels take (include/b200_e2tts.h)
+SUPPORTED_RESIDUAL_STREAMS = (1, 4)   # Transformer(num_residual_streams): 1 = plain residual, 4 = hyper-connections (the reference default)
 # x-transformers Attention keywords the kernels implement, with x-transformers' own defaults for a missing key
 ATTN_KWARGS_DEFAULTS = dict(gate_value_heads=False, softclamp_logits=False, logit_softclamp_value=50.)
 # text sub-blocks of layer i+1 overlap the audio sub-blocks of layer i on a second CUDA stream (Transformer._run_layers);
@@ -201,6 +202,14 @@ class HyperConnections(Module):  # A.5
     def params(self):
         return (self.norm.gamma, self.dynamic_alpha_fn, self.dynamic_alpha_scale, self.static_alpha, self.dynamic_beta_fn,
                 self.dynamic_beta_scale, self.static_beta)
+
+
+class Residual(Module):
+    """The reference's disabled hyper-connection (num_residual_streams=1, e2_tts.py:607): a plain residual `out + residual`, without
+    parameters. Kept in `hyper_conns` so that the module tree matches the reference's."""
+
+    def __init__(self, num_residual_streams=1, *, dim=None):
+        super().__init__()
 
 
 class RandomFourierEmbed(Module):  # e2_tts.py:355-364
@@ -410,8 +419,10 @@ class Transformer(_PackOwner):
         gate_value_heads, self.softclamp = _parse_attn_kwargs(attn_kwargs)
         if dict(ff_kwargs):
             _unsupported('ff_kwargs', ff_kwargs, 'e2_tts.py:552')
-        if num_residual_streams != 4:
-            _unsupported('num_residual_streams', num_residual_streams, 'e2_tts.py:547')
+        if num_residual_streams not in SUPPORTED_RESIDUAL_STREAMS:
+            raise NotImplementedError(
+                f'num_residual_streams={num_residual_streams!r} (e2_tts.py:547): supported values are 1 (plain residual) and 4 '
+                f'(hyper-connections; the kernels lay out 4 streams per token); there is no fallback path (SURVEY.md §2 row 8)')
         dim_text = default(dim_text, dim // 2)
         text_heads, text_dim_head = default(text_heads, heads), default(text_dim_head, dim_head)
         text_ff_mult, text_depth = default(text_ff_mult, ff_mult), default(text_depth, depth)
@@ -445,7 +456,7 @@ class Transformer(_PackOwner):
         self.time_cond_mlp = nn.Sequential(RandomFourierEmbed(dim), nn.Linear(dim + 1, dim), nn.SiLU()) if cond_on_time else Identity()
 
         layers, hyper_conns = [], []
-        hc = partial(HyperConnections, num_residual_streams)
+        hc = partial(HyperConnections if num_residual_streams != 1 else Residual, num_residual_streams)   # :607, disable = S == 1
         for ind in range(depth):
             first, later_half, has_text = ind == 0, ind >= depth // 2, ind < text_depth
             speech = ModuleList([
@@ -584,13 +595,25 @@ class Transformer(_PackOwner):
         # the next sub-block's width connection consumes it in one fused kernel (ops.HcDepthWidth); `close` materialises the streams
         # where something else reads them (cross-conditioning, skip path, final norm).
         fuse = ops.hc_can_fuse(xs.shape[0], xs.shape[1])
+        # num_residual_streams=1 (e2_tts.py:607, disable=True): every sub-block is x + branch(norm(x)). The width connection is then
+        # the branch norm alone (the conv sub-block has none) and hands x on as `rest`; the branch's last launch (the conv kernel, the
+        # to_out / FF-out GEMM epilogue) adds it, so the depth connection is nothing but a view back to [T, 1, D].
+        plain = self.num_streams == 1
 
         def width(res, hcm, gain, mode):
+            if plain:
+                x2 = res.view(res.shape[0], res.shape[-1])
+                if mode == 0:
+                    return x2, x2, None
+                br, xr = ops.BranchNorm.apply(x2, gain if mode == 1 else None, gain if mode == 2 else None, B, Np)
+                return br, xr, None
             if isinstance(res, tuple):
                 return ops.HcDepthWidth.apply(*res, *hcm.params(), gain, mode, Np)
             return ops.HcWidth.apply(res, *hcm.params(), gain, mode, Np)
 
         def depth(rest, y, beta):
+            if plain:
+                return y.view(y.shape[0], 1, y.shape[1])
             return (rest, y, beta) if fuse else ops.HcDepth.apply(rest, y, beta)
 
         def close(res):
@@ -598,7 +621,7 @@ class Transformer(_PackOwner):
 
         def sub_conv(res, hcm, conv):
             br, rest, beta = width(res, hcm, None, 0)
-            y = ops.DwConv.apply(br, conv.dw_conv1d[0].weight, conv.dw_conv1d[0].bias, mask_u8, B, Np)
+            y = ops.DwConv.apply(br, conv.dw_conv1d[0].weight, conv.dw_conv1d[0].bias, mask_u8, B, Np, plain)
             return depth(rest, y, beta)
 
         def sub_attn(res, hcm, gain, mode, attn, pk, vf, colscale, lfe=None):
@@ -610,13 +633,14 @@ class Transformer(_PackOwner):
                                         gate.bias if gate is not None else None, mix[0].weight if mix is not None else None,
                                         mix[0].bias if mix is not None else None, vf if mix is not None else None,
                                         pk['qkv'], cs, sn, mask_u8, B, Np, H, p_drop, next_seed(), self.softclamp, self._seed_dev, mbits)
-            y = ops.OutProj.apply(og, attn.to_out.weight, pk['out'], colscale, mask_u8, B, Np)
+            y = ops.OutProj.apply(og, attn.to_out.weight, pk['out'], colscale, mask_u8, B, Np, rest if plain else None)
             return depth(rest, y, beta), (v if vf is None else vf)
 
         def sub_ff(res, hcm, gain, mode, ff, pk, colscale):
             br, rest, beta = width(res, hcm, gain, mode)
             y = ops.FeedForward.apply(br, ff.ff[0].proj.weight, ff.ff[0].proj.bias, ff.ff[2].weight, ff.ff[2].bias,
-                                      pk['w1'], pk['b1'], pk['w2'], colscale, B, Np, p_drop, next_seed(), self._seed_dev)
+                                      pk['w1'], pk['b1'], pk['w2'], colscale, B, Np, p_drop, next_seed(), self._seed_dev,
+                                      rest if plain else None)
             return close(depth(rest, y, beta))
 
         def text_block(i, ts, tvf):  # the three text sub-blocks of layer i (:853-882)

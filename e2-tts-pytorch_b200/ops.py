@@ -232,18 +232,21 @@ class HcDepth(Function):
 
 # ---------------------------------------------------------------------------------------------------- depthwise conv
 class DwConv(Function):
-    """DepthwiseConv (e2_tts.py:295-328): mask -> depthwise conv k -> SiLU -> mask, on bf16 [B, Np, D]."""
+    """DepthwiseConv (e2_tts.py:295-328): mask -> depthwise conv k -> SiLU -> mask, on bf16 [B, Np, D]. residual=True: the plain
+    residual sub-block x + DepthwiseConv(x, mask) (:870-872, 900-902) in the same launch; masked rows keep x."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, mask, B, Np):
+    def forward(ctx, x, weight, bias, mask, B, Np, residual=False):
         D = x.shape[-1]
         w2 = weight.reshape(D, -1)
         y = torch.empty_like(x)
         pre = torch.empty_like(x) if any(ctx.needs_input_grad[:3]) else None   # bf16 pre-activation: backward does not redo the convolution
-        a = lib.make_args('b200_dwconv_args', x=x, mask=mask, weight=w2, bias=bias, y=y, B=B, Np=Np, D=D, ksize=w2.shape[1], pre=pre)
+        a = lib.make_args('b200_dwconv_args', x=x, mask=mask, weight=w2, bias=bias, y=y, B=B, Np=Np, D=D, ksize=w2.shape[1], pre=pre,
+                          residual=int(residual))
         lib.call('b200_dwconv_fwd', a, _stream())
         ctx.save_for_backward(x, weight, bias, mask, pre)
         ctx.meta = (B, Np)
+        ctx.residual = int(residual)
         return y
 
     @staticmethod
@@ -251,15 +254,52 @@ class DwConv(Function):
     def backward(ctx, dy):
         x, weight, bias, mask, pre = ctx.saved_tensors
         B, Np = ctx.meta
+        residual = ctx.residual
         D = x.shape[-1]
         w2 = weight.reshape(D, -1)
         dx = torch.empty_like(x)
         dw = _zeros(w2.shape, w2.device)
         db = _zeros(bias.shape, bias.device)
         a = lib.make_args('b200_dwconv_args', x=x, mask=mask, weight=w2, bias=bias, dy=_c(dy), dx=dx, dweight=dw, dbias=db,
-                          B=B, Np=Np, D=D, ksize=w2.shape[1], pre=pre)
+                          B=B, Np=Np, D=D, ksize=w2.shape[1], pre=pre, residual=residual)
         lib.call('b200_dwconv_bwd', a, _stream())
-        return dx, dw.view_as(weight), db, None, None, None
+        return dx, dw.view_as(weight), db, None, None, None, None
+
+
+class BranchNorm(Function):
+    """Pre-norm of a plain residual sub-block (Transformer(num_residual_streams=1), e2_tts.py:874-882, 906-939) on bf16 rows x [T, D]:
+    RMSNorm(g) (:875, 881 and the DurationPredictor) or, with `gains` (fp32 [B, D] = 1 + to_gamma(cond), one row per Np rows),
+    AdaptiveRMSNorm (:908, 937); the branch-norm mode of b200_final_norm_*. Returns (normed branch input, x): the second output IS x,
+    handed on as the sub-block's residual, so that its gradient (the residual add's dy) joins the norm's gradient inside the
+    backward kernel instead of in an autograd sum."""
+
+    @staticmethod
+    def forward(ctx, x, g, gains, B, Np):
+        T, D = x.shape
+        y = torch.empty_like(x)
+        a = lib.make_args('b200_final_norm_args', xres=x, g=None if gains is not None else g, y=y, B=B, N=Np, R=0, D=D, S=1,
+                          rows_per_batch=Np, gains=gains)
+        lib.call('b200_final_norm_fwd', a, _stream())
+        ctx.save_for_backward(x, g if gains is None else None, gains)
+        ctx.meta = (B, Np)
+        ctx.set_materialize_grads(False)
+        return y, x.view_as(x)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy, d_res):
+        x, g, gains = ctx.saved_tensors
+        B, Np = ctx.meta
+        T, D = x.shape
+        if dy is None:
+            return d_res, None, None, None, None
+        dx = torch.empty_like(x)
+        d_g = _zeros(g.shape, g.device) if g is not None else None
+        d_gains = _zeros(gains.shape, gains.device) if gains is not None else None
+        a = lib.make_args('b200_final_norm_args', xres=x, g=g, dy=_c(dy), d_xres=dx, g_g=d_g, B=B, N=Np, R=0, D=D, S=1,
+                          rows_per_batch=Np, gains=gains, d_gains=d_gains, d_res=_c(d_res))
+        lib.call('b200_final_norm_bwd', a, _stream())
+        return dx, d_g, d_gains, None, None
 
 
 # ---------------------------------------------------------------------------------------------------- attention
@@ -430,16 +470,30 @@ class FourierLinear(Function):
         return dx, dW, None, None, None
 
 
+def _rowgate_resid_bwd(dy, y, resid, cs, mask, B, rpb, D, want_bias=False):
+    """_rowgate_bwd for an epilogue that also added `resid` (the gate gradient reads the branch value as y - resid)."""
+    if cs is None:
+        return _rowgate_bwd(dy, y, cs, mask, B, rpb, D, want_bias)
+    dz = torch.empty_like(dy)
+    d_cs = _zeros(cs.shape, cs.device)
+    d_bias = _zeros(D, dy.device) if want_bias else None
+    lib.call('b200_rowgate_resid_bwd', dy, y, _c(resid), cs, mask, dz, d_cs, d_bias, B, rpb, D, _stream())
+    return (dz, d_cs, d_bias) if want_bias else (dz, d_cs)
+
+
 class OutProj(Function):
-    """Attention to_out (no bias) with the fused epilogue: zero padded rows (A.4 step 6) and AdaLNZero gate (:346-351)."""
+    """Attention to_out (no bias) with the fused epilogue: zero padded rows (A.4 step 6) and AdaLNZero gate (:346-351).
+    resid (bf16 [T, Dout], optional): the plain residual sub-block's add, x + gated output (:878, 916), in the same epilogue; its
+    gradient is dy itself."""
 
     @staticmethod
-    def forward(ctx, og, w, wpack, colscale, mask, B, Np):
+    def forward(ctx, og, w, wpack, colscale, mask, B, Np, resid=None):
         T, I = og.shape
         Dout = w.shape[0]
-        y = gemm(og, wpack, T, Dout, I, colscale=colscale, rows_per_batch=Np, rowmask=mask)
+        y = gemm(og, wpack, T, Dout, I, colscale=colscale, rows_per_batch=Np, rowmask=mask, resid=resid, ldr=Dout if resid is not None else 0)
         ctx.save_for_backward(og, wpack, colscale, mask, y)
         ctx.meta = (B, Np)
+        ctx.has_resid, ctx.resid = resid is not None, (resid if colscale is not None else None)   # the gated backward reads y - resid
         return y
 
     @staticmethod
@@ -447,26 +501,33 @@ class OutProj(Function):
     def backward(ctx, dy):
         og, wpack, colscale, mask, y = ctx.saved_tensors
         B, Np = ctx.meta
+        has_resid, resid = ctx.has_resid, ctx.resid
         T, I = og.shape
         Dout = y.shape[1]
-        dz, d_cs = _rowgate_bwd(_c(dy), y, colscale, mask, B, Np, Dout)
+        dy = _c(dy)
+        if resid is not None:
+            dz, d_cs = _rowgate_resid_bwd(dy, y, resid, colscale, mask, B, Np, Dout)
+        else:
+            dz, d_cs = _rowgate_bwd(dy, y, colscale, mask, B, Np, Dout)
         d_og = gemm(dz, wpack, T, I, Dout, b_mn=True)
         dW = grad_weight(dz, og, T, Dout, I)
-        return d_og, dW, None, d_cs, None, None, None
+        return d_og, dW, None, d_cs, None, None, None, (dy if has_resid else None)
 
 
 class FeedForward(Function):
-    """x-transformers FeedForward(glu=True) (A.2): GEGLU GEMM (+dropout) -> out GEMM (+bias, AdaLNZero gate)."""
+    """x-transformers FeedForward(glu=True) (A.2): GEGLU GEMM (+dropout) -> out GEMM (+bias, AdaLNZero gate). resid (bf16 [T, Din],
+    optional): the plain residual sub-block's add (:882, 939) in the out GEMM's epilogue; its gradient is dy itself."""
 
     @staticmethod
-    def forward(ctx, xn, w1, b1, w2, b2, w1pack, b1pack, w2pack, colscale, B, Np, dropout_p, seed, seed_dev):
+    def forward(ctx, xn, w1, b1, w2, b2, w1pack, b1pack, w2pack, colscale, B, Np, dropout_p, seed, seed_dev, resid=None):
         T, Din = xn.shape
         inner = w2.shape[1]
         ug = torch.empty((T, 2 * inner), device=xn.device, dtype=BF16)
         h = gemm(xn, w1pack, T, 2 * inner, Din, D2=ug, ldd2=2 * inner, bias=b1pack, geglu=True, dropout_p=dropout_p, seed=seed, seed_dev=seed_dev)
-        y = gemm(h, w2pack, T, Din, inner, bias=b2, colscale=colscale, rows_per_batch=Np)
+        y = gemm(h, w2pack, T, Din, inner, bias=b2, colscale=colscale, rows_per_batch=Np, resid=resid, ldr=Din if resid is not None else 0)
         ctx.save_for_backward(xn, ug, h, y, w1pack, w2pack, colscale)
         ctx.meta = (B, Np, dropout_p, seed, inner, seed_dev)
+        ctx.has_resid, ctx.resid = resid is not None, (resid if colscale is not None else None)   # the gated backward reads y - resid
         return y
 
     @staticmethod
@@ -474,12 +535,16 @@ class FeedForward(Function):
     def backward(ctx, dy):
         xn, ug, h, y, w1pack, w2pack, colscale = ctx.saved_tensors
         B, Np, dropout_p, seed, inner, seed_dev = ctx.meta
+        has_resid, resid = ctx.has_resid, ctx.resid
         T, Din = xn.shape
-        if colscale is not None:
+        dy = _c(dy)
+        if colscale is not None and resid is not None:
+            dz, d_cs, db2 = _rowgate_resid_bwd(dy, y, resid, colscale, None, B, Np, Din, want_bias=True)
+        elif colscale is not None:
             # y = cs * (h W2^T + b2): recover the pre-gate value through y / cs inside the kernel
-            dz, d_cs, db2 = _rowgate_bwd(_c(dy), y, colscale, None, B, Np, Din, want_bias=True)   # bias grad rides along
+            dz, d_cs, db2 = _rowgate_bwd(dy, y, colscale, None, B, Np, Din, want_bias=True)   # bias grad rides along
         else:
-            dz, d_cs = _c(dy), None
+            dz, d_cs = dy, None
             db2 = colsum(dz, T, Din, Din)
         dh = gemm(dz, w2pack, T, inner, Din, b_mn=True)
         dW2 = grad_weight(dz, h, T, Din, inner)
@@ -491,7 +556,7 @@ class FeedForward(Function):
         nb = inner // 64
         dW1 = dW1p.view(nb, 2, 64, Din).transpose(0, 1).reshape(2 * inner, Din)   # undo the GEGLU interleave (layout only)
         db1 = db1p.view(nb, 2, 64).transpose(0, 1).reshape(2 * inner)
-        return dx, dW1, db1, dW2, db2, None, None, None, d_cs, None, None, None, None, None
+        return dx, dW1, db1, dW2, db2, None, None, None, d_cs, None, None, None, None, None, (dy if has_resid else None)
 
 
 # ---------------------------------------------------------------------------------------------------- cross-stream GEMMs

@@ -249,11 +249,19 @@ int b200_geglu_bwd(const void* dh, const void* ug, void* dug, float* db_packed, 
 /* out[n] += sum_t X[t,n] (bf16 X, fp32 out; caller zeroes out) — nn.Linear bias gradients. */
 int b200_colsum(const void* X, int64_t T, int32_t ncols, int32_t ld, float* out, b200_stream_t stream);
 
-/* Drop registers, sum the S streams, final RMSNorm (e2_tts.py:943-952). y bf16 [B*N, D]. */
+/* Drop registers, sum the S streams, final RMSNorm (e2_tts.py:943-952). y bf16 [B*N, D].
+ * Branch-norm mode (rows_per_batch > 0): the pre-norm of a plain residual sub-block (Transformer(num_residual_streams=1),
+ *   e2_tts.py:870-882, 900-939): y[r] = F.normalize(x[r]) * sqrt(D) * gain, on rows x bf16 [B*N, D]; requires S == 1, R == 0 and
+ *   (B*N) % rows_per_batch == 0. gains == NULL: RMSNorm, gain = g [D], bwd ADDS into g_g [D]; gains != NULL: AdaptiveRMSNorm,
+ *   gain = gains[r / rows_per_batch] (fp32 [B*N / rows_per_batch, D], the 1 + gamma of b200_small_linear; g unused), bwd ADDS
+ *   into d_gains (same shape, zeroed by the caller; g_g unused). A zero row gives y = 0 and the finite gradient of F.normalize
+ *   (the norm clamped at 1e-12). bwd: d_res (optional bf16 [B*N, D]), the gradient of the residual path around the norm, is added
+ *   into d_xres. All four fields zero: the final norm above. */
 typedef struct {
     const void* xres; const float* g; void* y;
     const void* dy; void* d_xres; float* g_g;   /* bwd: d_xres [B,R+N,S,D] fully written, g_g accumulated */
     int32_t B, N, R, D, S;
+    int32_t rows_per_batch; const float* gains; float* d_gains; const void* d_res;   /* branch-norm mode (above) */
 } b200_final_norm_args;
 int b200_final_norm_fwd(const b200_final_norm_args* a, b200_stream_t stream);
 int b200_final_norm_bwd(const b200_final_norm_args* a, b200_stream_t stream);
@@ -279,6 +287,11 @@ int b200_flow_loss_bwd(const b200_flow_loss_args* a, b200_stream_t stream);
  * d_bias[:] += sum_rows dz (fp32 [D], caller zeroes). cs/mask/d_bias may be NULL. */
 int b200_rowgate_bwd(const void* dy, const void* y, const float* cs, const uint8_t* mask, void* dz, float* d_cs,
                      float* d_bias, int32_t B, int32_t rows_per_batch, int32_t D, b200_stream_t stream);
+/* The same for an epilogue that also added a residual, y = rowmask * colscale * (z + bias) + resid (the fused residual add of a plain
+ * residual sub-block): the gate gradient reads the branch value as y - resid (bf16 resid, required), so it carries the bf16 rounding
+ * of the sum y (at most 2^-9 |y| per element). dz and d_bias are those of b200_rowgate_bwd; resid's own gradient is dy. */
+int b200_rowgate_resid_bwd(const void* dy, const void* y, const void* resid, const float* cs, const uint8_t* mask, void* dz, float* d_cs,
+                           float* d_bias, int32_t B, int32_t rows_per_batch, int32_t D, b200_stream_t stream);
 int b200_cast_rows(const float* src, void* dst, int64_t rows, int32_t cols, int32_t ld, b200_stream_t stream);
 /* InterpolatedCharacterEmbed (e2_tts.py:414-482; E2TTS(interpolated_text=True) :1135, :1233): the per-token front half of
  *   te[b, n] = mask[b, n] * ( lerp[b, n] + Linear2( silu( pos[b, n] * w1 + b1 ) ) )
@@ -324,12 +337,15 @@ int b200_fourier_embed(const float* times, const float* weights, float* out, int
 /* Masked depthwise conv k (odd, <= 31) + SiLU (DepthwiseConv e2_tts.py:295-328) on bf16 [B, Np, D]:
  *   y = m * silu(conv1d_depthwise(m * x) + bias), weight fp32 [D, k]. fwd also stores the bf16 pre-activation (conv + bias) into
  *   `pre` [B, Np, D] when it is non-null; bwd REQUIRES it (caller-owned, like every saved tensor) instead of recomputing the
- *   convolution. dweight/dbias are ADDED into zero-initialised fp32 buffers. */
+ *   convolution. dweight/dbias are ADDED into zero-initialised fp32 buffers.
+ *   residual != 0 (the plain residual sub-block x + DepthwiseConv(x, mask), e2_tts.py:870-872, 900-902): y = x + m * silu(...), the
+ *   add itself unmasked (a masked row keeps x bit for bit) and rounded once; bwd dx = dy + the convolution's dx. y must not alias x. */
 typedef struct {
     const void* x; const uint8_t* mask; const float *weight, *bias; void* y;
     const void* dy; void* dx; float *dweight, *dbias;
     int32_t B, Np, D, ksize;
     void* pre;
+    int32_t residual;
 } b200_dwconv_args;
 int b200_dwconv_fwd(const b200_dwconv_args* a, b200_stream_t stream);
 int b200_dwconv_bwd(const b200_dwconv_args* a, b200_stream_t stream);

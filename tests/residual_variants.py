@@ -1,0 +1,45 @@
+"""Test infrastructure for Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True):
+the cases stored from the original e2_tts.py by tools/make_residual_golden.py, and a context that turns the oracle of
+oracle/e2tts_oracle.py into that backbone.
+
+With one stream the reference's hyper-connection modules are `Residual` (oracle/ref_leaves/hyper_connections.py): the width
+connection hands the stream itself to the branch and keeps it as the residual, the depth connection is `branch_out + residual`, and
+expand / reduce are identities. The oracle holds its streams as (b, n, S, d), so with S = 1 swapping its two hyper-connection leaves is
+all it takes; the stage rounding of the conditioning probe (O.STAGE_ROUND) stays on the residual sum, which the CUDA path stores in
+bf16 (the branch output itself is added in fp32 inside the producing kernel and never stored)."""
+import contextlib
+
+from oracle import e2tts_oracle as O
+
+KW1 = dict(dim=128, depth=2, heads=2, num_residual_streams=1)
+
+# forward + backward cases of the original: class, seed, transformer kwargs, (batch, frames), lens, text, drop_text_cond
+RESIDUAL1_CASES = {
+    'depth2': dict(cls='E2TTS', seed=62, tkw=KW1, mel=(2, 80), lens=[80, 80], text=['abc', 'a longer text than the first'], drop=False),
+    'depth4_lens': dict(cls='E2TTS', seed=64, tkw=dict(KW1, depth=4), mel=(2, 80), lens=[80, 51], text=['abc', 'a longer text than the first'],
+                        drop=False),
+    'text_dropped': dict(cls='E2TTS', seed=66, tkw=dict(KW1, heads=4), mel=(3, 64), lens=[64, 40, 17], text=['one', 'two words', ''],
+                         drop=True),
+    'duration': dict(cls='DurationPredictor', seed=68, tkw=KW1, mel=(3, 72), lens=[72, 50, 31], text=['abc', 'hello world', 'x']),
+}
+# E2TTS.sample: weights seed, cond (batch, frames), text, duration, steps, cfg_strength; y0 = first draw of generator 3000 + seed
+RESIDUAL1_SAMPLE = dict(seed=70, cond=(2, 20), text=['Hello', 'Goodbye then'], duration=[40, 33], steps=4, cfg_strength=1.0)
+
+
+def _width(sd, p, res, S):
+    return res[..., 0, :], res, None
+
+
+def _depth(rest, beta, y):
+    return O._rs(y[..., None, :] + rest)
+
+
+@contextlib.contextmanager
+def plain_residual_oracle():
+    """Inside the block the oracle computes the num_residual_streams=1 backbone (use it with TransformerCfg(num_residual_streams=1))."""
+    saved = O.hyper_width, O.hyper_depth
+    O.hyper_width, O.hyper_depth = _width, _depth
+    try:
+        yield
+    finally:
+        O.hyper_width, O.hyper_depth = saved
