@@ -31,6 +31,24 @@ __global__ void __launch_bounds__(256) flat_gather_kernel(const b200_chunk* __re
     for (int i = n4 * 4 + threadIdx.x; i < c.n; i += 256) dst[i] = __ldg(src + i) * scale;
 }
 
+// sumsq: the block partials go to a static device array and the last block to finish adds them in block order, so the norm is
+// the same bit for bit on every call with the same input (no float atomics whose order depends on the schedule): a resumed run
+// clips exactly as the uninterrupted one. One call at a time per device (stream order), like every other user of the buffer.
+constexpr int kSumsqMaxGrid = 4096;
+__device__ float g_sumsq_part[kSumsqMaxGrid];
+__device__ unsigned int g_sumsq_ticket;   // blocks of the current call that have written their partial; reset by the last one
+
+__device__ __forceinline__ float block_sum_256(float acc, float* part) {   // fixed order; the result is valid in thread 0
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    float s = 0.f;
+    if (threadIdx.x == 0)
+        for (int i = 0; i < 8; ++i) s += part[i];
+    return s;
+}
+
 __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x, long long n, float* __restrict__ out) {
     float acc = 0.f;
     const long long n4 = ((reinterpret_cast<uintptr_t>(x) & 15) == 0) ? (n >> 2) : 0;
@@ -39,15 +57,24 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ x,
         acc += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
     }
     for (long long i = n4 * 4 + (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) acc += x[i] * x[i];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     __shared__ float part[8];
-    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
-    __syncthreads();
+    __shared__ bool last;
+    const float s = block_sum_256(acc, part);
     if (threadIdx.x == 0) {
-        float s = 0.f;
-        for (int i = 0; i < 8; ++i) s += part[i];
-        atomicAdd(out, s);
+        g_sumsq_part[blockIdx.x] = s;
+        __threadfence();
+        last = atomicAdd(&g_sumsq_ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    float a = 0.f;
+    for (int i = threadIdx.x; i < (int)gridDim.x; i += 256) a += __ldcg(g_sumsq_part + i);
+    __syncthreads();   // part[] is reused
+    const float total = block_sum_256(a, part);
+    if (threadIdx.x == 0) {
+        *out = total;
+        g_sumsq_ticket = 0u;
     }
 }
 
@@ -57,7 +84,7 @@ struct AdoptP {
     float *m, *v, *ema;
     const float* gradnorm_sq;
     const float* used;
-    float max_grad_norm, lr, beta1, beta2, eps, weight_decay, ema_weight;
+    float max_grad_norm, lr, one_minus_beta1, one_minus_beta2, eps, weight_decay, ema_weight;
     int* chunk_state;
     int ema_mode;
 };
@@ -72,9 +99,9 @@ __device__ __forceinline__ void adopt_elem(const AdoptP& p, float g, float& w, f
     } else {
         if (p.weight_decay > 0.f) w *= (1.f - p.lr * p.weight_decay);
         const float u = g / fmaxf(sqrtf(v), p.eps);
-        m += (1.f - p.beta1) * (u - m);
+        m += p.one_minus_beta1 * (u - m);
         w -= p.lr * m;
-        v += (1.f - p.beta2) * (g * g - v);
+        v += p.one_minus_beta2 * (g * g - v);
     }
     if (p.ema_mode == 1) e += p.ema_weight * (w - e);
     else if (p.ema_mode == 2) e = w;
@@ -90,7 +117,10 @@ __global__ void __launch_bounds__(256) adopt_step_kernel(const AdoptP p) {
     __syncthreads();
     if (live && first && threadIdx.x == 0) p.chunk_state[blockIdx.x] = 1;
     float clip = 1.f;
-    if (p.gradnorm_sq && p.max_grad_norm > 0.f) clip = fminf(1.f, p.max_grad_norm / (sqrtf(__ldg(p.gradnorm_sq)) + 1e-6f));   // clip_grad_norm_
+    if (p.gradnorm_sq && p.max_grad_norm > 0.f) {   // clip_grad_norm_: clamp(max_norm / (norm + 1e-6), max=1), so a NaN norm gives a NaN
+        const float q = p.max_grad_norm / (sqrtf(__ldg(p.gradnorm_sq)) + 1e-6f);   // coefficient (every weight), not fminf's 1
+        clip = q > 1.f ? 1.f : q;
+    }
     const bool vec = ((reinterpret_cast<uintptr_t>(w) & 15) == 0) && ((off & 3) == 0);
     const int n4 = vec ? c.n >> 2 : 0;
     for (int i = threadIdx.x; i < n4; i += 256) {
@@ -141,13 +171,11 @@ extern "C" int b200_flat_scatter(const b200_chunk* chunks_dev, int32_t n_chunks,
 }
 
 extern "C" int b200_sumsq(const float* x, int64_t n, float* out, b200_stream_t stream) {
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B200_REQUIRE(x && out && n > 0, "sumsq: null pointer / empty buffer");
-    cudaError_t e = cudaMemsetAsync(out, 0, sizeof(float), st);
-    B200_REQUIRE(e == cudaSuccess, "sumsq: memset: %s", cudaGetErrorString(e));
     const long long blocks = (n / 4 + 255) / 256;
-    const int grid = (int)(blocks < 1 ? 1 : (blocks > (long long)num_sms() * 8 ? (long long)num_sms() * 8 : blocks));
-    sumsq_kernel<<<grid, 256, 0, st>>>(x, (long long)n, out);
+    const long long cap = (long long)num_sms() * 8 < kSumsqMaxGrid ? (long long)num_sms() * 8 : kSumsqMaxGrid;
+    const int grid = (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
+    sumsq_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(x, (long long)n, out);
     return check_launch("sumsq_kernel");
 }
 
@@ -158,7 +186,11 @@ extern "C" int b200_adopt_step(const b200_adopt_args* a, b200_stream_t stream) {
     AdoptP p{};
     p.chunks = a->chunks_dev; p.grad = a->grad_flat; p.m = a->m_flat; p.v = a->v_flat; p.ema = a->ema_flat;
     p.gradnorm_sq = a->gradnorm_sq; p.max_grad_norm = a->max_grad_norm; p.used = a->used;
-    p.lr = a->lr; p.beta1 = a->beta1; p.beta2 = a->beta2; p.eps = a->eps; p.weight_decay = a->weight_decay;
+    p.lr = a->lr;
+    // the lerp weights 1 - beta: formed in double by the caller (as torch's lerp_(x, 1. - beta) does) when given, else from the fp32 betas
+    p.one_minus_beta1 = a->one_minus_beta1 != 0.f ? a->one_minus_beta1 : 1.f - a->beta1;
+    p.one_minus_beta2 = a->one_minus_beta2 != 0.f ? a->one_minus_beta2 : 1.f - a->beta2;
+    p.eps = a->eps; p.weight_decay = a->weight_decay;
     p.chunk_state = a->chunk_state; p.ema_mode = a->ema_mode; p.ema_weight = a->ema_weight;
     adopt_step_kernel<<<a->n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("adopt_step_kernel");

@@ -203,7 +203,8 @@ class FusedAdoptEMA:
         a = lib.make_args('b200_adopt_args', chunks_dev=lay.param_table, n_chunks=lay.n_chunks, grad_flat=flat_grads, m_flat=self.m, v_flat=self.v,
                           ema_flat=self.ema, gradnorm_sq=self.norm_sq if clip else None, max_grad_norm=float(self.max_grad_norm), lr=float(self.lr),
                           beta1=float(self.betas[0]), beta2=float(self.betas[1]), eps=float(self.eps), weight_decay=float(wd), chunk_state=self.chunk_state,
-                          ema_mode=int(mode), ema_weight=float(weight), used=self.sync.used if flat_grads is self.sync.flat else None)
+                          ema_mode=int(mode), ema_weight=float(weight), used=self.sync.used if flat_grads is self.sync.flat else None,
+                          one_minus_beta1=float(1.0 - self.betas[0]), one_minus_beta2=float(1.0 - self.betas[1]))
         lib.call('b200_adopt_step', a, _stream())
         self.steps += 1
 

@@ -388,13 +388,18 @@ typedef struct { void* ptr; int64_t flat_offset; int32_t n; int32_t pidx; /* ind
 int b200_flat_gather(const b200_chunk* chunks_dev, int32_t n_chunks, float* flat, float scale, float* used, b200_stream_t stream);
 /* ptr[i] = flat[flat_offset + i] (e.g. EMA weights into a module's parameters) */
 int b200_flat_scatter(const b200_chunk* chunks_dev, int32_t n_chunks, const float* flat, b200_stream_t stream);
-/* *out = sum x[i]^2 (out: ONE device float, zeroed by the call): torch.nn.utils.clip_grad_norm_'s total norm, trainer.py:272-273 */
+/* *out = sum x[i]^2 (out: ONE device float, overwritten): torch.nn.utils.clip_grad_norm_'s total norm, trainer.py:272-273.
+ * Deterministic: the block partials are added in block order, so equal inputs give a bit-identical norm. The partials live in one
+ * static device buffer, so calls on one device must be ordered (one stream, or events between streams). */
 int b200_sumsq(const float* x, int64_t n, float* out, b200_stream_t stream);
 /* One pass over every parameter (trainer.py:272-279):
- *   g    = grad * min(1, max_grad_norm / (sqrt(*gradnorm_sq) + 1e-6))        (clip_grad_norm_; skipped when gradnorm_sq == NULL)
+ *   g    = grad * clamp(max_grad_norm / (sqrt(*gradnorm_sq) + 1e-6), max=1)  (clip_grad_norm_; skipped when gradnorm_sq == NULL;
+ *                                                                          a NaN norm gives a NaN coefficient, an infinite one 0)
  *   w   *= 1 - lr * weight_decay                                              (Adopt's decoupled weight decay, when > 0)
  *   first gradient of a parameter : v = g^2, m = 0, parameter untouched     (Adopt initialises its state on first sight)
  *   afterwards                    : m += (1-beta1) (g / max(sqrt(v), eps) - m);  w -= lr m;  v += (1-beta2) (g^2 - v)
+ *   (1-beta1, 1-beta2: one_minus_beta1 / one_minus_beta2 when non-zero — the complements formed in double and rounded once, as
+ *   torch's lerp_(x, 1. - beta) applies them; 0 keeps 1.f - beta formed in fp32 on the device, which is 16 u off for beta 0.99)
  *   ("first" is tracked per chunk in chunk_state (int32 [n_chunks], zeroed once by the caller): a parameter that received no
  *   gradient on the first steps — the text stream while the text is dropped — is initialised when its first gradient arrives)
  *   ema_mode 1: ema += ema_weight (w - ema)   (ema-pytorch lerp, ema_weight = 1 - current decay);  2: ema = w (copy phase);  0: none
@@ -409,6 +414,7 @@ typedef struct {
     int32_t* chunk_state;
     int32_t ema_mode; float ema_weight;
     const float* used;   /* optional fp32 [n_params]: parameters with used[pidx] == 0 keep w, m, v (only their EMA moves) */
+    float one_minus_beta1, one_minus_beta2;   /* optional: fp32(1 - beta) formed in double; 0 -> 1.f - beta on the device */
 } b200_adopt_args;
 int b200_adopt_step(const b200_adopt_args* a, b200_stream_t stream);
 
