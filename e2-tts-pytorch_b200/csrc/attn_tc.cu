@@ -316,18 +316,23 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 }
 
 // ================================================================================================ backward
-// One CTA per (128-key tile, head, batch), 384 threads:
-//   warpgroup 0, one thread : TMA producer — K, V once; Q_i / dO_i tiles (64 queries) through a 3-stage ring
-//   warpgroups 1, 2         : 64 keys each, per query tile i (all operands from smem, accumulators in registers):
+// One CTA per (128-key tile, head, batch), 256 threads:
+//   thread 0 also issues the TMA loads — K, V once; Q_i / dO_i tiles (64 queries) through a 3-stage ring, two tiles ahead
+//   warpgroups 0, 1         : 64 keys each, per query tile i (all operands from smem, accumulators in registers):
 //                             S^T = K Q_i^T, dP^T = V dO_i^T                 (wgmma m64n64k16, K-major operands)
 //                             recompute softclamp + softmax from the saved LSE, dS^T = P^T (dP^T - delta)(1 - tanh^2) scale
 //                             (unclamped mode: no tanh, dS^T = P^T (dP^T - delta) scale)
 //                             dV += P^T dO_i, dK += dS^T Q_i                 (register A operands, B MN-major)
-//                             dQ_i += dS K_w through a swizzled smem copy of dS^T (A MN-major), flushed with fp32 vector atomics.
+//                             and dS^T into a swizzled smem tile, double-buffered by the parity of the query tile.
+// dQ is reduced once per CTA and query tile: after a named barrier, the warpgroup whose index equals the tile's parity computes
+// dQ_i = dS_i K over all 128 keys from both dS^T tiles (A MN-major, 8 k-steps), stages the fp32 result in a swizzled smem tile and
+// adds it into dq with one TMA tensor reduction (a [B*H, Np, 64] map, so rows >= Np are clipped and the next head is never touched).
+// Barrier hand-offs per dS^T buffer b: DS_FULL (the other warpgroup arrives once its tile is written, the reducing one waits) and
+// DS_FREE (the reducing warpgroup arrives once its dQ MMAs have read the buffer, the other one waits before it rewrites it two tiles on).
+// The lse / delta of query tile i + 1 are loaded during tile i into smem, so no global load sits between the MMA wait and the score math.
 struct AttnBwdTcP {
     const unsigned int* maskbits; int mask_words;
     const float *lse, *delta;
-    float* dq_acc;                  // fp32 [B,H,Np,64], zeroed by the host wrapper
     __nv_bfloat16 *dk, *dv;
     int B, H, Np, nq;
     float scale, scale_over_clamp, clamp, dropout_p, keep_scale;
@@ -337,6 +342,8 @@ struct AttnBwdTcP {
     float scale_log2e;              // unclamped mode: scale * log2(e)
 };
 constexpr int QDO_STAGES = 3, TQB = 64;
+// named barriers of the backward consumers (ids 1, 2: per warpgroup)
+constexpr int BAR_DS_FULL = 3, BAR_DS_FREE = 5;   // + dS^T buffer
 
 // Backward prep, one 8-lane group per (b, h, n): dO = dOg * gate, d_gate = <dOg, O>, delta = gate * d_gate = <dO, O>
 struct AttnPrepP {
@@ -382,21 +389,39 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnPrepP p) {
 
 // P^T / dS^T of one query tile from the S^T / dP^T fragments (rows = keys kr, kr + 8; columns = queries qt0 + 8 g + cq + {0, 1}).
 // UNCLAMPED: P = 2^(s scale log2 e - lse log2 e), dS = P (dP - delta) scale (POLY is then unused).
+// sld: the tile's -lse log2 e (64 floats) then delta (64 floats), zero for queries >= Np.
+// Dropout: the thread's keys kr, kr + 8 have the parity of lane >> 2, so lanes L and L ^ 4 hold the two keys of every hash pair at the
+// same query columns. Each lane hashes one of its two columns (pair index drop_pair + 8 g half_stride + 4 i: the even-stride counter
+// (bh Np + q) stride + key, halved, in 32 bits) and the word its partner needs crosses with one shuffle.
 template <bool UNCLAMPED, bool POLY, bool DROP>
-__device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float (&s)[32], const float (&dp)[32], int bh, int qt0, int cq,
-                                               const bool (&kok)[2], const int (&key)[2], uint32_t seedmix, uint32_t (&ppk)[16], uint32_t (&dpk)[16]) {
+__device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float (&s)[32], const float (&dp)[32], const float* sld, int qt0, int cq,
+                                               const bool (&kok)[2], bool kodd, uint32_t drop_pair, uint32_t seedmix,
+                                               uint32_t (&ppk)[16], uint32_t (&dpk)[16]) {
     const uint32_t thr32 = drop_thresh32(p.drop_thresh);
+    const uint32_t pair_g = 8u * ((uint32_t)p.drop_stride >> 1);
     const float clog = p.clamp * LOG2E_F;
 #pragma unroll
     for (int g = 0; g < 8; ++g) {
+        const float2 nl2 = *reinterpret_cast<const float2*>(sld + 8 * g + cq);
+        const float2 dl2 = *reinterpret_cast<const float2*>(sld + 64 + 8 * g + cq);
+        bool keepw[2][2];   // [key i][query column c]
+        if constexpr (DROP) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const DropWords h = drop_words(seedmix, drop_pair + (uint32_t)g * pair_g + 4u * i);
+                const uint32_t other = __shfl_xor_sync(0xffffffffu, kodd ? h.a : h.b, 4);
+                const bool own = (kodd ? h.b : h.a) >= thr32, oth = other >= thr32;
+                keepw[i][0] = kodd ? oth : own;
+                keepw[i][1] = kodd ? own : oth;
+            }
+        }
         float pe[2][2], dsv[2][2];
 #pragma unroll
         for (int c = 0; c < 2; ++c) {
             const int qi = qt0 + 8 * g + cq + c;
             const bool qok = qi < p.Np;
-            const float nlse2 = qok ? -__ldg(p.lse + (size_t)bh * p.Np + qi) * LOG2E_F : 0.f;
-            const float dl = qok ? __ldg(p.delta + (size_t)bh * p.Np + qi) : 0.f;
-            const unsigned long long qbase = ((unsigned long long)bh * p.Np + (unsigned long long)qi) * (unsigned long long)p.drop_stride;
+            const float nlse2 = c ? nl2.y : nl2.x;
+            const float dl = c ? dl2.y : dl2.x;
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 const int e = 4 * g + 2 * i + c;
@@ -416,8 +441,7 @@ __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float 
                 }
                 float tt, pd;
                 if constexpr (DROP) {
-                    const DropWords h = drop_words(seedmix, (uint32_t)((qbase + (unsigned long long)key[i]) >> 1));
-                    const bool keep = ((key[i] & 1) ? h.b : h.a) >= thr32;
+                    const bool keep = keepw[i][c];
                     tt = __fmaf_rn(keep ? dp[e] : 0.f, p.keep_scale, -dl);
                     pd = keep ? pv : 0.f;   // dV uses the dropped probabilities, dS the un-dropped ones
                 } else {
@@ -437,17 +461,22 @@ __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float 
 }
 
 template <bool UNCLAMPED>
-__global__ void __launch_bounds__(384, 1)
+// 256 threads and no register hand-over: with a third (producer) warpgroup, ptxas allocates every thread against 168 registers
+// (3 warps per SM sub-partition) whatever setmaxnreg grants the consumers, and the consumer live set (S, dP, dV, dK fragments and the
+// packed P / dS) spills there. One consumer thread issues the TMA loads instead.
+__global__ void __launch_bounds__(256, 1)
 attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                      const __grid_constant__ CUtensorMap tmDO, const AttnBwdTcP p) {
+                      const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDQ, const AttnBwdTcP p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sK = smem;                          // 16 KB (128 keys)
     uint8_t* sV = sK + TILE16;                   // 16 KB
     uint8_t* sQ = sV + TILE16;                   // [3] x 8 KB (64 queries)
     uint8_t* sDO = sQ + QDO_STAGES * TILE8;      // [3] x 8 KB
-    uint8_t* sDS = sDO + QDO_STAGES * TILE8;     // [2 warpgroups] x 8 KB: dS^T (64 keys x 64 queries), 128B-swizzled
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sDS + 2 * TILE8);
+    uint8_t* sDS = sDO + QDO_STAGES * TILE8;     // [2 buffers][2 warpgroups] x 8 KB: dS^T (64 keys x 64 queries), 128B-swizzled
+    uint8_t* sDQ = sDS + 4 * TILE8;              // [2 warpgroups] x 16 KB: fp32 dQ staging, two 64 x 32 halves, 128B-swizzled
+    float* sLD = reinterpret_cast<float*>(sDQ + 2 * TILE16);   // [2 warpgroups][2 slots][-lse log2 e x 64 | delta x 64]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sLD + 2 * 2 * 128);
     uint64_t* kv_full = bars;                    // 1
     uint64_t* qdo_full = bars + 1;               // 3
     uint64_t* qdo_empty = bars + 4;              // 3 (one arrival per consumer warpgroup)
@@ -459,36 +488,32 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const int nq = p.nq;
 
     if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO);
+        tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO); tma_prefetch_desc(&tmDQ);
         mbar_init(kv_full, 1);
         for (int i = 0; i < QDO_STAGES; ++i) { mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 2); }
         fence_barrier_init();
     }
     __syncthreads();
 
-    if (wg == 0) {
-        regs_dealloc<40>();
-        if (threadIdx.x == 0) {
-            const int row_base = bh * p.Np;
-            mbar_arrive_expect_tx(kv_full, 2 * TILE16);
-            tma_load_2d(sK, &tmK, kv_full, 0, row_base + k0);
-            tma_load_2d(sV, &tmV, kv_full, 0, row_base + k0);
-            int st = 0;
-            uint32_t ph = 0;
-            for (int i = 0; i < nq; ++i) {
-                mbar_wait(&qdo_empty[st], ph ^ 1);
-                mbar_arrive_expect_tx(&qdo_full[st], 2 * TILE8);
-                const int qt_i = (i + kt) % nq;   // staggered query-tile order: the key-tile CTAs of one head never flush the same dQ rows together
-                tma_load_2d(sQ + st * TILE8, &tmQ, &qdo_full[st], 0, row_base + qt_i * TQB);
-                tma_load_2d(sDO + st * TILE8, &tmDO, &qdo_full[st], 0, row_base + qt_i * TQB);
-                if (++st == QDO_STAGES) { st = 0; ph ^= 1; }
-            }
-        }
-        return;
+    // TMA producer (thread 0): K, V once; query tile j into ring stage j % 3 once the tile j - 3 that used it has been released by
+    // both warpgroups. Tiles 0 and 1 go out here, tile it + 2 at the top of iteration it.
+    const int row_base = bh * p.Np;
+    auto load_qdo = [&](int j) {
+        const int s_j = j % QDO_STAGES;
+        if (j >= QDO_STAGES) mbar_wait(&qdo_empty[s_j], (uint32_t)((j / QDO_STAGES) & 1) ^ 1u);
+        mbar_arrive_expect_tx(&qdo_full[s_j], 2 * TILE8);
+        const int qt_j = (j + kt) % nq;   // staggered query-tile order: the key-tile CTAs of one head never flush the same dQ rows together
+        tma_load_2d(sQ + s_j * TILE8, &tmQ, &qdo_full[s_j], 0, row_base + qt_j * TQB);
+        tma_load_2d(sDO + s_j * TILE8, &tmDO, &qdo_full[s_j], 0, row_base + qt_j * TQB);
+    };
+    if (threadIdx.x == 0) {
+        mbar_arrive_expect_tx(kv_full, 2 * TILE16);
+        tma_load_2d(sK, &tmK, kv_full, 0, row_base + k0);
+        tma_load_2d(sV, &tmV, kv_full, 0, row_base + k0);
+        for (int j = 0; j < 2 && j < nq; ++j) load_qdo(j);
     }
 
-    regs_alloc<232>();
-    const int cw = wg - 1, t = threadIdx.x & 127, lane = t & 31, wq = t >> 5;
+    const int cw = wg, t = threadIdx.x & 127, lane = t & 31, wq = t >> 5;
     const int cq = 2 * (lane & 3);
     const int kr0 = cw * 64 + wq * 16 + (lane >> 2);   // fragment rows (keys) kr0, kr0 + 8 of the CTA's 128
     int key[2];
@@ -499,25 +524,56 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         kok[i] = key[i] < p.Np && ((p.maskbits[(size_t)b * p.mask_words + (key[i] >> 5)] >> (key[i] & 31)) & 1u);
     }
     const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
+    const bool kodd = (lane >> 2) & 1;
+    const bool active = k0 + cw * 64 < p.Np;   // a warpgroup whose 64 keys all lie at or past Np keeps only the barrier protocol
     const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + cw * TILE8), 16, 1024);        // K-major A of S^T
     const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + cw * TILE8), 16, 1024);        // K-major A of dP^T
-    const uint64_t kmn = make_smem_desc_sw128(smem_u32(sK + cw * TILE8), 64 * 128, 1024);    // MN-major B of dQ
-    uint8_t* ds_tile = sDS + cw * TILE8;
-    const uint64_t dsdesc = make_smem_desc_sw128(smem_u32(ds_tile), 64 * 128, 1024);         // MN-major A of dQ (dS^T stored)
+    const uint64_t kmn = make_smem_desc_sw128(smem_u32(sK), 64 * 128, 1024);                 // MN-major B of dQ: all 128 keys
+    uint8_t* dq_stage = sDQ + cw * TILE16;
+    float* ld_own = sLD + cw * 256;
+    // lse / delta of query tile `it` for this thread: threads 0-63 take -lse log2 e, threads 64-127 delta, 0 for queries >= Np
+    const int ld_j = t & 63;
+    const float* ld_src = (t < 64 ? p.lse : p.delta) + (size_t)bh * p.Np;
+    auto ld_tile = [&](int it) {
+        const int qi = ((it + kt) % nq) * TQB + ld_j;
+        float v = 0.f;
+        if (qi < p.Np) {
+            v = __ldg(ld_src + qi);
+            if (t < 64) v = -v * LOG2E_F;
+        }
+        return v;
+    };
     float dv[32], dk[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
 
+    if (active) {
+        ld_own[t] = ld_tile(0);
+    } else {
+        // dS^T = 0 for keys past Np in both buffers, written once: the dQ MMAs run over all 128 keys and add 0 x K for them
+#pragma unroll
+        for (int i = 0; i < 2 * TILE8 / 16 / 128; ++i) {
+            uint8_t* tile = sDS + (2 * (i & 1) + cw) * TILE8;
+            *reinterpret_cast<uint4*>(tile + ((i >> 1) * 128 + t) * 16) = make_uint4(0u, 0u, 0u, 0u);
+        }
+        fence_proxy_async();
+    }
+    named_bar_sync(1 + cw, 128);
     mbar_wait(kv_full, 0);
     int st = 0;
     uint32_t ph = 0;
     for (int it = 0; it < nq; ++it) {
         const int qt0 = ((it + kt) % nq) * TQB;
+        const int buf = it & 1;               // dS^T buffer of this tile, and the warpgroup that reduces its dQ
+        const bool reducer = cw == buf;
+        if (threadIdx.x == 0 && it + 2 < nq) load_qdo(it + 2);
+        const float ld_next = (active && it + 1 < nq) ? ld_tile(it + 1) : 0.f;
         mbar_wait(&qdo_full[st], ph);
-        const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + st * TILE8), 16, 1024);
-        const uint64_t dodesc = make_smem_desc_sw128(smem_u32(sDO + st * TILE8), 16, 1024);
+        uint8_t* ds_tile = sDS + (2 * buf + cw) * TILE8;
         uint32_t ppk[16], dpk[16];   // bf16-packed P_drop^T and dS^T fragments
-        {
+        if (active) {
+            const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + st * TILE8), 16, 1024);
+            const uint64_t dodesc = make_smem_desc_sw128(smem_u32(sDO + st * TILE8), 16, 1024);
             float s[32], dp[32];
             fence_regs(s); fence_regs(dp);
             wgmma_fence();
@@ -528,68 +584,98 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
             wgmma_commit();
             wgmma_wait<0>();
             fence_regs(s); fence_regs(dp);
+            ld_own[(buf ^ 1) * 128 + t] = ld_next;   // read at tile it + 1, after this tile's closing barrier
+            const float* sld = ld_own + buf * 128;
+            const uint32_t drop_pair = ((uint32_t)bh * (uint32_t)p.Np + (uint32_t)(qt0 + cq + kodd)) * ((uint32_t)p.drop_stride >> 1) +
+                                       ((uint32_t)key[0] >> 1);
             const bool drop = p.dropout_p > 0.f;
             if constexpr (UNCLAMPED) {
-                if (drop) bwd_score_math<true, false, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
-                else bwd_score_math<true, false, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                if (drop) bwd_score_math<true, false, true>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+                else bwd_score_math<true, false, false>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
             } else {
                 float amax = 0.f;
 #pragma unroll
                 for (int e = 0; e < 32; ++e) amax = fmaxf(amax, fabsf(s[e]));
                 const bool small = __all_sync(0xffffffffu, amax * fabsf(p.scale_over_clamp) <= TANH_POLY_MAX);   // same rule as the forward
                 if (small) {
-                    if (drop) bwd_score_math<false, true, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
-                    else bwd_score_math<false, true, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                    if (drop) bwd_score_math<false, true, true>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+                    else bwd_score_math<false, true, false>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
                 } else {
-                    if (drop) bwd_score_math<false, false, true>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
-                    else bwd_score_math<false, false, false>(p, s, dp, bh, qt0, cq, kok, key, seedmix, ppk, dpk);
+                    if (drop) bwd_score_math<false, false, true>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+                    else bwd_score_math<false, false, false>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
                 }
             }
         }
-        // dS^T into the warpgroup's swizzled smem tile (row = key, 64 queries = one 128-byte swizzle atom per row)
+        if (!reducer && it >= 2) named_bar_sync(BAR_DS_FREE + buf, 256);   // the dQ MMAs of tile it - 2 have read this buffer
+        if (active) {
+            // dS^T into the warpgroup's swizzled smem tile (row = key, 64 queries = one 128-byte swizzle atom per row)
 #pragma unroll
-        for (int g = 0; g < 8; ++g)
+            for (int g = 0; g < 8; ++g)
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int r = wq * 16 + (lane >> 2) + 8 * i;
-                *reinterpret_cast<uint32_t*>(ds_tile + r * 128 + ((g ^ (r & 7)) << 4) + cq * 2) = dpk[2 * g + i];
+                for (int i = 0; i < 2; ++i) {
+                    const int r = wq * 16 + (lane >> 2) + 8 * i;
+                    *reinterpret_cast<uint32_t*>(ds_tile + r * 128 + ((g ^ (r & 7)) << 4) + cq * 2) = dpk[2 * g + i];
+                }
+            fence_proxy_async();
+        }
+        if (!reducer) named_bar_arrive(BAR_DS_FULL + buf, 256);
+        if (active) {
+            // dV += P^T dO_i, dK += dS^T Q_i (register A: 16 queries per MMA)
+            const uint64_t domn = make_smem_desc_sw128(smem_u32(sDO + st * TILE8), 64 * 128, 1024);
+            const uint64_t qmn = make_smem_desc_sw128(smem_u32(sQ + st * TILE8), 64 * 128, 1024);
+            fence_regs(dv); fence_regs(dk);
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+                const uint32_t ap[4] = {ppk[4 * kk], ppk[4 * kk + 1], ppk[4 * kk + 2], ppk[4 * kk + 3]};
+                wgmma_rs_n64<1>(dv, ap, domn + (uint64_t)(kk * 128), 1u);
             }
-        fence_proxy_async();
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
-        // dV += P^T dO_i, dK += dS^T Q_i (register A: 16 queries per MMA), dQ_i = dS K_w
-        const uint64_t domn = make_smem_desc_sw128(smem_u32(sDO + st * TILE8), 64 * 128, 1024);
-        const uint64_t qmn = make_smem_desc_sw128(smem_u32(sQ + st * TILE8), 64 * 128, 1024);
-        float dq[32];
-        fence_regs(dv); fence_regs(dk); fence_regs(dq);
-        wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-            const uint32_t ap[4] = {ppk[4 * kk], ppk[4 * kk + 1], ppk[4 * kk + 2], ppk[4 * kk + 3]};
-            wgmma_rs_n64<1>(dv, ap, domn + (uint64_t)(kk * 128), 1u);
+            for (int kk = 0; kk < 4; ++kk) {
+                const uint32_t ad[4] = {dpk[4 * kk], dpk[4 * kk + 1], dpk[4 * kk + 2], dpk[4 * kk + 3]};
+                wgmma_rs_n64<1>(dk, ad, qmn + (uint64_t)(kk * 128), 1u);
+            }
+            wgmma_commit();
         }
+        if (reducer) {
+            // dQ_i = dS_i K over the CTA's keys: rows = queries, columns = head dims
+            if (t == 0) bulk_wait_group_read<0>();   // the reduction of tile it - 2 has read the staging tile
+            named_bar_sync(BAR_DS_FULL + buf, 256);
+            const uint64_t dsdesc = make_smem_desc_sw128(smem_u32(sDS + 2 * buf * TILE8), 64 * 128, 1024);   // MN-major A (dS^T stored)
+            float dq[32];
+            fence_regs(dq);
+            wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-            const uint32_t ad[4] = {dpk[4 * kk], dpk[4 * kk + 1], dpk[4 * kk + 2], dpk[4 * kk + 3]};
-            wgmma_rs_n64<1>(dk, ad, qmn + (uint64_t)(kk * 128), 1u);
+            for (int k = 0; k < 8; ++k) wgmma_ss_n64<1, 1>(dq, dsdesc + (uint64_t)(k * 128), kmn + (uint64_t)(k * 128), k > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(dq);
+            if (it + 2 < nq) named_bar_arrive(BAR_DS_FREE + buf, 256);
+            // stage as two 64 x 32 fp32 boxes in the 128B-swizzled layout of the tensor map (bank-conflict free float2 stores)
+#pragma unroll
+            for (int g = 0; g < 8; ++g)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int r = wq * 16 + (lane >> 2) + 8 * i;
+                    const int chunk = 2 * (g & 3) + (cq >> 2);
+                    *reinterpret_cast<float2*>(dq_stage + (g >> 2) * TILE8 + r * 128 + ((chunk ^ (r & 7)) << 4) + (cq & 3) * 4) =
+                        make_float2(dq[4 * g + 2 * i], dq[4 * g + 2 * i + 1]);
+                }
+            fence_proxy_async();
+        } else {
+            wgmma_wait<0>();
         }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_ss_n64<1, 1>(dq, dsdesc + (uint64_t)(k * 128), kmn + (uint64_t)(k * 128), k > 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(dv); fence_regs(dk); fence_regs(dq);
+        fence_regs(dv); fence_regs(dk);
         if (t == 0) mbar_arrive(&qdo_empty[st]);
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");   // every thread's MMAs have read the dS tile before it is rewritten
-        if (++st == QDO_STAGES) { st = 0; ph ^= 1; }
-        // dQ_i partial of this warpgroup's 64 keys: rows = queries, columns = head dims
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int qi = qt0 + wq * 16 + (lane >> 2) + 8 * i;
-            if (qi >= p.Np) continue;
-            float* dqr = p.dq_acc + ((size_t)bh * p.Np + qi) * DH;
-#pragma unroll
-            for (int g = 0; g < 8; ++g) atomicAdd(reinterpret_cast<float2*>(dqr + 8 * g + cq), make_float2(dq[4 * g + 2 * i], dq[4 * g + 2 * i + 1]));
+        named_bar_sync(1 + cw, 128);   // dQ staged; this tile's lse / delta slot read, the next one written
+        if (reducer && t == 0) {
+            tma_reduce_add_3d(&tmDQ, dq_stage, 0, qt0, bh);
+            tma_reduce_add_3d(&tmDQ, dq_stage + TILE8, 32, qt0, bh);
+            bulk_commit_group();
         }
+        if (++st == QDO_STAGES) { st = 0; ph ^= 1; }
     }
+    if (t == 0) bulk_wait_group<0>();
     // ---- dV (with the deferred 1/(1-p) of the dropped probabilities), dK: rows = keys
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
@@ -609,7 +695,7 @@ typedef CUresult (*PFN_encodeTiled2)(CUtensorMap*, CUtensorMapDataType, cuuint32
                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-static int make_head_map(CUtensorMap* m, const void* ptr, long long rows, int box_rows = 128) {
+static PFN_encodeTiled2 tensor_map_encoder() {
     static PFN_encodeTiled2 enc = nullptr;
     if (!enc) {
         void* fn = nullptr;
@@ -617,6 +703,11 @@ static int make_head_map(CUtensorMap* m, const void* ptr, long long rows, int bo
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
             enc = reinterpret_cast<PFN_encodeTiled2>(fn);
     }
+    return enc;
+}
+
+static int make_head_map(CUtensorMap* m, const void* ptr, long long rows, int box_rows = 128) {
+    const PFN_encodeTiled2 enc = tensor_map_encoder();
     B200_REQUIRE(enc, "cuTensorMapEncodeTiled entry point not available");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "attention: operand not 16-byte aligned");
     cuuint64_t gdim[2] = {64, (cuuint64_t)rows};
@@ -626,6 +717,22 @@ static int make_head_map(CUtensorMap* m, const void* ptr, long long rows, int bo
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                      CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     B200_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d)", (int)r);
+    return 0;
+}
+
+// fp32 dq [B*H, Np, 64] as a 3-D map with 64 x 32 boxes (128-byte rows, 128B swizzle): a box at rows >= Np is clipped by the
+// hardware instead of running into the next head
+static int make_dq_map(CUtensorMap* m, float* dq, int BH, int Np) {
+    const PFN_encodeTiled2 enc = tensor_map_encoder();
+    B200_REQUIRE(enc, "cuTensorMapEncodeTiled entry point not available");
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(dq) & 15) == 0, "attn_bwd: dq not 16-byte aligned");
+    cuuint64_t gdim[3] = {DH, (cuuint64_t)Np, (cuuint64_t)BH};
+    cuuint64_t gstride[2] = {DH * sizeof(float), (cuuint64_t)Np * DH * sizeof(float)};
+    cuuint32_t box[3] = {32, TQB, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, dq, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    B200_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (dq) failed (%d)", (int)r);
     return 0;
 }
 
@@ -723,7 +830,7 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     const size_t nelem = (size_t)a->B * a->H * a->Np * DH;
     cudaError_t e = cudaMemsetAsync(a->dq, 0, nelem * sizeof(float), st);
     B200_REQUIRE(e == cudaSuccess, "attn_bwd: memset: %s", cudaGetErrorString(e));
-    p.lse = a->lse; p.delta = a->ws_delta; p.dq_acc = reinterpret_cast<float*>(a->dq);
+    p.lse = a->lse; p.delta = a->ws_delta;
     p.dk = (__nv_bfloat16*)a->dk; p.dv = (__nv_bfloat16*)a->dv;
     p.B = a->B; p.H = a->H; p.Np = a->Np;
     p.scale = a->scale; p.scale_log2e = a->scale * LOG2E_F;
@@ -737,15 +844,17 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     p.keep_scale = 65536.f / (65536.f - (float)p.drop_thresh);
     p.drop_stride = (a->Np + 1) & ~1;
     p.seed = a->seed; p.seed_dev = reinterpret_cast<const unsigned long long*>(a->seed_dev);
-    CUtensorMap tq, tk, tv, tdo;
+    CUtensorMap tq, tk, tv, tdo, tdq;
     const long long rows = (long long)a->B * a->H * a->Np;
-    if (make_head_map(&tq, a->q, rows, TQB) || make_head_map(&tk, a->k, rows) || make_head_map(&tv, a->v, rows) || make_head_map(&tdo, a->ws_dO, rows, TQB)) return -1;
-    const int smem = 2 * TILE16 + 2 * QDO_STAGES * TILE8 + 2 * TILE8 + 128 + 1024;   // K, V, Q/dO rings, dS^T tiles, barriers, slack
+    if (make_head_map(&tq, a->q, rows, TQB) || make_head_map(&tk, a->k, rows) || make_head_map(&tv, a->v, rows) || make_head_map(&tdo, a->ws_dO, rows, TQB) ||
+        make_dq_map(&tdq, reinterpret_cast<float*>(a->dq), a->B * a->H, a->Np)) return -1;
+    // K, V, Q/dO rings, dS^T tiles, dQ staging, lse / delta slots, barriers, alignment slack
+    const int smem = 2 * TILE16 + 2 * QDO_STAGES * TILE8 + 4 * TILE8 + 2 * TILE16 + 2 * 2 * 128 * (int)sizeof(float) + 128 + 1024;
     static DeviceOnce once[2];
     const auto kern = a->unclamped ? attn_bwd_wgmma_kernel<true> : attn_bwd_wgmma_kernel<false>;
     cudaError_t e2 = set_max_smem_once(once[a->unclamped ? 1 : 0], kern, smem);
     B200_REQUIRE(e2 == cudaSuccess, "attn_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
     dim3 grid((a->Np + TKV - 1) / TKV, a->H, a->B);
-    kern<<<grid, 384, smem, st>>>(tq, tk, tv, tdo, p);
+    kern<<<grid, 256, smem, st>>>(tq, tk, tv, tdo, tdq, p);
     return check_launch("attn_bwd_wgmma_kernel");
 }

@@ -95,6 +95,13 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* s
                  ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
                  : "memory");
 }
+// TMA tile REDUCTION (shared -> global, element-wise add into the tensor, bulk async group), 3-D coordinates; the same ordering rules
+// as tma_store_2d, and the same hardware clipping of the box at the tensor's bounds.
+__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const void* smem_src, int c0, int c1, int c2) {
+    asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(m), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
 __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
@@ -103,6 +110,8 @@ __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.
 // named barriers (ids 1..15; __syncthreads owns id 0): bar.sync waits until `n` threads of the CTA have reached barrier `id`
 __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+// counts the calling threads towards barrier `id` without waiting: the producer side of a producer / consumer hand-off
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // 1-D bulk copy global -> shared (TMA engine, no tensor map): `bytes` a multiple of 16, both addresses 16-byte aligned
 __device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
