@@ -22,9 +22,11 @@
 
 namespace b200 {
 
-constexpr int TQ = 128, TKV = 128, DH = 64;
+constexpr int TQ = 128, TKV = 128;
 constexpr int TILE16 = 128 * 64 * 2;          // 16 KB: 128 rows x 64 bf16
 constexpr int TILE8 = 64 * 64 * 2;            // 8 KB: 64 rows x 64 bf16
+// A head row of DH bf16 is DH / 64 128-byte swizzle atoms: every Q / K / V / dO tile is stored as DH / 64 column blocks of 64
+// (one TMA box each), and a K-major operand steps to the next block every 4 k-steps.
 constexpr float LOG2E_F = 1.4426950408889634f;
 
 struct AttnTcP {
@@ -81,16 +83,17 @@ __global__ void attn_maskbits_kernel(const unsigned char* mask, unsigned int* bi
 // ------------------------------------------------------------------------------------------------ forward
 constexpr int KV_STAGES = 3;
 
-template <bool UNCLAMPED>
+template <bool UNCLAMPED, int DH>
 __global__ void __launch_bounds__(384, 1)
 attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const AttnTcP p) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* sQ = smem;                         // 16 KB
-    uint8_t* sK = sQ + TILE16;                  // [3] x 8 KB
-    uint8_t* sV = sK + KV_STAGES * TILE8;       // [3] x 8 KB
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * TILE8);
+    constexpr int NA = DH / 64;                 // column blocks (swizzle atoms) per head row
+    uint8_t* sQ = smem;                         // [NA] x 16 KB
+    uint8_t* sK = sQ + NA * TILE16;             // [3][NA] x 8 KB
+    uint8_t* sV = sK + KV_STAGES * NA * TILE8;  // [3][NA] x 8 KB
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sV + KV_STAGES * NA * TILE8);
     uint64_t* q_full = bars;                    // 1
     uint64_t* kv_full = bars + 1;               // 3
     uint64_t* kv_empty = bars + 4;              // 3 (one arrival per consumer warpgroup)
@@ -114,15 +117,19 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         if (threadIdx.x == 0) {
             // ---------------------------------------------------------------- TMA producer
             const int row_base = bh * p.Np;
-            mbar_arrive_expect_tx(q_full, TILE16);
-            tma_load_2d(sQ, &tmQ, q_full, 0, row_base + q0);
+            mbar_arrive_expect_tx(q_full, NA * TILE16);
+#pragma unroll
+            for (int a = 0; a < NA; ++a) tma_load_2d(sQ + a * TILE16, &tmQ, q_full, 64 * a, row_base + q0);
             int st = 0;
             uint32_t ph = 0;
             for (int j = 0; j < nkv; ++j) {
                 mbar_wait(&kv_empty[st], ph ^ 1);
-                mbar_arrive_expect_tx(&kv_full[st], 2 * TILE8);
-                tma_load_2d(sK + st * TILE8, &tmK, &kv_full[st], 0, row_base + j * 64);
-                tma_load_2d(sV + st * TILE8, &tmV, &kv_full[st], 0, row_base + j * 64);
+                mbar_arrive_expect_tx(&kv_full[st], 2 * NA * TILE8);
+#pragma unroll
+                for (int a = 0; a < NA; ++a) {
+                    tma_load_2d(sK + (st * NA + a) * TILE8, &tmK, &kv_full[st], 64 * a, row_base + j * 64);
+                    tma_load_2d(sV + (st * NA + a) * TILE8, &tmV, &kv_full[st], 64 * a, row_base + j * 64);
+                }
                 if (++st == KV_STAGES) { st = 0; ph ^= 1; }
             }
         }
@@ -149,9 +156,11 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     const uint32_t thr32 = drop_thresh32(p.drop_thresh);
     float l[2] = {0.f, 0.f};
     float m[2] = {-INFINITY, -INFINITY};   // unclamped mode: running row maximum of the raw scores
-    float o[32];
+    float o[NA][32];   // O columns 64 a + 8 j + cq + {0, 1}
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    for (int a = 0; a < NA; ++a)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[a][i] = 0.f;
 
     mbar_wait(q_full, 0);
     const uint64_t qdesc = make_smem_desc_sw128(smem_u32(sQ + cw * TILE8), 16, 1024);
@@ -162,9 +171,11 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         float s[32];
         fence_regs(s);
         wgmma_fence();
-        const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + st * TILE8), 16, 1024);
+        const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + st * NA * TILE8), 16, 1024);
 #pragma unroll
-        for (int k = 0; k < DH / 16; ++k) wgmma_ss_n64<0, 0>(s, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
+        for (int k = 0; k < DH / 16; ++k)
+            wgmma_ss_n64<0, 0>(s, qdesc + (uint64_t)((k >> 2) * (TILE16 >> 4) + (k & 3) * 2), kdesc + (uint64_t)((k >> 2) * (TILE8 >> 4) + (k & 3) * 2),
+                               k > 0 ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(s);
@@ -197,8 +208,11 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
                 float ls = 0.f;
 #pragma unroll
                 for (int g = 0; g < 8; ++g) {
-                    o[4 * g + 2 * i] *= alpha;
-                    o[4 * g + 2 * i + 1] *= alpha;
+#pragma unroll
+                    for (int a = 0; a < NA; ++a) {
+                        o[a][4 * g + 2 * i] *= alpha;
+                        o[a][4 * g + 2 * i + 1] *= alpha;
+                    }
                     s[4 * g + 2 * i] = ex2_approx(__fmaf_rn(s[4 * g + 2 * i], p.scale_log2e, nm));
                     s[4 * g + 2 * i + 1] = ex2_approx(__fmaf_rn(s[4 * g + 2 * i + 1], p.scale_log2e, nm));
                     ls += s[4 * g + 2 * i] + s[4 * g + 2 * i + 1];
@@ -274,18 +288,21 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
                 }
         }
         // O += P V: the accumulator fragment of S is, 16 keys at a time, the register A fragment of the next MMA
-        fence_regs(o);
+#pragma unroll
+        for (int a = 0; a < NA; ++a) fence_regs(o[a]);
         wgmma_fence();
-        const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + st * TILE8), 64 * 128, 1024);
+        const uint64_t vdesc = make_smem_desc_sw128(smem_u32(sV + st * NA * TILE8), 64 * 128, 1024);
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
             const uint32_t a[4] = {pack_bf16(s[8 * kk], s[8 * kk + 1]), pack_bf16(s[8 * kk + 2], s[8 * kk + 3]),
                                    pack_bf16(s[8 * kk + 4], s[8 * kk + 5]), pack_bf16(s[8 * kk + 6], s[8 * kk + 7])};
-            wgmma_rs_n64<1>(o, a, vdesc + (uint64_t)(kk * 128), 1u);
+#pragma unroll
+            for (int na = 0; na < NA; ++na) wgmma_rs_n64<1>(o[na], a, vdesc + (uint64_t)(na * (TILE8 >> 4) + kk * 128), 1u);
         }
         wgmma_commit();
         wgmma_wait<0>();
-        fence_regs(o);
+#pragma unroll
+        for (int a = 0; a < NA; ++a) fence_regs(o[a]);
         if (t == 0) mbar_arrive(&kv_empty[st]);
         if (++st == KV_STAGES) { st = 0; ph ^= 1; }
     }
@@ -302,12 +319,14 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         __nv_bfloat16* orow = p.o + ((size_t)bh * p.Np + qi) * DH;
         __nv_bfloat16* grow = p.og + ((size_t)b * p.Np + qi) * (size_t)(p.H * DH) + hh * DH;
 #pragma unroll
-        for (int g = 0; g < 8; ++g) {
-            const uint32_t u = pack_bf16(o[4 * g + 2 * i] * inv, o[4 * g + 2 * i + 1] * inv);
-            *reinterpret_cast<uint32_t*>(orow + 8 * g + cq) = u;
-            // gate the bf16-rounded output (what the backward pass sees) for consistency
-            *reinterpret_cast<uint32_t*>(grow + 8 * g + cq) = pack_bf16(bf16_lo(u) * gt, bf16_hi(u) * gt);
-        }
+        for (int a = 0; a < NA; ++a)
+#pragma unroll
+            for (int g = 0; g < 8; ++g) {
+                const uint32_t u = pack_bf16(o[a][4 * g + 2 * i] * inv, o[a][4 * g + 2 * i + 1] * inv);
+                *reinterpret_cast<uint32_t*>(orow + 64 * a + 8 * g + cq) = u;
+                // gate the bf16-rounded output (what the backward pass sees) for consistency
+                *reinterpret_cast<uint32_t*>(grow + 64 * a + 8 * g + cq) = pack_bf16(bf16_lo(u) * gt, bf16_hi(u) * gt);
+            }
         if ((lane & 3) == 0) {
             if constexpr (UNCLAMPED) p.lse[(size_t)bh * p.Np + qi] = __fmaf_rn(m[i], p.scale, logf(lt));
             else p.lse[(size_t)bh * p.Np + qi] = logf(lt);
@@ -345,7 +364,7 @@ constexpr int QDO_STAGES = 3, TQB = 64;
 // named barriers of the backward consumers (ids 1, 2: per warpgroup)
 constexpr int BAR_DS_FULL = 3, BAR_DS_FREE = 5;   // + dS^T buffer
 
-// Backward prep, one 8-lane group per (b, h, n): dO = dOg * gate, d_gate = <dOg, O>, delta = gate * d_gate = <dO, O>
+// Backward prep, one DH / 8-lane group per (b, h, n): dO = dOg * gate, d_gate = <dOg, O>, delta = gate * d_gate = <dO, O>
 struct AttnPrepP {
     const float* gate;              // [B*Np, H] or null
     const __nv_bfloat16* o;
@@ -355,10 +374,13 @@ struct AttnPrepP {
     __nv_bfloat16* dO_out;
     float* delta_out;
 };
+template <int DH>
 __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnPrepP p) {
+    constexpr int LANES = DH / 8, LOG2_LANES = DH == 64 ? 3 : 4;
+    static_assert(LANES == 1 << LOG2_LANES, "head dim 64 or 128");
     const long long gidx = (long long)blockIdx.x * 256 + threadIdx.x;
-    const long long rowid = gidx >> 3;
-    const int c = (int)(gidx & 7);
+    const long long rowid = gidx >> LOG2_LANES;
+    const int c = (int)(gidx & (LANES - 1));
     const long long total = (long long)p.B * p.H * p.Np;
     const bool ok = rowid < total;
     float dot = 0.f, gt = 1.f;
@@ -378,22 +400,22 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const AttnPrepP p) {
         }
         *reinterpret_cast<uint4*>(p.dO_out + (size_t)rowid * DH + c * 8) = make_uint4(w[0], w[1], w[2], w[3]);
     }
-    dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-    dot += __shfl_xor_sync(0xffffffffu, dot, 2);
-    dot += __shfl_xor_sync(0xffffffffu, dot, 4);
+#pragma unroll
+    for (int m = 1; m < LANES; m <<= 1) dot += __shfl_xor_sync(0xffffffffu, dot, m);
     if (ok && c == 0) {
         p.delta_out[rowid] = dot * gt;
         if (p.dgate) p.dgate[((size_t)b * p.Np + n) * p.H + hh] = dot;
     }
 }
 
-// P^T / dS^T of one query tile from the S^T / dP^T fragments (rows = keys kr, kr + 8; columns = queries qt0 + 8 g + cq + {0, 1}).
+// P^T / dS^T of one query tile from the S^T / dP^T fragments (rows = keys kr, kr + 8; columns = queries qt0 + 8 g + cq + {0, 1}),
+// for the column groups g = G0 .. G0 + NG - 1 (the head-dim-128 kernel splits the eight between its two warpgroups).
 // UNCLAMPED: P = 2^(s scale log2 e - lse log2 e), dS = P (dP - delta) scale (POLY is then unused).
 // sld: the tile's -lse log2 e (64 floats) then delta (64 floats), zero for queries >= Np.
 // Dropout: the thread's keys kr, kr + 8 have the parity of lane >> 2, so lanes L and L ^ 4 hold the two keys of every hash pair at the
 // same query columns. Each lane hashes one of its two columns (pair index drop_pair + 8 g half_stride + 4 i: the even-stride counter
 // (bh Np + q) stride + key, halved, in 32 bits) and the word its partner needs crosses with one shuffle.
-template <bool UNCLAMPED, bool POLY, bool DROP>
+template <bool UNCLAMPED, bool POLY, bool DROP, int G0 = 0, int NG = 8>
 __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float (&s)[32], const float (&dp)[32], const float* sld, int qt0, int cq,
                                                const bool (&kok)[2], bool kodd, uint32_t drop_pair, uint32_t seedmix,
                                                uint32_t (&ppk)[16], uint32_t (&dpk)[16]) {
@@ -401,7 +423,7 @@ __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float 
     const uint32_t pair_g = 8u * ((uint32_t)p.drop_stride >> 1);
     const float clog = p.clamp * LOG2E_F;
 #pragma unroll
-    for (int g = 0; g < 8; ++g) {
+    for (int g = G0; g < G0 + NG; ++g) {
         const float2 nl2 = *reinterpret_cast<const float2*>(sld + 8 * g + cq);
         const float2 dl2 = *reinterpret_cast<const float2*>(sld + 64 + 8 * g + cq);
         bool keepw[2][2];   // [key i][query column c]
@@ -461,12 +483,13 @@ __device__ __forceinline__ void bwd_score_math(const AttnBwdTcP& p, const float 
 }
 
 template <bool UNCLAMPED>
-// 256 threads and no register hand-over: with a third (producer) warpgroup, ptxas allocates every thread against 168 registers
+// Head dim 64. 256 threads and no register hand-over: with a third (producer) warpgroup, ptxas allocates every thread against 168 registers
 // (3 warps per SM sub-partition) whatever setmaxnreg grants the consumers, and the consumer live set (S, dP, dV, dK fragments and the
 // packed P / dS) spills there. One consumer thread issues the TMA loads instead.
 __global__ void __launch_bounds__(256, 1)
 attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                       const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDQ, const AttnBwdTcP p) {
+    constexpr int DH = 64;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* sK = smem;                          // 16 KB (128 keys)
@@ -690,6 +713,245 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     }
 }
 
+// Head dim 128. Doubling the head-dim-64 kernel does not fit: dK and dV of 64 keys x 128 dims would take 128 accumulator registers
+// per thread next to S^T, dP^T and their packed operands (~290 in all), and the tiles ~256 KB of shared memory. So the two
+// warpgroups share ONE 64-key tile and split the work instead of the keys — one CTA per (64-key tile, head, batch), 256 threads:
+//   warpgroup 0 computes S^T = K Q_i^T, warpgroup 1 dP^T = V dO_i^T (m64n64k16, 8 k-steps over both column blocks of the head);
+//   each hands the half of its fragment the other needs through shared memory (fp32, fragment order), so warpgroup 0 does the score
+//   math of query columns 0-31 and warpgroup 1 of columns 32-63 (the same fragment positions, so the dropout hash, its lane pairing
+//   and the score arithmetic are the head-dim-64 kernel's, element for element);
+//   both write their P^T / dS^T columns into swizzled bf16 tiles, and warpgroup w then owns head dims 64 w .. 64 w + 63 of
+//   dV += P^T dO_i, dK += dS^T Q_i and dQ_i = dS_i K (all operands from shared memory, 4 k-steps each), 96 accumulator registers.
+//   Each warpgroup stages its 64 x 64 fp32 dQ block and adds it into dq with two TMA reductions (a [B*H, Np, 128] map, 32-float
+//   boxes): one reduction per key tile, as in the head-dim-64 kernel.
+// Per query tile: BAR_X (exchange halves written; also orders the lse / delta slot) and BAR_PDS (P^T / dS^T written, dQ staging free).
+// Every warpgroup waits for its own MMAs before it reaches the next tile's BAR_X, so single exchange and P^T / dS^T buffers suffice.
+constexpr int BAR_X = 3, BAR_PDS = 4;
+// One warpgroup's half of the head-dim-128 score math for one query tile: warpgroup W holds S^T (W = 0) or dP^T (W = 1) in `acc`,
+// hands the other warpgroup the fragment elements of its query columns through sX, takes its own from the other's, and writes
+// P_drop^T and dS^T of query columns 32 W .. 32 W + 31 (column groups g = 4 W .. 4 W + 3) into the swizzled tiles.
+template <bool UNCLAMPED, int W>
+__device__ __forceinline__ void d128_score_half(const AttnBwdTcP& p, const float (&acc)[32], float* sX, float* sLD, int slot, float ld_next,
+                                                bool last, uint8_t* sP, uint8_t* sDS, int t, int kr0, int qt0, int cq, const bool (&kok)[2],
+                                                bool kodd, uint32_t drop_pair, uint32_t seedmix) {
+    constexpr int KEEP = 16 * W, GIVE = 16 - KEEP;   // first fragment element this warpgroup scores / hands over
+#pragma unroll
+    for (int e = 0; e < 16; ++e) sX[(W * 16 + e) * 128 + t] = acc[GIVE + e];
+    if (W == 0 && !last) sLD[(slot ^ 1) * 128 + t] = ld_next;   // read at the next tile, after its BAR_X
+    named_bar_sync(BAR_X, 256);
+    float oth[32];
+#pragma unroll
+    for (int e = 0; e < 16; ++e) oth[KEEP + e] = sX[((W ^ 1) * 16 + e) * 128 + t];
+    const float* sld = sLD + slot * 128;
+    const bool drop = p.dropout_p > 0.f;
+    uint32_t ppk[16], dpk[16];
+    auto score = [&](const float (&s)[32], const float (&dp)[32]) {
+        if constexpr (UNCLAMPED) {
+            if (drop) bwd_score_math<true, false, true, 4 * W, 4>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+            else bwd_score_math<true, false, false, 4 * W, 4>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+        } else {
+            float amax = 0.f;
+#pragma unroll
+            for (int e = KEEP; e < KEEP + 16; ++e) amax = fmaxf(amax, fabsf(s[e]));
+            if (__all_sync(0xffffffffu, amax * fabsf(p.scale_over_clamp) <= TANH_POLY_MAX)) {   // same rule as the forward
+                if (drop) bwd_score_math<false, true, true, 4 * W, 4>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+                else bwd_score_math<false, true, false, 4 * W, 4>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+            } else {
+                if (drop) bwd_score_math<false, false, true, 4 * W, 4>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+                else bwd_score_math<false, false, false, 4 * W, 4>(p, s, dp, sld, qt0, cq, kok, kodd, drop_pair, seedmix, ppk, dpk);
+            }
+        }
+    };
+    if constexpr (W == 0) score(acc, oth);
+    else score(oth, acc);
+#pragma unroll
+    for (int g = 4 * W; g < 4 * W + 4; ++g)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int r = kr0 + 8 * i;
+            const int off = r * 128 + ((g ^ (r & 7)) << 4) + cq * 2;
+            *reinterpret_cast<uint32_t*>(sP + off) = ppk[2 * g + i];
+            *reinterpret_cast<uint32_t*>(sDS + off) = dpk[2 * g + i];
+        }
+}
+
+template <bool UNCLAMPED>
+__global__ void __launch_bounds__(256, 1)
+attn_bwd_d128_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                           const __grid_constant__ CUtensorMap tmDO, const __grid_constant__ CUtensorMap tmDQ, const AttnBwdTcP p) {
+    constexpr int DH = 128;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    uint8_t* sK = smem;                          // [2 column blocks] x 8 KB (64 keys)
+    uint8_t* sV = sK + 2 * TILE8;                // [2] x 8 KB
+    uint8_t* sQ = sV + 2 * TILE8;                // [3 stages][2] x 8 KB (64 queries)
+    uint8_t* sDO = sQ + QDO_STAGES * 2 * TILE8;  // [3][2] x 8 KB
+    uint8_t* sP = sDO + QDO_STAGES * 2 * TILE8;  // P_drop^T (64 keys x 64 queries), 128B-swizzled
+    uint8_t* sDS = sP + TILE8;                   // dS^T, same layout
+    uint8_t* sDQ = sDS + TILE8;                  // [2 warpgroups] x 16 KB: fp32 dQ staging, two 64 x 32 boxes each, 128B-swizzled
+    float* sX = reinterpret_cast<float*>(sDQ + 2 * TILE16);   // [2 warpgroups][16 fragment elements][128 threads] fp32
+    float* sLD = sX + 2 * 16 * 128;              // [2 slots][-lse log2 e x 64 | delta x 64]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sLD + 2 * 128);
+    uint64_t* kv_full = bars;                    // 1
+    uint64_t* qdo_full = bars + 1;               // 3
+    uint64_t* qdo_empty = bars + 4;              // 3 (one arrival per consumer warpgroup)
+
+    const int wg = threadIdx.x >> 7;
+    const int kt = blockIdx.x, hh = blockIdx.y, b = blockIdx.z;
+    const int bh = b * p.H + hh;
+    const int k0 = kt * 64;
+    const int nq = p.nq;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmQ); tma_prefetch_desc(&tmK); tma_prefetch_desc(&tmV); tma_prefetch_desc(&tmDO); tma_prefetch_desc(&tmDQ);
+        mbar_init(kv_full, 1);
+        for (int i = 0; i < QDO_STAGES; ++i) { mbar_init(&qdo_full[i], 1); mbar_init(&qdo_empty[i], 2); }
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    const int row_base = bh * p.Np;
+    auto load_qdo = [&](int j) {
+        const int s_j = j % QDO_STAGES;
+        if (j >= QDO_STAGES) mbar_wait(&qdo_empty[s_j], (uint32_t)((j / QDO_STAGES) & 1) ^ 1u);
+        mbar_arrive_expect_tx(&qdo_full[s_j], 4 * TILE8);
+        const int qt_j = (j + kt) % nq;   // staggered query-tile order, as in the head-dim-64 kernel
+#pragma unroll
+        for (int a = 0; a < 2; ++a) {
+            tma_load_2d(sQ + (2 * s_j + a) * TILE8, &tmQ, &qdo_full[s_j], 64 * a, row_base + qt_j * TQB);
+            tma_load_2d(sDO + (2 * s_j + a) * TILE8, &tmDO, &qdo_full[s_j], 64 * a, row_base + qt_j * TQB);
+        }
+    };
+    if (threadIdx.x == 0) {
+        mbar_arrive_expect_tx(kv_full, 4 * TILE8);
+#pragma unroll
+        for (int a = 0; a < 2; ++a) {
+            tma_load_2d(sK + a * TILE8, &tmK, kv_full, 64 * a, row_base + k0);
+            tma_load_2d(sV + a * TILE8, &tmV, kv_full, 64 * a, row_base + k0);
+        }
+        for (int j = 0; j < 2 && j < nq; ++j) load_qdo(j);
+    }
+
+    const int cw = wg, t = threadIdx.x & 127, lane = t & 31, wq = t >> 5;
+    const int cq = 2 * (lane & 3);
+    const int kr0 = wq * 16 + (lane >> 2);   // fragment rows (keys) kr0, kr0 + 8 of the CTA's 64
+    int key[2];
+    bool kok[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        key[i] = k0 + kr0 + 8 * i;
+        kok[i] = key[i] < p.Np && ((p.maskbits[(size_t)b * p.mask_words + (key[i] >> 5)] >> (key[i] & 31)) & 1u);
+    }
+    const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
+    const bool kodd = (lane >> 2) & 1;
+    // S^T (warpgroup 0): A = K, B = Q_i; dP^T (warpgroup 1): A = V, B = dO_i — both K-major over the 128 head dims
+    const uint64_t adesc = make_smem_desc_sw128(smem_u32(cw == 0 ? sK : sV), 16, 1024);
+    const uint64_t kmn = make_smem_desc_sw128(smem_u32(sK + cw * TILE8), 64 * 128, 1024);   // MN-major B of dQ: this warpgroup's dims
+    const uint64_t pdesc = make_smem_desc_sw128(smem_u32(sP), 16, 1024);                     // K-major A of dV (P^T stored)
+    const uint64_t dskm = make_smem_desc_sw128(smem_u32(sDS), 16, 1024);                     // K-major A of dK
+    const uint64_t dsmn = make_smem_desc_sw128(smem_u32(sDS), 64 * 128, 1024);               // MN-major A of dQ
+    uint8_t* dq_stage = sDQ + cw * TILE16;
+    // lse / delta of query tile `it` (warpgroup 0 loads them): threads 0-63 take -lse log2 e, threads 64-127 delta, 0 for queries >= Np
+    const int ld_j = t & 63;
+    const float* ld_src = (t < 64 ? p.lse : p.delta) + (size_t)bh * p.Np;
+    auto ld_tile = [&](int it) {
+        const int qi = ((it + kt) % nq) * TQB + ld_j;
+        float v = 0.f;
+        if (qi < p.Np) {
+            v = __ldg(ld_src + qi);
+            if (t < 64) v = -v * LOG2E_F;
+        }
+        return v;
+    };
+    float dv[32], dk[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) { dv[i] = 0.f; dk[i] = 0.f; }
+
+    if (cw == 0) sLD[t] = ld_tile(0);
+    __syncthreads();
+    mbar_wait(kv_full, 0);
+    int st = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < nq; ++it) {
+        const int qt0 = ((it + kt) % nq) * TQB;
+        const int slot = it & 1;
+        if (threadIdx.x == 0 && it + 2 < nq) load_qdo(it + 2);
+        const float ld_next = (cw == 0 && it + 1 < nq) ? ld_tile(it + 1) : 0.f;
+        mbar_wait(&qdo_full[st], ph);
+        float acc[32];   // warpgroup 0: S^T, warpgroup 1: dP^T
+        {
+            const uint64_t bdesc = make_smem_desc_sw128(smem_u32((cw == 0 ? sQ : sDO) + 2 * st * TILE8), 16, 1024);
+            fence_regs(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < DH / 16; ++k) {
+                const uint64_t off = (uint64_t)((k >> 2) * (TILE8 >> 4) + (k & 3) * 2);
+                wgmma_ss_n64<0, 0>(acc, adesc + off, bdesc + off, k > 0 ? 1u : 0u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(acc);
+        }
+        const uint32_t drop_pair = ((uint32_t)bh * (uint32_t)p.Np + (uint32_t)(qt0 + cq + kodd)) * ((uint32_t)p.drop_stride >> 1) +
+                                   ((uint32_t)key[0] >> 1);
+        const bool last = it + 1 >= nq;
+        if (cw == 0) d128_score_half<UNCLAMPED, 0>(p, acc, sX, sLD, slot, ld_next, last, sP, sDS, t, kr0, qt0, cq, kok, kodd, drop_pair, seedmix);
+        else d128_score_half<UNCLAMPED, 1>(p, acc, sX, sLD, slot, ld_next, last, sP, sDS, t, kr0, qt0, cq, kok, kodd, drop_pair, seedmix);
+        fence_proxy_async();
+        if (t == 0) bulk_wait_group_read<0>();   // the reduction of the previous tile has read this warpgroup's dQ staging
+        named_bar_sync(BAR_PDS, 256);
+        // dV += P^T dO_i, dK += dS^T Q_i, dQ_i = dS_i K, each on this warpgroup's 64 head dims (column block cw)
+        float dq[32];
+        {
+            const uint64_t domn = make_smem_desc_sw128(smem_u32(sDO + (2 * st + cw) * TILE8), 64 * 128, 1024);
+            const uint64_t qmn = make_smem_desc_sw128(smem_u32(sQ + (2 * st + cw) * TILE8), 64 * 128, 1024);
+            fence_regs(dv); fence_regs(dk); fence_regs(dq);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_ss_n64<0, 1>(dv, pdesc + (uint64_t)(k * 2), domn + (uint64_t)(k * 128), 1u);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_ss_n64<0, 1>(dk, dskm + (uint64_t)(k * 2), qmn + (uint64_t)(k * 128), 1u);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) wgmma_ss_n64<1, 1>(dq, dsmn + (uint64_t)(k * 128), kmn + (uint64_t)(k * 128), k > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(dv); fence_regs(dk); fence_regs(dq);
+        }
+        if (t == 0) mbar_arrive(&qdo_empty[st]);
+        // stage as two 64 x 32 fp32 boxes in the 128B-swizzled layout of the tensor map (rows = queries)
+#pragma unroll
+        for (int g = 0; g < 8; ++g)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int r = kr0 + 8 * i;
+                const int chunk = 2 * (g & 3) + (cq >> 2);
+                *reinterpret_cast<float2*>(dq_stage + (g >> 2) * TILE8 + r * 128 + ((chunk ^ (r & 7)) << 4) + (cq & 3) * 4) =
+                    make_float2(dq[4 * g + 2 * i], dq[4 * g + 2 * i + 1]);
+            }
+        fence_proxy_async();
+        named_bar_sync(1 + cw, 128);
+        if (t == 0) {
+            tma_reduce_add_3d(&tmDQ, dq_stage, 64 * cw, qt0, bh);
+            tma_reduce_add_3d(&tmDQ, dq_stage + TILE8, 64 * cw + 32, qt0, bh);
+            bulk_commit_group();
+        }
+        if (++st == QDO_STAGES) { st = 0; ph ^= 1; }
+    }
+    if (t == 0) bulk_wait_group<0>();
+    // ---- dV (with the deferred 1/(1-p) of the dropped probabilities), dK: rows = keys, columns 64 cw + 8 g + cq + {0, 1}
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+        if (key[i] >= p.Np) continue;
+        __nv_bfloat16* dvp = p.dv + ((size_t)bh * p.Np + key[i]) * DH + 64 * cw;
+        __nv_bfloat16* dkp = p.dk + ((size_t)bh * p.Np + key[i]) * DH + 64 * cw;
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+            *reinterpret_cast<uint32_t*>(dvp + 8 * g + cq) = pack_bf16(dv[4 * g + 2 * i] * p.keep_scale, dv[4 * g + 2 * i + 1] * p.keep_scale);
+            *reinterpret_cast<uint32_t*>(dkp + 8 * g + cq) = pack_bf16(dk[4 * g + 2 * i], dk[4 * g + 2 * i + 1]);
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------- host
 typedef CUresult (*PFN_encodeTiled2)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -706,12 +968,13 @@ static PFN_encodeTiled2 tensor_map_encoder() {
     return enc;
 }
 
-static int make_head_map(CUtensorMap* m, const void* ptr, long long rows, int box_rows = 128) {
+// bf16 [rows, dh] with boxes of 64 columns (one 128-byte swizzle atom) x box_rows rows
+static int make_head_map(CUtensorMap* m, const void* ptr, long long rows, int dh, int box_rows) {
     const PFN_encodeTiled2 enc = tensor_map_encoder();
     B200_REQUIRE(enc, "cuTensorMapEncodeTiled entry point not available");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "attention: operand not 16-byte aligned");
-    cuuint64_t gdim[2] = {64, (cuuint64_t)rows};
-    cuuint64_t gstride[1] = {128};
+    cuuint64_t gdim[2] = {(cuuint64_t)dh, (cuuint64_t)rows};
+    cuuint64_t gstride[1] = {(cuuint64_t)dh * 2};
     cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -720,14 +983,14 @@ static int make_head_map(CUtensorMap* m, const void* ptr, long long rows, int bo
     return 0;
 }
 
-// fp32 dq [B*H, Np, 64] as a 3-D map with 64 x 32 boxes (128-byte rows, 128B swizzle): a box at rows >= Np is clipped by the
-// hardware instead of running into the next head
-static int make_dq_map(CUtensorMap* m, float* dq, int BH, int Np) {
+// fp32 dq [B*H, Np, dh] as a 3-D map with 64 x 32 boxes (128-byte rows, 128B swizzle; dh / 32 boxes per row): a box at rows >= Np
+// is clipped by the hardware instead of running into the next head
+static int make_dq_map(CUtensorMap* m, float* dq, int BH, int Np, int dh) {
     const PFN_encodeTiled2 enc = tensor_map_encoder();
     B200_REQUIRE(enc, "cuTensorMapEncodeTiled entry point not available");
     B200_REQUIRE((reinterpret_cast<uintptr_t>(dq) & 15) == 0, "attn_bwd: dq not 16-byte aligned");
-    cuuint64_t gdim[3] = {DH, (cuuint64_t)Np, (cuuint64_t)BH};
-    cuuint64_t gstride[2] = {DH * sizeof(float), (cuuint64_t)Np * DH * sizeof(float)};
+    cuuint64_t gdim[3] = {(cuuint64_t)dh, (cuuint64_t)Np, (cuuint64_t)BH};
+    cuuint64_t gstride[2] = {dh * sizeof(float), (cuuint64_t)Np * dh * sizeof(float)};
     cuuint32_t box[3] = {32, TQB, 1};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, dq, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -756,7 +1019,7 @@ extern "C" int b200_attn_maskbits(const uint8_t* keymask, void* ws_maskbits, int
 extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B200_REQUIRE(a && a->q && a->k && a->v && a->o && a->og && a->lse && a->ws_maskbits, "attn_fwd: null pointer");
-    B200_REQUIRE(a->dim_head == 64, "attn_fwd: only dim_head 64 is built (got %d)", a->dim_head);
+    B200_REQUIRE(a->dim_head == 64 || a->dim_head == 128, "attn_fwd: dim_head must be 64 or 128 (got %d)", a->dim_head);
     B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_fwd: bad shape");
     if (a->unclamped) {
         B200_REQUIRE(a->softclamp == 0.f, "attn_fwd: unclamped attention needs softclamp == 0 (got %g)", a->softclamp);
@@ -790,11 +1053,13 @@ extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) 
     p.drop_stride = (a->Np + 1) & ~1;
     CUtensorMap tq, tk, tv;
     const long long rows = (long long)a->B * a->H * a->Np;
-    if (make_head_map(&tq, a->q, rows) || make_head_map(&tk, a->k, rows, 64) || make_head_map(&tv, a->v, rows, 64)) return -1;
-    const int smem = TILE16 + 2 * KV_STAGES * TILE8 + 128 + 1024;   // Q, K/V rings, barriers, alignment slack
-    static DeviceOnce once[2];
-    const auto kern = a->unclamped ? attn_fwd_wgmma_kernel<true> : attn_fwd_wgmma_kernel<false>;
-    cudaError_t e = set_max_smem_once(once[a->unclamped ? 1 : 0], kern, smem);
+    const int dh = a->dim_head, na = dh / 64;
+    if (make_head_map(&tq, a->q, rows, dh, 128) || make_head_map(&tk, a->k, rows, dh, 64) || make_head_map(&tv, a->v, rows, dh, 64)) return -1;
+    const int smem = na * (TILE16 + 2 * KV_STAGES * TILE8) + 128 + 1024;   // Q, K/V rings, barriers, alignment slack
+    static DeviceOnce once[4];
+    const auto kern = dh == 64 ? (a->unclamped ? attn_fwd_wgmma_kernel<true, 64> : attn_fwd_wgmma_kernel<false, 64>)
+                               : (a->unclamped ? attn_fwd_wgmma_kernel<true, 128> : attn_fwd_wgmma_kernel<false, 128>);
+    cudaError_t e = set_max_smem_once(once[(a->unclamped ? 1 : 0) + (dh == 128 ? 2 : 0)], kern, smem);
     B200_REQUIRE(e == cudaSuccess, "attn_fwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     dim3 grid((a->Np + TQ - 1) / TQ, a->H, a->B);
     kern<<<grid, 384, smem, st>>>(tq, tk, tv, p);
@@ -805,7 +1070,7 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B200_REQUIRE(a && a->q && a->k && a->v && a->o && a->d_og && a->lse && a->ws_dO && a->ws_delta && a->dq && a->dk && a->dv && a->ws_maskbits,
                  "attn_bwd: null pointer");
-    B200_REQUIRE(a->dim_head == 64, "attn_bwd: only dim_head 64 is built (got %d)", a->dim_head);
+    B200_REQUIRE(a->dim_head == 64 || a->dim_head == 128, "attn_bwd: dim_head must be 64 or 128 (got %d)", a->dim_head);
     B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_bwd: bad shape");
     if (a->unclamped) {
         B200_REQUIRE(a->softclamp == 0.f, "attn_bwd: unclamped attention needs softclamp == 0 (got %g)", a->softclamp);
@@ -815,8 +1080,10 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
                  "running maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
     const AttnPrepP pp{a->gate, (const __nv_bfloat16*)a->o, a->B, a->H, a->Np, (const __nv_bfloat16*)a->d_og, a->d_gate,
                        (__nv_bfloat16*)a->ws_dO, a->ws_delta};
-    const long long prep_threads = (long long)a->B * a->H * a->Np * 8;
-    attn_bwd_prep_kernel<<<(unsigned)((prep_threads + 255) / 256), 256, 0, st>>>(pp);
+    const int dh = a->dim_head;
+    const long long prep_threads = (long long)a->B * a->H * a->Np * (dh / 8);
+    if (dh == 64) attn_bwd_prep_kernel<64><<<(unsigned)((prep_threads + 255) / 256), 256, 0, st>>>(pp);
+    else attn_bwd_prep_kernel<128><<<(unsigned)((prep_threads + 255) / 256), 256, 0, st>>>(pp);
     if (int rc = check_launch("attn_bwd_prep_kernel")) return rc;
     AttnBwdTcP p{};
     p.nq = (a->Np + TQB - 1) / TQB;
@@ -827,7 +1094,7 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
         attn_maskbits_kernel<<<(total + 127) / 128, 128, 0, st>>>(a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits), a->B, a->Np, p.mask_words);
         if (int rc = check_launch("attn_maskbits_kernel")) return rc;
     }
-    const size_t nelem = (size_t)a->B * a->H * a->Np * DH;
+    const size_t nelem = (size_t)a->B * a->H * a->Np * dh;
     cudaError_t e = cudaMemsetAsync(a->dq, 0, nelem * sizeof(float), st);
     B200_REQUIRE(e == cudaSuccess, "attn_bwd: memset: %s", cudaGetErrorString(e));
     p.lse = a->lse; p.delta = a->ws_delta;
@@ -846,15 +1113,26 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     p.seed = a->seed; p.seed_dev = reinterpret_cast<const unsigned long long*>(a->seed_dev);
     CUtensorMap tq, tk, tv, tdo, tdq;
     const long long rows = (long long)a->B * a->H * a->Np;
-    if (make_head_map(&tq, a->q, rows, TQB) || make_head_map(&tk, a->k, rows) || make_head_map(&tv, a->v, rows) || make_head_map(&tdo, a->ws_dO, rows, TQB) ||
-        make_dq_map(&tdq, reinterpret_cast<float*>(a->dq), a->B * a->H, a->Np)) return -1;
-    // K, V, Q/dO rings, dS^T tiles, dQ staging, lse / delta slots, barriers, alignment slack
-    const int smem = 2 * TILE16 + 2 * QDO_STAGES * TILE8 + 4 * TILE8 + 2 * TILE16 + 2 * 2 * 128 * (int)sizeof(float) + 128 + 1024;
+    const int kv_rows = dh == 64 ? TKV : 64;   // keys per CTA
+    if (make_head_map(&tq, a->q, rows, dh, TQB) || make_head_map(&tk, a->k, rows, dh, kv_rows) || make_head_map(&tv, a->v, rows, dh, kv_rows) ||
+        make_head_map(&tdo, a->ws_dO, rows, dh, TQB) || make_dq_map(&tdq, reinterpret_cast<float*>(a->dq), a->B * a->H, a->Np, dh)) return -1;
+    dim3 grid((a->Np + kv_rows - 1) / kv_rows, a->H, a->B);
+    if (dh == 64) {
+        // K, V, Q/dO rings, dS^T tiles, dQ staging, lse / delta slots, barriers, alignment slack
+        const int smem = 2 * TILE16 + 2 * QDO_STAGES * TILE8 + 4 * TILE8 + 2 * TILE16 + 2 * 2 * 128 * (int)sizeof(float) + 128 + 1024;
+        static DeviceOnce once[2];
+        const auto kern = a->unclamped ? attn_bwd_wgmma_kernel<true> : attn_bwd_wgmma_kernel<false>;
+        cudaError_t e2 = set_max_smem_once(once[a->unclamped ? 1 : 0], kern, smem);
+        B200_REQUIRE(e2 == cudaSuccess, "attn_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
+        kern<<<grid, 256, smem, st>>>(tq, tk, tv, tdo, tdq, p);
+        return check_launch("attn_bwd_wgmma_kernel");
+    }
+    // K, V (2 column blocks each), Q/dO rings, P^T and dS^T tiles, dQ staging, exchange halves, lse / delta slots, barriers, alignment
+    const int smem = 4 * TILE8 + 4 * QDO_STAGES * TILE8 + 2 * TILE8 + 2 * TILE16 + (2 * 16 * 128 + 2 * 128) * (int)sizeof(float) + 128 + 1024;
     static DeviceOnce once[2];
-    const auto kern = a->unclamped ? attn_bwd_wgmma_kernel<true> : attn_bwd_wgmma_kernel<false>;
+    const auto kern = a->unclamped ? attn_bwd_d128_wgmma_kernel<true> : attn_bwd_d128_wgmma_kernel<false>;
     cudaError_t e2 = set_max_smem_once(once[a->unclamped ? 1 : 0], kern, smem);
     B200_REQUIRE(e2 == cudaSuccess, "attn_bwd: cudaFuncSetAttribute: %s", cudaGetErrorString(e2));
-    dim3 grid((a->Np + TKV - 1) / TKV, a->H, a->B);
     kern<<<grid, 256, smem, st>>>(tq, tk, tv, tdo, tdq, p);
-    return check_launch("attn_bwd_wgmma_kernel");
+    return check_launch("attn_bwd_d128_wgmma_kernel");
 }

@@ -210,7 +210,8 @@ __global__ void rotary_table_kernel(float* cs, float* sn, int Np, int half) {
 
 // ------------------------------------------------------------------------------------------------ qkv post
 // qkvg [T, ld] = [q(I) | k(I) | v(I) | gate(h) | mix(h)] (raw GEMM output), or [q | k | v | mix(h)] without the head gate
-// (no_gate). Produces rotated q,k and the value-residual-mixed v in [B,H,Np,64] (A.3, A.4 steps 1-3), plus sigmoid(head gate) [T,H] fp32.
+// (no_gate), I = H * DH. Produces rotated q,k and the value-residual-mixed v in [B,H,Np,DH] (A.3, A.4 steps 1-3), plus sigmoid(head
+// gate) [T,H] fp32. One DH / 8-lane group per (token, head), 8 elements (4 rotary pairs) per lane; the rotary table is [Np, DH / 2].
 struct QkvP {
     const __nv_bfloat16* qkvg; int ld;
     const float *gate_b, *mix_b, *cs, *sn;
@@ -225,29 +226,32 @@ struct QkvP {
     int dq_fp32;
     int no_gate;
 };
+template <int DH>
 __global__ void __launch_bounds__(256) qkv_post_fwd_kernel(const QkvP p) {
-    const long long total = (long long)p.B * p.Np * p.H * 8;
-    const int I = p.H * 64;
+    constexpr int LANES = DH / 8, LOG2_LANES = DH == 64 ? 3 : 4;
+    static_assert(LANES == 1 << LOG2_LANES, "head dim 64 or 128");
+    const long long total = (long long)p.B * p.Np * p.H * LANES;
+    const int I = p.H * DH;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < total; i += (long long)gridDim.x * 256) {
-        const int c = (int)(i & 7);
-        const int hh = (int)((i >> 3) % p.H);
-        const long long tok = (i >> 3) / p.H;
+        const int c = (int)(i & (LANES - 1));
+        const int hh = (int)((i >> LOG2_LANES) % p.H);
+        const long long tok = (i >> LOG2_LANES) / p.H;
         const int n = (int)(tok % p.Np), b = (int)(tok / p.Np);
         const __nv_bfloat16* row = p.qkvg + (size_t)tok * p.ld;
-        const size_t dst = (((size_t)b * p.H + hh) * p.Np + n) * 64 + c * 8;
+        const size_t dst = (((size_t)b * p.H + hh) * p.Np + n) * DH + c * 8;
         float cs[4], sn[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) { cs[j] = p.cs[n * 32 + c * 4 + j]; sn[j] = p.sn[n * 32 + c * 4 + j]; }
+        for (int j = 0; j < 4; ++j) { cs[j] = p.cs[n * (DH / 2) + c * 4 + j]; sn[j] = p.sn[n * (DH / 2) + c * 4 + j]; }
         float x[8], y[8];
-        unpack8(*reinterpret_cast<const uint4*>(row + hh * 64 + c * 8), x);
+        unpack8(*reinterpret_cast<const uint4*>(row + hh * DH + c * 8), x);
 #pragma unroll
         for (int j = 0; j < 4; ++j) { y[2 * j] = x[2 * j] * cs[j] - x[2 * j + 1] * sn[j]; y[2 * j + 1] = x[2 * j + 1] * cs[j] + x[2 * j] * sn[j]; }
         *reinterpret_cast<uint4*>(p.q + dst) = pack8(y);
-        unpack8(*reinterpret_cast<const uint4*>(row + I + hh * 64 + c * 8), x);
+        unpack8(*reinterpret_cast<const uint4*>(row + I + hh * DH + c * 8), x);
 #pragma unroll
         for (int j = 0; j < 4; ++j) { y[2 * j] = x[2 * j] * cs[j] - x[2 * j + 1] * sn[j]; y[2 * j + 1] = x[2 * j + 1] * cs[j] + x[2 * j] * sn[j]; }
         *reinterpret_cast<uint4*>(p.k + dst) = pack8(y);
-        unpack8(*reinterpret_cast<const uint4*>(row + 2 * I + hh * 64 + c * 8), x);
+        unpack8(*reinterpret_cast<const uint4*>(row + 2 * I + hh * DH + c * 8), x);
         if (p.v_first) {
             const float mix = sigmoidf_(__bfloat162float(row[3 * I + (p.no_gate ? 0 : p.H) + hh]) + p.mix_b[hh]);
             float vf[8];
@@ -259,25 +263,28 @@ __global__ void __launch_bounds__(256) qkv_post_fwd_kernel(const QkvP p) {
         if (c == 0 && !p.no_gate) p.gate[(size_t)tok * p.H + hh] = sigmoidf_(__bfloat162float(row[3 * I + hh]) + p.gate_b[hh]);
     }
 }
+template <int DH>
 __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
-    const long long total = (long long)p.B * p.Np * p.H * 8;
-    const int I = p.H * 64;
+    constexpr int LANES = DH / 8, LOG2_LANES = DH == 64 ? 3 : 4;
+    static_assert(LANES == 1 << LOG2_LANES, "head dim 64 or 128");
+    const long long total = (long long)p.B * p.Np * p.H * LANES;
+    const int I = p.H * DH;
     const long long i = (long long)blockIdx.x * 256 + threadIdx.x;
     const bool ok = i < total;
     float dmix = 0.f, mix = 0.f;
     int c = 0, hh = 0;
     long long tok = 0;
     if (ok) {
-        c = (int)(i & 7);
-        hh = (int)((i >> 3) % p.H);
-        tok = (i >> 3) / p.H;
+        c = (int)(i & (LANES - 1));
+        hh = (int)((i >> LOG2_LANES) % p.H);
+        tok = (i >> LOG2_LANES) / p.H;
         const int n = (int)(tok % p.Np), b = (int)(tok / p.Np);
         const __nv_bfloat16* row = p.qkvg + (size_t)tok * p.ld;
         __nv_bfloat16* drow = p.d_qkvg + (size_t)tok * p.ld;
-        const size_t src = (((size_t)b * p.H + hh) * p.Np + n) * 64 + c * 8;
+        const size_t src = (((size_t)b * p.H + hh) * p.Np + n) * DH + c * 8;
         float cs[4], sn[4];
 #pragma unroll
-        for (int j = 0; j < 4; ++j) { cs[j] = p.cs[n * 32 + c * 4 + j]; sn[j] = p.sn[n * 32 + c * 4 + j]; }
+        for (int j = 0; j < 4; ++j) { cs[j] = p.cs[n * (DH / 2) + c * 4 + j]; sn[j] = p.sn[n * (DH / 2) + c * 4 + j]; }
         float x[8], y[8];
         if (p.dq_fp32) {
             const float4 a0 = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.dq) + src);
@@ -288,11 +295,11 @@ __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
         }
 #pragma unroll
         for (int j = 0; j < 4; ++j) { y[2 * j] = x[2 * j] * cs[j] + x[2 * j + 1] * sn[j]; y[2 * j + 1] = x[2 * j + 1] * cs[j] - x[2 * j] * sn[j]; }
-        *reinterpret_cast<uint4*>(drow + hh * 64 + c * 8) = pack8(y);
+        *reinterpret_cast<uint4*>(drow + hh * DH + c * 8) = pack8(y);
         unpack8(*reinterpret_cast<const uint4*>(p.dk + src), x);
 #pragma unroll
         for (int j = 0; j < 4; ++j) { y[2 * j] = x[2 * j] * cs[j] + x[2 * j + 1] * sn[j]; y[2 * j + 1] = x[2 * j + 1] * cs[j] - x[2 * j] * sn[j]; }
-        *reinterpret_cast<uint4*>(drow + I + hh * 64 + c * 8) = pack8(y);
+        *reinterpret_cast<uint4*>(drow + I + hh * DH + c * 8) = pack8(y);
         unpack8(*reinterpret_cast<const uint4*>(p.dv + src), x);
         if (p.dv_extra) {
             float xe[8];
@@ -303,17 +310,16 @@ __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
         if (p.v_first) {
             mix = sigmoidf_(__bfloat162float(row[3 * I + (p.no_gate ? 0 : p.H) + hh]) + p.mix_b[hh]);
             float vr[8], vf[8], o[8];
-            unpack8(*reinterpret_cast<const uint4*>(row + 2 * I + hh * 64 + c * 8), vr);
+            unpack8(*reinterpret_cast<const uint4*>(row + 2 * I + hh * DH + c * 8), vr);
             unpack8(*reinterpret_cast<const uint4*>(p.v_first + src), vf);
 #pragma unroll
             for (int j = 0; j < 8; ++j) { dmix += x[j] * (vr[j] - vf[j]); o[j] = x[j] * (1.f - mix); x[j] *= mix; }
             *reinterpret_cast<uint4*>(p.d_vfirst + src) = pack8(o);
         }
-        *reinterpret_cast<uint4*>(drow + 2 * I + hh * 64 + c * 8) = pack8(x);
+        *reinterpret_cast<uint4*>(drow + 2 * I + hh * DH + c * 8) = pack8(x);
     }
-    dmix += __shfl_xor_sync(0xffffffffu, dmix, 1);
-    dmix += __shfl_xor_sync(0xffffffffu, dmix, 2);
-    dmix += __shfl_xor_sync(0xffffffffu, dmix, 4);
+#pragma unroll
+    for (int m = 1; m < LANES; m <<= 1) dmix += __shfl_xor_sync(0xffffffffu, dmix, m);
     if (ok && c == 0) {
         __nv_bfloat16* drow = p.d_qkvg + (size_t)tok * p.ld;
         if (!p.no_gate) {
@@ -872,15 +878,18 @@ extern "C" int b200_embed_bwd(const float* d_tok, const int32_t* ids, float* d_e
     return check_launch("embed_bwd_kernel");
 }
 extern "C" int b200_rotary_table(float* cos_out, float* sin_out, int32_t Np, int32_t dim_head, b200_stream_t stream) {
-    B200_REQUIRE(cos_out && sin_out && Np > 0 && dim_head == 64, "rotary_table: only dim_head 64 is built");
-    rotary_table_kernel<<<(Np * 32 + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(cos_out, sin_out, Np, 32);
+    B200_REQUIRE(cos_out && sin_out && Np > 0, "rotary_table: bad arguments");
+    B200_REQUIRE(dim_head == 64 || dim_head == 128, "rotary_table: dim_head must be 64 or 128 (got %d)", dim_head);
+    const int half = dim_head / 2;
+    rotary_table_kernel<<<(Np * half + 255) / 256, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(cos_out, sin_out, Np, half);
     return check_launch("rotary_table_kernel");
 }
 
 static int fill_qkv(QkvP& p, const b200_qkv_post_args* a) {
     B200_REQUIRE(a && a->qkvg && a->rot_cos && a->rot_sin && (a->no_gate || (a->gate_bias && a->gate)), "qkv_post: null pointer");
-    B200_REQUIRE(a->dim_head == 64, "qkv_post: only dim_head 64 is built");
-    B200_REQUIRE(a->ld % 8 == 0 && a->ld >= 3 * a->H * 64 + ((a->no_gate ? 0 : 1) + (a->v_first ? 1 : 0)) * a->H, "qkv_post: bad row pitch %d", a->ld);
+    B200_REQUIRE(a->dim_head == 64 || a->dim_head == 128, "qkv_post: dim_head must be 64 or 128 (got %d)", a->dim_head);
+    B200_REQUIRE(a->ld % 8 == 0 && a->ld >= 3 * a->H * a->dim_head + ((a->no_gate ? 0 : 1) + (a->v_first ? 1 : 0)) * a->H, "qkv_post: bad row pitch %d",
+                 a->ld);
     B200_REQUIRE(!a->v_first || a->mix_bias, "qkv_post: value residual needs the mix bias");
     p.qkvg = (const __nv_bfloat16*)a->qkvg; p.ld = a->ld; p.gate_b = a->gate_bias; p.mix_b = a->mix_bias; p.cs = a->rot_cos; p.sn = a->rot_sin;
     p.v_first = (const __nv_bfloat16*)a->v_first; p.gate = a->gate; p.B = a->B; p.H = a->H; p.Np = a->Np;
@@ -892,7 +901,9 @@ extern "C" int b200_qkv_post_fwd(const b200_qkv_post_args* a, b200_stream_t stre
     if (fill_qkv(p, a)) return -1;
     B200_REQUIRE(a->q && a->k && a->v, "qkv_post_fwd: null output");
     p.q = (__nv_bfloat16*)a->q; p.k = (__nv_bfloat16*)a->k; p.v = (__nv_bfloat16*)a->v;
-    qkv_post_fwd_kernel<<<grid_for((long long)a->B * a->Np * a->H * 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+    const long long threads = (long long)a->B * a->Np * a->H * (a->dim_head / 8);
+    if (a->dim_head == 64) qkv_post_fwd_kernel<64><<<grid_for(threads), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+    else qkv_post_fwd_kernel<128><<<grid_for(threads), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("qkv_post_fwd_kernel");
 }
 extern "C" int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stream) {
@@ -901,8 +912,9 @@ extern "C" int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stre
     B200_REQUIRE(a->dq && a->dk && a->dv && (a->no_gate || a->d_gate) && a->d_qkvg && (!a->v_first || a->d_vfirst), "qkv_post_bwd: null pointer");
     p.dq = (const __nv_bfloat16*)a->dq; p.dk = (const __nv_bfloat16*)a->dk; p.dv = (const __nv_bfloat16*)a->dv; p.d_gate = a->d_gate;
     p.d_qkvg = (__nv_bfloat16*)a->d_qkvg; p.d_vfirst = (__nv_bfloat16*)a->d_vfirst; p.dq_fp32 = a->dq_fp32; p.dv_extra = (const __nv_bfloat16*)a->dv_extra;
-    const long long total = (long long)a->B * a->Np * a->H * 8;
-    qkv_post_bwd_kernel<<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+    const long long total = (long long)a->B * a->Np * a->H * (a->dim_head / 8);
+    if (a->dim_head == 64) qkv_post_bwd_kernel<64><<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+    else qkv_post_bwd_kernel<128><<<(unsigned)((total + 255) / 256), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(p);
     return check_launch("qkv_post_bwd_kernel");
 }
 

@@ -29,6 +29,7 @@ BF16, F32 = torch.bfloat16, torch.float32
 SOFTCLAMP = 50.0  # x-transformers logit_softclamp_value default (A.4)
 SOFTCLAMP_MAX = 64.0  # largest clamp the clamped attention kernels take (include/b200_e2tts.h)
 SUPPORTED_RESIDUAL_STREAMS = (1, 4)   # Transformer(num_residual_streams): 1 = plain residual, 4 = hyper-connections (the reference default)
+SUPPORTED_DIM_HEADS = (64, 128)       # Transformer(dim_head, text_dim_head): head widths the attention kernels are built for
 # x-transformers Attention keywords the kernels implement, with x-transformers' own defaults for a missing key
 ATTN_KWARGS_DEFAULTS = dict(gate_value_heads=False, softclamp_logits=False, logit_softclamp_value=50.)
 # text sub-blocks of layer i+1 overlap the audio sub-blocks of layer i on a second CUDA stream (Transformer._run_layers);
@@ -142,7 +143,7 @@ class Attention(Module):  # A.4
     def __init__(self, dim, heads, dim_head, learned_value_residual_mix, gate_value_heads=True):
         super().__init__()
         inner = heads * dim_head
-        self.heads = heads
+        self.heads, self.dim_head = heads, dim_head
         self.to_q = nn.Linear(dim, inner, bias=False)
         self.to_k = nn.Linear(dim, inner, bias=False)
         self.to_v = nn.Linear(dim, inner, bias=False)
@@ -426,10 +427,12 @@ class Transformer(_PackOwner):
         dim_text = default(dim_text, dim // 2)
         text_heads, text_dim_head = default(text_heads, heads), default(text_dim_head, dim_head)
         text_ff_mult, text_depth = default(text_ff_mult, ff_mult), default(text_depth, depth)
-        if dim_head != 64 or text_dim_head != 64:
-            _unsupported('dim_head', (dim_head, text_dim_head), 'e2_tts.py:527 (attention kernels are built for head dim 64)')
-        if text_heads != heads:
-            _unsupported('text_heads', text_heads, 'e2_tts.py:530')
+        for name, value in (('dim_head', dim_head), ('text_dim_head', text_dim_head)):
+            if value not in SUPPORTED_DIM_HEADS:
+                raise NotImplementedError(
+                    f'{name}={value!r} (e2_tts.py:527, :531): supported head dims are 64 and 128, the widths the attention kernels are '
+                    f'built for; there is no fallback path (SURVEY.md §2 row 8)')
+        assert heads >= 1 and text_heads >= 1, 'heads and text_heads must be >= 1'
         assert 1 <= text_depth <= depth
         assert dim % 64 == 0 and dim_text % 64 == 0 and dim <= 1024, 'kernels need dim, dim_text multiples of 64 and dim <= 1024'
         assert int(dim * ff_mult) % 64 == 0 and int(dim_text * text_ff_mult) % 64 == 0
@@ -438,6 +441,7 @@ class Transformer(_PackOwner):
         self.abs_pos_emb = nn.Embedding(max_seq_len, dim) if abs_pos_emb else None
         self.dim, self.dim_text, self.depth, self.text_depth = dim, dim_text, depth, text_depth
         self.heads, self.dim_head = heads, dim_head
+        self.text_heads, self.text_dim_head = text_heads, text_dim_head
         self.has_freq_axis = False
         self.dropout = dropout
         self.num_streams = num_residual_streams
@@ -496,8 +500,7 @@ class Transformer(_PackOwner):
     # ------------------------------------------------------------------ packed operands
     def _add_weights(self, pack):
         """Add every per-layer GEMM operand and the stacked to_gamma weights to `pack`; -> dict(layers=[per-layer handles], cond=...)."""
-        d, dt, H = self.dim, self.dim_text, self.heads
-        I = H * 64
+        d, dt = self.dim, self.dim_text
         packed = []
         e = pack.buffer
         cond_rows = []
@@ -510,6 +513,7 @@ class Transformer(_PackOwner):
                 ff = mods[7] if pre == 'a' else mods[4]
                 has_mix = attn.to_value_residual_mix is not None
                 has_gate = attn.to_v_head_gate is not None
+                H, I = attn.heads, attn.heads * attn.dim_head   # per stream: the text attention may have its own geometry
                 qkv = e(3 * I + (int(has_gate) + int(has_mix)) * H, din)   # rows [q | k | v | gate | mix], gate and mix optional
                 for j, lin in enumerate((attn.to_q, attn.to_k, attn.to_v)):
                     pack.add(lin.weight, qkv, row_off=j * I)
@@ -554,11 +558,11 @@ class Transformer(_PackOwner):
             cond = dict(W=W_all, b=b_all, lins=cond_rows)
         return dict(layers=packed, cond=cond)
 
-    def _rotary(self, Np, dev):
+    def _rotary(self, Np, dim_head, dev):
         rot = self._derived.setdefault('rot', {})
-        if Np not in rot:
-            rot[Np] = ops.rotary_table(Np, dev)
-        return rot[Np]
+        if (Np, dim_head) not in rot:
+            rot[Np, dim_head] = ops.rotary_table(Np, dev, dim_head)
+        return rot[Np, dim_head]
 
     # ------------------------------------------------------------------ conditioning vectors
     def _cond_gains(self, times, batch, c):
@@ -579,8 +583,8 @@ class Transformer(_PackOwner):
     # ------------------------------------------------------------------ the block stack
     def _run_layers(self, P, xs, ts, gains, mask_u8, B, Np, seed):
         """P: the per-layer packed operands; xs bf16 [T,S,d], ts bf16 [T,S,dt] | None -> final residual streams. Layer loop of e2_tts.py:825-939."""
-        H = self.heads
-        cs, sn = self._rotary(Np, xs.device)
+        # the audio and the text attention may differ in head count and width: each call takes both, and the rotary table, from its module
+        rot = {dh: self._rotary(Np, dh, xs.device) for dh in {self.dim_head, self.text_dim_head}}
         p_drop = self.dropout if self.training else 0.0
         mbits = ops.attn_maskbits(mask_u8, B, Np, xs.device) if xs.is_cuda else None   # one key-mask bitmask for all 2 * depth attention calls
         skips = []
@@ -629,10 +633,12 @@ class Transformer(_PackOwner):
             if lfe is not None:   # attn_input_fourier_embed (:909): between the attention norm (fused into the width kernel) and the attention
                 br = ops.FourierLinear.apply(br, lfe.linear.weight, pk['lfe'], *lfe.split_dims)
             mix, gate = attn.to_value_residual_mix, attn.to_v_head_gate
+            cs, sn = rot[attn.dim_head]
             og, v = ops.Attention.apply(br, attn.to_q.weight, attn.to_k.weight, attn.to_v.weight, gate.weight if gate is not None else None,
                                         gate.bias if gate is not None else None, mix[0].weight if mix is not None else None,
                                         mix[0].bias if mix is not None else None, vf if mix is not None else None,
-                                        pk['qkv'], cs, sn, mask_u8, B, Np, H, p_drop, next_seed(), self.softclamp, self._seed_dev, mbits)
+                                        pk['qkv'], cs, sn, mask_u8, B, Np, attn.heads, p_drop, next_seed(), self.softclamp, self._seed_dev, mbits,
+                                        attn.dim_head)
             y = ops.OutProj.apply(og, attn.to_out.weight, pk['out'], colscale, mask_u8, B, Np, rest if plain else None)
             return depth(rest, y, beta), (v if vf is None else vf)
 
@@ -658,7 +664,7 @@ class Transformer(_PackOwner):
         two = TWO_STREAM and has_text(0) and xs.is_cuda
         if two:
             main, side = torch.cuda.current_stream(xs.device), _side_stream(xs.device)
-            for t in (mask_u8, cs, sn, mbits):
+            for t in (mask_u8, mbits, *[x for pair in rot.values() for x in pair]):
                 if t is not None:
                     t.record_stream(side)
 

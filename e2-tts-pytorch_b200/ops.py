@@ -99,10 +99,11 @@ def pack_weights(table_dev, n):
     lib.call('b200_pack_weights', table_dev, n, _stream())
 
 
-def rotary_table(Np, device):
-    cs = torch.empty((Np, 32), device=device, dtype=F32)
-    sn = torch.empty((Np, 32), device=device, dtype=F32)
-    lib.call('b200_rotary_table', cs, sn, Np, 64, _stream())
+def rotary_table(Np, device, dim_head=64):
+    """cos / sin fp32 [Np, dim_head / 2] of the rotary embedding (A.3), dim_head 64 or 128"""
+    cs = torch.empty((Np, dim_head // 2), device=device, dtype=F32)
+    sn = torch.empty((Np, dim_head // 2), device=device, dtype=F32)
+    lib.call('b200_rotary_table', cs, sn, Np, dim_head, _stream())
     return cs, sn
 
 
@@ -313,7 +314,7 @@ def _clamp_args(softclamp):
 
 
 def _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits=None):
-    """b200_attn_fwd on q, k, v bf16 [B, H, Np, 64] -> og (gated, head-merged bf16 [B*Np, H*64]), o (bf16 [B, H, Np, 64]), lse (fp32
+    """b200_attn_fwd on q, k, v bf16 [B, H, Np, dh] (dh 64 or 128) -> og (gated, head-merged bf16 [B*Np, H*dh]), o (bf16 [B, H, Np, dh]), lse (fp32
     [B, H, Np]). `maskbits` is attn_maskbits(mask), shared by every layer of a step; without it the call builds its own. `gate` may be
     None (no head gate), `softclamp` None (no logit soft-clamp)."""
     B, H, Np, dh = q.shape
@@ -329,7 +330,7 @@ def _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev, ma
 
 
 def _attn_core_bwd(d_og, q, k, v, o, lse, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits=None):
-    """b200_attn_bwd -> dq (fp32: accumulated across key tiles with atomics), dk, dv (bf16 [B, H, Np, 64]), d_gate (fp32 [B*Np, H],
+    """b200_attn_bwd -> dq (fp32: accumulated across key tiles with atomics), dk, dv (bf16 [B, H, Np, dh]), d_gate (fp32 [B*Np, H],
     None without a gate)."""
     B, H, Np, dh = q.shape
     dq = torch.empty(q.shape, device=q.device, dtype=F32)
@@ -370,24 +371,26 @@ class Attention(Function):
     residual + gate post-processing, wgmma flash attention (softclamp, key mask, dropout, head gate). Returns the gated
     head-merged output (input of to_out) and this layer's values (the first layer's feed every later layer, e2_tts.py:878,916).
     One autograd node: q/k/v never enter the graph, and dq stays fp32 from the attention backward into the rotary inverse.
-    wg, bg None: no head gate (x-transformers gate_value_heads=False; packed rows [q|k|v|mix]); softclamp None: no logit soft-clamp."""
+    wg, bg None: no head gate (x-transformers gate_value_heads=False; packed rows [q|k|v|mix]); softclamp None: no logit soft-clamp.
+    dim_head: 64 or 128, H heads of it (I = H * dim_head); cs / sn the rotary table of that head dim."""
 
     @staticmethod
-    def forward(ctx, xn, wq, wk, wv, wg, bg, wm, bm, v_first, wpack, cs, sn, mask, B, Np, H, dropout_p, seed, softclamp, seed_dev, maskbits=None):
+    def forward(ctx, xn, wq, wk, wv, wg, bg, wm, bm, v_first, wpack, cs, sn, mask, B, Np, H, dropout_p, seed, softclamp, seed_dev, maskbits=None,
+                dim_head=64):
         ctx.set_materialize_grads(False)   # only the first layer's values are consumed downstream: no zero-filled d_v for the others
         T, Din = xn.shape
-        I = H * 64
+        I = H * dim_head
         dev = xn.device
         has_mix = wm is not None
         has_gate = wg is not None
         ncat = 3 * I + (int(has_gate) + int(has_mix)) * H
         ld = (ncat + 7) // 8 * 8
         qkvg = gemm(xn, wpack, T, ncat, Din, ldd=ld)
-        q = torch.empty((B, H, Np, 64), device=dev, dtype=BF16)
+        q = torch.empty((B, H, Np, dim_head), device=dev, dtype=BF16)
         k, v = torch.empty_like(q), torch.empty_like(q)
         gate = torch.empty((T, H), device=dev, dtype=F32) if has_gate else None
         a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
-                          q=q, k=k, v=v, gate=gate, B=B, H=H, Np=Np, dim_head=64, no_gate=int(not has_gate))
+                          q=q, k=k, v=v, gate=gate, B=B, H=H, Np=Np, dim_head=dim_head, no_gate=int(not has_gate))
         lib.call('b200_qkv_post_fwd', a, _stream())
         og, o, lse = _attn_core_fwd(q, k, v, gate, mask, dropout_p, seed, softclamp, seed_dev, maskbits)
         ctx.maskbits = maskbits
@@ -399,18 +402,19 @@ class Attention(Function):
     @once_differentiable
     def backward(ctx, d_og, d_v_extra):
         xn, qkvg, gate, v_first, wpack, cs, sn, bg, bm, q, k, v, o, lse, mask = ctx.saved_tensors
-        if d_og is None:   # (only the values were used: not a case the model produces, kept for completeness)
-            d_og = torch.zeros((xn.shape[0], ctx.meta[2] * 64), device=xn.device, dtype=BF16)
         B, Np, H, ncat, ld, has_mix, dropout_p, seed, softclamp, seed_dev, has_gate = ctx.meta
+        dh = q.shape[-1]
+        if d_og is None:   # (only the values were used: not a case the model produces, kept for completeness)
+            d_og = torch.zeros((xn.shape[0], H * dh), device=xn.device, dtype=BF16)
         T, Din = xn.shape
-        I = H * 64
+        I = H * dh
         dev = xn.device
         dq, dk, dv, d_gate = _attn_core_bwd(d_og, q, k, v, o, lse, gate, mask, dropout_p, seed, softclamp, seed_dev, ctx.maskbits)
         d_qkvg = torch.empty((T, ld), device=dev, dtype=BF16)
         d_vfirst = torch.empty_like(v_first) if v_first is not None else None
         a = lib.make_args('b200_qkv_post_args', qkvg=qkvg, ld=ld, gate_bias=bg, mix_bias=bm, rot_cos=cs, rot_sin=sn, v_first=v_first,
                           gate=gate, dq=dq, dk=dk, dv=dv, dv_extra=_c(d_v_extra), d_gate=d_gate, d_qkvg=d_qkvg, d_vfirst=d_vfirst,
-                          B=B, H=H, Np=Np, dim_head=64, dq_fp32=1, no_gate=int(not has_gate))
+                          B=B, H=H, Np=Np, dim_head=dh, dq_fp32=1, no_gate=int(not has_gate))
         lib.call('b200_qkv_post_bwd', a, _stream())
         dx = gemm(d_qkvg, wpack, T, Din, ncat, lda=ld, ldb=Din, b_mn=True)
         dW = grad_weight(d_qkvg, xn, T, ncat, Din, ldy=ld)
@@ -419,7 +423,7 @@ class Attention(Function):
         m0 = H if has_gate else 0                           # first mix column past 3 I
         return (dx, dW[:I], dW[I:2 * I], dW[2 * I:3 * I], dW[3 * I:3 * I + H] if has_gate else None, db[:H] if has_gate else None,
                 dW[3 * I + m0:3 * I + m0 + H] if has_mix else None, db[m0:m0 + H] if has_mix else None,
-                d_vfirst, None, None, None, None, None, None, None, None, None, None, None, None)
+                d_vfirst, None, None, None, None, None, None, None, None, None, None, None, None, None)
 
 
 def attn_maskbits(mask_u8, B, Np, device):

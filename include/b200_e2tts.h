@@ -80,9 +80,9 @@ int b200_gemm(const b200_gemm_args* a, b200_stream_t stream);
 int b200_seed_advance(uint64_t* seed_dev, b200_stream_t stream);   /* *seed_dev = splitmix64 step of *seed_dev (one thread) */
 
 /* ------------------------------------------------------------------------------------------------
- * Fused softclamped attention, head_dim 64 (x-transformers Attend as configured by the reference: A.4
- * steps 4-5, call sites e2_tts.py:875, :911). q,k,v,o: bf16 [B,H,Np,64]; keymask: u8 [B,Np] (1 = keep) or
- * NULL; gate: fp32 [B*Np, H] = sigmoid(to_v_head_gate(x)) or NULL; og: bf16 [B*Np, H*64] gated, merged
+ * Fused softclamped attention, dim_head (= dh) 64 or 128; any other value is refused (x-transformers Attend as configured by the
+ * reference: A.4 steps 4-5, call sites e2_tts.py:875, :911). q,k,v,o: bf16 [B,H,Np,dh]; keymask: u8 [B,Np] (1 = keep) or
+ * NULL; gate: fp32 [B*Np, H] = sigmoid(to_v_head_gate(x)) or NULL; og: bf16 [B*Np, H*dh] gated, merged
  * heads (the input of to_out); lse: fp32 [B,H,Np] (natural log of the softmax denominator of the CLAMPED
  * logits). Dropout on P uses a counter-based hash of (seed, b,h,i,j) that backward recomputes.
  * Logits: softclamp * tanh(scale q.k / softclamp) with softclamp in (0, 64] (x-transformers softclamp_logits), or, when
@@ -112,9 +112,9 @@ int b200_attn_maskbits(const uint8_t* keymask, void* ws_maskbits, int32_t B, int
  * unclamped: softclamp must be 0 */
 int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream);
 
-/* backward: d_og bf16 [B*Np, H*64] -> dk,dv bf16 [B,H,Np,64], dq FP32 [B,H,Np,64] (accumulated with atomics across key
- * tiles), d_gate fp32 [B*Np,H] (grad wrt the sigmoid gate VALUE;
- * may be NULL). ws_dO (bf16 [B,H,Np,64]), ws_delta (fp32 [B,H,Np]) and ws_maskbits are caller workspaces. */
+/* backward, dim_head (= dh) 64 or 128: d_og bf16 [B*Np, H*dh] -> dk,dv bf16 [B,H,Np,dh], dq FP32 [B,H,Np,dh] (accumulated with
+ * TMA reductions across key tiles), d_gate fp32 [B*Np,H] (grad wrt the sigmoid gate VALUE;
+ * may be NULL). ws_dO (bf16 [B,H,Np,dh]), ws_delta (fp32 [B,H,Np]) and ws_maskbits are caller workspaces. */
 typedef struct {
     const void *q, *k, *v, *o, *d_og;
     const uint8_t* keymask;
@@ -219,12 +219,14 @@ int b200_assemble_fwd(const b200_assemble_args* a, b200_stream_t stream);
 int b200_assemble_bwd(const b200_assemble_args* a, b200_stream_t stream);
 int b200_embed_bwd(const float* d_tok, const int32_t* ids, float* d_emb, int32_t ntok, int32_t D, int32_t vocab, b200_stream_t stream);
 
-/* Rotary table cos/sin [Np, 32] for dim_head 64, positions 0..Np-1 including registers (A.3; e2_tts.py:793). */
+/* Rotary table cos/sin [Np, dim_head / 2], dim_head 64 or 128: inv_freq_i = 10000^(-2i / dim_head), positions 0..Np-1 including
+ * registers (A.3; e2_tts.py:793, :798). */
 int b200_rotary_table(float* cos_out, float* sin_out, int32_t Np, int32_t dim_head, b200_stream_t stream);
 
 /* Post-processing of the fused [q|k|v|gate|mix] projection (A.4 steps 1-3, 5): interleaved-pair rotary on
  * q,k; v = lerp(v_first, v, sigmoid(mix)) when v_first != NULL; gate = sigmoid(gate_logit + bias) fp32 [T,H];
- * q,k,v written as [B,H,Np,64]. bwd inverts all of it into d_qkvg (same packed layout) and d_vfirst.
+ * q,k,v written as [B,H,Np,dim_head], I = H * dim_head, dim_head 64 or 128 (rot_cos / rot_sin: the table of that dim_head).
+ * bwd inverts all of it into d_qkvg (same packed layout) and d_vfirst.
  * no_gate != 0 (x-transformers Attention without gate_value_heads): the layout is [q|k|v|mix], the mix logits at column 3I;
  * gate, gate_bias and d_gate are then neither read nor written (may be NULL). */
 typedef struct {
@@ -233,7 +235,7 @@ typedef struct {
     const void* v_first;
     void *q, *k, *v; float* gate;
     const void *dq, *dk, *dv; const float* d_gate;
-    const void* dv_extra;   /* optional bf16 [B,H,Np,64] added to dv (value-residual gradients of later layers into layer 0) */
+    const void* dv_extra;   /* optional bf16 [B,H,Np,dim_head] added to dv (value-residual gradients of later layers into layer 0) */
     void *d_qkvg, *d_vfirst;
     int32_t B, H, Np, dim_head;
     int32_t dq_fp32;   /* bwd: dq is fp32 (wgmma attention backward) instead of bf16 */

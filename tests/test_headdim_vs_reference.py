@@ -1,0 +1,111 @@
+"""CPU: the attention geometry knobs of Transformer (e2_tts.py:527-531) — 128-wide heads (dim_head, text_dim_head) and a text stream
+with its own head count (text_heads). The oracle of tests/headdim_variants.py against what the original e2_tts.py computed with them
+(tests/golden/reference/headdim_*.pt, tools/make_headdim_golden.py), the package's parameter layout against the original's, the head
+dims that still raise, and the C-ABI validation of dim_head."""
+import pytest
+import torch
+
+from headdim_variants import HEADDIM_CASES, HEADDIM_SAMPLE, cfg, headdim_oracle
+from oracle import e2tts_oracle as O
+from oracle import reference_cases as RC
+from test_oracle_vs_reference import _check_grads, _grad_sd
+
+import e2_tts_pytorch_b200 as pkg
+
+
+@pytest.mark.parametrize('name', list(HEADDIM_CASES))
+def test_oracle_vs_reference(name):
+    """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
+    c = HEADDIM_CASES[name]
+    g = RC.load('headdim_' + name)
+    sd = _grad_sd(RC.state_dict(c['cls'], c['seed'], c['tkw']))
+    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
+    lens = torch.tensor(c['lens'])
+    text = O.list_str_to_tensor(c['text'])
+    with headdim_oracle(c['tkw']):
+        if c['cls'] == 'E2TTS':
+            x0 = RC.randn(mel.shape, c['seed'] + 2000)
+            o = O.e2tts_forward(sd, cfg(c['tkw']), mel, text, lens=lens, x0=x0, times=g['times'], span_mask=g['span_mask'],
+                                drop_text_cond=c['drop'])
+            loss = o['loss']
+            assert RC.compact_rel_l2(o['pred'], g['pred']) < 1e-4
+            assert abs(float(o['pred'].detach().double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
+        else:
+            torch.manual_seed(c['seed'])
+            rand_frac = mel.new_zeros(mel.shape[0]).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
+            loss = O.duration_forward(sd, cfg(c['tkw'], cond_on_time=False), mel, text, lens=lens, rand_frac=rand_frac)
+    assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
+    loss.backward()
+    if c['cls'] == 'E2TTS':
+        _check_grads(sd, g['grads'])
+    else:
+        _check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+    if c['drop']:   # the text stream is skipped: its parameters get no gradient
+        assert g['grads']['transformer.layers.0.1.2.to_q.weight'] is None
+
+
+def test_sample_vs_reference():
+    s = HEADDIM_SAMPLE
+    g = RC.load('headdim_sample')
+    cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
+    with torch.no_grad(), headdim_oracle(s['tkw']):
+        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), cfg(s['tkw']), cond, O.list_str_to_tensor(s['text']),
+                             duration=torch.tensor(s['duration']), y0=RC.randn(g['shape'], 3000 + s['seed']), steps=s['steps'],
+                             cfg_strength=s['cfg_strength'])
+    assert tuple(got.shape) == g['shape']
+    assert RC.compact_rel_l2(got, g['out']) < 1e-4
+
+
+@pytest.mark.parametrize('name', list(HEADDIM_CASES))
+def test_state_dict_matches_reference(name):
+    """keys and shapes of the original's model with the same geometry: its checkpoints load"""
+    c = HEADDIM_CASES[name]
+    want = RC.load('headdim_' + name)['shapes']
+    t = dict(dropout=0., max_seq_len=128, **c['tkw'])
+    m = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
+    got = {k: tuple(v.shape) for k, v in m.state_dict().items()}
+    assert got == want
+
+
+def test_geometry_is_recorded():
+    t = pkg.Transformer(dim=256, depth=2, heads=2, dim_head=128, text_heads=1, text_dim_head=64)
+    assert (t.heads, t.dim_head, t.text_heads, t.text_dim_head) == (2, 128, 1, 64)
+    audio, text = t.layers[0][0][3], t.layers[0][1][2]
+    assert (audio.heads, audio.dim_head, text.heads, text.dim_head) == (2, 128, 1, 64)
+    assert audio.to_q.weight.shape == (256, 256) and text.to_q.weight.shape == (64, 128)
+
+
+@pytest.mark.parametrize('kw', [dict(dim_head=32), dict(dim_head=96), dict(text_dim_head=32), dict(text_dim_head=96),
+                                dict(dim_head=128, text_dim_head=256)])
+def test_other_head_dims_raise(kw):
+    name = next(iter(kw))
+    with pytest.raises(NotImplementedError, match=f'{name}=.*supported head dims are 64 and 128'):
+        pkg.Transformer(dim=128, depth=2, heads=2, **kw)
+    with pytest.raises(NotImplementedError, match='supported head dims are 64 and 128'):
+        pkg.E2TTS(transformer=dict(dim=128, depth=2, heads=2, **kw), use_vocos=False)
+
+
+def test_cabi_dim_head_validation_without_gpu():
+    """dim_head is checked before the device is touched (placeholder pointers, never read)"""
+    ptrs = dict.fromkeys(('q', 'k', 'v', 'o', 'lse', 'ws_maskbits'), 256)
+    bwd = dict(d_og=256, ws_dO=256, ws_delta=256, dq=256, dk=256, dv=256)
+    for dh in (32, 96, 256):
+        shape = dict(B=1, H=1, Np=64, dim_head=dh, scale=dh ** -0.5, softclamp=50.0)
+        for name, extra in (('b200_attn_fwd', dict(og=256)), ('b200_attn_bwd', bwd)):
+            a = pkg.lib.make_args(name + '_args', **ptrs, **shape, **extra)
+            with pytest.raises(RuntimeError, match='dim_head must be 64 or 128'):
+                pkg.lib.call(name, a, None)
+        q = dict(qkvg=256, rot_cos=256, rot_sin=256, q=256, k=256, v=256, B=1, H=2, Np=8, dim_head=dh, ld=3 * 2 * 128 + 8, no_gate=1)
+        a = pkg.lib.make_args('b200_qkv_post_args', **q)
+        with pytest.raises(RuntimeError, match='dim_head must be 64 or 128'):
+            pkg.lib.call('b200_qkv_post_fwd', a, None)
+        a = pkg.lib.make_args('b200_qkv_post_args', **q, dq=256, dk=256, dv=256, d_qkvg=256)
+        with pytest.raises(RuntimeError, match='dim_head must be 64 or 128'):
+            pkg.lib.call('b200_qkv_post_bwd', a, None)
+        with pytest.raises(RuntimeError, match='dim_head must be 64 or 128'):
+            pkg.lib.call('b200_rotary_table', 256, 256, 8, dh, None)
+    # the row pitch follows the head dim: 3 H dim_head columns (+ H per gate / mix logit)
+    q = dict(qkvg=256, rot_cos=256, rot_sin=256, q=256, k=256, v=256, B=1, H=2, Np=8, dim_head=128, no_gate=1)
+    a = pkg.lib.make_args('b200_qkv_post_args', ld=3 * 2 * 64, **q)
+    with pytest.raises(RuntimeError, match='row pitch'):
+        pkg.lib.call('b200_qkv_post_fwd', a, None)
