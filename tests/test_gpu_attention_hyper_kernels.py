@@ -532,11 +532,12 @@ def host_maskbits(m, Np):
 
 
 def warp_tile_amax(q, k):
-    """max |s| over each forward warp's fragment (16 query rows x 64 keys), over the rows the TMA boxes read: past the end of a head
-    they are the next head's rows, past the end of the tensor zeros"""
-    B, H, Np, _ = q.shape
-    Qf, Kf = h64(q).reshape(-1, 64), h64(k).reshape(-1, 64)
-    Qf, Kf = torch.cat([Qf, torch.zeros(1, 64, dtype=F64)]), torch.cat([Kf, torch.zeros(1, 64, dtype=F64)])
+    """max |s| over each forward warp's fragment (16 query rows x 64 keys, the dot product over all dh head dims: the head-dim-128
+    forward has the same 128-query / 64-key tiles), over the rows the TMA boxes read: past the end of a head they are the next head's
+    rows, past the end of the tensor zeros"""
+    B, H, Np, dh = q.shape
+    Qf, Kf = h64(q).reshape(-1, dh), h64(k).reshape(-1, dh)
+    Qf, Kf = torch.cat([Qf, torch.zeros(1, dh, dtype=F64)]), torch.cat([Kf, torch.zeros(1, dh, dtype=F64)])
     total = B * H * Np
     nq, nk = -(-Np // TQ) * TQ, -(-Np // TKV_FWD) * TKV_FWD
     out_all, out_valid = [], []
@@ -674,18 +675,23 @@ def attn_bwd(pkg, q, k, v, o, lse, gate, mask, dog, clamp, p_drop, seed, ws=None
     return r
 
 
-def attn_inputs(B, H, Np, regime, masks, gate, seed):
+def attn_inputs(B, H, Np, regime, masks, gate, seed, dh=64, device=None):
+    """regime: the logit regime assert_regime proves ('big': |scale s| > 90 somewhere, for the unclamped kernels). The clamp argument
+    u = s dh^-1/2 / clamp of scores of standard deviation sd^2 dh^1/2 does not depend on dh, so the recipes hold at every head dim.
+    masks: one kind per batch element (cycled) — 'edges', 'tail', 'random', 'none', 'empty' (no valid key)."""
     g = torch.Generator().manual_seed(seed)
     rn = lambda *s: torch.randn(*s, generator=g)
     if regime == 'deg9':
-        # s = 64 a_i b_j + noise along one sign vector per head: |u| = |s| / 400 up to just under 0.5, so whole tiles need degree 9
-        sv = torch.where(rn(B, H, 1, 64) > 0, 1.0, -1.0)
-        a = 1.75 * (0.5 + 0.5 * torch.rand(B, H, Np, 1, generator=g))
-        b = 1.75 * (2 * torch.rand(B, H, Np, 1, generator=g) - 1)
-        q, k = sv * a + 0.01 * rn(B, H, Np, 64), sv * b
+        # s = dh c^2 a_i b_j + noise along one sign vector per head, c^2 dh^1/2 constant: |u| up to just under 0.5 (|s| / 400 at
+        # dh = 64), so whole tiles need degree 9
+        c = 1.75 * (64 / dh) ** 0.25
+        sv = torch.where(rn(B, H, 1, dh) > 0, 1.0, -1.0)
+        a = c * (0.5 + 0.5 * torch.rand(B, H, Np, 1, generator=g))
+        b = c * (2 * torch.rand(B, H, Np, 1, generator=g) - 1)
+        q, k = sv * a + 0.01 * rn(B, H, Np, dh), sv * b
     else:
-        sd = {'deg5': 1.0, 'mixed': 1.0, 'tanh': 7.0, 'sat': 60.0}[regime]
-        q, k = rn(B, H, Np, 64) * sd, rn(B, H, Np, 64) * sd
+        sd = {'deg5': 1.0, 'mixed': 1.0, 'tanh': 7.0, 'sat': 60.0, 'big': 6.0}[regime]
+        q, k = rn(B, H, Np, dh) * sd, rn(B, H, Np, dh) * sd
         if regime == 'mixed':
             k[:, :, ::7] *= 16                                        # every 7th key far outside the polynomial range
             # and every warp tile with a row of the head beyond the degree-5 range: the first key of each 64-key tile and the last
@@ -693,10 +699,13 @@ def attn_inputs(B, H, Np, regime, masks, gate, seed):
             k[:, :, ::64] = 16.0
             k[:, :, -1] = 16.0
             q[:, :, -1] = 4.0
-    v = rn(B, H, Np, 64)
+    v = rn(B, H, Np, dh)
     m = torch.ones(B, Np, dtype=torch.bool)
     for b in range(B):
         kind = masks[b % len(masks)]
+        if kind == 'empty':
+            m[b] = False
+            continue
         if kind == 'edges':                                         # both sides of the 32-bit word, 64-key tile and 128-key tile edges
             for n in (31, 32, 63, 64, 127, 128):
                 if n < Np:
@@ -709,14 +718,21 @@ def attn_inputs(B, H, Np, regime, masks, gate, seed):
             m[b] = torch.rand(Np, generator=g) > 0.3
         m[b, 0] = True                                              # (the model's register keys are always valid)
     gt = torch.rand(B * Np, H, generator=g) if gate else None
-    dog = rn(B * Np, H * 64)
-    to = lambda t: None if t is None else t.to(dev()).contiguous()
+    dog = rn(B * Np, H * dh)
+    to = lambda t: None if t is None else t.to(dev() if device is None else device).contiguous()
     return (to(q.to(BF16)), to(k.to(BF16)), to(v.to(BF16)), to(gt), m, to(m.to(torch.uint8)) if masks != ('none',) else None,
             to(dog.to(BF16)))
 
 
 def assert_regime(regime, q, k, m, clamp, w=1e-3):
-    soc = SCALE / clamp
+    """the case's scores lie where the regime's name says (score scale dh^-1/2); returns max |u| per forward warp tile over the
+    head's own rows and keys (inf for warps without a query row of the head), None for the unclamped 'big'"""
+    scale = q.shape[-1] ** -0.5
+    if regime == 'big':          # unclamped: 2^(scale s log2 e) of some valid score is beyond fp32 without the running maximum
+        sv = (h64(q) @ h64(k).transpose(-1, -2)).abs() * scale
+        assert clamp is None and float(sv[m[:, None, None, :].expand_as(sv)].max()) > 90
+        return None
+    soc = scale / clamp
     amax, amax_valid = warp_tile_amax(q, k)
     ua = amax * soc
     uv = (h64(q) @ h64(k).transpose(-1, -2)).abs() * soc

@@ -42,24 +42,28 @@ def _clamp_fields(clamp):
     return dict(softclamp=0.0, unclamped=1) if clamp is None else dict(softclamp=clamp, unclamped=0)
 
 
-def attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed):
+def attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed, ws=None, ready=0, seed_dev=None):
     B, H, Np, dh = q.shape
     o, og, lse = nans(q.shape, BF16), nans((B * Np, H * dh), BF16), nans((B, H, Np), F32)
-    ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
+    if ws is None:
+        ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
     a = pkg.lib.make_args('b200_attn_fwd_args', q=q, k=k, v=v, keymask=mask, gate=gate, o=o, og=og, lse=lse, B=B, H=H, Np=Np, dim_head=dh,
-                          scale=dh ** -0.5, dropout_p=p_drop, seed=seed, ws_maskbits=ws, **_clamp_fields(clamp))
+                          scale=dh ** -0.5, dropout_p=p_drop, seed=seed, ws_maskbits=ws, seed_dev=seed_dev, maskbits_ready=ready,
+                          **_clamp_fields(clamp))
     pkg.lib.call('b200_attn_fwd', a, stream())
     return dict(o=o, og=og, lse=lse, ws=ws)
 
 
-def attn_bwd(pkg, q, k, v, o, lse, gate, mask, dog, clamp, p_drop, seed):
+def attn_bwd(pkg, q, k, v, o, lse, gate, mask, dog, clamp, p_drop, seed, ws=None, ready=0, seed_dev=None):
     B, H, Np, dh = q.shape
     r = dict(dq=nans(q.shape, F32), dk=nans(q.shape, BF16), dv=nans(q.shape, BF16), ws_dO=nans(q.shape, BF16), ws_delta=nans((B, H, Np), F32),
              d_gate=nans((B * Np, H), F32) if gate is not None else None)
-    ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
+    if ws is None:
+        ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
     a = pkg.lib.make_args('b200_attn_bwd_args', q=q, k=k, v=v, o=o, d_og=dog, keymask=mask, gate=gate, lse=lse, ws_dO=r['ws_dO'],
                           ws_delta=r['ws_delta'], d_gate=r['d_gate'], dq=r['dq'], dk=r['dk'], dv=r['dv'], B=B, H=H, Np=Np, dim_head=dh,
-                          scale=dh ** -0.5, dropout_p=p_drop, seed=seed, ws_maskbits=ws, **_clamp_fields(clamp))
+                          scale=dh ** -0.5, dropout_p=p_drop, seed=seed, ws_maskbits=ws, seed_dev=seed_dev, maskbits_ready=ready,
+                          **_clamp_fields(clamp))
     pkg.lib.call('b200_attn_bwd', a, stream())
     return r
 
