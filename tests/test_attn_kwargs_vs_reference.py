@@ -6,9 +6,9 @@ import pytest
 import torch
 
 from attn_variants import ATTN_KWARGS_CASES, clamp_of, variant_oracle
+from model_checks import check_grads, grad_sd
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
-from test_oracle_vs_reference import _check_grads, _grad_sd
 
 import e2_tts_pytorch_b200 as pkg
 
@@ -22,7 +22,7 @@ def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
     c = ATTN_KWARGS_CASES[name]
     g = RC.load('attn_kwargs_' + name)
-    sd = _grad_sd(RC.state_dict(c['cls'], c['seed'], _tkw(c)))
+    sd = grad_sd(RC.state_dict(c['cls'], c['seed'], _tkw(c)))
     mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
     lens = torch.tensor(c['lens'])
     text = O.list_str_to_tensor(c['text'])
@@ -40,9 +40,9 @@ def test_oracle_vs_reference(name):
     assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
     loss.backward()
     if c['cls'] == 'E2TTS':
-        _check_grads(sd, g['grads'])
+        check_grads(sd, g['grads'])
     else:
-        _check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+        check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
 
 
 @pytest.mark.parametrize('name', list(ATTN_KWARGS_CASES))

@@ -6,36 +6,23 @@ put 1, 32, 64, 65 and 127 valid keys into the last key tile (64 and 1 leave the 
 one row next to another head (a reduction at the wrong row or head coordinates lands in the neighbouring head's dq; the rows the box
 covers past N' carry dS = 0, so these outputs cannot tell a clipped box from one that adds zeros there), grids below one wave and of
 several waves, dropout at odd N' (the keep mask hashed once per key pair), clamped and unclamped. Every output of every head is held
-to the element-wise float64 bounds of tests/test_gpu_attention_hyper_kernels.py / tests/test_gpu_attention_variants.py, and a batch
-element launched alone gives
+to the element-wise float64 bounds of the restatement of tests/attn_ref.py, and a batch element launched alone gives
 bit-identical dk, dv and d_gate: only dq is summed in an order that depends on the launch."""
 import pytest
 import torch
 
-from test_gpu_attention_hyper_kernels import F64, assert_regime, attn_bwd, attn_fwd, attn_inputs, attn_restate, h64
-from test_gpu_attention_variants import inputs as u_inputs, restate as u_restate, ubwd, ufwd
-from test_gpu_leaf_kernels import check_b, check_e, check_f
+from attn_ref import assert_regime, attn_bwd, attn_fwd, attn_inputs, restate, unclamped_inputs
+from kernel_checks import F64, check_b, check_e, check_f, pkg
 
 pytestmark = pytest.mark.gpu
 
 CLAMP = 50.0
 
 
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
 def _run(pkg, unclamped, q, k, v, gate, mask, dog, p_drop, seed):
-    if unclamped:
-        fw = ufwd(pkg, q, k, v, gate, mask, p_drop, seed)
-        bw = ubwd(pkg, q, k, v, fw['o'], fw['lse'], gate, mask, dog, p_drop, seed)
-    else:
-        fw = attn_fwd(pkg, q, k, v, gate, mask, CLAMP, p_drop, seed)
-        bw = attn_bwd(pkg, q, k, v, fw['o'], fw['lse'], gate, mask, dog, CLAMP, p_drop, seed)
+    clamp = None if unclamped else CLAMP
+    fw = attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed)
+    bw = attn_bwd(pkg, q, k, v, fw['o'], fw['lse'], gate, mask, dog, clamp, p_drop, seed)
     torch.cuda.synchronize()
     return fw, bw
 
@@ -55,7 +42,7 @@ CASES = [
 def test_attention_bwd_schedule(pkg, name, B, H, Np, unclamped, p_drop):
     seed = 424242 + Np
     if unclamped:
-        q, k, v, gate, m, mask, dog = u_inputs(B, H, Np, 'random', seed=Np * 13 + H)
+        q, k, v, gate, m, mask, dog = unclamped_inputs(B, H, Np, 'random', seed=Np * 13 + H)
     else:
         q, k, v, gate, m, mask, dog = attn_inputs(B, H, Np, 'mixed', ('tail', 'random'), True, seed=Np * 13 + H)
         # a batch element launched alone makes the same degree-5 / degree-9 choice per warp tile only outside the degree-5 range
@@ -65,12 +52,12 @@ def test_attention_bwd_schedule(pkg, name, B, H, Np, unclamped, p_drop):
         assert Np % 2 == 1
     fw, bw = _run(pkg, unclamped, q, k, v, gate, mask, dog, p_drop, seed)
     if unclamped:
-        r = u_restate(q, k, v, gate, m, p_drop, seed, dog, fw['o'], fw['lse'])
+        r = restate(q, k, v, gate, m, None, p_drop, seed, dog, fw['o'], fw['lse'])
         okq = r['row_ok'][..., None].expand(B, H, Np, 64)
         zero = torch.zeros(B, H, Np, 64, dtype=F64)
         dq_v, dq_e = torch.where(okq, r['dq'].v, zero), torch.where(okq, r['dq'].e, zero)
     else:
-        r = attn_restate(q, k, v, gate, m, CLAMP, p_drop, seed, dog, fw['o'], fw['lse'])
+        r = restate(q, k, v, gate, m, CLAMP, p_drop, seed, dog, fw['o'], fw['lse'])
         dq_v, dq_e = r['dq'].v, r['dq'].e
     check_b(f'{name} dv', bw['dv'], r['dv'].v, r['dv'].e)
     check_b(f'{name} dk', bw['dk'], r['dk'].v, r['dk'].e)

@@ -3,7 +3,7 @@
 Forward (attn_fwd_wgmma_kernel<*, 128>): one CTA per (128-query tile, head, batch) on 64-key tiles through a 3-stage K / V ring; each
 consumer warp picks its tanh evaluation (degree-5 polynomial, degree 9, or tanh.approx for the outliers) over its 16 query rows x 64
 keys, with the dot products over all 128 dims, over the rows the TMA boxes read: past a head's end the next head's, past the tensor's
-end zeros (test_gpu_attention_hyper_kernels.warp_tile_amax, whose tiles are this kernel's).
+end zeros (attn_ref.warp_tile_amax, whose tiles are this kernel's).
 Backward (attn_bwd_d128_wgmma_kernel): one CTA per (64-key tile, head, batch); the query tiles run in the order (j + kt) % nq through
 a 3-stage Q / dO ring; warpgroup 0 computes S^T and warpgroup 1 dP^T and each hands the other half of its fragment over through one
 fp32 exchange buffer, so warpgroup w scores query columns 32 w .. 32 w + 31; the lse / delta of the next query tile travel through a
@@ -11,8 +11,8 @@ two-slot buffer; each warpgroup adds its 64 dQ columns into dq as two 32-float T
 backward's per-warp choice between `tanh_poly2` everywhere and `tanh_poly2` / tanh.approx per element changes no value (both branches
 evaluate `tanh_poly2` for |x| <= 0.5), so only the forward's degree-5 / degree-9 choice bears on isolation.
 
-Every output starts NaN-filled and is held to the element-wise float64 bounds of test_gpu_headdim128.restate (clamped and unclamped;
-the Rv method of test_gpu_attention_hyper_kernels.py), the restatement itself to float64 autograd where the size allows. Rows without
+Every output starts NaN-filled and is held to the element-wise float64 bounds of attn_ref.restate (clamped and unclamped;
+the Rv method of kernel_checks.py), the restatement itself to float64 autograd where the size allows. Rows without
 a valid key give exactly o = 0, lse = -inf, dq = 0. Exact properties are held bit for bit. The host tests at the end feed the same
 checks the restated values with one schedule fault injected each and require every fault to be rejected."""
 import math
@@ -20,26 +20,15 @@ import math
 import pytest
 import torch
 
-import test_gpu_headdim128 as h128
-from test_gpu_attention_hyper_kernels import (BF16, F32, F64, TQ, TQB, Rv, U, agree, assert_regime, attn_inputs, dev, h64,
-                                              host_maskbits)
-from test_gpu_headdim128 import attn_bwd, attn_fwd, autograd64, restate
-from test_gpu_leaf_kernels import check_b, check_e, check_f, gamma
-from test_gpu_parity_full import _dropout_keep
+import attn_ref
+from attn_ref import TQ, TQB, assert_regime, attn_bwd, attn_fwd, attn_inputs, autograd64, dropout_keep, host_maskbits, restate
+from kernel_checks import BF16, F32, F64, U, Rv, agree, check_b, check_e, check_f, dev, gamma, h64, pkg
 
 DH = 128
 TKB = 64            # keys per backward CTA
 QDO_STAGES = 3      # the backward's Q / dO ring
 H100_SMS = 132      # H100 SXM
 W = 1e-3            # relative window of assert_regime around each polynomial threshold
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
 
 
 # ------------------------------------------------------------------------------------------------------------------ launch rules
@@ -248,7 +237,7 @@ def test_attention_d128_shared_bitmask_and_device_seed(pkg, clamp):
         check_e(f'shared bitmask + device seed {key}', f[key], ref_f[key])
     for key in ('dk', 'dv', 'd_gate', 'ws_dO', 'ws_delta'):
         check_e(f'shared bitmask + device seed {key}', b[key], ref_b[key])
-    keep = _dropout_keep(total, B, H, Np, p_drop)
+    keep = dropout_keep(total, B, H, Np, p_drop)
     assert 0.05 < 1 - float(keep.double().mean()) < 0.15                # the summed seed's dropout pattern is the one applied
     r = restate(q, k, v, gate, m, clamp, p_drop, total, dog, f['o'], f['lse'])
     check_outputs('device seed', B, H, Np, gate, f, b, r)
@@ -302,7 +291,7 @@ def test_d128_checks_reject_a_flipped_dropout_keep_bit(host_case, monkeypatch, p
     """one keep bit wrong at the even (parity 0) or odd (1) key of a hashed pair — the half a lane takes from its partner through
     the lane-pair shuffle — at a query column of warpgroup 1 (32 .. 63 of its tile), for dv and for dk"""
     (q, k, v, gate, m, dog, o_k, lse_k), r = host_case
-    keep = _dropout_keep(TSEED, TB, TH, TN, TDROP)
+    keep = dropout_keep(TSEED, TB, TH, TN, TDROP)
     p = _probs(q, k, m)
     dP = r['dO'].v @ h64(v).transpose(-1, -2)
     cols = (torch.arange(TN) % TQB >= 32)[:, None] & (torch.arange(TN) % 2 == parity)[None, :]
@@ -311,7 +300,7 @@ def test_d128_checks_reject_a_flipped_dropout_keep_bit(host_case, monkeypatch, p
         i = int(vis.flatten().argmax())
         flipped = keep.clone()
         flipped.view(-1)[i] = ~flipped.view(-1)[i]
-        monkeypatch.setattr(h128, '_dropout_keep', lambda *a: flipped)
+        monkeypatch.setattr(attn_ref, 'dropout_keep', lambda *a: flipped)
         rf = restate(q, k, v, gate, m, TCLAMP, TDROP, TSEED, dog, o_k, lse_k)
         monkeypatch.undo()
         _rejects(check_b, f'flipped keep bit {out}', rf[out].v.to(BF16), r[out].v, r[out].e)

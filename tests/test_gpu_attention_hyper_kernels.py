@@ -1,24 +1,14 @@
 """Element-wise float64 bounds for the attention (csrc/attn_tc.cu) and hyper-connection (csrc/hyper.cu) kernels.
 
-Method of tests/test_gpu_leaf_kernels.py: every output of b200_attn_maskbits / b200_attn_fwd / b200_attn_bwd (with its prep kernel) and
+Method of tests/kernel_checks.py: every output of b200_attn_maskbits / b200_attn_fwd / b200_attn_bwd (with its prep kernel) and
 b200_hc_width_fwd / _bwd (unfused and fused) / b200_hc_depth_fwd / _bwd is compared element by element with a float64 restatement
 computed on the host from the exact bf16 / fp32 tensors the kernel received. The C ABI is called directly with NaN-prefilled output
 buffers, so an element the kernel never writes fails. Every bound is E (bit-identical), F (fp32) or B (one bf16 rounding of an F
 value, check_b).
 
-The F bounds are carried by `Rv`: each intermediate of the kernel's sequence of operations is held as its exact float64 value `v` and
-a bound `e` on the distance of the kernel's fp32 value from it. Each operation adds the propagated error of its inputs (taken at the
-largest magnitude the computed inputs can have, |v| + e) and its own roundings (standard model fl(a op b) = (a op b)(1 + d), |d| <= u;
-a sum or inner product of n terms in any order, warp shuffles and atomics included, is within gamma_n sum|terms|: Higham, Accuracy and
-Stability of Numerical Algorithms, 2nd ed., (3.4)-(3.5)). Figures for functions and instructions:
-  tanhf 2 ulp, logf 1 ulp (CUDA C++ Programming Guide, appendix "Mathematical Functions"); sqrtf and / correctly rounded;
-  tanh.approx.f32: 2^-10.987 absolute, the PTX ISA's maximum error for it (its later wording, 2^-11 relative, is smaller for |tanh| <= 1);
-  ex2.approx.ftz.f32: 2 ulp relative (PTX ISA, ex2), and results below 2^-126 flush to zero;
-  the odd Taylor polynomials of tanh (Abramowitz and Stegun 4.5.64: u - u^3/3 + 2u^5/15 - 17u^7/315 + 62u^9/2835 - 1382u^11/155925 ...)
-  alternate in sign with decreasing terms for |u| < pi/2, so truncating after u^5 (u^9) errs by at most the u^7 (u^11) term;
-  a Horner evaluation of degree n in x^2 with fp32 coefficients is within gamma_(2n + 6) sum |c_i||x|^(2i+1) (Higham (5.3), plus the
-  rounding of x^2, of the last product by x and of each coefficient); the attention forward folds clamp * log2(e) * scale^(2i+1) /
-  clamp^(2i+1) into its coefficients with at most 16 fp32 roundings each, hence gamma_(2n + 22) there.
+The F bounds are carried by `Rv` (tests/kernel_checks.py). Figures for functions: tanhf 2 ulp, logf 1 ulp (CUDA C++ Programming
+Guide, appendix "Mathematical Functions"); sqrtf and / correctly rounded. The attention restatement, its error model and the
+figures for the instructions it uses are those of tests/attn_ref.py.
 The reference values come from the oracle (float64 autograd of O.hyper_width / O.hyper_depth, kernels' max(||r||, 1e-12) semantics)
 and, for attention, from the float64 restatement itself, which is checked against float64 autograd of the softmax attention where
 the case is small enough. Each restatement must agree with that reference to a thousandth of its own bound.
@@ -31,140 +21,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from attn_ref import (TQ, assert_regime, attn_bwd, attn_fwd, attn_inputs, autograd64, dropout_keep, host_maskbits,
+                      restate)
+from hyper_conv_ref import S, hc_common, hc_fwd, hc_inputs, hc_params
+from kernel_checks import (BF16, F32, F64, U, Rv, _rnd, add, agree, check_b, check_e, check_f, chk_b, chk_f, dev, dot, dots,
+                           exact, fma, gamma, h64, mono, mul, nans, neg, ones_rv, pkg, sms, stream, to_bf16)
+from model_checks import whole_model
 from oracle import e2tts_oracle as O
-from test_gpu_leaf_kernels import U, U16, check_b, check_e, check_f, gamma
-from test_gpu_parity_full import _dropout_keep, _whole_model
 
 pytestmark = pytest.mark.gpu
-
-F64, BF16, F32 = torch.float64, torch.bfloat16, torch.float32
-LOG2E = 1.0 / math.log(2.0)
-S = 4                         # residual streams (the only count the library builds)
-TANH_APPROX = 2.0 ** -10.987  # tanh.approx.f32
-EX2_REL = 2.0 ** -22          # ex2.approx.ftz.f32: 2 ulp
-FTZ = 2.0 ** -126
-TANH_C = [1.0, -1 / 3, 2 / 15, -17 / 315, 62 / 2835, -1382 / 155925]
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def nans(shape, dtype):
-    return torch.full(shape, float('nan'), device=dev(), dtype=dtype)
-
-
-def h64(t):
-    return t.detach().to(F64).cpu()
-
-
-# ---------------------------------------------------------------------------------------------------------------- running bounds
-class Rv:
-    """exact float64 value v of an fp32 quantity of the kernel, and a bound e on |kernel value - v|"""
-
-    def __init__(self, v, e=None):
-        self.v = v
-        self.e = torch.zeros_like(v) if e is None else e + torch.zeros_like(v)
-
-    def mag(self):
-        return self.v.abs() + self.e
-
-    def __getitem__(self, i):
-        return Rv(self.v[i], self.e[i])
-
-    def reshape(self, *shape):
-        return Rv(self.v.reshape(*shape), self.e.reshape(*shape))
-
-
-def exact(t):
-    return Rv(h64(t))
-
-
-def _rnd(v, p, n=1):
-    """n roundings of a result whose inputs carry the propagated error p"""
-    return Rv(v, p + gamma(n) * (v.abs() + p))
-
-
-def mul(a, b, n=1):
-    return _rnd(a.v * b.v, a.mag() * b.e + a.e * b.v.abs(), n)
-
-
-def add(a, b, n=1):
-    return _rnd(a.v + b.v, a.e + b.e, n)
-
-
-def neg(a):
-    return Rv(-a.v, a.e)
-
-
-def fma(a, b, c):
-    return _rnd(a.v * b.v + c.v, a.mag() * b.e + a.e * b.v.abs() + c.e, 1)
-
-
-def dots(pairs, n):
-    """sum of inner products einsum(eq, a, b) over n terms in all, any order"""
-    v = p = m = 0
-    for eq, a, b in pairs:
-        v = v + torch.einsum(eq, a.v, b.v)
-        p = p + torch.einsum(eq, a.mag(), b.e) + torch.einsum(eq, a.e, b.v.abs())
-        m = m + torch.einsum(eq, a.mag(), b.mag())
-    return Rv(v, p + gamma(n) * m)
-
-
-def dot(eq, a, b, n):
-    return dots([(eq, a, b)], n)
-
-
-def mono(a, f, rel, lo=None):
-    """f monotone on [v - e, v + e] (clipped below at lo), result rounded with relative error rel"""
-    v = f(a.v)
-    x0 = a.v - a.e if lo is None else torch.clamp(a.v - a.e, min=lo)
-    p = torch.maximum((f(a.v + a.e) - v).abs(), (f(x0) - v).abs())
-    return Rv(v, p + rel * (v.abs() + p))
-
-
-def to_bf16(a):
-    return Rv(a.v, a.e + U16 * a.mag())
-
-
-def ones_rv(*shape):
-    return Rv(torch.ones(*shape, dtype=F64))
-
-
-def agree(name, r, ref):
-    """the restatement r computes the reference value to a thousandth of its bound; returns the bound to hold the kernel to"""
-    ref = ref.detach().to(F64).cpu().reshape(r.v.shape)
-    slack = 1e-3 * r.e + 1e-12 * ref.abs() + 1e-300
-    bad = (r.v - ref).abs() > slack
-    assert not bool(bad.any()), f'{name}: the float64 restatement disagrees with the reference ({int(bad.sum())} elements)'
-    return ref, r.e + slack
-
-
-def chk_f(name, got, r, ref):
-    ref, bound = agree(name, r, ref)
-    check_f(name, got, ref, bound)
-
-
-def chk_b(name, got, r, ref):
-    """r: the fp32 value before the kernel's final bf16 rounding"""
-    ref, bound = agree(name, r, ref)
-    check_b(name, got, ref, bound)
 
 
 # ================================================================================================================ hyper-connections
@@ -193,49 +58,6 @@ def depth_bwd_warps(T):
     return min(-(-T // 8), sms() * 8) * 8
 
 
-def hc_params(D, seed):
-    g = torch.Generator().manual_seed(seed)
-    P = dict(gamma=torch.randn(D, generator=g) * 0.1, afn=torch.randn(D, S + 1, generator=g) * 0.05, ascale=torch.tensor(0.5),
-             salpha=torch.randn(S, S + 1, generator=g) * 0.5 + 0.3, bfn=torch.randn(D, generator=g) * 0.05, bscale=torch.tensor(0.7),
-             sbeta=torch.randn(S, generator=g) * 0.3 + 1)
-    return {k: v.to(dev()) for k, v in P.items()}
-
-
-def hc_inputs(T, D, rpb, mode, fused, seed, zero_tokens=()):
-    g = torch.Generator().manual_seed(seed)
-    x = (torch.randn(T, S, D, generator=g) * 1.5).to(BF16)
-    y = torch.randn(T, D, generator=g).to(BF16) if fused else None
-    bp = (1 + 0.3 * torch.randn(T, S, generator=g)) if fused else None
-    for tok, streams in zero_tokens:
-        x[tok, list(streams)] = 0
-    ng = None
-    if mode == 2:
-        ng = 1 + 0.2 * torch.randn(T // rpb, D, generator=g)
-    elif mode == 1:
-        ng = 1 + 0.2 * torch.randn(D, generator=g)
-    d_branch = torch.randn(T, D, generator=g).to(BF16)
-    d_res = torch.randn(T, S, D, generator=g).to(BF16)
-    d_beta = torch.randn(T, S, generator=g)
-    to = lambda t: None if t is None else t.to(dev()).contiguous()
-    return dict(x=to(x), y=to(y), bp=to(bp), ng=to(ng), d_branch=to(d_branch), d_res=to(d_res), d_beta=to(d_beta))
-
-
-def _hc_common(P, x, mode, ng, rpb, y, bp):
-    T, _, D = x.shape
-    return dict(xres=x, norm_gamma=P['gamma'], dynamic_alpha_fn=P['afn'], dynamic_alpha_scale=P['ascale'], static_alpha=P['salpha'],
-                dynamic_beta_fn=P['bfn'], dynamic_beta_scale=P['bscale'], static_beta=P['sbeta'], norm_mode=mode, norm_gain=ng,
-                rows_per_batch=rpb, T=T, D=D, num_streams=S, y_prev=y, beta_prev=bp)
-
-
-def hc_fwd(pkg, P, x, mode, ng, rpb, y=None, bp=None):
-    T, _, D = x.shape
-    out = dict(branch=nans((T, D), BF16), res=nans((T, S, D), BF16), beta=nans((T, S), F32), stats=nans((T, 32), F32))
-    a = pkg.lib.make_args('b200_hc_width_args', **_hc_common(P, x, mode, ng, rpb, y, bp), branch=out['branch'], res_out=out['res'],
-                          beta_out=out['beta'], stats_out=out['stats'])
-    pkg.lib.call('b200_hc_width_fwd', a, stream())
-    return out
-
-
 def hc_bwd(pkg, P, x, mode, ng, rpb, stats, d_branch, d_res, d_beta, y=None, bp=None):
     T, _, D = x.shape
     fused = y is not None
@@ -243,7 +65,7 @@ def hc_bwd(pkg, P, x, mode, ng, rpb, stats, d_branch, d_res, d_beta, y=None, bp=
     g = {k: torch.zeros_like(v) for k, v in P.items()}     # the kernel ADDS into the parameter gradients
     g_ng = torch.zeros_like(ng) if mode else None
     ws = nans((T * 20 + D * 8,), F32)                      # the workspace size of include/b200_e2tts.h
-    a = pkg.lib.make_args('b200_hc_width_args', **_hc_common(P, x, mode, ng, rpb, y, bp), d_branch=d_branch, d_res=d_res, d_beta=d_beta,
+    a = pkg.lib.make_args('b200_hc_width_args', **hc_common(P, x, mode, ng, rpb, y, bp), d_branch=d_branch, d_res=d_res, d_beta=d_beta,
                           d_xres=out['d_xres'], g_norm_gamma=g['gamma'], g_dynamic_alpha_fn=g['afn'], g_dynamic_alpha_scale=g['ascale'],
                           g_static_alpha=g['salpha'], g_dynamic_beta_fn=g['bfn'], g_dynamic_beta_scale=g['bscale'], g_static_beta=g['sbeta'],
                           g_norm_gain=g_ng, ws_records=ws, stats=stats, d_y_prev=out['d_y'], d_beta_prev=out['d_bp'])
@@ -509,247 +331,10 @@ def test_whole_model_single_short_clip(pkg):
     GEMM result (D * 8 floats) is larger than its coefficient rows (T * 20 floats)"""
     T, D = 1 * (100 + 32), 512
     assert T * 20 < D * 8
-    _whole_model(pkg, dict(dim=512, depth=2, heads=8), B=1, N=100, lens=[100], seed=70)
+    whole_model(pkg, dict(dim=512, depth=2, heads=8), B=1, N=100, lens=[100], seed=70)
 
 
 # ================================================================================================================ attention
-SCALE = 0.125   # 64 ** -0.5
-TQ, TKV_FWD, TQB = 128, 64, 64
-
-
-def mask_words(Np):
-    return ((Np + 127) // 128) * 4
-
-
-def host_maskbits(m, Np):
-    """the layout of attn_maskbits_kernel: bit n % 32 of word n / 32 set iff key n < Np is kept; words per batch padded to 4 per 128 keys"""
-    B = m.shape[0]
-    W = mask_words(Np)
-    keep = torch.zeros(B, W * 32, dtype=torch.int64)
-    keep[:, :Np] = m.to(torch.int64)
-    w = (keep.view(B, W, 32) << torch.arange(32, dtype=torch.int64)).sum(-1)
-    return torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32).flatten()
-
-
-def warp_tile_amax(q, k):
-    """max |s| over each forward warp's fragment (16 query rows x 64 keys, the dot product over all dh head dims: the head-dim-128
-    forward has the same 128-query / 64-key tiles), over the rows the TMA boxes read: past the end of a head they are the next head's
-    rows, past the end of the tensor zeros"""
-    B, H, Np, dh = q.shape
-    Qf, Kf = h64(q).reshape(-1, dh), h64(k).reshape(-1, dh)
-    Qf, Kf = torch.cat([Qf, torch.zeros(1, dh, dtype=F64)]), torch.cat([Kf, torch.zeros(1, dh, dtype=F64)])
-    total = B * H * Np
-    nq, nk = -(-Np // TQ) * TQ, -(-Np // TKV_FWD) * TKV_FWD
-    out_all, out_valid = [], []
-    for bh in range(B * H):
-        qi = (bh * Np + torch.arange(nq)).clamp(max=total)
-        ki = (bh * Np + torch.arange(nk)).clamp(max=total)
-        s = (Qf[qi] @ Kf[ki].t()).abs()
-        out_all.append(s.view(nq // 16, 16, nk // 64, 64).amax((1, 3)))
-        sv = s.clone()
-        sv[Np:] = 0
-        sv[:, Np:] = 0
-        sv = sv.view(nq // 16, 16, nk // 64, 64).amax((1, 3))
-        sv[(torch.arange(nq // 16) * 16 >= Np)] = math.inf        # warps without a query row of this head write nothing
-        out_valid.append(sv)
-    return torch.stack(out_all), torch.stack(out_valid)
-
-
-def poly_mag(au, n):
-    return sum(abs(TANH_C[i]) * au ** (2 * i + 1) for i in range(n))
-
-
-def logit_eval_err(au, fwd, w=1e-3):
-    """bound on |computed tanh(u) - tanh(u)| of the forward (fwd: the folded polynomials in the raw score, degree 5 for a warp tile within
-    |u| <= 0.15, degree 9 within 0.5, tanh.approx beyond) or of the backward (degree 9 for |u| <= 0.5, tanh.approx beyond). A path is
-    allowed for an element when its own |u| permits it, with a relative window w around each threshold for the fp32 score's error."""
-    c = 22 if fwd else 6
-    e5 = abs(TANH_C[3]) * au ** 7 + gamma(4 + c) * poly_mag(au, 3)
-    e9 = abs(TANH_C[5]) * au ** 11 + gamma(8 + c) * poly_mag(au, 5)
-    et = TANH_APPROX + gamma(2) * au
-    e = torch.zeros_like(au)
-    if fwd:
-        e = torch.where(au <= 0.15 * (1 + w), torch.maximum(e, e5), e)
-    e = torch.where(au <= 0.5 * (1 + w), torch.maximum(e, e9), e)
-    return torch.where(au >= 0.5 * (1 - w), torch.maximum(e, et), e)
-
-
-def ex2_rv(arg, valid):
-    """p = ex2.approx.ftz(arg) for valid elements, exactly 0 elsewhere"""
-    v = torch.exp2(arg.v)
-    e = v * (torch.exp2(arg.e) * (1 + EX2_REL) - 1) + FTZ
-    z = torch.zeros_like(v)
-    return Rv(torch.where(valid, v, z), torch.where(valid, e, z))
-
-
-def attn_restate(q, k, v, gate, m, clamp, p_drop, seed, dog, o_k, lse_k):
-    """forward and backward of attn_tc.cu as Rv on [B, H, Np(query), Np(key)]; o_k / lse_k: the kernel's saved forward outputs"""
-    B, H, Np, _ = q.shape
-    Q, K, V = exact(q), exact(k), exact(v)
-    soc = SCALE / clamp
-    clog = clamp * LOG2E
-    thr = int(p_drop * 65536)
-    ks = 65536 / (65536 - thr)
-    ksR = Rv(torch.tensor(ks, dtype=F64), U * ks if p_drop > 0 else 0.0)
-    valid = m[:, None, None, :].expand(B, H, Np, Np)
-    keep = _dropout_keep(seed, B, H, Np, p_drop).to(F64) if p_drop > 0 else torch.ones(B, H, Np, Np, dtype=F64)
-    s = dot('bhid,bhjd->bhij', Q, K, 64)
-    u = s.v * soc
-    au = u.abs()
-    # forward: y = clamp log2(e) tanh(u), p = 2^y on kept keys, l = sum p, lse = ln l, o = (sum bf16(p keep) v) ks / l
-    y = Rv(clog * torch.tanh(u), LOG2E * SCALE * s.e + clog * logit_eval_err(au, True) + gamma(3) * clog * torch.tanh(u).abs())
-    p = ex2_rv(y, valid)
-    l = dot('bhij,j->bhi', p, ones_rv(Np), Np)
-    lse = mono(l, torch.log, 2 * U)                                  # logf: 1 ulp
-    pk = to_bf16(Rv(p.v * keep, p.e * keep))
-    oacc = dot('bhij,bhjd->bhid', pk, V, Np)
-    inv = mono(l, lambda t: ks / t, gamma(2))                        # keep_scale (rounded) / l
-    o = mul(oacc, inv[..., None])
-    G = Rv(h64(gate).view(B, Np, H).permute(0, 2, 1)[..., None]) if gate is not None else Rv(torch.ones(B, H, Np, 1, dtype=F64))
-    og = mul(to_bf16(o), G)                                          # gate times the kernel's bf16 o, rounded again to bf16
-    # backward
-    DOG = Rv(h64(dog).view(B, Np, H, 64).permute(0, 2, 1, 3))
-    dO = to_bf16(mul(DOG, G))
-    ok64 = h64(o_k)
-    dgate_own = (DOG.v * ok64).sum(-1)                               # prep: <dog, o> with the kernel's own o
-    dgate_e = gamma(64) * (DOG.v.abs() * ok64.abs()).sum(-1)
-    delta = Rv((dO.v * o.v).sum(-1),
-               G.v[..., 0].abs() * ((DOG.v.abs() * (ok64 - o.v).abs()).sum(-1) + gamma(65) * (DOG.v.abs() * ok64.abs()).sum(-1)))
-    dP = dot('bhid,bhjd->bhij', dO, V, 64)
-    th = Rv(torch.tanh(u), soc * s.e + logit_eval_err(au, False))
-    dlse = (h64(lse_k) - lse.v).abs()
-    arg = Rv(clog * th.v - lse.v[..., None] * LOG2E)
-    arg.e = (clog * th.e + gamma(2) * clog * th.v.abs() + LOG2E * dlse[..., None] + gamma(2) * LOG2E * h64(lse_k).abs()[..., None])
-    arg = _rnd(arg.v, arg.e)                                         # the fma rounds once
-    pb = ex2_rv(arg, valid)
-    dsc = _rnd(SCALE * (1 - th.v ** 2), SCALE * (2 * th.v.abs() * th.e + th.e ** 2))
-    if p_drop > 0:                                                   # fma(keep ? dP : 0, keep_scale, -delta)
-        tt = _rnd(keep * ks * dP.v - delta.v[..., None], keep * (ks * dP.e + dP.v.abs() * ksR.e) + delta.e[..., None])
-    else:
-        tt = _rnd(dP.v - delta.v[..., None], dP.e + delta.e[..., None])
-    ds = to_bf16(mul(mul(pb, tt), dsc))
-    dk = dot('bhij,bhid->bhjd', ds, Q, Np)
-    dq = dot('bhij,bhjd->bhid', ds, K, Np)
-    dv = mul(dot('bhij,bhid->bhjd', to_bf16(Rv(pb.v * keep, pb.e * keep)), dO, Np), ksR)
-    return dict(o=o, og=og, lse=lse, dO=dO, dgate_own=dgate_own, dgate_e=dgate_e, dq=dq, dk=dk, dv=dv, s=s)
-
-
-def attn_autograd64(q, k, v, gate, m, clamp, p_drop, seed, dog):
-    """float64 autograd of the softmax attention the kernels implement (x-transformers Attend as the reference configures it)"""
-    B, H, Np, _ = q.shape
-    qr, kr, vr = (h64(t).requires_grad_() for t in (q, k, v))
-    sim = torch.tanh(torch.einsum('bhid,bhjd->bhij', qr, kr) * SCALE / clamp) * clamp
-    sim = sim.masked_fill(~m[:, None, None, :], -math.inf)
-    lse = torch.logsumexp(sim, -1)
-    attn = torch.softmax(sim, -1)
-    if p_drop > 0:
-        attn = attn * _dropout_keep(seed, B, H, Np, p_drop) * (65536 / (65536 - int(p_drop * 65536)))
-    o = attn @ vr
-    g = h64(gate).view(B, Np, H).permute(0, 2, 1)[..., None] if gate is not None else 1.0
-    dog4 = h64(dog).view(B, Np, H, 64).permute(0, 2, 1, 3)
-    dq, dk, dv = torch.autograd.grad(o * g, [qr, kr, vr], dog4)
-    return dict(o=o.detach(), lse=lse.detach(), dq=dq, dk=dk, dv=dv)
-
-
-def attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed, ws=None, ready=0, seed_dev=None):
-    B, H, Np, _ = q.shape
-    o, og, lse = nans(q.shape, BF16), nans((B * Np, H * 64), BF16), nans((B, H, Np), F32)
-    if ws is None:
-        ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
-    a = pkg.lib.make_args('b200_attn_fwd_args', q=q, k=k, v=v, keymask=mask, gate=gate, o=o, og=og, lse=lse, B=B, H=H, Np=Np, dim_head=64,
-                          scale=SCALE, softclamp=clamp, dropout_p=p_drop, seed=seed, ws_maskbits=ws, seed_dev=seed_dev, maskbits_ready=ready)
-    pkg.lib.call('b200_attn_fwd', a, stream())
-    return dict(o=o, og=og, lse=lse, ws=ws)
-
-
-def attn_bwd(pkg, q, k, v, o, lse, gate, mask, dog, clamp, p_drop, seed, ws=None, ready=0, seed_dev=None):
-    B, H, Np, _ = q.shape
-    r = dict(dq=nans(q.shape, F32), dk=nans(q.shape, BF16), dv=nans(q.shape, BF16), ws_dO=nans(q.shape, BF16), ws_delta=nans((B, H, Np), F32),
-             d_gate=nans((B * Np, H), F32))
-    if ws is None:
-        ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
-    a = pkg.lib.make_args('b200_attn_bwd_args', q=q, k=k, v=v, o=o, d_og=dog, keymask=mask, gate=gate, lse=lse, ws_dO=r['ws_dO'],
-                          ws_delta=r['ws_delta'], d_gate=r['d_gate'], dq=r['dq'], dk=r['dk'], dv=r['dv'], B=B, H=H, Np=Np, dim_head=64,
-                          scale=SCALE, softclamp=clamp, dropout_p=p_drop, seed=seed, ws_maskbits=ws, seed_dev=seed_dev, maskbits_ready=ready)
-    pkg.lib.call('b200_attn_bwd', a, stream())
-    return r
-
-
-def attn_inputs(B, H, Np, regime, masks, gate, seed, dh=64, device=None):
-    """regime: the logit regime assert_regime proves ('big': |scale s| > 90 somewhere, for the unclamped kernels). The clamp argument
-    u = s dh^-1/2 / clamp of scores of standard deviation sd^2 dh^1/2 does not depend on dh, so the recipes hold at every head dim.
-    masks: one kind per batch element (cycled) — 'edges', 'tail', 'random', 'none', 'empty' (no valid key)."""
-    g = torch.Generator().manual_seed(seed)
-    rn = lambda *s: torch.randn(*s, generator=g)
-    if regime == 'deg9':
-        # s = dh c^2 a_i b_j + noise along one sign vector per head, c^2 dh^1/2 constant: |u| up to just under 0.5 (|s| / 400 at
-        # dh = 64), so whole tiles need degree 9
-        c = 1.75 * (64 / dh) ** 0.25
-        sv = torch.where(rn(B, H, 1, dh) > 0, 1.0, -1.0)
-        a = c * (0.5 + 0.5 * torch.rand(B, H, Np, 1, generator=g))
-        b = c * (2 * torch.rand(B, H, Np, 1, generator=g) - 1)
-        q, k = sv * a + 0.01 * rn(B, H, Np, dh), sv * b
-    else:
-        sd = {'deg5': 1.0, 'mixed': 1.0, 'tanh': 7.0, 'sat': 60.0, 'big': 6.0}[regime]
-        q, k = rn(B, H, Np, dh) * sd, rn(B, H, Np, dh) * sd
-        if regime == 'mixed':
-            k[:, :, ::7] *= 16                                        # every 7th key far outside the polynomial range
-            # and every warp tile with a row of the head beyond the degree-5 range: the first key of each 64-key tile and the last
-            # key are |s| ~ 16 |sum q| (std 128), the last query row meets them at s = 64 * 4 * 16
-            k[:, :, ::64] = 16.0
-            k[:, :, -1] = 16.0
-            q[:, :, -1] = 4.0
-    v = rn(B, H, Np, dh)
-    m = torch.ones(B, Np, dtype=torch.bool)
-    for b in range(B):
-        kind = masks[b % len(masks)]
-        if kind == 'empty':
-            m[b] = False
-            continue
-        if kind == 'edges':                                         # both sides of the 32-bit word, 64-key tile and 128-key tile edges
-            for n in (31, 32, 63, 64, 127, 128):
-                if n < Np:
-                    m[b, n] = False
-        elif kind == 'tail':                                        # a padded tail and the key before the last valid one
-            n_valid = max(Np - Np // 4 - 1, 2)
-            m[b, n_valid:] = False
-            m[b, n_valid - 2] = False
-        elif kind == 'random':
-            m[b] = torch.rand(Np, generator=g) > 0.3
-        m[b, 0] = True                                              # (the model's register keys are always valid)
-    gt = torch.rand(B * Np, H, generator=g) if gate else None
-    dog = rn(B * Np, H * dh)
-    to = lambda t: None if t is None else t.to(dev() if device is None else device).contiguous()
-    return (to(q.to(BF16)), to(k.to(BF16)), to(v.to(BF16)), to(gt), m, to(m.to(torch.uint8)) if masks != ('none',) else None,
-            to(dog.to(BF16)))
-
-
-def assert_regime(regime, q, k, m, clamp, w=1e-3):
-    """the case's scores lie where the regime's name says (score scale dh^-1/2); returns max |u| per forward warp tile over the
-    head's own rows and keys (inf for warps without a query row of the head), None for the unclamped 'big'"""
-    scale = q.shape[-1] ** -0.5
-    if regime == 'big':          # unclamped: 2^(scale s log2 e) of some valid score is beyond fp32 without the running maximum
-        sv = (h64(q) @ h64(k).transpose(-1, -2)).abs() * scale
-        assert clamp is None and float(sv[m[:, None, None, :].expand_as(sv)].max()) > 90
-        return None
-    soc = scale / clamp
-    amax, amax_valid = warp_tile_amax(q, k)
-    ua = amax * soc
-    uv = (h64(q) @ h64(k).transpose(-1, -2)).abs() * soc
-    uv = uv[m[:, None, None, :].expand_as(uv)]
-    if regime == 'deg5':
-        assert bool((ua <= 0.15 * (1 - w)).all())                  # every warp tile on the degree-5 polynomial
-    elif regime == 'deg9':
-        assert bool((ua <= 0.5 * (1 - w)).all()) and bool((ua > 0.15 * (1 + w)).any())
-    elif regime == 'mixed':
-        assert bool((ua > 0.5 * (1 + w)).any()) and 0 < float((uv > 0.5).double().mean()) < 0.5
-    elif regime == 'tanh':
-        assert float((uv > 0.5 * (1 + w)).double().mean()) > 0.5  # mostly tanh.approx
-    elif regime == 'sat':
-        assert clamp == 64.0 and float((uv > 4).double().mean()) > 0.9   # tanh(4) = 0.99933: the clamp saturates
-    return amax_valid * soc
-
-
 # (name, B, H, N', logit regime, softclamp, dropout, per-batch masks, gate, isolation)
 ATTN_CASES = [
     ('n33-b1-h1', 1, 1, 33, 'mixed', 50.0, 0.0, ('edges',), True, False),
@@ -778,13 +363,13 @@ def test_attention_kernels(pkg, name, B, H, Np, regime, clamp, p_drop, masks, us
     if p_drop > 0:
         assert Np % 2 == 1                                          # odd N': the dropout row pitch is N' + 1
     fw = attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed)
-    bw = attn_bwd(pkg, q, k, v, fw['o'], fw['lse'], gate, mask, dog, clamp, p_drop, seed)
+    bw = attn_bwd(pkg, q, k, v, fw['o'], fw['lse'], gate, mask, dog, clamp, p_drop, seed, d_gate=True)
     torch.cuda.synchronize()
     mb = fw['ws'].cpu()
     assert torch.equal(mb, host_maskbits(m, Np)), f'{name}: key bitmask'
-    r = attn_restate(q, k, v, gate, m, clamp, p_drop, seed, dog, fw['o'], fw['lse'])
+    r = restate(q, k, v, gate, m, clamp, p_drop, seed, dog, fw['o'], fw['lse'])
     if B * H * Np * Np <= 3_000_000:
-        ag = attn_autograd64(q, k, v, gate, m, clamp, p_drop, seed, dog)
+        ag = autograd64(q, k, v, gate, m, clamp, p_drop, seed, dog)
         for key in ('o', 'lse', 'dq', 'dk', 'dv'):
             agree(f'{name} {key} (restatement vs float64 autograd)', r[key], ag[key])
     check_b(f'{name} o', fw['o'], r['o'].v, r['o'].e)
@@ -811,7 +396,7 @@ def test_attention_kernels(pkg, name, B, H, Np, regime, clamp, p_drop, masks, us
                 ms = mask[b:b + 1].contiguous() if mask is not None else None
                 dogs = dog.view(B, Np, H, 64)[b, :, hh].contiguous()
                 f1 = attn_fwd(pkg, sl(q), sl(k), sl(v), gs, ms, clamp, p_drop, seed)
-                b1 = attn_bwd(pkg, sl(q), sl(k), sl(v), f1['o'], f1['lse'], gs, ms, dogs, clamp, p_drop, seed)
+                b1 = attn_bwd(pkg, sl(q), sl(k), sl(v), f1['o'], f1['lse'], gs, ms, dogs, clamp, p_drop, seed, d_gate=True)
                 torch.cuda.synchronize()
                 tag = f'{name} isolation b{b} h{hh}'
                 check_e(f'{tag} o', f1['o'], sl(fw['o']))
@@ -844,8 +429,8 @@ def test_attention_shared_bitmask_and_device_seed(pkg):
         check_e(f'shared bitmask + device seed {key}', f[key], ref_f[key])
     for key in ('dk', 'dv', 'd_gate', 'ws_dO', 'ws_delta'):
         check_e(f'shared bitmask + device seed {key}', b[key], ref_b[key])
-    keep = _dropout_keep(total, B, H, Np, p_drop)
+    keep = dropout_keep(total, B, H, Np, p_drop)
     assert 0.05 < 1 - float(keep.double().mean()) < 0.15              # the summed seed's dropout pattern is the one applied
-    r = attn_restate(q, k, v, gate, m, clamp, p_drop, total, dog, f['o'], f['lse'])
+    r = restate(q, k, v, gate, m, clamp, p_drop, total, dog, f['o'], f['lse'])
     check_b('device seed o', f['o'], r['o'].v, r['o'].e)
     check_f('device seed dq', b['dq'], r['dq'].v, r['dq'].e)

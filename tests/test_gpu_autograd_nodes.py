@@ -27,27 +27,14 @@ import pytest
 import torch
 
 import bench
-import test_gpu_attention_hyper_kernels as A
-import test_gpu_conv_melspec_kernels as C
-from test_gpu_gemm_schedule import U, U16, assert_close, check_bf16, drop_mask, gamma, ref64
-from test_gpu_leaf_kernels import check_e
+from attn_ref import attn_fwd
+from hyper_conv_ref import CV_TN, S, cdiv, dw_ref, hc_fwd, hc_inputs, hc_params
+from kernel_checks import U, U16, assert_close, check_bf16, check_e, dev, drop_mask, gamma, h64, nans, pkg, ref64
 
 pytestmark = pytest.mark.gpu
 
 F64, BF16, F32 = torch.float64, torch.bfloat16, torch.float32
 U8 = torch.uint8
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
 
 
 # ------------------------------------------------------------------------------------------------------------ widths of config 2
@@ -73,10 +60,6 @@ def rnd(shape, g, scale=1.0, dtype=BF16, grad=False):
 
 def param(shape, g, scale, grad=True):
     return rnd(shape, g, scale, F32, grad)
-
-
-def nans(shape, dtype):
-    return torch.full(shape, float('nan'), device=dev(), dtype=dtype)
 
 
 def _2d(t):
@@ -235,7 +218,7 @@ def attn_case(pkg, rec, pool, *, B, Np, H, Din, lens, has_mix, extra, p_drop, us
     pkg.lib.call('b200_qkv_post_fwd', a, ops._stream())
     for nm, got, want in (('q', q, q2), ('k', k, k2), ('v', v_s, v2), ('gate', gate, gate2), ('returned v', v, v2)):
         ce(f'{nm} {tag}', got, want)
-    r = A.attn_fwd(pkg, q2, k2, v2, gate2, mask, SOFTCLAMP, p_drop, s, seed_dev=sdev)
+    r = attn_fwd(pkg, q2, k2, v2, gate2, mask, SOFTCLAMP, p_drop, s, seed_dev=sdev)
     ce(f'og {tag}', og, r['og'])
     ce(f'o {tag}', o, r['o'])
     ce(f'lse {tag}', lse, r['lse'])
@@ -501,7 +484,6 @@ def cross_case(pkg, rec, pool, *, T, D, Dt, has_at, with_dto, seed):
             GEMM bound, the residual add, bf16.
       dWta = dxo^T [x | t], dWat = dto^T [x | t]: GEMM bound over T*S rows, fp32."""
     ops = pkg.ops
-    S = A.S
     g = rng(seed)
     R, Kc = T * S, D + Dt
     xs = rnd((T, S, D), g, grad=True)
@@ -563,7 +545,6 @@ def skip_case(pkg, rec, pool, *, T, D, seed):
     """ops.SkipProj: out = [x | skip] W^T over T*S rows (GEMM bound over K = 2D, bf16); dx = dy W[:, :D], dskip = dy W[:, D:]
     (GEMM bound, bf16); dW = dy^T [x | skip] (GEMM bound over T*S, fp32)."""
     ops = pkg.ops
-    S = A.S
     g = rng(seed)
     R = T * S
     xs, sk = rnd((T, S, D), g, grad=True), rnd((T, S, D), g, grad=True)
@@ -832,9 +813,9 @@ def test_hc_width_wiring(pkg, rec, pool, mode, fused):
     input it belongs to. T = 480 tokens of 3 elements (160 rows per batch, T * S a multiple of 64 as the fused backward needs), D = 200."""
     ops = pkg.ops
     T, D, rpb = 480, 200, 160
-    assert ops.hc_can_fuse(T, A.S)
-    P = A.hc_params(D, 100 + mode)
-    inp = A.hc_inputs(T, D, rpb, mode, fused, 101 + mode)
+    assert ops.hc_can_fuse(T, S)
+    P = hc_params(D, 100 + mode)
+    inp = hc_inputs(T, D, rpb, mode, fused, 101 + mode)
     params, ng = hc_leaves(P, inp, mode)
     x = inp['x'].clone().requires_grad_()
     extra = ()
@@ -846,7 +827,7 @@ def test_hc_width_wiring(pkg, rec, pool, mode, fused):
     branch, res, beta = node.apply(x, *extra, *params, ng, mode, rpb)
     ctx = branch.grad_fn
     assert ctx.meta == (mode, rpb)
-    r = A.hc_fwd(pkg, P, inp['x'], mode, inp['ng'], rpb, inp['y'] if fused else None, inp['bp'] if fused else None)
+    r = hc_fwd(pkg, P, inp['x'], mode, inp['ng'], rpb, inp['y'] if fused else None, inp['bp'] if fused else None)
     for nm, got in (('branch', branch), ('res', res), ('beta', beta)):
         ce(f'{nm} mode{mode} fused={fused}', got, r[nm])
     stats = ctx.saved_tensors[3 if fused else 1]
@@ -877,7 +858,7 @@ def test_hc_width_wiring(pkg, rec, pool, mode, fused):
 def test_hc_depth(pkg):
     """ops.HcDepth: out = res + beta y (one product and one add, or one FMA: gamma_2, bf16); backward: d_res is the incoming gradient
     bit for bit, d_y = sum_s beta d_out (gamma_S, bf16), d_beta = sum_d d_out y (gamma_D, fp32). T = 450, D = 200, 4 streams."""
-    T, D, S = 450, 200, A.S
+    T, D = 450, 200
     g = rng(110)
     res, y = rnd((T, S, D), g, grad=True), rnd((T, D), g, grad=True)
     beta = (torch.randn((T, S), device=dev(), generator=g) + 1).requires_grad_()
@@ -913,14 +894,14 @@ def test_dwconv_node(pkg, pool):
     y.backward(dy)
     slab_only(pool)
     m = mask.bool().cpu()
-    r = C.dw_ref(C.h64(x).view(B, Np, D), m, C.h64(w).view(D, ks), C.h64(b), C.h64(dy).view(B, Np, D), C.h64(pre).view(B, Np, D))
+    r = dw_ref(h64(x).view(B, Np, D), m, h64(w).view(D, ks), h64(b), h64(dy).view(B, Np, D), h64(pre).view(B, Np, D))
     mm = m[..., None].expand(B, Np, D).reshape(T, D).to(dev())
     cb('pre', pre, r['conv'].reshape(T, D).to(dev()), r['e_pre'].reshape(T, D).to(dev()))
     for nm, got, key in (('y', y, 'y'), ('dx', x.grad, 'dx')):
         ref, e = r[key].reshape(T, D).to(dev()), r['e_' + key].reshape(T, D).to(dev())
         cb(nm, got.detach()[mm], ref[mm], e[mm])
         ce(f'{nm} masked rows', got.detach()[~mm], torch.zeros_like(got.detach()[~mm]))
-    n = B * C.cdiv(Np, C.CV_TN) * C.CV_TN + 1
+    n = B * cdiv(Np, CV_TN) * CV_TN + 1
     assert w.grad.shape == w.shape
     cf('dweight', w.grad.view(D, ks), r['dW'].to(dev()), gamma(n) * r['dWabs'].to(dev()) + r['dWcar'].to(dev()))
     cf('dbias', b.grad, r['db'].to(dev()), gamma(n) * r['dbabs'].to(dev()) + r['dbcar'].to(dev()))

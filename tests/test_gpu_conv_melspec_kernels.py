@@ -17,50 +17,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from hyper_conv_ref import CV_TN, cdiv, corr, dw_mask, dw_ref, model_mask
+from kernel_checks import F32, F64, BF16, U, check_b, check_e, check_f, dev, gamma, gen, h64, nans, pkg, stream
 from oracle import e2tts_oracle as O
-from test_gpu_attention_hyper_kernels import Rv, add, mul, neg
-from test_gpu_leaf_kernels import U, check_b, check_e, check_f, gamma, sig_err
 
 pytestmark = pytest.mark.gpu
 
-F64, BF16, F32 = torch.float64, torch.bfloat16, torch.float32
-FDIV = 4 * U      # __fdividef: 2 ulp, i.e. at most 4u relative
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def nans(shape, dtype):
-    return torch.full(shape, float('nan'), device=dev(), dtype=dtype)
-
-
-def h64(t):
-    return t.detach().to(F64).cpu()
-
-
-def gen(seed):
-    return torch.Generator().manual_seed(seed)
-
-
-def cdiv(a, b):
-    return -(-a // b)
-
 
 # ======================================================================================================== depthwise conv
-CV_TN, CV_TC, CV_FWD_TILES, CV_BWD_TILES = 64, 64, 2, 4   # token tile, channel tile, tiles per forward / backward block
+CV_TC, CV_FWD_TILES, CV_BWD_TILES = 64, 2, 4   # channel tile, tiles per forward / backward block (token tile: CV_TN)
 
 
 def dw_geometry(Np, D):
@@ -71,40 +36,6 @@ def dw_geometry(Np, D):
     fwd_blocks, bwd_blocks, ctiles = cdiv(ntiles, CV_FWD_TILES), cdiv(ntiles, CV_BWD_TILES), cdiv(D, CV_TC)
     return (ntiles - CV_FWD_TILES * (fwd_blocks - 1), ntiles - CV_BWD_TILES * (bwd_blocks - 1), Np - CV_TN * (ntiles - 1),
             (D - CV_TC * (ctiles - 1)) // 2)
-
-
-def corr(t, w):
-    """out[b, n, c] = sum_k w[c, k] t[b, n + k - ks/2, c] (zero outside the sequence): F.conv1d's depthwise cross-correlation
-    with padding ks/2, on [B, Np, D]"""
-    ks, Np = w.shape[1], t.shape[1]
-    tp = F.pad(t, (0, 0, ks // 2, ks // 2))
-    return sum(w[:, k] * tp[:, k:k + Np] for k in range(ks))
-
-
-def tap_sums(d, t, ks):
-    """out[c, k] = sum_{b, n} d[b, n, c] t[b, n + k - ks/2, c]: the weight gradient of corr"""
-    Np = t.shape[1]
-    tp = F.pad(t, (0, 0, ks // 2, ks // 2))
-    return torch.stack([(d * tp[:, k:k + Np]).sum((0, 1)) for k in range(ks)], 1)
-
-
-def dw_mask(Np, spec, g):
-    """one batch row's validity: 'all', 'none', an int L (tokens n < L valid: a suffix mask, or with L >= 32 the model's register
-    prefix followed by a ragged audio suffix) or 'holes' (random interior holes, a single valid token between two masked ones and
-    masked tokens on both sides of a tile edge)"""
-    if spec == 'all':
-        return torch.ones(Np, dtype=torch.bool)
-    if spec == 'none':
-        return torch.zeros(Np, dtype=torch.bool)
-    if isinstance(spec, int):
-        return torch.arange(Np) < spec
-    m = torch.rand(Np, generator=g) > 0.25
-    if Np >= 3:
-        c = Np // 2
-        m[c - 1], m[c], m[c + 1] = False, True, False
-    if Np > 66:
-        m[63], m[64] = False, False
-    return m
 
 
 def dw_launch_fwd(pkg, x, mask, w, b, with_pre=True):
@@ -122,46 +53,6 @@ def dw_launch_bwd(pkg, x, mask, w, b, dy, pre, dw0, db0):
                           ksize=w.shape[1], pre=pre)
     pkg.lib.call('b200_dwconv_bwd', a, stream())
     return dx, dw, db
-
-
-def dw_ref(x, m, w, b, dy, pre):
-    """float64 restatement on the host, [B, Np, D] (a channel subset is exact: the convolution is per channel).
-    x, dy, pre: the bf16 values the kernel read; m: bool [B, Np]; w [D, k], b [D]: the fp32 parameters.
-
-    pre = conv(m x) + b: the kernel's fp32 value is bias + k FMAs (the zero-padded taps of the 31-wide window add exact zeros),
-        within gamma(k + 1) (|b| + sum|w||m x|) = e_pre; then one bf16 rounding (check_b).
-    y = m silu(pre): the kernel evaluates __fdividef(p, 1 + __expf(-p)) at its fp32 p. |silu'| <= 1.1 carries e_pre; at |p| <= P =
-        |pre| + e_pre the evaluation errs by <= P (sig_err(P) + 4u) (sig_err: the __expf and 1 + e rounding and a rounded
-        quotient; __fdividef's 2 ulp add 4u). This absolute bound also covers p < -87.3, where 1 + e exceeds 2^126 and __fdividef
-        returns 0 for a true value below 1e-36. Masked rows are exactly +0.
-    d_pre = dy silu'(pre_bf16), from the saved bf16 pre the kernel reads, so the designed rounding of pre is not an error of the
-        backward: s = __fdividef(1, 1 + __expf(-p)) within sig_err(|p|) + 4u, then the fp32 evaluation of s (1 + p (1 - s)) and the
-        product with dy, one rounding per operation (Rv). Masked rows and rows outside the sequence: exactly 0.
-    dx = flipped conv of d_pre: k FMAs from 0, gamma(k) sum|w||d_pre| plus sum|w| e_dpre carried, then bf16; masked rows +0.
-    dW[c, k] = sum d_pre x[n + k - k/2], dbias = sum d_pre over B Np tokens (register sums, shared atomics, global atomics into
-        the initial value: any order) within gamma(B Np64 + 1) sum|terms| (Np64: Np rounded up to whole tiles; the initial value is
-        one term) plus the carried sum e_dpre |x|."""
-    ks = w.shape[1]
-    mx = torch.where(m[..., None], x, torch.zeros((), dtype=F64))
-    aw = w.abs()
-    conv = corr(mx, w) + b
-    e_pre = gamma(ks + 1) * (b.abs() + corr(mx.abs(), aw))
-    P = conv.abs() + e_pre
-    y = torch.where(m[..., None], F.silu(conv), torch.zeros((), dtype=F64))
-    e_y = 1.1 * e_pre + P * (sig_err(P) + FDIV)
-    p = torch.where(m[..., None], pre, torch.zeros((), dtype=F64))
-    s = torch.sigmoid(p)
-    one = Rv(torch.ones_like(p))
-    t = mul(Rv(s, sig_err(p) + FDIV), add(one, mul(Rv(p), add(one, neg(Rv(s, sig_err(p) + FDIV))))))
-    dp = mul(Rv(torch.where(m[..., None], dy, torch.zeros((), dtype=F64))), t)
-    dpv = torch.where(m[..., None], dp.v, torch.zeros((), dtype=F64))
-    edp = torch.where(m[..., None], dp.e, torch.zeros((), dtype=F64))
-    wf = w.flip(1)
-    dx = corr(dpv, wf)
-    e_dx = gamma(ks) * corr(dpv.abs() + edp, wf.abs()) + corr(edp, wf.abs())
-    return dict(conv=conv, e_pre=e_pre, y=y, e_y=e_y, dpre=dpv, e_dpre=edp, dx=dx, e_dx=e_dx,
-                dW=tap_sums(dpv, mx, ks), dWabs=tap_sums(dpv.abs() + edp, mx.abs(), ks), dWcar=tap_sums(edp, mx.abs(), ks),
-                db=dpv.sum((0, 1)), dbabs=(dpv.abs() + edp).sum((0, 1)), dbcar=edp.sum((0, 1)))
 
 
 def check_dwconv(pkg, B, Np, D, ks, masks, seed, scale=1.0, poison=False, chans=None, tag=''):
@@ -203,13 +94,6 @@ def check_dwconv(pkg, B, Np, D, ks, masks, seed, scale=1.0, poison=False, chans=
     return dict(m=m, x=x, w=w, b=b, dy=dy, y=y, pre=pre, dx=dx, r=r)
 
 
-def _model_mask(B, Np, g, R=32):
-    """the model's layer mask: R register tokens, then each clip's audio length (ragged, the longest fills the row)"""
-    lens = torch.randint(Np // 3, Np - R + 1, (B,), generator=g)
-    lens[0] = Np - R
-    return [R + int(n) for n in lens]
-
-
 # name, B, Np, D, ksize, per-row masks (None: null mask pointer), x scale, poison, channel subset,
 # expected (tiles of the last forward block, of the last backward block, tokens of the last tile, pairs of the last channel tile)
 DW_CASES = [
@@ -247,7 +131,7 @@ def test_dwconv_kernels(pkg, name, B, Np, D, ks, masks, scale, poison, subset, g
     assert dw_geometry(Np, D) == geo
     seed = sum(map(ord, name))
     if masks == 'model':
-        masks = _model_mask(B, Np, gen(seed + 1))
+        masks = model_mask(B, Np, gen(seed + 1))
     chans = None
     if subset:      # first, a middle and the last channel tile
         mid = (cdiv(D, CV_TC) // 2) * CV_TC

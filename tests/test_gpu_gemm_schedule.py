@@ -14,31 +14,9 @@ import math
 import pytest
 import torch
 
+from kernel_checks import BF16, F32, F64, U, U16, assert_close, check_bf16, dev, drop_mask, pkg, ref64, sms
+
 pytestmark = pytest.mark.gpu
-
-F64, BF16, F32 = torch.float64, torch.bfloat16, torch.float32
-U = 2.0 ** -24
-U16 = 2.0 ** -8
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def gamma(n):
-    return n * U / (1 - n * U)
 
 
 # ---------------------------------------------------------------------------------------------- restated host selection (b200_gemm)
@@ -74,29 +52,6 @@ def operands(M, N, K, seed, scale=1.0):
     A = torch.randn(M, K, device=dev(), generator=g).to(BF16)
     B = (torch.randn(N, K, device=dev(), generator=g) * scale).to(BF16)
     return A, B
-
-
-def ref64(A, B):
-    """exact-operand float64 product and the accumulation bound gamma_K * sum |a b|"""
-    a, b = A.to(F64), B.to(F64)
-    return a @ b.t(), gamma(A.shape[1]) * (a.abs() @ b.abs().t())
-
-
-def assert_close(name, got, ref, bound):
-    got = got.to(F64)
-    err = (got - ref).abs()
-    bad = ~(err <= bound)            # NaN fails
-    if bool(bad.any()):
-        i = int(bad.flatten().nonzero()[0, 0])
-        idx = divmod(i, ref.shape[1])
-        raise AssertionError(f'{name}: {int(bad.sum())} of {ref.numel()} elements out of bound, first at {idx}: '
-                             f'got {got.flatten()[i].item():.9g}, ref {ref.flatten()[i].item():.9g}, bound {bound.flatten()[i].item():.3g}')
-
-
-def check_bf16(name, got, ref, acc_bound, extra=0.0):
-    """bf16 output: one rounding of an fp32 value within acc_bound (+ extra) of ref"""
-    b = acc_bound + extra
-    assert_close(name, got, ref, b + U16 * (ref.abs() + b))
 
 
 def nan_out(M, ld, fp32=False):
@@ -241,21 +196,6 @@ def test_split_k_at_the_64_cap(pkg):
 
 
 # ---------------------------------------------------------------------------------------------- GEGLU + dropout
-def drop_mask(seed, rows, hidden):
-    """kept (True) / dropped pattern of the GEGLU epilogue, restated in torch integer arithmetic (ptx.cuh drop_words):
-    pair = (row * hidden + col) >> 1 (low 32 bits); x = pair * 0x9E3779B1 + seedmix; x ^= x >> 15; word = x * (0x85EBCA6B for even
-    col, 0xC2B2AE35 for odd col), all mod 2^32; keep iff word >= thresh16 << 16."""
-    M32 = 0xFFFFFFFF
-    seedmix = (seed & M32) ^ (((seed >> 32) * 0x85EBCA77) & M32)
-    r = torch.arange(rows, dtype=torch.int64, device=dev())[:, None]
-    c = torch.arange(hidden, dtype=torch.int64, device=dev())[None, :]
-    pair = ((r * hidden + c) >> 1) & M32
-    x = (pair * 0x9E3779B1 + seedmix) & M32
-    x = x ^ (x >> 15)
-    word = torch.where(c % 2 == 0, (x * 0x85EBCA6B) & M32, (x * 0xC2B2AE35) & M32)
-    return word
-
-
 @pytest.mark.parametrize('M,N,K', [(T2, 4096, 512), (T2, 2048, 256), (1096, 512, 320), (1096, 512, 192)])
 def test_geglu_dropout(pkg, M, N, K):
     p, seed = 0.1, 1234

@@ -2,193 +2,28 @@
 kernels up to the whole model.
 
 Kernels: b200_attn_fwd / b200_attn_bwd at dim_head 128 (the <*, 128> forward instantiations and attn_bwd_d128_wgmma_kernel), clamped
-and unclamped, with and without the head gate, against element-wise float64 bounds in the method of
-tests/test_gpu_attention_hyper_kernels.py (its Rv helpers, imported); outputs start NaN-filled. The restatement below is that file's
-(clamped) and tests/test_gpu_attention_variants.py's (unclamped) with the head dim a parameter: the dot products run over 128 terms
-and the score scale is 128 ** -0.5. Rows whose keys are all masked give o = og = 0, lse = -inf and zero gradients.
+and unclamped, with and without the head gate, against the element-wise float64 bounds of the restatement of tests/attn_ref.py;
+outputs start NaN-filled. At head dim 128 its dot products run over 128 terms and the score scale is 128 ** -0.5. Rows whose keys
+are all masked give o = og = 0, lse = -inf and zero gradients.
 Then b200_qkv_post_* and b200_rotary_table at dim_head 128, the ops.Attention / AttnCore nodes, and whole models against the oracle
-within the bounds of tests/test_gpu_parity_full.py."""
+within the bounds of tests/model_checks.py."""
 import math
-import random
 
 import pytest
 import torch
 
+from attn_ref import attn_bwd, attn_fwd, autograd64, d128_inputs, dropout_keep, host_maskbits, restate
 from attn_variants import variant_oracle
+from conftest import rel_l2
 from headdim_variants import cfg, headdim_oracle
+from kernel_checks import BF16, F32, F64, U, Rv, agree, check_b, check_e, check_f, dev, gamma, h64, nans, pkg, stream
+from model_checks import cos, small_model, whole_model
 from oracle import e2tts_oracle as O
 from residual_variants import plain_residual_oracle
-from test_gpu_attention_hyper_kernels import (EX2_REL, F64, FTZ, BF16, F32, LOG2E, Rv, U, _rnd, agree, dev, dot, exact, ex2_rv, h64,
-                                              host_maskbits, logit_eval_err, mask_words, mono, mul, nans, ones_rv, stream, to_bf16)
-from test_gpu_leaf_kernels import check_b, check_e, check_f, gamma
-from conftest import rel_l2
-from test_gpu_parity_full import _dropout_keep, _whole_model, cos
 
 pytestmark = pytest.mark.gpu
 
 DH = 128
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-# ------------------------------------------------------------------------------------------------------------------ launches
-def _clamp_fields(clamp):
-    return dict(softclamp=0.0, unclamped=1) if clamp is None else dict(softclamp=clamp, unclamped=0)
-
-
-def attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed, ws=None, ready=0, seed_dev=None):
-    B, H, Np, dh = q.shape
-    o, og, lse = nans(q.shape, BF16), nans((B * Np, H * dh), BF16), nans((B, H, Np), F32)
-    if ws is None:
-        ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
-    a = pkg.lib.make_args('b200_attn_fwd_args', q=q, k=k, v=v, keymask=mask, gate=gate, o=o, og=og, lse=lse, B=B, H=H, Np=Np, dim_head=dh,
-                          scale=dh ** -0.5, dropout_p=p_drop, seed=seed, ws_maskbits=ws, seed_dev=seed_dev, maskbits_ready=ready,
-                          **_clamp_fields(clamp))
-    pkg.lib.call('b200_attn_fwd', a, stream())
-    return dict(o=o, og=og, lse=lse, ws=ws)
-
-
-def attn_bwd(pkg, q, k, v, o, lse, gate, mask, dog, clamp, p_drop, seed, ws=None, ready=0, seed_dev=None):
-    B, H, Np, dh = q.shape
-    r = dict(dq=nans(q.shape, F32), dk=nans(q.shape, BF16), dv=nans(q.shape, BF16), ws_dO=nans(q.shape, BF16), ws_delta=nans((B, H, Np), F32),
-             d_gate=nans((B * Np, H), F32) if gate is not None else None)
-    if ws is None:
-        ws = torch.full((mask_words(Np) * B,), -1, device=dev(), dtype=torch.int32)
-    a = pkg.lib.make_args('b200_attn_bwd_args', q=q, k=k, v=v, o=o, d_og=dog, keymask=mask, gate=gate, lse=lse, ws_dO=r['ws_dO'],
-                          ws_delta=r['ws_delta'], d_gate=r['d_gate'], dq=r['dq'], dk=r['dk'], dv=r['dv'], B=B, H=H, Np=Np, dim_head=dh,
-                          scale=dh ** -0.5, dropout_p=p_drop, seed=seed, ws_maskbits=ws, seed_dev=seed_dev, maskbits_ready=ready,
-                          **_clamp_fields(clamp))
-    pkg.lib.call('b200_attn_bwd', a, stream())
-    return r
-
-
-# ------------------------------------------------------------------------------------------------------------------ inputs
-def inputs(B, H, Np, kind, gate, masked, seed, dh=DH):
-    """kind: 'small' (|u| mostly in the polynomial ranges), 'mixed' (every 7th key far outside them), 'big' (unclamped: |scale s| > 90
-    somewhere). masked: random key masks, and batch element 1 (if any) without a valid key."""
-    g = torch.Generator().manual_seed(seed)
-    rn = lambda *s: torch.randn(*s, generator=g)
-    q, k = rn(B, H, Np, dh), rn(B, H, Np, dh)
-    if kind == 'mixed':
-        k[:, :, ::7] *= 16
-    elif kind == 'big':
-        q, k = q * 5.0, k * 5.0
-    v = rn(B, H, Np, dh)
-    m = torch.ones(B, Np, dtype=torch.bool)
-    if masked:
-        m = torch.rand(B, Np, generator=g) > 0.3
-        m[:, 0] = True
-        if B > 1:
-            m[1] = False
-    gt = torch.rand(B * Np, H, generator=g) if gate else None
-    dog = rn(B * Np, H * dh)
-    to = lambda t: None if t is None else t.to(dev()).contiguous()
-    return (to(q.to(BF16)), to(k.to(BF16)), to(v.to(BF16)), to(gt), m, to(m.to(torch.uint8)) if masked else None, to(dog.to(BF16)))
-
-
-# ------------------------------------------------------------------------------------------------------------------ restatement
-def restate(q, k, v, gate, m, clamp, p_drop, seed, dog, o_k, lse_k):
-    """forward and backward of attn_tc.cu at head dim dh as Rv on [B, H, Np(query), Np(key)]; clamp None: the unclamped kernels.
-    o_k / lse_k: the kernel's saved forward outputs. Rows without a valid key are left to the caller."""
-    B, H, Np, dh = q.shape
-    scale = dh ** -0.5
-    sl2 = scale * LOG2E
-    nkv = -(-Np // 64)
-    Q, K, V = exact(q), exact(k), exact(v)
-    thr = int(p_drop * 65536)
-    ks = 65536 / (65536 - thr)
-    ksR = Rv(torch.tensor(ks, dtype=F64), U * ks if p_drop > 0 else 0.0)
-    valid = m[:, None, None, :].expand(B, H, Np, Np)
-    row_ok = valid.any(-1, keepdim=True)
-    keep = _dropout_keep(seed, B, H, Np, p_drop).to(F64) if p_drop > 0 else torch.ones(B, H, Np, Np, dtype=F64)
-    s = dot('bhid,bhjd->bhij', Q, K, dh)
-    zero = torch.zeros_like(s.v)
-    if clamp is None:
-        M = torch.where(valid, s.v, torch.full_like(s.v, -math.inf)).amax(-1, keepdim=True)
-        M = torch.where(row_ok, M, torch.zeros_like(M))
-        Mabs = torch.where(valid, s.v.abs() + s.e, zero).amax(-1, keepdim=True)
-        A = sl2 * (s.e + 4 * U * (s.v.abs() + Mabs)) + nkv * sl2 * 3 * U * 2 * Mabs
-        r = torch.exp2(A) * (1 + EX2_REL) ** (nkv + 1) - 1
-        pv = torch.where(valid, torch.exp2(sl2 * (s.v - M)), zero)
-        p = Rv(pv, torch.where(valid, pv * r + FTZ, zero))
-        l = dot('bhij,j->bhi', p, ones_rv(Np), Np + 2 * nkv)
-        nacc = Np + 2 * nkv
-    else:
-        soc, clog = scale / clamp, clamp * LOG2E
-        u = s.v * soc
-        y = Rv(clog * torch.tanh(u), LOG2E * scale * s.e + clog * logit_eval_err(u.abs(), True) + gamma(3) * clog * torch.tanh(u).abs())
-        p = ex2_rv(y, valid)
-        l = dot('bhij,j->bhi', p, ones_rv(Np), Np)
-        nacc = Np
-    l1 = Rv(torch.where(row_ok[..., 0], l.v, torch.ones_like(l.v)), l.e)
-    lnl = mono(l1, torch.log, 2 * U)
-    if clamp is None:
-        lse = Rv(M[..., 0] * scale + lnl.v, lnl.e + U * (M[..., 0].abs() * scale + lnl.v.abs()) * 2)
-    else:
-        lse = lnl
-    pk = to_bf16(Rv(p.v * keep, p.e * keep))
-    oacc = dot('bhij,bhjd->bhid', pk, V, nacc)
-    inv = mono(l1, lambda t: ks / t, gamma(2))
-    o = mul(oacc, inv[..., None])
-    G = Rv(h64(gate).view(B, Np, H).permute(0, 2, 1)[..., None]) if gate is not None else Rv(torch.ones(B, H, Np, 1, dtype=F64))
-    og = mul(to_bf16(o), G)
-    # backward: P recomputed from the kernel's lse
-    DOG = Rv(h64(dog).view(B, Np, H, dh).permute(0, 2, 1, 3))
-    dO = to_bf16(mul(DOG, G))
-    ok64 = h64(o_k)
-    dgate_own = (DOG.v * ok64).sum(-1)
-    dgate_e = gamma(dh) * (DOG.v.abs() * ok64.abs()).sum(-1)
-    delta = Rv((dO.v * o.v).sum(-1),
-               G.v[..., 0].abs() * ((DOG.v.abs() * (ok64 - o.v).abs()).sum(-1) + gamma(dh + 1) * (DOG.v.abs() * ok64.abs()).sum(-1)))
-    dP = dot('bhid,bhjd->bhij', dO, V, dh)
-    lk = torch.where(row_ok[..., 0], h64(lse_k), torch.zeros_like(lse.v))
-    dlse = (lk - torch.where(row_ok[..., 0], lse.v, torch.zeros_like(lse.v))).abs()
-    lv = torch.where(row_ok, lse.v[..., None], torch.zeros_like(lse.v[..., None]))
-    if clamp is None:
-        arg = _rnd(sl2 * s.v - lv * LOG2E, sl2 * s.e + LOG2E * dlse[..., None] + gamma(2) * (sl2 * s.v.abs() + LOG2E * lk.abs()[..., None]))
-        dsc = Rv(torch.tensor(scale, dtype=F64))
-    else:
-        th = Rv(torch.tanh(u), soc * s.e + logit_eval_err(u.abs(), False))
-        arg = _rnd(clog * th.v - lv * LOG2E, clog * th.e + gamma(2) * clog * th.v.abs() + LOG2E * dlse[..., None] +
-                   gamma(2) * LOG2E * lk.abs()[..., None])
-        dsc = _rnd(scale * (1 - th.v ** 2), scale * (2 * th.v.abs() * th.e + th.e ** 2))
-    pb = ex2_rv(arg, valid)
-    if p_drop > 0:
-        tt = _rnd(keep * ks * dP.v - delta.v[..., None], keep * (ks * dP.e + dP.v.abs() * ksR.e) + delta.e[..., None])
-    else:
-        tt = _rnd(dP.v - delta.v[..., None], dP.e + delta.e[..., None])
-    ds = to_bf16(mul(mul(pb, tt), dsc))
-    dk = dot('bhij,bhid->bhjd', ds, Q, Np)
-    dq = dot('bhij,bhjd->bhid', ds, K, Np)
-    dv = mul(dot('bhij,bhid->bhjd', to_bf16(Rv(pb.v * keep, pb.e * keep)), dO, Np), ksR)
-    return dict(o=o, og=og, lse=lse, dO=dO, dgate_own=dgate_own, dgate_e=dgate_e, dq=dq, dk=dk, dv=dv, row_ok=row_ok[..., 0])
-
-
-def autograd64(q, k, v, gate, m, clamp, p_drop, seed, dog):
-    """float64 autograd of the softmax attention the kernels implement (rows with a valid key)"""
-    B, H, Np, dh = q.shape
-    qr, kr, vr = (h64(t).requires_grad_() for t in (q, k, v))
-    sim = torch.einsum('bhid,bhjd->bhij', qr, kr) * dh ** -0.5
-    if clamp is not None:
-        sim = torch.tanh(sim / clamp) * clamp
-    valid = m[:, None, None, :].expand_as(sim)
-    row_ok = valid.any(-1, keepdim=True)
-    sim = torch.where(row_ok, sim.masked_fill(~valid, -math.inf), torch.zeros_like(sim))
-    lse = torch.logsumexp(sim, -1)
-    attn = torch.where(row_ok, torch.softmax(sim, -1), torch.zeros_like(sim))
-    if p_drop > 0:
-        attn = attn * _dropout_keep(seed, B, H, Np, p_drop) * (65536 / (65536 - int(p_drop * 65536)))
-    o = attn @ vr
-    g = h64(gate).view(B, Np, H).permute(0, 2, 1)[..., None] if gate is not None else 1.0
-    dog4 = h64(dog).view(B, Np, H, dh).permute(0, 2, 1, 3)
-    dq, dk, dv = torch.autograd.grad(o * g, [qr, kr, vr], dog4)
-    return dict(o=o.detach(), lse=lse.detach(), dq=dq, dk=dk, dv=dv)
 
 
 # (name, B, H, N', logits, softclamp (None: unclamped), dropout, gate, masked)
@@ -210,7 +45,7 @@ CASES = [
 @pytest.mark.parametrize('name,B,H,Np,kind,clamp,p_drop,use_gate,masked', CASES, ids=[c[0] for c in CASES])
 def test_attention_kernels_d128(pkg, name, B, H, Np, kind, clamp, p_drop, use_gate, masked):
     seed = 97531 + Np
-    q, k, v, gate, m, mask, dog = inputs(B, H, Np, kind, use_gate, masked, seed=Np * 13 + H)
+    q, k, v, gate, m, mask, dog = d128_inputs(B, H, Np, kind, use_gate, masked, seed=Np * 13 + H)
     fw = attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed)
     bw = attn_bwd(pkg, q, k, v, fw['o'], fw['lse'], gate, mask, dog, clamp, p_drop, seed)
     torch.cuda.synchronize()
@@ -252,7 +87,7 @@ def test_dropout_kept_set_equals_dim_head_64(pkg, clamp):
     on v = [v64 | v'] gives, in its first 64 columns, bit for bit what the dim_head-64 kernel gives on v64 with the same seed — the
     kept set is indexed by (b, h, query, key) whatever the head width"""
     B, H, Np, p_drop, seed = 2, 3, 193, 0.1, 0xBADC0DE
-    q, k, v, gate, m, mask, dog = inputs(B, H, Np, 'small', True, True, seed=3)
+    q, k, v, gate, m, mask, dog = d128_inputs(B, H, Np, 'small', True, True, seed=3)
     q = torch.zeros_like(q)
     f128 = attn_fwd(pkg, q, k, v, gate, mask, clamp, p_drop, seed)
     sl = lambda t: t[..., :64].contiguous()
@@ -260,7 +95,7 @@ def test_dropout_kept_set_equals_dim_head_64(pkg, clamp):
     torch.cuda.synchronize()
     check_e('kept set: o', sl(f128['o']), f64['o'])
     check_e('kept set: lse', f128['lse'], f64['lse'])
-    keep = _dropout_keep(seed, B, H, Np, p_drop)
+    keep = dropout_keep(seed, B, H, Np, p_drop)
     assert 0.05 < 1 - float(keep.double().mean()) < 0.15
 
 
@@ -436,7 +271,7 @@ def test_attention_node_d128(pkg, B, Np, H, Din, has_mix, has_gate, clamp):
 def test_attn_core_node_d128(pkg):
     """AttnCore at head dim 128 against float64 autograd (cfg2's 4 x 128 heads at N' = 1056 with a masked batch element)"""
     B, H, Np = 2, 4, 1056
-    q, k, v, gate, m, mask, dog = inputs(B, H, Np, 'small', True, True, seed=21)
+    q, k, v, gate, m, mask, dog = d128_inputs(B, H, Np, 'small', True, True, seed=21)
     m[1] = torch.rand(Np) > 0.5
     m[1, 0] = True
     mask = m.to(torch.uint8).to(dev())
@@ -457,39 +292,29 @@ def test_attn_core_node_d128(pkg):
 # ------------------------------------------------------------------------------------------------------------------ whole models
 def test_e2tts_d512_depth8_heads4x128_vs_oracle(pkg):
     """cfg2's width (d512, depth 8) with 4 heads of 128 (I = 512, as 8 x 64): N = 1024 ragged, loss, prediction and every gradient"""
-    _whole_model(pkg, dict(dim=512, depth=8, heads=4, dim_head=128), B=2, N=1024, lens=[1024, 800], seed=40)
+    whole_model(pkg, dict(dim=512, depth=8, heads=4, dim_head=128), B=2, N=1024, lens=[1024, 800], seed=40)
 
 
 def test_e2tts_mixed_geometry_vs_oracle(pkg):
     """audio 8 x 64, text 2 x 128: two rotary tables, two qkv packings"""
     text = dict(text_heads=2, text_dim_head=128)
     with headdim_oracle(dict(heads=8, dim_head=64, **text)):
-        _whole_model(pkg, dict(dim=512, depth=2, heads=8, dim_head=64), B=2, N=224, lens=[224, 170], seed=41, model_kw=text)
+        whole_model(pkg, dict(dim=512, depth=2, heads=8, dim_head=64), B=2, N=224, lens=[224, 170], seed=41, model_kw=text)
 
 
 def test_e2tts_plain_residual_unclamped_d128_vs_oracle(pkg):
     """dim_head 128 with num_residual_streams=1 and attn_kwargs=dict() (no clamp, no head gate), at cfg2's shape like the 64-wide
     tests of these switches"""
     with plain_residual_oracle(), variant_oracle(dict()):
-        _whole_model(pkg, dict(dim=512, depth=8, heads=4, dim_head=128, num_residual_streams=1), B=2, N=1024, lens=[1024, 800], seed=40,
+        whole_model(pkg, dict(dim=512, depth=8, heads=4, dim_head=128, num_residual_streams=1), B=2, N=1024, lens=[1024, 800], seed=40,
                      model_kw=dict(attn_kwargs=dict()))
-
-
-def _small(pkg, seed, tkw, cls='E2TTS'):
-    torch.manual_seed(seed)
-    random.seed(seed)
-    t = dict(dropout=0., max_seq_len=256, **tkw)
-    model = pkg.E2TTS(transformer=t, use_vocos=False) if cls == 'E2TTS' else pkg.DurationPredictor(transformer=t)
-    sd = O.randomize_zero_init({k: v.clone() for k, v in model.state_dict().items()}, seed=seed + 1)
-    model.load_state_dict(sd)
-    return model.to(dev()), sd
 
 
 SMALL = dict(dim=128, depth=2, heads=1, dim_head=128, text_heads=2, text_dim_head=64)
 
 
 def test_sample_32_steps_d128_vs_oracle(pkg):
-    model, sd = _small(pkg, 90, SMALL)
+    model, sd = small_model(pkg, 90, **SMALL)
     torch.manual_seed(91)
     cond = torch.randn(2, 24, 100)
     text = ['Hello', 'Goodbye']
@@ -503,7 +328,7 @@ def test_sample_32_steps_d128_vs_oracle(pkg):
 
 
 def test_duration_predictor_d128_vs_oracle(pkg):
-    model, sd = _small(pkg, 92, SMALL, cls='DurationPredictor')
+    model, sd = small_model(pkg, 92, 'DurationPredictor', **SMALL)
     model.train()
     mel = torch.randn(3, 72, 100)
     lens = torch.tensor([72, 50, 31])
@@ -527,7 +352,7 @@ def test_duration_predictor_d128_vs_oracle(pkg):
 
 def test_graphed_step_matches_eager_d128(pkg):
     """GraphedTrainStep replays the eager step's gradients at head dim 128 (audio) / 64 (text, 2 heads)"""
-    model, _ = _small(pkg, 93, SMALL)
+    model, _ = small_model(pkg, 93, **SMALL)
     model.train()
     model.cond_drop_prob = 0.0
     B, N = 2, 96

@@ -4,15 +4,9 @@ Each entry point runs on the GPU and is compared, element by element, with a flo
 on the host from the exact bf16 / fp32 tensors the kernel received (backward references: float64 autograd of that expression).
 Where the oracle (oracle/e2tts_oracle.py) has the leaf, the reference is built on it.
 
-Every bound belongs to one of three classes; the helpers below carry the derivations.
-  E  bit-identical to the torch expression (copies, casts, packing, gathers: __float2bfloat16 and Tensor.to(torch.bfloat16) both
-     round to nearest even).
-  F  fp32 outputs: a sum of n terms is within gamma(n) * sum|terms| of the exact sum for ANY order of the additions (so for warp
-     shuffles and atomics too), plus the documented error of the fp32 library functions and intrinsics the kernel calls (CUDA C++
-     Programming Guide, appendix "Mathematical Functions": expf, sinf/cosf/sincosf, erff 2 ulp, log1pf 1 ulp, powf 4 ulp,
-     __expf 2 + floor(1.173 |x|) ulp; correctly rounded + - * / and sqrtf).
-  B  bf16 outputs: one round-to-nearest of an fp32 value within `atol` of the exact one (check_b).
-Where a case exists to reach a code path behind a size threshold, the test asserts that it is on the intended side.
+Every bound is E (bit-identical), F (fp32) or B (one bf16 rounding of an F value), the classes of tests/kernel_checks.py; the helpers
+below carry the derivations. Where a case exists to reach a code path behind a size threshold, the test asserts that it is on the
+intended side.
 """
 import math
 
@@ -21,98 +15,15 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from kernel_checks import BF16, F32, F64, U, U16, bf16_ulp, check_b, check_e, check_f, check_zero, dev, gamma, gen, pkg, sig_err
 from oracle import e2tts_oracle as O
 
 pytestmark = pytest.mark.gpu
-
-F64, BF16, F32 = torch.float64, torch.bfloat16, torch.float32
-U = 2.0 ** -24      # fp32 unit roundoff (24-bit significand, round to nearest)
-U16 = 2.0 ** -8     # bf16 unit roundoff (8-bit significand)
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
-def gen(seed):
-    return torch.Generator().manual_seed(seed)
 
 
 def bfr(t):
     """round to bf16 (host copy): the exact values a bf16 kernel input holds"""
     return t.to(BF16)
-
-
-# ---------------------------------------------------------------------------------------------------------------------- bounds
-def gamma(n):
-    """Higham's gamma_n = n u / (1 - n u) (Accuracy and Stability of Numerical Algorithms, 2nd ed., eqs. (3.4), (4.4)): a sum of
-    n + 1 terms, or an inner product of n terms, evaluated in fp32 in any order is within gamma_n * sum|terms| of the exact value."""
-    return n * U / (1 - n * U)
-
-
-def sig_err(a):
-    """|sigmoidf_(fl(x + b)) - sigmoid(x + b)| for the kernels' 1 / (1 + __expf(-a)):  the fp32 add of logit and bias rounds
-    (<= u|a|, sigmoid' <= 1/4); __expf(-a) is within 2 + floor(1.173|a|) ulp, i.e. 2(2 + 1.173|a|) u relative, which moves
-    1 / (1 + e) by sigma (1 - sigma) times that (<= 1/4 of it); 1 + e and the division round once each (<= 2u sigma <= 2u)."""
-    a = a.abs()
-    return U * (a / 4 + (2 + 1.173 * a) / 2 + 2)
-
-
-def _report(name, got, ref, bound):
-    over = (got - ref).abs() - bound
-    over = torch.where(torch.isnan(over), torch.full_like(over, math.inf), over)
-    i = int(torch.argmax(over))
-    idx = tuple(int(j) for j in np.unravel_index(i, tuple(ref.shape))) if ref.dim() else ()
-    return (f'{name}: |got - ref| exceeds the bound at {idx}: got {got.flatten()[i].item():.9g}, ref {ref.flatten()[i].item():.9g}, '
-            f'bound {bound.flatten()[i].item():.3g}; {int((over > 0).sum())} of {ref.numel()} elements')
-
-
-def check_f(name, got, ref, bound):
-    """element-wise |got - ref| <= bound (F: the caller derives the bound; NaN never passes)"""
-    ref = ref.detach().to(F64).cpu()
-    got = got.detach().to(F64).cpu().reshape(ref.shape)
-    bound = torch.as_tensor(bound, dtype=F64).cpu().expand_as(ref)
-    ok = (got - ref).abs() <= bound
-    assert bool(ok.all()), _report(name, got, ref, bound)
-
-
-def check_b(name, got, ref, atol):
-    """B: got = bf16(v) with v an fp32 value, |v - ref| <= atol. Round to nearest with an 8-bit significand moves v by at most
-    2^-8 |v|, so |got - ref| <= 2^-8 |v| + atol <= 2^-8 |ref| + (1 + 2^-8) atol."""
-    assert got.dtype == BF16, got.dtype
-    ref = ref.detach().to(F64).cpu()
-    check_f(name, got, ref, U16 * ref.abs() + (1 + U16) * torch.as_tensor(atol, dtype=F64).cpu())
-
-
-def check_e(name, got, want):
-    """E: bit-identical, compared as integers (so +0 and -0 differ)"""
-    got, want = got.detach().cpu().contiguous(), want.detach().cpu().contiguous()
-    assert got.dtype == want.dtype and got.shape == want.shape, (name, got.dtype, want.dtype, got.shape, want.shape)
-    it = {BF16: torch.int16, F32: torch.int32}[got.dtype]
-    bad = got.view(it) != want.view(it)
-    if bool(bad.any()):
-        i = int(bad.flatten().nonzero()[0])
-        idx = tuple(int(j) for j in np.unravel_index(i, tuple(got.shape)))
-        raise AssertionError(f'{name}: {int(bad.sum())} of {bad.numel()} elements differ, first at {idx}: '
-                             f'got {got.flatten()[i].item()!r}, want {want.flatten()[i].item()!r}')
-
-
-def check_zero(name, got):
-    check_e(name, got, torch.zeros_like(got.cpu()))
-
-
-def bf16_ulp(x):
-    """spacing of bf16 numbers at |x| (8-bit significand; subnormal spacing 2^-133 below 2^-126)"""
-    e = torch.floor(torch.log2(x.abs().clamp(min=2.0 ** -126)))
-    return torch.pow(2.0, e - 7)
 
 
 # ---------------------------------------------------------------------------------------------------------------------- small linear

@@ -6,21 +6,10 @@ import pytest
 import torch
 
 from conftest import rel_l2
+from kernel_checks import dev, pkg
 from oracle import optim_oracle as OO
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
 
 
 SHAPES = [(5,), (3, 7), (), (40000,), (16384,), (129, 515), (1,), (64, 64)]

@@ -1,7 +1,7 @@
 """Element-wise float64 bounds for the optimiser-step kernels of csrc/optim.cu: b200_flat_gather, b200_sumsq, b200_adopt_step and
 b200_flat_scatter, and FusedAdoptEMA / GradSync around them.
 
-Method of tests/test_gpu_attention_hyper_kernels.py: each entry point is called through the C ABI (lib.call / lib.make_args) over
+Method of tests/kernel_checks.py: each entry point is called through the C ABI (lib.call / lib.make_args) over
 chunk tables built by optim.FlatLayout, with NaN-prefilled outputs and a sentinel in the flat buffers' padding slots (parameter
 offsets are rounded up to 4 elements; no kernel may write those slots). References are computed in float64 (torch's float64 ops,
 on the device for the 64 M-element layouts) from the exact fp32 inputs of the same call. Every bound is E (bit for bit) or F:
@@ -47,11 +47,11 @@ import pytest
 import torch
 
 from oracle import optim_oracle as OO
-from test_gpu_leaf_kernels import U, check_e as check_e_fp, gamma
+from kernel_checks import F32, F64, U, Rv, _rnd, check_e, dev, gamma, mul, pkg, sms, stream
 
 pytestmark = pytest.mark.gpu
 
-F64, F32, I32 = torch.float64, torch.float32, torch.int32
+I32 = torch.int32
 CHUNK = 16384                         # optim.CHUNK: elements per chunk-table entry
 SUMSQ_MAX_GRID = 4096                 # optim.cu kSumsqMaxGrid
 SENTINEL = -1234.5                    # padding slots
@@ -59,35 +59,6 @@ EDGE_SHAPES = [(1,), (3,), (4,), (5,), (16383,), (16384,), (16385,), (3 * CHUNK 
 EDGE_W_SHIFT = [0, 1, 0, 2, 3, 0, 1, 3, 2]     # storage offset (elements) of each parameter in its buffer: 1, 2, 3 -> misaligned w
 EDGE_G_SHIFT = [1, 0, 3, 0, 2, 1, 0, 0, 3]     # the same for the gradients (flat_gather's scalar path)
 TEXT = re.compile(r'(text|^transformer\.(layers|hyper_conns)\.\d+\.1\.)')   # parameters without a gradient when the text is dropped
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
-def sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def check_e(name, got, want):
-    """bit for bit: fp32 through test_gpu_leaf_kernels.check_e, int32 (chunk_state) directly"""
-    if got.dtype != I32:
-        return check_e_fp(name, got, want)
-    got, want = got.cpu(), want.cpu()
-    bad = got != want
-    assert not bool(bad.any()), f'{name}: {int(bad.sum())} of {bad.numel()} differ, first at {int(bad.nonzero()[0, 0])}: got {got[bad][0]}, want {want[bad][0]}'
 
 
 def gamma64(n):
@@ -211,25 +182,6 @@ def fcheck_e(name, sl, got, want, mask):
 
 
 # ------------------------------------------------------------------------------------------------------------- running bounds
-class Rv:
-    """exact float64 value v of an fp32 quantity of the kernel, and a bound e on |kernel value - v|"""
-
-    def __init__(self, v, e=0.0):
-        self.v = v
-        self.e = e + torch.zeros_like(v)
-
-    def mag(self):
-        return self.v.abs() + self.e
-
-
-def _rnd(v, p, n=1):
-    return Rv(v, p + gamma(n) * (v.abs() + p))
-
-
-def mul(a, b, n=1):
-    return _rnd(a.v * b.v, a.mag() * b.e + a.e * b.v.abs(), n)
-
-
 def sub(a, b, n=1):
     return _rnd(a.v - b.v, a.e + b.e, n)
 

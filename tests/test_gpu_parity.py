@@ -13,6 +13,8 @@ import torch
 import torch.nn.functional as F
 
 from conftest import GOLDEN, rel_l2
+from kernel_checks import dev, pkg
+from model_checks import cos
 from oracle import e2tts_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -20,25 +22,8 @@ pytestmark = pytest.mark.gpu
 LEAF_TOL = 2e-2
 
 
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
 def bf(t):
     return t.to(torch.bfloat16).contiguous()
-
-
-def cos(a, b):
-    a, b = a.double().flatten(), b.double().flatten()
-    return float((a @ b) / (a.norm() * b.norm() + 1e-30))
 
 
 def check(name, got, want, tol=LEAF_TOL):

@@ -3,43 +3,21 @@ tiles, hyper-connection kernels at D = 512 / 1024, wgmma attention at N' = 1056 
 a d1024 / 16-head model — against the fp32 oracle (oracle/e2tts_oracle.py) computed on the box's CPU inside the test, never against
 a sibling kernel. All calls go through the C ABI. Tolerances as in test_gpu_parity.py (bf16 tensor-core path vs fp32 oracle).
 """
-import math
-import random
-
 import pytest
 import torch
 import torch.nn.functional as F
 
+from attn_ref import dropout_keep
 from conftest import rel_l2
+from kernel_checks import dev, pkg
+from model_checks import check, cos, small_model, whole_model
 from oracle import e2tts_oracle as O
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
 def bf(t):
     return t.to(torch.bfloat16).contiguous()
-
-
-def cos(a, b):
-    a, b = a.double().flatten(), b.double().flatten()
-    return float((a @ b) / (a.norm() * b.norm() + 1e-30))
-
-
-def check(name, got, want, tol):
-    e = rel_l2(got.float().cpu(), want.float().cpu())
-    assert e < tol, f'{name}: rel-L2 {e:.4g} >= {tol}'
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -181,24 +159,6 @@ def test_hyper_depth_width_fused(pkg, D):
 # (d) wgmma attention core against an fp32 softmax written here (x-transformers Attend as the reference configures it, SURVEY A.4
 #     steps 4-5: scale, tanh soft clamp 50, key-padding mask, fp32 softmax, dropout, per-head gate), at the benchmark's sequence length
 #     and at short, unmasked and dropout cases
-def _mul32(x, c):
-    """(x * c) mod 2^32 for int64 tensors x < 2^32 and a 32-bit constant c, without overflowing int64."""
-    return (x * (c & 0xFFFF) + ((x * (c >> 16)) & 0xFFFF) * 65536) & 0xFFFFFFFF
-
-
-def _dropout_keep(seed, B, H, Np, p):
-    """The kernels' attention-dropout mask (ptx.cuh: seed_mix32, drop_words) for element ((b*H + h)*Np + i)*stride + j, as bool
-    [B, H, Np, Np]: keep iff the 32-bit word of the element >= thresh16 << 16, thresh16 = int(p * 65536)."""
-    stride = (Np + 1) & ~1
-    seedmix = (seed & 0xFFFFFFFF) ^ (((seed >> 32) * 0x85EBCA77) & 0xFFFFFFFF)
-    row = torch.arange(B * H * Np, dtype=torch.int64).view(B, H, Np, 1)
-    idx = row * stride + torch.arange(Np, dtype=torch.int64)
-    x = (_mul32((idx >> 1) & 0xFFFFFFFF, 0x9E3779B1) + seedmix) & 0xFFFFFFFF
-    x = x ^ (x >> 15)
-    word = torch.where((idx & 1) == 1, _mul32(x, 0xC2B2AE35), _mul32(x, 0x85EBCA6B))
-    return word >= (int(p * 65536) << 16)
-
-
 def _attn_core_ref(q, k, v, gate, mask, clamp=50.0, dropout=0.0, seed=0):
     """-> og [B*Np, H*dh] (gated, head-merged), o [B, H, Np, dh], lse [B, H, Np] (log-sum-exp of the clamped, masked logits). With
     dropout the kept probabilities are scaled by 65536 / (65536 - thresh16), the kernels' exact 1 / (1 - p)."""
@@ -210,7 +170,7 @@ def _attn_core_ref(q, k, v, gate, mask, clamp=50.0, dropout=0.0, seed=0):
     attn = torch.softmax(sim, dim=-1)
     if dropout > 0:
         thresh16 = int(dropout * 65536)
-        attn = attn * _dropout_keep(seed, B, H, Np, dropout) * (65536 / (65536 - thresh16))
+        attn = attn * dropout_keep(seed, B, H, Np, dropout) * (65536 / (65536 - thresh16))
     o = torch.einsum('bhij,bhjd->bhid', attn, v)
     og = o * gate.view(B, Np, H).permute(0, 2, 1)[..., None]
     return og.permute(0, 2, 1, 3).reshape(B * Np, H * dh), o, torch.logsumexp(sim, dim=-1)
@@ -253,83 +213,29 @@ def test_attention_core_vs_fp32_softmax(pkg, Np, H, big_logits, masked, dropout)
 
 # ----------------------------------------------------------------------------------------------------------------------
 # (a), (e) whole model at the BASELINE widths against the oracle run on the host CPU
-def _whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, model_kw=None, e2tts_kw=None):
-    torch.manual_seed(seed)
-    random.seed(seed)   # the hyper-connections draw their initial stream with python's randrange: the same case on every run
-    model = pkg.E2TTS(transformer=dict(dropout=0., max_seq_len=N, **tkw, **(model_kw or {})), use_vocos=False, **(e2tts_kw or {}))
-    # dyn_scale 0.05 (5x the reference's init of the hyper-connections' dynamic scales): with the 0.5 of the 2-layer fixtures a depth-8
-    # stack amplifies bf16 rounding of the residual streams ~10x — the fp32 oracle with its OWN stage outputs rounded to bf16
-    # (O.STAGE_ROUND) then moves its prediction by 12.6 %, exactly what the kernels showed. The probe below
-    # keeps this test honest: the case must be well conditioned for a bf16 path before the kernels are held to 3e-2.
-    sd = O.randomize_zero_init({k: v.clone() for k, v in model.state_dict().items()}, seed=seed + 1, dyn_scale=0.05)
-    model.load_state_dict(sd)
-    model.to(dev()).train()
-    mel = torch.randn(B, N, 100)
-    text = ['Hello', 'Goodbye'][:B]
-    x0, times = torch.randn(B, N, 100), torch.rand(B)
-    lens_t = torch.tensor(lens)
-    span = torch.zeros(B, N, dtype=torch.bool)
-    for b in range(B):
-        span[b, lens[b] // 8: lens[b] - lens[b] // 10] = True
-    with pkg.inject_randomness(x0=x0.to(dev()), times=times.to(dev()), span_mask=span.to(dev()), drop_text_cond=False):
-        out = model(mel.to(dev()), text=text, lens=lens_t.to(dev()))
-    out.loss.backward()
-    torch.cuda.synchronize()
-    # oracle on the host (fp32, all cores)
-    osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    ref = O.e2tts_forward(osd, O.TransformerCfg(**tkw), mel, O.list_str_to_tensor(text), x0=x0, times=times, span_mask=span, lens=lens_t)
-    ref['loss'].backward()
-    O.STAGE_ROUND = O.bf16_ste
-    try:
-        with torch.no_grad():
-            probe = O.e2tts_forward(sd, O.TransformerCfg(**tkw), mel, O.list_str_to_tensor(text), x0=x0, times=times, span_mask=span, lens=lens_t)
-    finally:
-        O.STAGE_ROUND = None
-    e_probe = rel_l2(probe['pred'], ref['pred'].detach())
-    assert e_probe < 1.5e-2, f'test case is ill-conditioned for bf16 activations (oracle vs bf16-stage oracle: {e_probe:.3g})'
-    loss, rloss = float(out.loss), float(ref['loss'])
-    assert abs(loss - rloss) <= 1e-2 * abs(rloss), (loss, rloss)
-    check('pred', out.pred_flow, ref['pred'].detach(), tol_pred)
-    print(f'pred rel-L2 {rel_l2(out.pred_flow.float().cpu(), ref["pred"].detach()):.4g} (bf16-stage oracle probe {e_probe:.4g})')
-    total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())
-    worst = (1.0, None)
-    for k, p in model.named_parameters():
-        gr = osd[k].grad
-        if gr is None:
-            assert p.grad is None or float(p.grad.abs().max()) == 0.0, f'{k} should be unused'
-            continue
-        assert p.grad is not None, k
-        if float(gr.norm()) < 1e-4 * total:     # negligible next to the whole gradient: direction is rounding noise in any bf16 path
-            continue
-        cs_ = cos(p.grad.cpu(), gr)
-        worst = min(worst, (cs_, k))
-        assert cs_ >= 0.99, (k, cs_)
-    print(f'whole model {tkw}: loss {loss:.5f} (oracle {rloss:.5f}), worst grad cosine {worst}')
-
-
 def test_e2tts_cfg2_shape_vs_oracle(pkg):
     """BASELINE cfg2's model (d512, depth 8, 8 heads) at its sequence length (N = 1024, N' = 1056), B = 2 with a ragged batch:
     T = 2112 rows -> the 128 x 256 GEMM tile, hc_width_*<2,true>, 9-tile wgmma attention — what bench.py times."""
-    _whole_model(pkg, dict(dim=512, depth=8, heads=8), B=2, N=1024, lens=[1024, 800], seed=40)
+    whole_model(pkg, dict(dim=512, depth=8, heads=8), B=2, N=1024, lens=[1024, 800], seed=40)
 
 
 def test_e2tts_cfg3_kernels_vs_oracle(pkg):
     """cfg3 / cfg5's width (d1024, 16 heads, dim_text 512) at N = 2048 (N' = 2080): hc_width_*<4,false>, 16-head qkv packing,
     17-tile attention; depth 2 keeps the host oracle within seconds."""
-    _whole_model(pkg, dict(dim=1024, depth=2, heads=16), B=1, N=2048, lens=[1900], seed=50)
+    whole_model(pkg, dict(dim=1024, depth=2, heads=16), B=1, N=2048, lens=[1900], seed=50)
 
 
 def test_e2tts_attn_fourier_embed_input_vs_oracle(pkg):
     """SURVEY §8f row 4, first variant: Transformer(attn_fourier_embed_input=True) (e2_tts.py:545-546; LinearFourierEmbed :368-386 on the
     attention input, :909) — wgmma GEMM + b200_fourier_feat_* against the oracle, which tests/test_oracle_vs_reference.py pins to the
     reference's own code with the switch on. Loss, prediction and every parameter gradient incl. `layers.{i}.0.4.linear.weight`."""
-    _whole_model(pkg, dict(dim=256, depth=2, heads=4), B=2, N=224, lens=[224, 170], seed=60, model_kw=dict(attn_fourier_embed_input=True))
+    whole_model(pkg, dict(dim=256, depth=2, heads=4), B=2, N=224, lens=[224, 170], seed=60, model_kw=dict(attn_fourier_embed_input=True))
 
 
 def test_e2tts_concat_cond_vs_oracle(pkg):
     """SURVEY §8f row 4, third variant: E2TTS(concat_cond=True) (e2_tts.py:1134, :1200-1201, :1263-1267): the stem GEMM reads
     cat(cond, x) (b200_stem_prepare concat layout) against ONE packed Linear(2C -> dim); oracle pinned to the reference's own code."""
-    _whole_model(pkg, dict(dim=256, depth=2, heads=4), B=2, N=224, lens=[224, 190], seed=80, e2tts_kw=dict(concat_cond=True))
+    whole_model(pkg, dict(dim=256, depth=2, heads=4), B=2, N=224, lens=[224, 190], seed=80, e2tts_kw=dict(concat_cond=True))
 
 
 def test_e2tts_interpolated_text_vs_oracle(pkg):
@@ -337,23 +243,17 @@ def test_e2tts_interpolated_text_vs_oracle(pkg):
     b200_interp_text_* + the abs-pos Linear as a wgmma GEMM with bias / residual / row-mask epilogue, against the oracle (pinned to
     the reference's own code in tests/test_oracle_vs_reference.py): ragged text and audio lengths, gradients of the embedding table
     and both abs_pos_mlp linears included."""
-    _whole_model(pkg, dict(dim=256, depth=2, heads=4), B=2, N=224, lens=[224, 150], seed=70, e2tts_kw=dict(interpolated_text=True))
+    whole_model(pkg, dict(dim=256, depth=2, heads=4), B=2, N=224, lens=[224, 150], seed=70, e2tts_kw=dict(interpolated_text=True))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
 # (f) sampling: euler, 32 steps, autoguidance null model — against the oracle's fixed-grid ODE on the host
-def _small_model(pkg, seed, depth=2):
-    torch.manual_seed(seed)
-    random.seed(seed)
-    tkw = dict(dim=128, depth=depth, heads=2)
-    model = pkg.E2TTS(transformer=dict(dropout=0., max_seq_len=256, **tkw), use_vocos=False)
-    sd = O.randomize_zero_init({k: v.clone() for k, v in model.state_dict().items()}, seed=seed + 1)
-    model.load_state_dict(sd)
-    return model.to(dev()), sd, O.TransformerCfg(**tkw)
+SMALL = dict(dim=128, depth=2, heads=2)
 
 
 def test_sample_32_steps_vs_oracle(pkg):
-    model, sd, cfg = _small_model(pkg, 60)
+    model, sd = small_model(pkg, 60, **SMALL)
+    cfg = O.TransformerCfg(**SMALL)
     torch.manual_seed(61)
     cond = torch.randn(2, 24, 100)
     text = ['Hello', 'Goodbye']
@@ -368,8 +268,9 @@ def test_sample_32_steps_vs_oracle(pkg):
 def test_sample_euler_and_null_model(pkg):
     """odeint method 'euler' (e2_tts.py:1122-1126 odeint_kwargs) and `cfg_null_model` autoguidance (:1318-1321: the null prediction
     comes from a second, weaker model WITH text instead of this model without text)."""
-    model, sd, cfg = _small_model(pkg, 70)
-    weak, wsd, _ = _small_model(pkg, 80)
+    model, sd = small_model(pkg, 70, **SMALL)
+    cfg = O.TransformerCfg(**SMALL)
+    weak, wsd = small_model(pkg, 80, **SMALL)
     model.odeint_kwargs = dict(method='euler')
     torch.manual_seed(71)
     cond = torch.randn(2, 20, 100)
@@ -401,8 +302,9 @@ def test_sample_euler_and_null_model(pkg):
 # SURVEY §8f row 2: velocity-consistency loss (e2_tts.py:1556-1576; trainer hook trainer.py:259-268) — a second, no-grad forward of the
 # EMA model at t + delta through the same kernels, fused into the loss head
 def test_velocity_consistency_loss_vs_oracle(pkg):
-    model, sd, cfg = _small_model(pkg, 90)
-    ema, esd, _ = _small_model(pkg, 91)
+    model, sd = small_model(pkg, 90, **SMALL)
+    cfg = O.TransformerCfg(**SMALL)
+    ema, esd = small_model(pkg, 91, **SMALL)
     ema.eval()
     model.train()
     model.velocity_consistency_weight = 0.7

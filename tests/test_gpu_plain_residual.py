@@ -1,6 +1,6 @@
 """GPU: Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True).
 
-Kernels, element-wise against float64 with NaN-filled outputs (the method of test_gpu_leaf_kernels.py / test_gpu_conv_melspec_kernels.py):
+Kernels, element-wise against float64 with NaN-filled outputs (the method of kernel_checks.py, the depthwise reference of hyper_conv_ref.py):
   * the branch-norm mode of b200_final_norm_* (RMSNorm(g) and per-batch AdaptiveRMSNorm gains, the residual gradient d_res, zero rows);
   * the residual mode of b200_dwconv_* (y = x + the masked conv, dx = dy + the conv's dx).
 Bit-exact properties: masked rows of the residual convolution keep x (and pass dy); its pre-activation equals the plain launch's;
@@ -14,28 +14,11 @@ import torch
 from conftest import rel_l2
 from oracle import e2tts_oracle as O
 from residual_variants import plain_residual_oracle
-from test_gpu_conv_melspec_kernels import CV_TN, _model_mask, cdiv, dw_mask, dw_ref, h64, nans, stream
-from test_gpu_leaf_kernels import U, U16, BF16, F32, check_b, check_e, check_f, gamma
-from test_gpu_parity_full import _whole_model
+from hyper_conv_ref import CV_TN, cdiv, dw_mask, dw_ref, model_mask
+from kernel_checks import BF16, F64, U, U16, check_b, check_e, check_f, dev, gamma, gen, h64, nans, pkg, stream
+from model_checks import small_model, whole_model
 
 pytestmark = pytest.mark.gpu
-F64 = torch.float64
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
-
-
-def dev():
-    return torch.device('cuda:0')
-
-
-def gen(seed):
-    return torch.Generator().manual_seed(seed)
 
 
 # ================================================================================================================ branch norm
@@ -190,7 +173,7 @@ def test_residual_dwconv_kernels(pkg, name, B, Np, D, masks, subset):
     seed = sum(map(ord, name))
     g = gen(seed)
     if masks == 'model':
-        masks = _model_mask(B, Np, gen(seed + 1))
+        masks = model_mask(B, Np, gen(seed + 1))
     m = torch.stack([dw_mask(Np, s, g) for s in masks])
     x = torch.randn(B, Np, D, generator=g).to(BF16)
     w = torch.randn(D, ks, generator=g) / ks ** 0.5 + 0.1 * torch.arange(ks) / ks
@@ -309,24 +292,16 @@ def test_nodes_with_residual(pkg):
 # ================================================================================================================ model
 def test_e2tts_cfg2_shape_plain_residual_vs_oracle(pkg):
     """BASELINE cfg2's model (d512, depth 8, 8 heads, N = 1024, ragged B = 2) with num_residual_streams=1: conditioning probe < 1.5 %,
-    loss within 1e-2, prediction rel-L2 within 3e-2, every gradient cosine >= 0.99 (the bounds of tests/test_gpu_parity_full.py)"""
+    loss within 1e-2, prediction rel-L2 within 3e-2, every gradient cosine >= 0.99 (the bounds of tests/model_checks.py)"""
     with plain_residual_oracle():
-        _whole_model(pkg, dict(dim=512, depth=8, heads=8, num_residual_streams=1), B=2, N=1024, lens=[1024, 800], seed=40)
+        whole_model(pkg, dict(dim=512, depth=8, heads=8, num_residual_streams=1), B=2, N=1024, lens=[1024, 800], seed=40)
 
 
-def _small(pkg, seed, cls='E2TTS'):
-    import random
-    torch.manual_seed(seed)
-    random.seed(seed)
-    t = dict(dim=128, depth=2, heads=2, dropout=0., max_seq_len=256, num_residual_streams=1)
-    model = pkg.E2TTS(transformer=t, use_vocos=False) if cls == 'E2TTS' else pkg.DurationPredictor(transformer=t)
-    sd = O.randomize_zero_init({k: v.clone() for k, v in model.state_dict().items()}, seed=seed + 1)
-    model.load_state_dict(sd)
-    return model.to(dev()), sd
+SMALL = dict(dim=128, depth=2, heads=2, num_residual_streams=1)
 
 
 def test_sample_32_steps_plain_residual_vs_oracle(pkg):
-    model, sd = _small(pkg, 70)
+    model, sd = small_model(pkg, 70, **SMALL)
     torch.manual_seed(71)
     cond = torch.randn(2, 24, 100)
     text = ['Hello', 'Goodbye']
@@ -342,7 +317,7 @@ def test_sample_32_steps_plain_residual_vs_oracle(pkg):
 
 def test_graphed_step_matches_eager_and_launches_no_hyper_connection(pkg, monkeypatch):
     """GraphedTrainStep replays the eager step's gradients; neither launches a hyper-connection entry point"""
-    model, _ = _small(pkg, 3)
+    model, _ = small_model(pkg, 3, **SMALL)
     model.train()
     model.cond_drop_prob = 0.0
     B, N = 2, 96
@@ -378,7 +353,7 @@ def test_graphed_step_matches_eager_and_launches_no_hyper_connection(pkg, monkey
 
 def test_duration_predictor_plain_residual_vs_oracle(pkg):
     """DurationPredictor(num_residual_streams=1): loss within 1e-2 of the oracle, gradient cosines >= 0.99"""
-    model, sd = _small(pkg, 41, cls='DurationPredictor')
+    model, sd = small_model(pkg, 41, 'DurationPredictor', **SMALL)
     model.train()
     mel = torch.randn(3, 72, 100)
     lens = torch.tensor([72, 50, 31])

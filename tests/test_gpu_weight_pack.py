@@ -14,11 +14,11 @@ import pytest
 import torch
 
 from conftest import rel_l2
+from kernel_checks import U, dev, pkg
 from oracle import e2tts_oracle as O
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24      # fp32 unit roundoff
 B, N, C = 2, 96, 100
 STEPS = 3           # sample(): 2 midpoint steps = 4 function evaluations, each a text pass and a null pass
 TKW = dict(dim=128, depth=2, heads=2, dropout=0.0)
@@ -29,14 +29,6 @@ BUILD = {
     'duration': lambda pkg: pkg.DurationPredictor(transformer=dict(TKW)),
     'transformer': lambda pkg: pkg.Transformer(**TKW),
 }
-
-
-@pytest.fixture(scope='module')
-def pkg():
-    import e2_tts_pytorch_b200 as pkg
-    assert torch.cuda.is_available()
-    pkg.lib.load()
-    return pkg
 
 
 @pytest.fixture
@@ -63,10 +55,6 @@ def pack_log(pkg, monkeypatch):
     monkeypatch.setattr(ops, 'pack_weights', lambda *a: (log.append('pack'), pack_weights(*a))[1])
     monkeypatch.setattr(ops, 'axpy', lambda *a: (log.append('axpy'), axpy(*a))[1])
     return log
-
-
-def dev():
-    return torch.device('cuda:0')
 
 
 def build(pkg, kind, sd=None, seed=0):

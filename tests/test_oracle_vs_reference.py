@@ -7,33 +7,14 @@ import pytest
 import torch
 
 from oracle import e2tts_oracle as O
+from model_checks import check_grads, grad_sd
 from oracle import reference_cases as RC
-
-
-def _grad_sd(sd):
-    return {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-
-
-def _check_grads(sd, rec, rel=2e-4, floor=1e-7):
-    """Elementwise on the stored sample: |got - want| <= rel * max|want| + floor (the tolerance of a full comparison), plus max|g| and
-    the norm. A parameter the original left without a gradient must get none (or an all-zero one) from the oracle."""
-    for k, r in rec.items():
-        got = sd[k].grad
-        if r is None:
-            assert got is None or float(got.abs().max()) == 0.0, k
-            continue
-        assert got is not None, k
-        g = got.detach().double().flatten()
-        tol = rel * r['max'] + floor
-        assert float((g[RC.sample_index(g.numel())] - r['values'].double()).abs().max()) <= tol, k
-        assert abs(float(g.abs().max()) - r['max']) <= tol, k
-        assert abs(float(g.norm()) - r['norm']) <= 5 * rel * r['norm'] + floor, k
 
 
 def _forward_case(name):
     c = RC.FORWARD_CASES[name]
     g = RC.load('forward_' + name)
-    sd = _grad_sd(RC.state_dict('E2TTS', c['seed'], c['tkw'], **c['kw']))
+    sd = grad_sd(RC.state_dict('E2TTS', c['seed'], c['tkw'], **c['kw']))
     mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
     x0 = RC.randn(mel.shape, c['seed'] + 2000)
     lens_t = torch.tensor(c['lens']) if c['lens'] else None
@@ -44,7 +25,7 @@ def _forward_case(name):
     assert abs(float(o['loss'].detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
     assert RC.compact_rel_l2(o['pred'], g['pred']) < 1e-4
     assert abs(float(o['pred'].double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
-    _check_grads(sd, g['grads'])
+    check_grads(sd, g['grads'])
     return sd
 
 
@@ -113,7 +94,7 @@ def test_sample_vs_reference(steps, cfg_strength, duration):
 def test_duration_predictor_vs_reference():
     """DurationPredictor.forward (:1042-1113): random prefix mask, masked mean pool, softplus head, L1-on-frames loss."""
     g = RC.load('duration')
-    sd = _grad_sd(RC.state_dict('DurationPredictor', 41))
+    sd = grad_sd(RC.state_dict('DurationPredictor', 41))
     mel = RC.randn((3, 72, 100), 1041)
     torch.manual_seed(5)
     rand_frac = mel.new_zeros(3).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
@@ -121,7 +102,7 @@ def test_duration_predictor_vs_reference():
                              lens=torch.tensor([72, 50, 31]), rand_frac=rand_frac)
     assert abs(float(got) - g['loss']) <= 1e-4 * abs(g['loss'])
     got.backward()
-    _check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+    check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
 
 
 def test_mask_helpers_bit_exact_vs_reference():
@@ -154,7 +135,7 @@ def test_velocity_consistency_loss_vs_reference():
     gradients of the online model against the oracle's restatement."""
     g = RC.load('velocity_consistency')
     s = RC.VELOCITY_SEED
-    sd = _grad_sd(RC.state_dict('E2TTS', s, velocity_consistency_weight=0.7))
+    sd = grad_sd(RC.state_dict('E2TTS', s, velocity_consistency_weight=0.7))
     mel = RC.randn((2, 64, 100), 1000 + s)
     o = O.e2tts_forward(sd, O.TransformerCfg(**RC.KW), mel, O.list_str_to_tensor(['abc', 'some text']), lens=torch.tensor([64, 50]),
                         x0=RC.randn(mel.shape, 2000 + s), times=g['times'], span_mask=g['span_mask'], velocity_sd=RC.state_dict('E2TTS', s + 1),

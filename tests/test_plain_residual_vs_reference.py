@@ -5,10 +5,10 @@ C-ABI validation of the branch-norm and residual-convolution fields."""
 import pytest
 import torch
 
+from model_checks import check_grads, grad_sd
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
 from residual_variants import RESIDUAL1_CASES, RESIDUAL1_SAMPLE, plain_residual_oracle
-from test_oracle_vs_reference import _check_grads, _grad_sd
 
 import e2_tts_pytorch_b200 as pkg
 
@@ -22,7 +22,7 @@ def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
     c = RESIDUAL1_CASES[name]
     g = RC.load('residual1_' + name)
-    sd = _grad_sd(RC.state_dict(c['cls'], c['seed'], c['tkw']))
+    sd = grad_sd(RC.state_dict(c['cls'], c['seed'], c['tkw']))
     assert not any('.hyper_conns.' in k for k in sd)
     mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
     lens = torch.tensor(c['lens'])
@@ -41,9 +41,9 @@ def test_oracle_vs_reference(name):
     assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
     loss.backward()
     if c['cls'] == 'E2TTS':
-        _check_grads(sd, g['grads'])
+        check_grads(sd, g['grads'])
     else:
-        _check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+        check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
     if c.get('drop'):   # the text stream is skipped: its parameters get no gradient
         assert g['grads']['transformer.layers.0.1.2.to_q.weight'] is None
 
