@@ -75,6 +75,18 @@ def _rs(x):
     return x if STAGE_ROUND is None or x is None else STAGE_ROUND(x)
 
 
+# Dropout hook (test infrastructure): DROPOUT, when set, is called as DROPOUT(name, x) at the two places the reference drops and
+# returns the dropped tensor — the softmax probabilities of `attention` (name `<prefix>.attn_dropout`) and the GEGLU hidden of
+# `feedforward` (name `<prefix>.ff.1`); the names are the qualified names of the x-transformers nn.Dropout modules
+# (oracle/ref_leaves/x_transformers/x_transformers.py:53, :113). tests use it to give the oracle a known mask: the reference's
+# dropped by a seeded recipe, or the kernels' own hash masks. None (default) = no dropout, as the reference with dropout=0.
+DROPOUT = None
+
+
+def drop(name, x):
+    return x if DROPOUT is None else DROPOUT(name, x)
+
+
 # --------------------------------------------------------------------------------------------------
 # helpers (:113-124, :173-235)
 
@@ -145,7 +157,7 @@ def attention(sd, p, x, mask, freqs, value_residual, heads, dim_head, softclamp)
     sim = torch.tanh(sim / softclamp) * softclamp
     if mask is not None:
         sim = sim.masked_fill(~mask[:, None, None, :], -torch.finfo(sim.dtype).max)
-    attn = torch.softmax(sim.float(), dim=-1).to(sim.dtype)
+    attn = drop(p + '.attn_dropout', torch.softmax(sim.float(), dim=-1).to(sim.dtype))
     out = torch.einsum('bhij,bhjd->bhid', attn, v)
     gate = torch.sigmoid(x @ sd[p + '.to_v_head_gate.weight'].t() + sd[p + '.to_v_head_gate.bias'])
     out = out * gate.permute(0, 2, 1)[..., None]
@@ -155,10 +167,10 @@ def attention(sd, p, x, mask, freqs, value_residual, heads, dim_head, softclamp)
     return out, orig_v
 
 
-def feedforward(sd, p, x):  # A.2 GEGLU (exact erf GELU)
+def feedforward(sd, p, x):  # A.2 GEGLU (exact erf GELU), nn.Dropout between the GLU and the output Linear
     h = x @ sd[p + '.ff.0.proj.weight'].t() + sd[p + '.ff.0.proj.bias']
     u, g = h.chunk(2, dim=-1)
-    return (u * F.gelu(g)) @ sd[p + '.ff.2.weight'].t() + sd[p + '.ff.2.bias']
+    return drop(p + '.ff.1', u * F.gelu(g)) @ sd[p + '.ff.2.weight'].t() + sd[p + '.ff.2.bias']
 
 
 def depthwise_conv(sd, p, x, mask):  # :312-328

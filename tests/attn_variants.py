@@ -46,7 +46,7 @@ def attention(sd, p, x, mask, freqs, value_residual, heads, dim_head, softclamp)
         sim = torch.tanh(sim / softclamp) * softclamp
     if mask is not None:
         sim = sim.masked_fill(~mask[:, None, None, :], -torch.finfo(sim.dtype).max)
-    attn = torch.softmax(sim.float(), dim=-1).to(sim.dtype)
+    attn = O.drop(p + '.attn_dropout', torch.softmax(sim.float(), dim=-1).to(sim.dtype))
     out = torch.einsum('bhij,bhjd->bhid', attn, v)
     if p + '.to_v_head_gate.weight' in sd:
         gate = torch.sigmoid(x @ sd[p + '.to_v_head_gate.weight'].t() + sd[p + '.to_v_head_gate.bias'])

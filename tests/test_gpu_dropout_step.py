@@ -1,0 +1,293 @@
+"""Training steps with dropout on, against the oracle given the kernels' own masks.
+
+Every attention and feed-forward call of a step gets a seed from Transformer._run_layers (`next_seed()`), the text sub-blocks
+included, which run on the side stream; the kernels hash their masks from (seed + device seed word) mod 2^64. `SeedRecorder`
+(tests/dropout_ref.py) records which seed and whether a device word each call took, and `KernelMasks` rebuilds the masks on the host
+with the float64 restatements of the kernels' hashes, through the oracle's O.DROPOUT hook (pinned to the reference's own code by
+tests/test_dropout_vs_reference.py). A layer reusing another's seed, the text stream's masks keyed to the wrong row count, a graph
+replay drawing its masks from another word than the one it left behind, or a race between the two streams moves the prediction away
+from the oracle's; a negative control in every case gives the oracle the masks of seed + 1 and must miss the prediction tolerance by
+3x. Each case runs on both schedules: the text sub-blocks of layer i + 1 on the side stream (default) and all on one stream
+(modules.TWO_STREAM = False), which call next_seed() in different orders."""
+import random
+
+import pytest
+import torch
+
+from conftest import rel_l2
+from dropout_ref import KernelMasks, SeedRecorder, splitmix64, with_dropout
+from headdim_variants import cfg, headdim_oracle
+from kernel_checks import F64, dev, pkg  # noqa: F401  (pytest fixture)
+from model_checks import cos
+from oracle import e2tts_oracle as O
+
+pytestmark = pytest.mark.gpu
+
+TOL_PRED, TOL_LOSS, PROBE, COS = 3e-2, 1e-2, 1.5e-2, 0.99     # the criteria of model_checks.whole_model
+SMALL = dict(dim=128, depth=2, heads=2)
+# Dropout p of the small models (the kernels' 16-bit threshold drops with probability exactly p at 0.25 and 0.5). With the AdaLNZero
+# gates open (bias 0, `build`) the masks of seed + 1 move the small E2TTS models' prediction by 7-8 % at p = 0.25 (the oracle against
+# itself), short of 3x the 3e-2 tolerance, and by 13-15 % at 0.5. The DurationPredictor's final-normed transformer output separates
+# at 0.25 (~15 %).
+P_SMALL = 0.5
+P_CFG2 = 0.75
+CASES = {   # transformer kwargs, batch, frames, lens, seed, dropout p; f64=False: the oracle in fp32 (float64 elsewhere)
+    'depth4_lens': dict(cls='E2TTS', tkw=dict(dim=128, depth=4, heads=2), B=2, N=96, lens=[96, 61], seed=201, p=P_SMALL),
+    'residual1': dict(cls='E2TTS', tkw=dict(SMALL, num_residual_streams=1), B=2, N=96, lens=[96, 70], seed=202, p=P_SMALL),
+    'a128_t64': dict(cls='E2TTS', tkw=dict(dim=256, depth=2, heads=2, dim_head=128, text_heads=2, text_dim_head=64), B=2, N=96,
+                     lens=[96, 53], seed=203, p=P_SMALL),
+    'gate_unclamped': dict(cls='E2TTS', tkw=dict(SMALL, attn_kwargs=dict(gate_value_heads=True)), B=2, N=96, lens=[96, 77], seed=204,
+                           p=P_SMALL),
+    # O.duration_forward's mse_loss against lens.float() does not take a float64 prediction
+    'duration': dict(cls='DurationPredictor', tkw=SMALL, B=3, N=72, lens=[72, 50, 31], seed=205, p=0.25, f64=False),
+    # cfg2's model with test_gpu_parity_full.test_e2tts_cfg2_shape_vs_oracle's weights (AdaLNZero gates as initialised: with them
+    # open, the gradient of the scalar hyper_conns.0.1.0.dynamic_alpha_scale is a near-cancelling sum whose sign the kernels and the
+    # oracle do not share). At the benchmarked dropout 0.1 the masks of seed + 1 move the prediction by only ~3.3 %: this case holds
+    # the kernels to the criteria but its negative control only has to miss the tolerance (neg=1); at 0.75 it separates by 3x.
+    'cfg2_p0.1': dict(cls='E2TTS', tkw=dict(dim=512, depth=8, heads=8), B=2, N=1024, lens=[1024, 800], seed=40, p=0.1, f64=False, neg=1,
+                      open_gates=False),
+    'cfg2': dict(cls='E2TTS', tkw=dict(dim=512, depth=8, heads=8), B=2, N=1024, lens=[1024, 800], seed=40, p=P_CFG2, f64=False,
+                 open_gates=False),
+}
+SCHEDULES = ['two_stream', 'serial']
+TEXT = ['Hello', 'Goodbye', 'x']
+
+
+@pytest.fixture(params=SCHEDULES)
+def schedule(request, pkg, monkeypatch):
+    if request.param == 'serial':
+        monkeypatch.setattr(pkg.modules, 'TWO_STREAM', False)
+    return request.param
+
+
+def build(pkg, c, p):
+    """the case's model with dropout p on the GPU and its state dict: weights as model_checks.whole_model seeds them, but (unless
+    the case says open_gates=False) the AdaLNZero gates open at sigmoid(0) = 1/2 instead of the reference's initial sigmoid(-2)
+    (to_gamma.bias 0), so that what the attention and feed-forward branches add, dropout included, weighs 4x more in the prediction"""
+    torch.manual_seed(c['seed'])
+    random.seed(c['seed'])
+    t = dict(dropout=p, max_seq_len=max(c['N'], 128), **c['tkw'])
+    model = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
+    sd = O.randomize_zero_init({k: v.clone() for k, v in model.state_dict().items()}, seed=c['seed'] + 1, dyn_scale=0.05)
+    for k in sd:
+        if k.endswith('to_gamma.bias') and c.get('open_gates', True):
+            sd[k].zero_()
+    model.load_state_dict(sd)
+    return model.to(dev()).train(), sd
+
+
+def inputs(c):
+    g = torch.Generator().manual_seed(c['seed'] + 7)
+    B, N = c['B'], c['N']
+    span = torch.zeros(B, N, dtype=torch.bool)
+    for b, n in enumerate(c['lens']):
+        span[b, n // 8: n - n // 10] = True
+    x = dict(mel=torch.randn(B, N, 100, generator=g), x0=torch.randn(B, N, 100, generator=g), times=torch.rand(B, generator=g),
+             span=span, lens=torch.tensor(c['lens']), rand_frac=torch.tensor([0.9, 0.6, 0.3][:B]), text=TEXT[:B])
+    # the injected draws on the device, held as long as the inputs: a captured graph reads them on every replay
+    x['dev'] = {k: x[k].to(dev()) for k in ('x0', 'times', 'span', 'rand_frac')}
+    return x
+
+
+def randomness(pkg, c, x):
+    d = x['dev']
+    if c['cls'] == 'E2TTS':
+        return pkg.inject_randomness(x0=d['x0'], times=d['times'], span_mask=d['span'], drop_text_cond=False)
+    return pkg.inject_randomness(duration_rand_frac=d['rand_frac'])
+
+
+def gpu_step(pkg, model, c, x, pin_host=None, backward=True):
+    """one eager training step -> (loss, prediction, recorder); the DurationPredictor's prediction is its final-normed transformer
+    output [B, N, d]"""
+    with randomness(pkg, c, x), SeedRecorder(pkg, model, pin_host) as rec:
+        out = model(x['mel'].to(dev()), text=x['text'], lens=x['lens'].to(dev()))
+    loss = out.loss if c['cls'] == 'E2TTS' else out
+    if backward:
+        loss.backward()
+    torch.cuda.synchronize()
+    pred = out.pred_flow if c['cls'] == 'E2TTS' else rec.final[-1].view(c['B'], c['N'], -1)
+    return float(loss), pred.detach().float().cpu(), rec
+
+
+def oracle(c, sd, x, masks, grad=True, probe=False):
+    """(loss, prediction, {name: gradient}) of the oracle with O.DROPOUT = masks, in float64 unless the case says otherwise;
+    probe: its stage outputs rounded to bf16 (O.STAGE_ROUND), no gradients"""
+    dt = F64 if c.get('f64', True) else torch.float32
+    osd = {k: (v.detach().clone().to(dt).requires_grad_(grad) if v.is_floating_point() else v) for k, v in sd.items()}
+    mel, lens, text = x['mel'].to(dt), x['lens'], O.list_str_to_tensor(x['text'])
+    old = torch.get_default_dtype()
+    torch.set_default_dtype(dt)
+    O.STAGE_ROUND = O.bf16_ste if probe else None
+    cap = {}
+    inner = O.transformer_forward
+
+    def transformer_forward(*a, **k):
+        cap['y'] = inner(*a, **k)
+        return cap['y']
+    O.transformer_forward = transformer_forward
+    try:
+        with headdim_oracle(c['tkw']), torch.set_grad_enabled(grad):
+            if c['cls'] == 'E2TTS':
+                o = with_dropout(masks, O.e2tts_forward, osd, cfg(c['tkw']), mel, text, x0=x['x0'].to(dt), times=x['times'].to(dt),
+                                 span_mask=x['span'], lens=lens)
+                loss, pred = o['loss'], o['pred']
+            else:
+                loss = with_dropout(masks, O.duration_forward, osd, cfg(c['tkw'], cond_on_time=False), mel, text, lens=lens,
+                                    rand_frac=x['rand_frac'].to(dt))
+                pred = cap['y']
+        if grad:
+            loss.backward()
+    finally:
+        O.transformer_forward = inner
+        O.STAGE_ROUND = None
+        torch.set_default_dtype(old)
+    grads = {k: v.grad for k, v in osd.items() if grad and v.is_floating_point()}
+    return float(loss), pred.detach(), grads
+
+
+def check_vs_oracle(model, c, sd, x, loss, pred, calls, word, tag):
+    """model_checks.whole_model's criteria against the oracle with the masks of `calls` at device word `word`, and the negative
+    control: the masks of every effective seed + 1 miss the prediction tolerance by 3x (by c['neg'] x where the case says so)"""
+    masks = KernelMasks(calls, word)
+    rloss, rpred, rgrads = oracle(c, sd, x, masks)
+    assert sorted(masks.used) == sorted(calls), f'{tag}: the oracle dropped at {sorted(masks.used)}, the kernels at {sorted(calls)}'
+    masks.used.clear()
+    _, ppred, _ = oracle(c, sd, x, masks, grad=False, probe=True)
+    e_probe = rel_l2(ppred, rpred)
+    assert e_probe < PROBE, f'{tag}: ill-conditioned for bf16 activations (probe {e_probe:.3g})'
+    assert abs(loss - rloss) <= TOL_LOSS * abs(rloss), (tag, loss, rloss)
+    e_pred = rel_l2(pred, rpred)
+    assert e_pred < TOL_PRED, f'{tag}: pred rel-L2 {e_pred:.4g}'
+    total = float(torch.cat([g.flatten() for g in rgrads.values() if g is not None]).norm())
+    worst = (1.0, None)
+    for k, prm in model.named_parameters():
+        gr = rgrads[k]
+        if gr is None:
+            assert prm.grad is None or float(prm.grad.abs().max()) == 0.0, f'{k} should be unused'
+            continue
+        assert prm.grad is not None, k
+        if float(gr.norm()) < 1e-4 * total:
+            continue
+        worst = min(worst, (cos(prm.grad.cpu(), gr), k))
+    assert worst[0] >= COS, (tag, worst)
+    _, npred, _ = oracle(c, sd, x, KernelMasks(calls, word, offset=1), grad=False)
+    e_neg, need = rel_l2(pred, npred), c.get('neg', 3) * TOL_PRED
+    assert e_neg >= need, f'{tag}: the masks of seed + 1 give pred rel-L2 {e_neg:.4g}, not >= {need}'
+    print(f'{tag}: loss {loss:.5f} (oracle {rloss:.5f}), pred rel-L2 {e_pred:.4g} (probe {e_probe:.4g}, seed + 1 {e_neg:.4g}), '
+          f'worst grad cosine {worst}')
+
+
+def check_calls(model, calls, p, device_word):
+    """one call per attention and feed-forward module that ran, every one with dropout p, distinct seeds"""
+    assert calls, 'no dropout call recorded'
+    assert all(cl.p == p and cl.device_word == device_word for cl in calls.values()), calls
+    seeds = [cl.seed for cl in calls.values()]
+    assert len(set(seeds)) == len(seeds), 'two modules share a dropout seed'
+    depth = len(model.transformer.layers)
+    text_layers = sum(1 for n in calls if n.endswith('.1.2.attn_dropout'))
+    assert text_layers == depth, 'every layer has text sub-blocks in these cases'
+    assert sum(1 for n in calls if n.endswith('.attn_dropout')) == 2 * depth
+    assert sum(1 for n in calls if n.endswith('.ff.1')) == 2 * depth
+
+
+@pytest.mark.parametrize('name', list(CASES))
+def test_dropout_step_vs_oracle(pkg, schedule, name):
+    c = CASES[name]
+    model, sd = build(pkg, c, c['p'])
+    x = inputs(c)
+    loss, pred, rec = gpu_step(pkg, model, c, x)
+    calls = rec.calls()
+    check_calls(model, calls, c['p'], False)
+    check_vs_oracle(model, c, sd, x, loss, pred, calls, 0, f'{name} {schedule}')
+
+
+def test_schedules_agree_without_dropout(pkg, monkeypatch):
+    """p = 0: the serial and the two-stream schedule compute the same step. The prediction is bit-identical across runs and
+    schedules; every gradient is within the run-to-run scatter of DESIGN §5 (<= 3.8e-3 relative L2 at cfg2) of the serial one.
+    Gradients are not held bit for bit across schedules even where two serial runs agree: the column sums and the split-K partial
+    sums combine through fp32 atomics in an order that depends on what else runs on the GPU at the time — the text stream, on the
+    two-stream schedule (on an H100 the layer-0 audio head-gate bias gradient agreed in two serial runs and differed on two streams)"""
+    c = CASES['cfg2']
+    model, _ = build(pkg, c, 0.0)
+    x = inputs(c)
+
+    def run():
+        model.zero_grad(set_to_none=True)
+        loss, pred, _ = gpu_step(pkg, model, c, x)
+        return loss, pred, {k: p.grad.detach().clone() for k, p in model.named_parameters() if p.grad is not None}
+
+    monkeypatch.setattr(pkg.modules, 'TWO_STREAM', False)
+    s1, s2 = run(), run()
+    monkeypatch.setattr(pkg.modules, 'TWO_STREAM', True)
+    t = run()
+    assert torch.equal(s1[1], s2[1]) and torch.equal(s1[1], t[1]), 'the prediction differs between runs or schedules'
+    assert set(s1[2]) == set(t[2])
+    assert abs(t[0] - s1[0]) <= 1e-6 * abs(s1[0])
+    same_serial = sum(torch.equal(s1[2][k], s2[2][k]) for k in s1[2])
+    same_sched = sum(torch.equal(s1[2][k], t[2][k]) for k in s1[2])
+    worst = 0.0
+    for k in s1[2]:
+        e = rel_l2(t[2][k].cpu(), s1[2][k].cpu())
+        worst = max(worst, e)
+        assert e <= 4e-3, (k, e)
+    print(f'gradients bit-identical: {same_serial} of {len(s1[2])} between serial runs, {same_sched} across schedules; '
+          f'largest difference across schedules {worst:.3g} relative L2')
+
+
+def test_graph_replays_with_dropout_vs_oracle(pkg, schedule):
+    """GraphedTrainStep with dropout on: every replay first steps the device seed word (splitmix64, checked exactly in host
+    arithmetic) and its loss, prediction and gradients match the oracle with the masks of the captured seeds at that word; an
+    eager step with the word and the captured host seed pinned gives a bit-identical prediction"""
+    c = dict(cls='E2TTS', tkw=SMALL, B=2, N=96, lens=[96, 61], seed=206, p=P_SMALL)
+    model, sd = build(pkg, c, c['p'])
+    model.cond_drop_prob = 0.0
+    x = inputs(c)
+    mel, lens = x['mel'].to(dev()), x['lens'].to(dev())
+    text = pkg.list_str_to_tensor(x['text']).to(dev())
+    with randomness(pkg, c, x), SeedRecorder(pkg, model) as rec:
+        step = pkg.GraphedTrainStep(model, mel, text=text, lens=lens)
+    captured = rec.calls(len(rec.log) // len(rec.host))   # the calls of the last forward (after the warm-up): the capture's
+    host = rec.host[-1]
+    check_calls(model, captured, c['p'], True)
+    word_of = lambda: int(step._seed_dev.item()) % 2 ** 64
+    seen = set()
+    for r in (1, 2):
+        torch.cuda.synchronize()
+        w0 = word_of()
+        loss = float(step())
+        torch.cuda.synchronize()
+        w = word_of()
+        assert w == splitmix64(w0), f'replay {r}: seed word {w:#x}, splitmix64 of {w0:#x} is {splitmix64(w0):#x}'
+        assert w not in seen
+        seen.add(w)
+        pred = step.out.pred_flow.detach().float().cpu()
+        check_vs_oracle(model, c, sd, x, loss, pred, captured, w, f'replay {r} {schedule}')
+        # the eager step with this word and the captured host seed draws the same masks
+        model.transformer._seed_dev = torch.tensor([w - 2 ** 64 if w >= 2 ** 63 else w], dtype=torch.int64, device=dev())
+        try:
+            _, epred, erec = gpu_step(pkg, model, c, x, pin_host=host, backward=False)
+        finally:
+            model.transformer._seed_dev = step._seed_dev
+        assert erec.host == [host] and erec.calls() == captured
+        assert torch.equal(epred, pred), f'replay {r}: the eager step with its seeds differs from the replay'
+
+
+def test_eval_ignores_dropout(pkg):
+    """model.eval(): a dropout-0.1 model and the same weights at dropout 0 give bit-identical forward and sample() output"""
+    c = dict(cls='E2TTS', tkw=SMALL, B=2, N=96, lens=[96, 61], seed=207)
+    m1, sd = build(pkg, c, 0.1)
+    m0, _ = build(pkg, c, 0.0)
+    m0.load_state_dict(sd)
+    x = inputs(c)
+    y0 = torch.randn(2, 64, 100, generator=torch.Generator().manual_seed(208)).to(dev())
+    cond = x['mel'][:, :24].to(dev())
+    outs = []
+    for m in (m1, m0):
+        m.eval()
+        with torch.no_grad():
+            loss, pred, _ = gpu_step(pkg, m, c, x, backward=False)
+            with pkg.inject_randomness(y0=y0):
+                s = m.sample(cond, text=x['text'], duration=64, steps=4, cfg_strength=1.0, return_raw_output=True)
+        outs.append((loss, pred, s.float().cpu()))
+    assert torch.equal(outs[0][1], outs[1][1]) and torch.equal(outs[0][2], outs[1][2])
+    assert abs(outs[0][0] - outs[1][0]) <= 1e-6 * abs(outs[1][0])    # the loss's masked mean is an atomic reduction (DESIGN §5)
