@@ -336,12 +336,16 @@ __global__ void __launch_bounds__(256) qkv_post_bwd_kernel(const QkvP p) {
     }
 }
 
-// ------------------------------------------------------------------------------------------------ GEGLU backward
+// ------------------------------------------------------------------------------------------------ GLU backward
 // ug packed [T, 2*inner] ([u(64)|gate(64)] per 128 columns), dh [T, inner] -> dug packed; the bias gradient of the GLU
-// projection (column sums of dug, packed order) is accumulated in the same pass (db must be zeroed by the caller).
+// projection (column sums of dug, packed order) is accumulated in the same pass (db must be zeroed by the caller), and with MULT the
+// gradient of the hidden-unit multiplier (dmult[c] += sum_rows drop(dh) u act(g), zeroed by the caller, may be NULL).
+// ACT: 1 exact erf GELU, 2 SiLU, 3 ReLU^2 (the activation codes of b200_gemm's GLU epilogue).
 constexpr int GB_ROWS = 256;   // rows per block (8 row lanes x 32)
-__global__ void __launch_bounds__(256) geglu_bwd_kernel(const __nv_bfloat16* dh, const __nv_bfloat16* ug, __nv_bfloat16* dug, float* db, long long T,
-                                                         int inner, float dropout_p, unsigned long long seed, const unsigned long long* seed_dev) {
+template <int ACT, bool MULT>
+__global__ void __launch_bounds__(256) glu_bwd_kernel(const __nv_bfloat16* dh, const __nv_bfloat16* ug, __nv_bfloat16* dug, float* db,
+                                                       const float* mult, float* dmult, long long T,
+                                                       int inner, float dropout_p, unsigned long long seed, const unsigned long long* seed_dev) {
     __shared__ float red[8][32][17];
     const int nchunk = inner >> 3;
     const int cl = threadIdx.x & 31, rl = threadIdx.x >> 5;
@@ -350,8 +354,14 @@ __global__ void __launch_bounds__(256) geglu_bwd_kernel(const __nv_bfloat16* dh,
     const float ks = dropout_p > 0.f ? 65536.f / (65536.f - (float)thr) : 1.f;
     const uint32_t seedmix = seed_mix32(seed + (seed_dev ? __ldg(seed_dev) : 0ull));
     float su[8] = {0, 0, 0, 0, 0, 0, 0, 0}, sg[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    float sm[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // MULT only
     if (c < nchunk) {
         const int hcol = c * 8;
+        float m[8];
+        if constexpr (MULT) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) m[j] = __ldg(mult + hcol + j);
+        }
         const long long r1 = min(T, (long long)(blockIdx.y + 1) * GB_ROWS);
         for (long long row = (long long)blockIdx.y * GB_ROWS + rl; row < r1; row += 8) {
             const size_t pu = (size_t)row * 2 * inner + (hcol >> 6) * 128 + (hcol & 63);
@@ -359,7 +369,7 @@ __global__ void __launch_bounds__(256) geglu_bwd_kernel(const __nv_bfloat16* dh,
             unpack8(*reinterpret_cast<const uint4*>(dh + (size_t)row * inner + hcol), d);
             unpack8(*reinterpret_cast<const uint4*>(ug + pu), u);
             unpack8(*reinterpret_cast<const uint4*>(ug + pu + 64), g);
-            if (dropout_p > 0.f) {   // same pair hash as the GEGLU epilogue of the forward GEMM
+            if (dropout_p > 0.f) {   // same pair hash as the GLU epilogue of the forward GEMM
                 const uint32_t pbase = (uint32_t)(((unsigned long long)row * (unsigned long long)inner + hcol) >> 1);
 #pragma unroll
                 for (int j = 0; j < 8; j += 2) {
@@ -370,10 +380,26 @@ __global__ void __launch_bounds__(256) geglu_bwd_kernel(const __nv_bfloat16* dh,
             }
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                const float cdf = 0.5f * (1.f + erff(g[j] * 0.70710678118654752440f));
-                const float pdf = 0.3989422804014327f * __expf(-0.5f * g[j] * g[j]);
-                du[j] = d[j] * g[j] * cdf;
-                dg[j] = d[j] * u[j] * (cdf + g[j] * pdf);
+                float a;                       // act(g), MULT only
+                const float dd = MULT ? d[j] * m[j] : d[j];   // the gradient reaching u * act(g)
+                if constexpr (ACT == 1) {
+                    const float cdf = 0.5f * (1.f + erff(g[j] * 0.70710678118654752440f));
+                    const float pdf = 0.3989422804014327f * __expf(-0.5f * g[j] * g[j]);
+                    du[j] = dd * g[j] * cdf;
+                    dg[j] = dd * u[j] * (cdf + g[j] * pdf);
+                    a = g[j] * cdf;
+                } else if constexpr (ACT == 2) {
+                    const float s = 1.f / (1.f + __expf(-g[j]));   // sigmoid; 0 where exp(-g) overflows
+                    a = g[j] * s;
+                    du[j] = dd * a;
+                    dg[j] = dd * u[j] * (s + a * (1.f - s));      // silu'(g) = s (1 + g (1 - s))
+                } else {
+                    const float r = fmaxf(g[j], 0.f);
+                    a = r * r;
+                    du[j] = dd * a;
+                    dg[j] = dd * u[j] * (2.f * r);
+                }
+                if constexpr (MULT) sm[j] += d[j] * u[j] * a;
             }
             const uint4 pu4 = pack8(du), pg4 = pack8(dg);
             *reinterpret_cast<uint4*>(dug + pu) = pu4;
@@ -398,6 +424,21 @@ __global__ void __launch_bounds__(256) geglu_bwd_kernel(const __nv_bfloat16* dh,
             for (int k = 0; k < 8; ++k) s += red[k][cc][j];
             const int hcol = chunk * 8 + (j & 7);
             atomicAdd(db + (hcol >> 6) * 128 + (hcol & 63) + (j >= 8 ? 64 : 0), s);
+        }
+    }
+    if (MULT && dmult) {
+        if (db) __syncthreads();   // the bias reduction has read `red`
+#pragma unroll
+        for (int j = 0; j < 8; ++j) red[rl][cl][j] = sm[j];
+        __syncthreads();
+        for (int i = threadIdx.x; i < 32 * 8; i += 256) {
+            const int cc = i >> 3, j = i & 7;
+            const int chunk = blockIdx.x * 32 + cc;
+            if (chunk >= nchunk) continue;
+            float s = 0.f;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) s += red[k][cc][j];
+            atomicAdd(dmult + chunk * 8 + j, s);
         }
     }
 }
@@ -918,13 +959,31 @@ extern "C" int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stre
     return check_launch("qkv_post_bwd_kernel");
 }
 
+extern "C" int b200_glu_bwd(const b200_glu_bwd_args* a, b200_stream_t stream) {
+    B200_REQUIRE(a && a->dh && a->ug && a->dug, "glu_bwd: null pointer");
+    B200_REQUIRE(a->T > 0 && a->inner > 0 && (a->inner % 64) == 0, "glu_bwd: inner must be a multiple of 64");
+    B200_REQUIRE(a->act >= 1 && a->act <= 3, "glu_bwd: act=%d is not an activation code (1 GELU, 2 SiLU, 3 ReLU^2)", (int)a->act);
+    B200_REQUIRE(!a->d_mult || a->mult, "glu_bwd: d_mult needs mult");
+    dim3 grid((a->inner / 8 + 31) / 32, (unsigned)((a->T + GB_ROWS - 1) / GB_ROWS));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const auto dh = (const __nv_bfloat16*)a->dh, ug = (const __nv_bfloat16*)a->ug;
+    const auto dug = (__nv_bfloat16*)a->dug;
+    const auto sd = reinterpret_cast<const unsigned long long*>(a->seed_dev);
+    auto kern = glu_bwd_kernel<1, false>;
+    if (a->mult) kern = a->act == 1 ? glu_bwd_kernel<1, true> : a->act == 2 ? glu_bwd_kernel<2, true> : glu_bwd_kernel<3, true>;
+    else kern = a->act == 1 ? glu_bwd_kernel<1, false> : a->act == 2 ? glu_bwd_kernel<2, false> : glu_bwd_kernel<3, false>;
+    kern<<<grid, 256, 0, st>>>(dh, ug, dug, a->db_packed, a->mult, a->d_mult, a->T, a->inner, a->dropout_p, a->seed, sd);
+    return check_launch("glu_bwd_kernel");
+}
+
 extern "C" int b200_geglu_bwd(const void* dh, const void* ug, void* dug, float* db_packed, int64_t T, int32_t inner, float dropout_p, uint64_t seed,
                               const uint64_t* seed_dev, b200_stream_t stream) {
     B200_REQUIRE(dh && ug && dug && T > 0 && inner > 0 && (inner % 64) == 0, "geglu_bwd: inner must be a multiple of 64");
-    dim3 grid((inner / 8 + 31) / 32, (unsigned)((T + GB_ROWS - 1) / GB_ROWS));
-    geglu_bwd_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        (const __nv_bfloat16*)dh, (const __nv_bfloat16*)ug, (__nv_bfloat16*)dug, db_packed, T, inner, dropout_p, seed, reinterpret_cast<const unsigned long long*>(seed_dev));
-    return check_launch("geglu_bwd_kernel");
+    b200_glu_bwd_args a{};
+    a.dh = dh; a.ug = ug; a.dug = dug; a.db_packed = db_packed;
+    a.T = T; a.inner = inner; a.act = 1;
+    a.dropout_p = dropout_p; a.seed = seed; a.seed_dev = seed_dev;
+    return b200_glu_bwd(&a, stream);
 }
 
 extern "C" int b200_colsum(const void* X, int64_t T, int32_t ncols, int32_t ld, float* out, b200_stream_t stream) {

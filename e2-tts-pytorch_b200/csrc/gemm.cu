@@ -35,11 +35,14 @@ struct GemmParams {
     const float* colscale; int rows_per_batch;
     const unsigned char* rowmask;
     const void* resid; long long ldr;
-    int geglu; float dropout_p; unsigned long long seed;
+    int geglu; float dropout_p; unsigned long long seed;   // geglu: 0 none, else the GLU activation (GLU_GELU / GLU_SILU / GLU_RELU2)
     const unsigned long long* seed_dev;   // optional device addend of the seed (CUDA-graph replays)
     int atomic_out;
     int tma_store;   // bf16 output through the smem staging slices and TMA stores (tmD)
+    const float* glu_mult;   // optional [N/2] multiplier of the hidden units (x-transformers GLU mult_bias), hidden-unit order
 };
+
+constexpr int GLU_GELU = 1, GLU_SILU = 2, GLU_RELU2 = 3;
 
 // Tiles: (BM * MH) x BN. MH == 2 gives each consumer warpgroup 128 rows (two m64 MMAs per k-step share one B tile); BN == 256 gives it
 // one m64n256 MMA per k-step. Both halve the smem -> tensor-core bytes per FLOP of the 128 x 128 tile; 128 fp32 accumulators per thread.
@@ -75,6 +78,85 @@ __device__ __forceinline__ float2 gelu_erf2(float2 x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(t.x));
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ey) : "f"(t.y));
     return ffma2(make_float2(-a.x, -a.y), make_float2(ex, ey), make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f)));
+}
+
+// SiLU (x-transformers FeedForward(swish=True)) for a PAIR: silu(x) = x / (1 + 2^(-x log2 e)), one MUFU.EX2 and one MUFU.RCP (inside
+// __fdividef) per element. The rounded exponent argument, ex2.approx (2^-22 relative), the add and __fdividef (2 ulp) keep the relative
+// error below (8 + 1.5 |x|) 2^-24: under 4e-6 for |x| <= 40, 0.2 % of a bf16 half-ulp. Where 1 + 2^(-x log2 e) exceeds 2^126 (x < -87)
+// the value is 0, and |silu(x)| < 1e-36 there; for large positive x the exponent underflows to 0 and silu(x) = x exactly.
+// (The same arithmetic with an explicit rcp.approx and product makes the 128 x 256 tile spill 8 bytes; this form does not.)
+__device__ __forceinline__ float2 silu2(float2 x) {
+    const float2 t = fmul2(x, make_float2(-1.4426950408889634f, -1.4426950408889634f));
+    float ex, ey;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ex) : "f"(t.x));
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(ey) : "f"(t.y));
+    const float2 d = fadd2(make_float2(ex, ey), make_float2(1.f, 1.f));
+    return make_float2(__fdividef(x.x, d.x), __fdividef(x.y, d.y));
+}
+
+// ReLU^2 (x-transformers FeedForward(relu_squared=True)) for a PAIR: one max and one product per element, exactly 0 for x <= 0.
+__device__ __forceinline__ float2 relu2_2(float2 x) {
+    const float2 r = make_float2(fmaxf(x.x, 0.f), fmaxf(x.y, 0.f));
+    return fmul2(r, r);
+}
+
+template <int ACT>
+__device__ __forceinline__ float2 glu_act2(float2 g) {
+    if constexpr (ACT == GLU_GELU) return gelu_erf2(g);
+    else if constexpr (ACT == GLU_SILU) return silu2(g);
+    else return relu2_2(g);
+}
+
+// GLU epilogue on the accumulator fragments: every 128 packed columns hold [0,64) = u, [64,128) = gate of the same 64 hidden units, so a
+// thread holds both halves of each of its hidden units (fragment groups j and j + 8 of the 128-column group).
+// h = u * act(gate) (* glu_mult) (* dropout keep / (1 - p)), bf16; D2 <- the bf16 pre-activations.
+template <int ACT, int BN, int MH>
+__device__ __forceinline__ void glu_epilogue(const GemmParams& p, float (&acc)[MH][BN / 2], int tm, int tn, int cw, int wq, int lane) {
+    constexpr int BMT = BM * MH;
+    const int cq = 2 * (lane & 3);
+    const bool do_drop = p.dropout_p > 0.f;
+    const float keep_scale = do_drop ? 65536.f / (65536.f - (float)(uint32_t)(p.dropout_p * 65536.f)) : 1.f;
+    const uint32_t seedmix = do_drop ? seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull)) : 0u;
+    const uint32_t thr32 = drop_thresh32((uint32_t)(p.dropout_p * 65536.f));
+#pragma unroll
+    for (int h = 0; h < MH; ++h) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
+            if (row >= p.M) continue;
+#pragma unroll
+            for (int sub = 0; sub < BN / 128; ++sub) {
+                const int colg = tn * BN + sub * 128;   // first packed column of the group (N % 128 == 0)
+                if (colg >= p.N) continue;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    const int cu = colg + 8 * j + cq;           // packed column of u; the gate is 64 further
+                    const int hcol = colg / 2 + 8 * j + cq;     // hidden-unit column
+                    float2 u = make_float2(acc[h][4 * (sub * 16 + j) + 2 * i], acc[h][4 * (sub * 16 + j) + 2 * i + 1]);
+                    float2 g = make_float2(acc[h][4 * (sub * 16 + 8 + j) + 2 * i], acc[h][4 * (sub * 16 + 8 + j) + 2 * i + 1]);
+                    if (p.bias) {
+                        u = fadd2(u, make_float2(__ldg(p.bias + cu), __ldg(p.bias + cu + 1)));
+                        g = fadd2(g, make_float2(__ldg(p.bias + cu + 64), __ldg(p.bias + cu + 65)));
+                    }
+                    const uint32_t wu = pack_bf16(u.x, u.y), wgt = pack_bf16(g.x, g.y);
+                    if (p.D2) {
+                        __nv_bfloat16* d2 = reinterpret_cast<__nv_bfloat16*>(p.D2) + (long long)row * p.ldd2 + cu;
+                        *reinterpret_cast<uint32_t*>(d2) = wu;
+                        *reinterpret_cast<uint32_t*>(d2 + 64) = wgt;
+                    }
+                    // the backward pass recomputes from the bf16-rounded pre-activations: use them here too
+                    float2 h2 = fmul2(make_float2(bf16_lo(wu), bf16_hi(wu)), glu_act2<ACT>(make_float2(bf16_lo(wgt), bf16_hi(wgt))));
+                    if (p.glu_mult) h2 = fmul2(h2, make_float2(__ldg(p.glu_mult + hcol), __ldg(p.glu_mult + hcol + 1)));
+                    if (do_drop) {
+                        // hidden-unit pairs (2k, 2k+1) of one row share a 32-bit hash; N/2 is even, so (row * N/2 + hcol) >> 1 pairs them
+                        const DropWords hsh = drop_words(seedmix, (uint32_t)(((unsigned long long)row * (unsigned long long)(p.N / 2) + hcol) >> 1));
+                        h2 = fmul2(h2, make_float2(hsh.a >= thr32 ? keep_scale : 0.f, hsh.b >= thr32 ? keep_scale : 0.f));
+                    }
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + hcol) = pack_bf16(h2.x, h2.y);
+                }
+            }
+        }
+    }
 }
 
 
@@ -327,51 +409,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                 }
             }
+        } else if (p.geglu == GLU_GELU) {   // one copy of the GLU epilogue per activation: no per-element branch on it
+            glu_epilogue<GLU_GELU, BN, MH>(p, acc, tm, tn, cw, wq, lane);
+        } else if (p.geglu == GLU_SILU) {
+            glu_epilogue<GLU_SILU, BN, MH>(p, acc, tm, tn, cw, wq, lane);
         } else {
-            // GEGLU: every 128 packed columns hold [0,64) = u, [64,128) = gate of the same 64 hidden units, so a thread holds both
-            // halves of each of its hidden units (fragment groups j and j + 8 of the 128-column group)
-            const bool do_drop = p.dropout_p > 0.f;
-            const float keep_scale = do_drop ? 65536.f / (65536.f - (float)(uint32_t)(p.dropout_p * 65536.f)) : 1.f;
-            const uint32_t seedmix = do_drop ? seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull)) : 0u;
-            const uint32_t thr32 = drop_thresh32((uint32_t)(p.dropout_p * 65536.f));
-#pragma unroll
-            for (int h = 0; h < MH; ++h) {
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
-                    if (row >= p.M) continue;
-#pragma unroll
-                    for (int sub = 0; sub < BN / 128; ++sub) {
-                        const int colg = tn * BN + sub * 128;   // first packed column of the group (N % 128 == 0)
-                        if (colg >= p.N) continue;
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const int cu = colg + 8 * j + cq;           // packed column of u; the gate is 64 further
-                            const int hcol = colg / 2 + 8 * j + cq;     // hidden-unit column
-                            float2 u = make_float2(acc[h][4 * (sub * 16 + j) + 2 * i], acc[h][4 * (sub * 16 + j) + 2 * i + 1]);
-                            float2 g = make_float2(acc[h][4 * (sub * 16 + 8 + j) + 2 * i], acc[h][4 * (sub * 16 + 8 + j) + 2 * i + 1]);
-                            if (p.bias) {
-                                u = fadd2(u, make_float2(__ldg(p.bias + cu), __ldg(p.bias + cu + 1)));
-                                g = fadd2(g, make_float2(__ldg(p.bias + cu + 64), __ldg(p.bias + cu + 65)));
-                            }
-                            const uint32_t wu = pack_bf16(u.x, u.y), wgt = pack_bf16(g.x, g.y);
-                            if (p.D2) {
-                                __nv_bfloat16* d2 = reinterpret_cast<__nv_bfloat16*>(p.D2) + (long long)row * p.ldd2 + cu;
-                                *reinterpret_cast<uint32_t*>(d2) = wu;
-                                *reinterpret_cast<uint32_t*>(d2 + 64) = wgt;
-                            }
-                            // the backward pass recomputes from the bf16-rounded pre-activations: use them here too
-                            float2 h2 = fmul2(make_float2(bf16_lo(wu), bf16_hi(wu)), gelu_erf2(make_float2(bf16_lo(wgt), bf16_hi(wgt))));
-                            if (do_drop) {
-                                // hidden-unit pairs (2k, 2k+1) of one row share a 32-bit hash; N/2 is even, so (row * N/2 + hcol) >> 1 pairs them
-                                const DropWords hsh = drop_words(seedmix, (uint32_t)(((unsigned long long)row * (unsigned long long)(p.N / 2) + hcol) >> 1));
-                                h2 = fmul2(h2, make_float2(hsh.a >= thr32 ? keep_scale : 0.f, hsh.b >= thr32 ? keep_scale : 0.f));
-                            }
-                            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + hcol) = pack_bf16(h2.x, h2.y);
-                        }
-                    }
-                }
-            }
+            glu_epilogue<GLU_RELU2, BN, MH>(p, acc, tm, tn, cw, wq, lane);
         }
     }
     if (t == 0) bulk_wait_group<0>();   // the staging slices stay valid until the last store has completed
@@ -496,7 +539,10 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     p.D2 = a->D2; p.ldd2 = a->ldd2;
     p.bias = a->bias; p.colscale = a->colscale; p.rows_per_batch = (int)(a->rows_per_batch > 0 ? a->rows_per_batch : 1);
     p.rowmask = a->rowmask; p.resid = a->resid; p.ldr = a->ldr;
+    B200_REQUIRE(a->geglu >= 0 && a->geglu <= GLU_RELU2, "gemm: geglu=%d is not an activation code (0 none, 1 GELU, 2 SiLU, 3 ReLU^2)", (int)a->geglu);
+    B200_REQUIRE(!a->glu_mult || a->geglu, "gemm: glu_mult needs the GLU epilogue (geglu != 0)");
     p.geglu = a->geglu; p.dropout_p = a->dropout_p; p.seed = a->seed; p.seed_dev = reinterpret_cast<const unsigned long long*>(a->seed_dev);
+    p.glu_mult = a->glu_mult;
     if (p.atomic_out) {
         B200_REQUIRE(a->d_fp32, "gemm: split-K requires an fp32 output");
         B200_REQUIRE(!a->bias && !a->colscale && !a->rowmask && !a->resid && !a->geglu, "gemm: split-K supports no epilogue");

@@ -32,6 +32,11 @@ SUPPORTED_RESIDUAL_STREAMS = (1, 4)   # Transformer(num_residual_streams): 1 = p
 SUPPORTED_DIM_HEADS = (64, 128)       # Transformer(dim_head, text_dim_head): head widths the attention kernels are built for
 # x-transformers Attention keywords the kernels implement, with x-transformers' own defaults for a missing key
 ATTN_KWARGS_DEFAULTS = dict(gate_value_heads=False, softclamp_logits=False, logit_softclamp_value=50.)
+# x-transformers FeedForward keywords besides those the reference passes itself (dim, mult, glu, dropout), with x-transformers' defaults.
+# The last five have no kernel and are refused unless set to their default.
+FF_KWARGS_DEFAULTS = dict(swish=False, relu_squared=False, glu_mult_bias=False, no_bias=False, zero_init_output=False,
+                          custom_activation=None, solu=False, post_act_ln=False, sublayer_dropout=0., dim_out=None)
+GLU_GELU, GLU_SILU, GLU_RELU2 = ops.GLU_GELU, ops.GLU_SILU, ops.GLU_RELU2
 # text sub-blocks of layer i+1 overlap the audio sub-blocks of layer i on a second CUDA stream (Transformer._run_layers);
 # B200_TWO_STREAM=0 serialises them on the current stream (developer A/B switch)
 import os as _os
@@ -157,16 +162,22 @@ class Attention(Module):  # A.4
 
 
 class _GLU(Module):
-    def __init__(self, dim_in, dim_out):
+    def __init__(self, dim_in, dim_out, mult_bias=False):
         super().__init__()
-        self.proj = nn.Linear(dim_in, dim_out * 2)
+        self.proj = nn.Linear(dim_in, dim_out * 2)   # x-transformers' GLU keeps this bias whatever no_bias says
+        self.mult_bias = nn.Parameter(torch.ones(dim_out)) if mult_bias else None
 
 
 class FeedForward(Module):  # A.2
-    def __init__(self, dim, mult, dropout):
+    def __init__(self, dim, mult, dropout, act=GLU_GELU, glu_mult_bias=False, no_bias=False, zero_init_output=False):
         super().__init__()
         inner = int(dim * mult)
-        self.ff = nn.Sequential(_GLU(dim, inner), nn.Dropout(dropout), nn.Linear(inner, dim))
+        self.act = act
+        self.ff = nn.Sequential(_GLU(dim, inner, glu_mult_bias), nn.Dropout(dropout), nn.Linear(inner, dim, bias=not no_bias))
+        if zero_init_output:
+            nn.init.zeros_(self.ff[2].weight)
+            if self.ff[2].bias is not None:
+                nn.init.zeros_(self.ff[2].bias)
 
 
 class TextAudioCrossCondition(Module):  # e2_tts.py:486-513
@@ -399,6 +410,24 @@ def _parse_attn_kwargs(attn_kwargs):
     return bool(kw['gate_value_heads']), clamp
 
 
+def _parse_ff_kwargs(ff_kwargs):
+    """x-transformers FeedForward keywords (e2_tts.py:552, passed to both the audio and the text FeedForward) -> the keyword arguments of
+    FeedForward above. A missing key takes x-transformers' default; a refused switch set to its default value is accepted."""
+    taken = sorted(set(ff_kwargs) & {'dim', 'mult', 'glu', 'dropout'})
+    if taken:   # the reference passes these itself: its FeedForward(...) call fails the same way
+        raise TypeError(f'FeedForward() got multiple values for keyword argument {taken[0]!r} (ff_kwargs, e2_tts.py:552)')
+    unknown = sorted(set(ff_kwargs) - set(FF_KWARGS_DEFAULTS))
+    if unknown:
+        _unsupported(f'ff_kwargs[{unknown[0]!r}]', ff_kwargs[unknown[0]], 'e2_tts.py:552')
+    kw = {**FF_KWARGS_DEFAULTS, **ff_kwargs}
+    for key in ('custom_activation', 'solu', 'post_act_ln', 'sublayer_dropout', 'dim_out'):
+        if kw[key] != FF_KWARGS_DEFAULTS[key]:
+            _unsupported(f'ff_kwargs[{key!r}]', kw[key], 'e2_tts.py:552')
+    act = GLU_RELU2 if kw['relu_squared'] else GLU_SILU if kw['swish'] else GLU_GELU   # x-transformers' precedence
+    return dict(act=act, glu_mult_bias=bool(kw['glu_mult_bias']), no_bias=bool(kw['no_bias']),
+                zero_init_output=bool(kw['zero_init_output']))
+
+
 class Transformer(_PackOwner):
     """Multistream flow-matching backbone — constructor and forward signature of the reference's Transformer
     (e2_tts.py:518-952). Non-default research switches raise (no kernels, no fallback)."""
@@ -418,8 +447,7 @@ class Transformer(_PackOwner):
         if attn_laser:
             _unsupported('attn_laser', attn_laser, 'e2_tts.py:543')
         gate_value_heads, self.softclamp = _parse_attn_kwargs(attn_kwargs)
-        if dict(ff_kwargs):
-            _unsupported('ff_kwargs', ff_kwargs, 'e2_tts.py:552')
+        ff_kw = _parse_ff_kwargs(dict(ff_kwargs))
         if num_residual_streams not in SUPPORTED_RESIDUAL_STREAMS:
             raise NotImplementedError(
                 f'num_residual_streams={num_residual_streams!r} (e2_tts.py:547): supported values are 1 (plain residual) and 4 '
@@ -471,7 +499,7 @@ class Transformer(_PackOwner):
                 LinearFourierEmbed(dim, p=attn_fourier_embed_input_frac) if attn_fourier_embed_input else nn.Identity(),   # :639
                 post_klass(),
                 norm_klass(dim),
-                FeedForward(dim, ff_mult, dropout),
+                FeedForward(dim, ff_mult, dropout, **ff_kw),
                 post_klass(),
                 None, None, None,
             ])
@@ -483,7 +511,7 @@ class Transformer(_PackOwner):
                     RMSNorm(dim_text),
                     Attention(dim_text, text_heads, text_dim_head, not first, gate_value_heads),
                     RMSNorm(dim_text),
-                    FeedForward(dim_text, text_ff_mult, dropout),
+                    FeedForward(dim_text, text_ff_mult, dropout, **ff_kw),
                     TextAudioCrossCondition(dim, dim_text, cond_audio_to_text=ind != text_depth - 1),
                 ])
                 text_hc = ModuleList([hc(dim=dim_text), hc(dim=dim_text), hc(dim=dim_text)])
@@ -646,7 +674,7 @@ class Transformer(_PackOwner):
             br, rest, beta = width(res, hcm, gain, mode)
             y = ops.FeedForward.apply(br, ff.ff[0].proj.weight, ff.ff[0].proj.bias, ff.ff[2].weight, ff.ff[2].bias,
                                       pk['w1'], pk['b1'], pk['w2'], colscale, B, Np, p_drop, next_seed(), self._seed_dev,
-                                      rest if plain else None)
+                                      rest if plain else None, ff.act, ff.ff[0].mult_bias)
             return close(depth(rest, y, beta))
 
         def text_block(i, ts, tvf):  # the three text sub-blocks of layer i (:853-882)

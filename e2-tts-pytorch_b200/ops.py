@@ -62,8 +62,9 @@ def _zeros(shape, device):
 
 def gemm(A, B, M, N, K, *, lda=None, ldb=None, A2=None, lda2=0, K1=0, a_mn=False, b_mn=False, out=None, ldd=None,
          out_fp32=False, D2=None, ldd2=0, bias=None, colscale=None, rows_per_batch=0, rowmask=None, resid=None, ldr=0,
-         geglu=False, dropout_p=0.0, seed=0, split_k=1, force_tile=0, seed_dev=None):
-    """D[M,N] = epilogue(sum_k A[m,k] B[n,k]) on the wgmma GEMM (include/b200_e2tts.h: b200_gemm)."""
+         geglu=False, dropout_p=0.0, seed=0, split_k=1, force_tile=0, seed_dev=None, glu_mult=None):
+    """D[M,N] = epilogue(sum_k A[m,k] B[n,k]) on the wgmma GEMM (include/b200_e2tts.h: b200_gemm). geglu: the GLU activation code
+    (GLU_GELU, GLU_SILU, GLU_RELU2; True is GELU), glu_mult: fp32 [N/2] multiplier of the hidden units."""
     dev = A.device
     n_out = N // 2 if geglu else N
     if ldd is None:
@@ -74,13 +75,17 @@ def gemm(A, B, M, N, K, *, lda=None, ldb=None, A2=None, lda2=0, K1=0, a_mn=False
         A, lda if lda is not None else (M if a_mn else K), A2, lda2, K1,
         B, ldb if ldb is not None else (N if b_mn else K), M, N, K, int(a_mn), int(b_mn),
         out, ldd, int(out_fp32), D2, ldd2, bias, colscale, rows_per_batch,
-        rowmask, resid, ldr, int(geglu), float(dropout_p), int(seed), int(split_k), int(force_tile), seed_dev))
+        rowmask, resid, ldr, int(geglu), float(dropout_p), int(seed), int(split_k), int(force_tile), seed_dev, glu_mult))
     lib.call('b200_gemm', args, _stream())
     return out
 
 
 _GEMM_FIELDS = ('A', 'lda', 'A2', 'lda2', 'K1', 'B', 'ldb', 'M', 'N', 'K', 'a_mn_major', 'b_mn_major', 'D', 'ldd', 'd_fp32', 'D2', 'ldd2',
-                'bias', 'colscale', 'rows_per_batch', 'rowmask', 'resid', 'ldr', 'geglu', 'dropout_p', 'seed', 'split_k', 'force_tile', 'seed_dev')
+                'bias', 'colscale', 'rows_per_batch', 'rowmask', 'resid', 'ldr', 'geglu', 'dropout_p', 'seed', 'split_k', 'force_tile', 'seed_dev',
+                'glu_mult')
+
+# GLU activation codes of b200_gemm's GLU epilogue and b200_glu_bwd (x-transformers FeedForward: default, swish=True, relu_squared=True)
+GLU_GELU, GLU_SILU, GLU_RELU2 = 1, 2, 3
 
 
 def grad_weight(dY, X, T, n_out, n_in, *, ldy=None, ldx=None, out=None, ldd=None):
@@ -519,18 +524,23 @@ class OutProj(Function):
 
 
 class FeedForward(Function):
-    """x-transformers FeedForward(glu=True) (A.2): GEGLU GEMM (+dropout) -> out GEMM (+bias, AdaLNZero gate). resid (bf16 [T, Din],
-    optional): the plain residual sub-block's add (:882, 939) in the out GEMM's epilogue; its gradient is dy itself."""
+    """x-transformers FeedForward(glu=True) (A.2): GLU GEMM (+dropout) -> out GEMM (+bias, AdaLNZero gate). resid (bf16 [T, Din],
+    optional): the plain residual sub-block's add (:882, 939) in the out GEMM's epilogue; its gradient is dy itself.
+    act: the GLU activation code (GLU_GELU, GLU_SILU, GLU_RELU2); mult (fp32 [inner], optional): GLU(mult_bias=True), h = u act(g) mult;
+    b2 None: the output Linear without bias (FeedForward(no_bias=True))."""
 
     @staticmethod
-    def forward(ctx, xn, w1, b1, w2, b2, w1pack, b1pack, w2pack, colscale, B, Np, dropout_p, seed, seed_dev, resid=None):
+    def forward(ctx, xn, w1, b1, w2, b2, w1pack, b1pack, w2pack, colscale, B, Np, dropout_p, seed, seed_dev, resid=None, act=GLU_GELU,
+                mult=None):
         T, Din = xn.shape
         inner = w2.shape[1]
         ug = torch.empty((T, 2 * inner), device=xn.device, dtype=BF16)
-        h = gemm(xn, w1pack, T, 2 * inner, Din, D2=ug, ldd2=2 * inner, bias=b1pack, geglu=True, dropout_p=dropout_p, seed=seed, seed_dev=seed_dev)
+        h = gemm(xn, w1pack, T, 2 * inner, Din, D2=ug, ldd2=2 * inner, bias=b1pack, geglu=act, dropout_p=dropout_p, seed=seed, seed_dev=seed_dev,
+                 glu_mult=mult)
         y = gemm(h, w2pack, T, Din, inner, bias=b2, colscale=colscale, rows_per_batch=Np, resid=resid, ldr=Din if resid is not None else 0)
         ctx.save_for_backward(xn, ug, h, y, w1pack, w2pack, colscale)
-        ctx.meta = (B, Np, dropout_p, seed, inner, seed_dev)
+        ctx.meta = (B, Np, dropout_p, seed, inner, seed_dev, act, b2 is not None)
+        ctx.mult = mult
         ctx.has_resid, ctx.resid = resid is not None, (resid if colscale is not None else None)   # the gated backward reads y - resid
         return y
 
@@ -538,29 +548,38 @@ class FeedForward(Function):
     @once_differentiable
     def backward(ctx, dy):
         xn, ug, h, y, w1pack, w2pack, colscale = ctx.saved_tensors
-        B, Np, dropout_p, seed, inner, seed_dev = ctx.meta
-        has_resid, resid = ctx.has_resid, ctx.resid
+        B, Np, dropout_p, seed, inner, seed_dev, act, has_b2 = ctx.meta
+        has_resid, resid, mult = ctx.has_resid, ctx.resid, ctx.mult
         T, Din = xn.shape
         dy = _c(dy)
+        db2 = None
         if colscale is not None and resid is not None:
-            dz, d_cs, db2 = _rowgate_resid_bwd(dy, y, resid, colscale, None, B, Np, Din, want_bias=True)
+            dz, d_cs, *db2 = _rowgate_resid_bwd(dy, y, resid, colscale, None, B, Np, Din, want_bias=has_b2)
         elif colscale is not None:
             # y = cs * (h W2^T + b2): recover the pre-gate value through y / cs inside the kernel
-            dz, d_cs, db2 = _rowgate_bwd(dy, y, colscale, None, B, Np, Din, want_bias=True)   # bias grad rides along
+            dz, d_cs, *db2 = _rowgate_bwd(dy, y, colscale, None, B, Np, Din, want_bias=has_b2)   # bias grad rides along
         else:
             dz, d_cs = dy, None
-            db2 = colsum(dz, T, Din, Din)
+            db2 = [colsum(dz, T, Din, Din)] if has_b2 else []
+        db2 = db2[0] if db2 else None
         dh = gemm(dz, w2pack, T, inner, Din, b_mn=True)
         dW2 = grad_weight(dz, h, T, Din, inner)
         dug = torch.empty_like(ug)
         db1p = _zeros(2 * inner, xn.device)
-        lib.call('b200_geglu_bwd', dh, ug, dug, db1p, T, inner, float(dropout_p), int(seed), seed_dev, _stream())
+        d_mult = None
+        if act == GLU_GELU and mult is None:
+            lib.call('b200_geglu_bwd', dh, ug, dug, db1p, T, inner, float(dropout_p), int(seed), seed_dev, _stream())
+        else:
+            d_mult = _zeros(inner, xn.device) if mult is not None and ctx.needs_input_grad[16] else None
+            lib.call('b200_glu_bwd', lib.make_args('b200_glu_bwd_args', dh=dh, ug=ug, dug=dug, db_packed=db1p, mult=mult, d_mult=d_mult, T=T,
+                                                   inner=inner, act=int(act), dropout_p=float(dropout_p), seed=int(seed),
+                                                   seed_dev=seed_dev), _stream())
         dx = gemm(dug, w1pack, T, Din, 2 * inner, b_mn=True)
         dW1p = grad_weight(dug, xn, T, 2 * inner, Din)
         nb = inner // 64
         dW1 = dW1p.view(nb, 2, 64, Din).transpose(0, 1).reshape(2 * inner, Din)   # undo the GEGLU interleave (layout only)
         db1 = db1p.view(nb, 2, 64).transpose(0, 1).reshape(2 * inner)
-        return dx, dW1, db1, dW2, db2, None, None, None, d_cs, None, None, None, None, None, (dy if has_resid else None)
+        return dx, dW1, db1, dW2, db2, None, None, None, d_cs, None, None, None, None, None, (dy if has_resid else None), None, d_mult
 
 
 # ---------------------------------------------------------------------------------------------------- cross-stream GEMMs

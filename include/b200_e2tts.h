@@ -46,8 +46,11 @@ uint64_t b200_launch_count(void);
  * Epilogue (applied in this order, each optional):
  *   + bias[n] (fp32)   * colscale[(m / rows_per_batch), n] (fp32, AdaLNZero gate :346-351)
  *   zero rows where rowmask[m]==0 (A.4 step 6)   + resid[m,n] (bf16)
- *   geglu=1: B rows are packed [u(64) | gate(64)] per 128-column tile (b200_pack_weight mode 2);
- *            D2[M,N] <- pre-activation (bf16), D[M,N/2] <- u * gelu_erf(gate) * dropout  (A.2)
+ *   geglu!=0: GLU (A.2); B rows are packed [u(64) | gate(64)] per 128-column tile (b200_pack_weight mode 2);
+ *            D2[M,N] <- pre-activation (bf16), D[M,N/2] <- u * act(gate) [* glu_mult] * dropout, where geglu selects act:
+ *            1 = exact erf GELU, 2 = SiLU (x-transformers swish=True), 3 = ReLU^2 (relu_squared=True); other values are refused.
+ *            glu_mult (fp32 [N/2], hidden-unit order, NULL = none): x-transformers GLU(mult_bias=True); refused without geglu.
+ *            The dropout keep set and D2 do not depend on the activation or on glu_mult.
  *   split_k>1: fp32 atomic accumulation into D (D is zeroed by the call); d_fp32 must be 1. split_k<0: the library picks the
  *            split that fills the SMs once for the tile shape it selects (weight-gradient GEMMs: few tiles, very long K).
  */
@@ -68,6 +71,7 @@ typedef struct {
     int32_t force_tile;   /* 0 = auto, 1 = 128 x 128 CTA tiles, 2 = 256 x 128 CTA tiles (two MMAs per k-step share one B tile),
                            * 3 = 128 x 256 CTA tiles (one m64n256 MMA per warpgroup and k-step); auto picks 3 for M >= 512, N >= 256 */
     const uint64_t* seed_dev;   /* optional DEVICE word added to `seed` when the kernel runs (see "dropout seeds" below); NULL = none */
+    const float* glu_mult;      /* optional GLU hidden-unit multiplier (see geglu above); NULL = none */
 } b200_gemm_args;
 int b200_gemm(const b200_gemm_args* a, b200_stream_t stream);
 
@@ -248,6 +252,18 @@ int b200_qkv_post_bwd(const b200_qkv_post_args* a, b200_stream_t stream);
  * zeroed by the caller, may be NULL) receives the bias gradient of the GLU projection in the same pass. */
 int b200_geglu_bwd(const void* dh, const void* ug, void* dug, float* db_packed, int64_t T, int32_t inner, float dropout_p, uint64_t seed,
                    const uint64_t* seed_dev, b200_stream_t stream);
+/* GLU backward of any activation of b200_gemm's GLU epilogue (A.2; b200_geglu_bwd is act = 1 with mult = NULL, bit for bit).
+ * dh bf16 [T, inner] (gradient of the GLU output h = drop(u * act(g) [* mult])), ug bf16 packed pre-activations [T, 2*inner] ->
+ * dug bf16 packed. db_packed (fp32 [2*inner], packed order, may be NULL) += column sums of the bf16 dug. mult (fp32 [inner],
+ * hidden-unit order) may be NULL; d_mult (fp32 [inner], may be NULL, needs mult) += sum over rows of drop(dh) * u * act(g).
+ * db_packed and d_mult are zeroed by the caller. act: 1 GELU, 2 SiLU, 3 ReLU^2. Dropout: the hash of the forward epilogue. */
+typedef struct {
+    const void* dh; const void* ug; void* dug; float* db_packed;
+    const float* mult; float* d_mult;
+    int64_t T; int32_t inner; int32_t act;
+    float dropout_p; uint64_t seed; const uint64_t* seed_dev;
+} b200_glu_bwd_args;
+int b200_glu_bwd(const b200_glu_bwd_args* a, b200_stream_t stream);
 /* out[n] += sum_t X[t,n] (bf16 X, fp32 out; caller zeroes out) — nn.Linear bias gradients. */
 int b200_colsum(const void* X, int64_t T, int32_t ncols, int32_t ld, float* out, b200_stream_t stream);
 
