@@ -462,8 +462,16 @@ class Transformer(_PackOwner):
                     f'built for; there is no fallback path (SURVEY.md §2 row 8)')
         assert heads >= 1 and text_heads >= 1, 'heads and text_heads must be >= 1'
         assert 1 <= text_depth <= depth
-        assert dim % 64 == 0 and dim_text % 64 == 0 and dim <= 1024, 'kernels need dim, dim_text multiples of 64 and dim <= 1024'
-        assert int(dim * ff_mult) % 64 == 0 and int(dim_text * text_ff_mult) % 64 == 0
+        for name, width, line in (('dim', dim, ':523'), ('dim_text', dim_text, ':524, :566')):
+            if width % 64 or width > 1024:
+                raise NotImplementedError(
+                    f'{name}={width!r} (e2_tts.py{line}): the kernels take model widths that are multiples of 64 up to 1024; there is no '
+                    f'fallback path (SURVEY.md §2 row 8)')
+        for name, width, mult, line in (('ff_mult', dim, ff_mult, ':646'), ('text_ff_mult', dim_text, text_ff_mult, ':692')):
+            if int(width * mult) % 64:
+                raise NotImplementedError(
+                    f'{name}={mult!r} (e2_tts.py{line}): the feed-forward inner width int({width} * {mult!r}) = {int(width * mult)} is not a '
+                    f'multiple of 64; the GLU kernels pack the hidden units in 64-column halves; there is no fallback path (SURVEY.md §2 row 8)')
 
         self.max_seq_len = max_seq_len
         self.abs_pos_emb = nn.Embedding(max_seq_len, dim) if abs_pos_emb else None

@@ -45,10 +45,12 @@ class TransformerCfg:
     depth: int = 8
     heads: int = 8
     dim_head: int = 64
-    ff_mult: int = 4
+    ff_mult: float = 4
+    text_ff_mult: float | None = None
     dim_text: int | None = None
     text_depth: int | None = None
     cond_on_time: bool = True
+    abs_pos_emb: bool = True
     kernel_size: int = 31
     num_registers: int = 32
     num_residual_streams: int = 4
@@ -56,7 +58,9 @@ class TransformerCfg:
 
     def __post_init__(self):
         self.dim_text = self.dim_text or self.dim // 2  # :566
+        self.text_ff_mult = self.text_ff_mult or self.ff_mult  # :571 (feedforward reads its width from the weights)
         self.text_depth = self.text_depth or self.depth  # :572
+        assert 1 <= self.text_depth <= self.depth  # :574
 
 
 # --------------------------------------------------------------------------------------------------
@@ -218,7 +222,8 @@ def transformer_forward(sd, cfg: TransformerCfg, x, times=None, mask=None, text_
     dev = x.device
     assert (times is not None) == cfg.cond_on_time  # :756
 
-    x = x + sd[P + '.abs_pos_emb.weight'][:n]  # :760-763
+    if cfg.abs_pos_emb:  # :760-763
+        x = x + sd[P + '.abs_pos_emb.weight'][:n]
     x = torch.cat((sd[P + '.registers'][None].expand(b, -1, -1), x), dim=1)  # :767-768
     if mask is not None:
         mask = F.pad(mask, (R, 0), value=True)  # :771

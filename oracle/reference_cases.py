@@ -75,7 +75,7 @@ def grad_record(grads):
             rec[k] = None
             continue
         g = g.detach().double().flatten()
-        rec[k] = dict(max=float(g.abs().max()), norm=float(g.norm()), values=g[sample_index(g.numel())].float())
+        rec[k] = dict(max=float(g.abs().max()) if g.numel() else 0.0, norm=float(g.norm()), values=g[sample_index(g.numel())].float())
     return rec
 
 

@@ -21,7 +21,8 @@ def check(name, got, want, tol):
     assert e < tol, f'{name}: rel-L2 {e:.4g} >= {tol}'
 
 
-def whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, model_kw=None, e2tts_kw=None):
+def whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, model_kw=None, e2tts_kw=None, drop_text_cond=False, dyn_scale=0.05,
+                grads=True):
     torch.manual_seed(seed)
     random.seed(seed)   # the hyper-connections draw their initial stream with python's randrange: the same case on every run
     model = pkg.E2TTS(transformer=dict(dropout=0., max_seq_len=N, **tkw, **(model_kw or {})), use_vocos=False, **(e2tts_kw or {}))
@@ -29,28 +30,29 @@ def whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, model_kw=None, e2tts_
     # stack amplifies bf16 rounding of the residual streams ~10x — the fp32 oracle with its OWN stage outputs rounded to bf16
     # (O.STAGE_ROUND) then moves its prediction by 12.6 %, exactly what the kernels showed. The probe below
     # keeps this test honest: the case must be well conditioned for a bf16 path before the kernels are held to 3e-2.
-    sd = O.randomize_zero_init({k: v.clone() for k, v in model.state_dict().items()}, seed=seed + 1, dyn_scale=0.05)
+    sd = O.randomize_zero_init({k: v.clone() for k, v in model.state_dict().items()}, seed=seed + 1, dyn_scale=dyn_scale)
     model.load_state_dict(sd)
     model.to(dev()).train()
     mel = torch.randn(B, N, 100)
-    text = ['Hello', 'Goodbye'][:B]
+    text = ['Hello', 'Goodbye', 'Good day'][:B]
     x0, times = torch.randn(B, N, 100), torch.rand(B)
     lens_t = torch.tensor(lens)
     span = torch.zeros(B, N, dtype=torch.bool)
     for b in range(B):
         span[b, lens[b] // 8: lens[b] - lens[b] // 10] = True
-    with pkg.inject_randomness(x0=x0.to(dev()), times=times.to(dev()), span_mask=span.to(dev()), drop_text_cond=False):
+    with pkg.inject_randomness(x0=x0.to(dev()), times=times.to(dev()), span_mask=span.to(dev()), drop_text_cond=drop_text_cond):
         out = model(mel.to(dev()), text=text, lens=lens_t.to(dev()))
     out.loss.backward()
     torch.cuda.synchronize()
     # oracle on the host (fp32, all cores)
     osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    ref = O.e2tts_forward(osd, O.TransformerCfg(**tkw), mel, O.list_str_to_tensor(text), x0=x0, times=times, span_mask=span, lens=lens_t)
+    kw = dict(x0=x0, times=times, span_mask=span, lens=lens_t, drop_text_cond=drop_text_cond)
+    ref = O.e2tts_forward(osd, O.TransformerCfg(**tkw), mel, O.list_str_to_tensor(text), **kw)
     ref['loss'].backward()
     O.STAGE_ROUND = O.bf16_ste
     try:
         with torch.no_grad():
-            probe = O.e2tts_forward(sd, O.TransformerCfg(**tkw), mel, O.list_str_to_tensor(text), x0=x0, times=times, span_mask=span, lens=lens_t)
+            probe = O.e2tts_forward(sd, O.TransformerCfg(**tkw), mel, O.list_str_to_tensor(text), **kw)
     finally:
         O.STAGE_ROUND = None
     e_probe = rel_l2(probe['pred'], ref['pred'].detach())
@@ -59,6 +61,8 @@ def whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, model_kw=None, e2tts_
     assert abs(loss - rloss) <= 1e-2 * abs(rloss), (loss, rloss)
     check('pred', out.pred_flow, ref['pred'].detach(), tol_pred)
     print(f'pred rel-L2 {rel_l2(out.pred_flow.float().cpu(), ref["pred"].detach()):.4g} (bf16-stage oracle probe {e_probe:.4g})')
+    if not grads:   # a case whose gradients are ill-conditioned for any bf16 path: loss and prediction only
+        return dict(probe=e_probe, worst_cos=None)
     total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())
     worst = (1.0, None)
     for k, p in model.named_parameters():
@@ -73,6 +77,7 @@ def whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, model_kw=None, e2tts_
         worst = min(worst, (cs_, k))
         assert cs_ >= 0.99, (k, cs_)
     print(f'whole model {tkw}: loss {loss:.5f} (oracle {rloss:.5f}), worst grad cosine {worst}')
+    return dict(probe=e_probe, worst_cos=worst)
 
 
 def small_model(pkg, seed, cls='E2TTS', **transformer_kw):
@@ -101,6 +106,9 @@ def check_grads(sd, rec, rel=2e-4, floor=1e-7):
             continue
         assert got is not None, k
         g = got.detach().double().flatten()
+        if r['values'].numel() == 0:    # an empty parameter (Transformer(num_registers=0).registers)
+            assert g.numel() == 0, k
+            continue
         tol = rel * r['max'] + floor
         assert float((g[RC.sample_index(g.numel())] - r['values'].double()).abs().max()) <= tol, k
         assert abs(float(g.abs().max()) - r['max']) <= tol, k

@@ -112,6 +112,11 @@ DW_CASES = [
     ('cfg2-audio', 16, 1056, 512, 31, 'model', 1.0, False, True, (1, 1, 32, 32)),
     ('cfg2-text', 16, 1056, 256, 31, 'model', 1.0, False, True, (1, 1, 32, 32)),
     ('cfg3', 4, 2080, 1024, 31, 'model', 1.0, False, True, (1, 1, 32, 32)),
+    # model widths off the powers of two (3, 6, 12 channel tiles) with the short kernels of Transformer(kernel_size=...)
+    ('d192-k7', 2, 300, 192, 7, ['holes', 250], 1.0, False, False, (1, 1, 44, 32)),
+    ('d384-k1-model', 2, 1056, 384, 1, 'model', 1.0, False, False, (1, 1, 32, 32)),
+    ('d768-k7', 3, 130, 768, 7, [100, 'holes', 'all'], 1.0, False, False, (1, 3, 2, 32)),
+    ('d768-k1', 2, 65, 768, 1, [64, 'holes'], 1.0, False, False, (2, 2, 1, 32)),
 ]
 
 

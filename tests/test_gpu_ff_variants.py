@@ -97,6 +97,7 @@ GLU_SHAPES = [
     (1096, 512, 320),     # M tail, K tail
     (1096, 512, 192),
     (100, 256, 200),      # fewer rows than one tile
+    (2112, 640, 128),     # a text FF-in of dim_text 128, text_ff_mult 2.5: inner 320, an odd number of 64-wide halves
 ]
 
 
@@ -124,14 +125,20 @@ def test_glu_gemm(pkg, M, N, K, act):
 
 
 @pytest.mark.parametrize('force_tile', [0, 1, 2, 3])
-def test_glu_gemm_every_force_tile(pkg, force_tile):
-    M, N, K = 1096, 768, 320
+def test_glu_gemm_every_force_tile(pkg, force_tile, N=768):
+    M, K = 1096, 320
     A, W = operands(M, N, K, 90 + force_tile)
     g = torch.Generator(device=dev()).manual_seed(91)
     bias, mult = torch.randn(N, device=dev(), generator=g) * 0.3, 1 + 0.5 * torch.randn(N // 2, device=dev(), generator=g)
     for act in ACTS:
         D2, out = glu_gemm(pkg, A, W, act, bias=bias, mult=mult, p=0.25, seed=77, force_tile=force_tile)
-        check_glu(f'{ACTS[act]} tile {force_tile}', act, D2, out, mult, 0.25, 77)
+        check_glu(f'{ACTS[act]} N{N} tile {force_tile}', act, D2, out, mult, 0.25, 77)
+
+
+@pytest.mark.parametrize('force_tile', [0, 1, 2, 3])
+def test_glu_gemm_every_force_tile_inner320(pkg, force_tile):
+    """inner 320 (N = 640): five [u(64) | g(64)] blocks, so a 256-wide tile row ends on half a tile"""
+    test_glu_gemm_every_force_tile(pkg, force_tile, N=640)
 
 
 def regime_operands(gate_bias):
@@ -220,7 +227,7 @@ def bwd_refs(act, dh, ug, mult, p, seed):
 
 
 @pytest.mark.parametrize('act', list(ACTS), ids=list(ACTS.values()))
-@pytest.mark.parametrize('T,inner', [(1, 64), (257, 2048), (1056, 512)])
+@pytest.mark.parametrize('T,inner', [(1, 64), (257, 2048), (1056, 512), (33, 320), (1056, 320)])
 def test_glu_bwd(pkg, act, T, inner):
     g = gen(inner + T + act)
     nb = inner // 64

@@ -142,10 +142,9 @@ def test_small_linear(pkg, B, K, xpath, dxpath):
 
 
 @pytest.mark.parametrize('B', [4, 32])
-def test_small_linear_seg_major_gains(pkg, B):
+def test_small_linear_seg_major_gains(pkg, B, d=512, L=18):
     """the batched gain projection of a deep d = 512 stack: act 5, seg = d, seg-major output, N = 4 L d; large enough that a warp
     computes several outputs and the dX slab is the full 256 features"""
-    d, L = 512, 18
     N = 4 * L * d
     npw, slab = _sl_launch(N, torch.cuda.get_device_properties(0).multi_processor_count)
     assert npw > 1 and slab == SL_SLAB
@@ -154,6 +153,12 @@ def test_small_linear_seg_major_gains(pkg, B):
     W = torch.randn(N, d, generator=g) * (4 / math.sqrt(d))
     bias = torch.randn(N, generator=g)
     _check_small_linear(pkg.ops, X, W, bias, 5, seg=d, seg_major=True, seed=B, tag='gains ')
+
+
+@pytest.mark.parametrize('B', [2, 16])
+def test_small_linear_seg_major_gains_depth24_d1024(pkg, B):
+    """the same projection at the width and depth of the d1024 depth-24 models: N = 4 * 24 * 1024 = 98 304 gains"""
+    test_small_linear_seg_major_gains(pkg, B, d=1024, L=24)
 
 
 def test_small_linear_duration_head(pkg):
@@ -494,10 +499,11 @@ def test_interp_text_packed_operand(pkg):
 # ---------------------------------------------------------------------------------------------------------------------- final norm
 @pytest.mark.parametrize('S', [1, 4])
 @pytest.mark.parametrize('R', [0, 32])
-@pytest.mark.parametrize('D', [128, 264, 512, 1024])
+@pytest.mark.parametrize('D', [128, 264, 512, 1024, 192, 384, 640, 768, 896])
 def test_final_norm(pkg, D, R, S):
     """ops.FinalNorm against O.rmsnorm(xres[:, R:].sum(2), g): all three per-thread widths (D <= 256, <= 512, <= 1024) and
-    D = 264, whose 33 chunks leave most lanes of a warp's second pass idle. Register rows of d_xres are exactly 0.
+    D = 264, whose 33 chunks leave most lanes of a warp's second pass idle; D = 192, 384, 640, 768, 896 (24, 48, 80, 96, 112 chunks):
+    model widths that leave lanes of the last pass of their width idle. Register rows of d_xres are exactly 0.
     x = the fp32 sum of S bf16 streams, within dx = gamma(S - 1) sum|streams|. cn = sqrt(D) / ||x||: the D squares and their sum
     carry gamma(D + 1) of ||x||^2 (half of it for ||x||), sqrtf(D), sqrtf and the division 3u, and dx moves ||x|| by ||dx|| (rc)."""
     g = gen(D * 10 + R + S)
@@ -675,7 +681,7 @@ def test_colsum(pkg, ncols, ld, cl, T):
 
 # ---------------------------------------------------------------------------------------------------------------------- GEGLU backward
 @pytest.mark.parametrize('T', [1, 257])
-@pytest.mark.parametrize('inner', [64, 2048])
+@pytest.mark.parametrize('inner', [64, 2048, 320])
 def test_geglu_bwd(pkg, inner, T):
     """b200_geglu_bwd (dropout 0) against float64 autograd of u * gelu(g) with the exact erf GELU, on the packed [u(64) | g(64)]
     layout; the packed bias gradient is the column sum of what the kernel wrote (the bf16 values the weight GEMM reads).

@@ -78,7 +78,9 @@ def bn_check(name, x, gain_rows, dy, d_res, y, dx, acc, acc0, rpb):
 
 # D, batches, rows per batch: every per-thread width, a batch that is not a multiple of the block's rows, a batch of one block
 # row, and a cfg2 row count (T = 2 x 1056)
-BN_CASES = [(128, 3, 37), (256, 2, 1056), (512, 4, 150), (1024, 3, 77), (512, 1, 8), (264, 2, 45)]
+# D = 192, 384, 640, 768, 896: model widths off the powers of two, whose last 16-byte-chunk pass leaves lanes of the warp idle
+BN_CASES = [(128, 3, 37), (256, 2, 1056), (512, 4, 150), (1024, 3, 77), (512, 1, 8), (264, 2, 45),
+            (192, 2, 99), (384, 3, 50), (640, 2, 45), (768, 2, 1056), (896, 1, 77)]
 
 
 @pytest.mark.parametrize('gain_mode', ['g', 'gains'])
