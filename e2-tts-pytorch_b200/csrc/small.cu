@@ -530,12 +530,27 @@ __global__ void __launch_bounds__(256) cfg_apply_kernel(const float* pred, const
 }
 
 // ------------------------------------------------------------------------------------------------ MelSpec
-// torchaudio MelSpectrogram(n_fft = win, hop, center/reflect, power 1, HTK fb) -> log(clamp(., 1e-5)) (e2_tts.py:248-290).
-// One block per (frame, batch): the windowed frame goes through an in-place radix-2 FFT in shared memory (bit-reversed load,
-// log2(n_fft) butterfly stages, one smem twiddle table per block), magnitudes of the n_fft/2+1 bins, then the mel filterbank
-// restricted to each filter's non-zero band (HTK triangles: 1 008 of the 51 300 entries of the reference's 513 x 100 matrix are
-// non-zero; the bands are found once per call by mel_bands_kernel), log. Output [B, n_mels, frames] like the reference.
+// torchaudio MelSpectrogram -> log(clamp(., 1e-5)) (e2_tts.py:248-290), with the reference's mel_spec_kwargs: a periodic Hann window of
+// win_length <= n_fft taps placed at (n_fft - win_length) / 2 (torch.stft), reflect-padded (center) or valid-only framing, |X| times
+// a normalisation scale, raised to `power`. One block per (frame, batch item): the windowed frame goes through a shared-memory FFT,
+// the n_fft/2+1 bins become |X|^power, then the mel filterbank restricted to each filter's non-zero band (HTK triangles: 1 008 of
+// the 51 300 entries of the reference's 513 x 100 matrix are non-zero; the bands are found once per call by mel_bands_kernel), log.
+// Output [B, n_mels, frames] like the reference, or [B, frames, n_mels].
+// Two FFTs: power-of-two n_fft keeps the in-place radix-2 kernel (bit-reversed load, log2(n_fft) butterfly stages, an n_fft/2
+// twiddle table); any other 5-smooth n_fft runs a Stockham autosort FFT of radix-4/2/3/5 stages, ping-ponging between two
+// shared-memory buffers so that no digit-reversal permutation is needed (twiddle table of n_fft entries).
 // (Round 1 used a direct O(n^2) DFT and the dense filterbank: ~1 M serial FMAs per frame.)
+constexpr int MEL_MAX_STAGES = 12;   // 4096 = 4^6; the longest 5-smooth factorisation below 4096 is 3^7 (2187)
+
+struct MelParams {
+    const float* wave; const float* window; const float* fb; const int2* bands; float* out; const int* wave_lens;
+    int nw_max, n_fft, hop, n_mels, frames, out_bnd;
+    int win_off, win_len, center;
+    float power, scale;
+    int log2n;                                          // radix-2 kernel
+    int nstages; int radix[MEL_MAX_STAGES];             // Stockham kernel, in stage order
+};
+
 __global__ void mel_bands_kernel(const float* __restrict__ fb, int nbins, int n_mels, int2* __restrict__ bands) {
     const int m = blockIdx.x * blockDim.x + threadIdx.x;
     if (m >= n_mels) return;
@@ -545,29 +560,78 @@ __global__ void mel_bands_kernel(const float* __restrict__ fb, int nbins, int n_
     bands[m] = make_int2(lo, hi);   // empty filter: lo >= hi
 }
 
-__global__ void __launch_bounds__(256) melspec_kernel(const float* __restrict__ wave, const float* __restrict__ window, const float* __restrict__ fb,
-                                                       const int2* __restrict__ bands, float* __restrict__ out, int nw_max, int n_fft, int log2n,
-                                                       int hop, int n_mels, int frames, const int* __restrict__ wave_lens, int out_bnd) {
+__device__ __forceinline__ size_t mel_out_index(const MelParams& p, int b, int f, int m) {
+    return p.out_bnd ? ((size_t)b * p.frames + f) * p.n_mels + m : ((size_t)b * p.n_mels + m) * p.frames + f;
+}
+
+// ragged batch (on-device collate, trainer.py:61-82): sample b has wave_lens[b] samples and its own frame count (centred: reflect-
+// padded at ITS end, valid framing: 1 + (len - n_fft) / hop); the frames behind them are the collate's zero padding, and an item
+// too short for any frame (len <= n_fft/2 centred, len < n_fft otherwise) is all zeros. Returns the item's length, or -1 after
+// writing frame f's zero row.
+__device__ __forceinline__ int mel_frame_len(const MelParams& p, int f, int b) {
+    const int nw = p.wave_lens ? min(__ldg(p.wave_lens + b), p.nw_max) : p.nw_max;
+    if (p.wave_lens) {
+        const int pad = p.center ? p.n_fft / 2 : 0;
+        if (nw <= pad || nw + 2 * pad < p.n_fft || f >= 1 + (nw + 2 * pad - p.n_fft) / p.hop) {
+            if (p.out_bnd) {           // one contiguous row
+                float* row = p.out + ((size_t)b * p.frames + f) * p.n_mels;
+                for (int m = threadIdx.x; m < p.n_mels; m += 256) row[m] = 0.f;
+            } else {
+                for (int m = threadIdx.x; m < p.n_mels; m += 256) p.out[((size_t)b * p.n_mels + m) * p.frames + f] = 0.f;
+            }
+            return -1;
+        }
+    }
+    return nw;
+}
+
+// sample n of frame f times its window tap (0 outside the window's win_len taps at win_off). PLAIN: the defaults (win_len = n_fft,
+// center, power 1, scale 1) compiled without the switches, so the default path runs the instructions it always ran.
+template <bool PLAIN>
+__device__ __forceinline__ float mel_sample(const MelParams& p, int b, int nw, int f, int n) {
+    const unsigned t = (unsigned)(n - p.win_off);
+    if (!PLAIN && t >= (unsigned)p.win_len) return 0.f;
+    int j = f * p.hop + n;
+    if (PLAIN || p.center) {                   // reflect padding by n_fft/2
+        j -= p.n_fft / 2;
+        if (j < 0) j = -j;
+        if (j >= nw) j = 2 * (nw - 1) - j;
+    }
+    return __ldg(p.wave + (size_t)b * p.nw_max + j) * __ldg(p.window + t);   // read-only path: the struct carries no __restrict__
+}
+
+// |X_k| * scale raised to the power, then the band-limited filterbank and the log
+template <bool PLAIN>
+__device__ __forceinline__ void mel_finish(const MelParams& p, const float2* z, float* mag, int b, int f) {
+    const int nbins = p.n_fft / 2 + 1;
+    for (int k = threadIdx.x; k < nbins; k += 256) {
+        const float a = sqrtf(z[k].x * z[k].x + z[k].y * z[k].y);
+        if (PLAIN) { mag[k] = a; continue; }
+        const float m = a * p.scale;
+        mag[k] = p.power == 1.f ? m : (p.power == 2.f ? m * m : powf(m, p.power));
+    }
+    __syncthreads();
+    for (int m = threadIdx.x; m < p.n_mels; m += 256) {
+        const int2 bd = __ldg(p.bands + m);
+        float acc = 0.f;
+        for (int k = bd.x; k < bd.y; ++k) acc += mag[k] * __ldg(p.fb + (size_t)k * p.n_mels + m);
+        p.out[mel_out_index(p, b, f, m)] = logf(fmaxf(acc, 1e-5f));
+    }
+}
+
+template <bool PLAIN>
+__global__ void __launch_bounds__(256) melspec_kernel(const MelParams p) {
     extern __shared__ float2 zsm[];
+    const int n_fft = p.n_fft, log2n = p.log2n;
     float2* z = zsm;                 // [n_fft] in-place FFT buffer
     float2* tw = z + n_fft;          // [n_fft/2] twiddles e^{-2 pi i k / n_fft}
     float* mag = reinterpret_cast<float*>(tw + n_fft / 2);   // [n_fft/2 + 1]
     const int f = blockIdx.x, b = blockIdx.y;
-    const int pad = n_fft / 2, nbins = n_fft / 2 + 1;
-    // ragged batch (on-device collate, trainer.py:61-82): sample b has wave_lens[b] samples -> 1 + len/hop frames, reflect-padded at ITS
-    // end; the frames behind them are the collate's zero padding
-    const int nw = wave_lens ? min(wave_lens[b], nw_max) : nw_max;
-    if (wave_lens && (f >= 1 + nw / hop || nw <= pad)) {
-        for (int m = threadIdx.x; m < n_mels; m += 256)
-            out[out_bnd ? ((size_t)b * frames + f) * n_mels + m : ((size_t)b * n_mels + m) * frames + f] = 0.f;
-        return;
-    }
+    const int nw = mel_frame_len(p, f, b);
+    if (nw < 0) return;
     for (int n = threadIdx.x; n < n_fft; n += 256) {
-        int j = f * hop + n - pad;               // center=True, reflect padding
-        if (j < 0) j = -j;
-        if (j >= nw) j = 2 * (nw - 1) - j;
         const int r = (int)(__brev((unsigned)n) >> (32 - log2n));
-        z[r] = make_float2(wave[(size_t)b * nw_max + j] * window[n], 0.f);
+        z[r] = make_float2(mel_sample<PLAIN>(p, b, nw, f, n), 0.f);
         if (n < n_fft / 2) {
             float sn, cs;
             sincospif(-2.f * (float)n / (float)n_fft, &sn, &cs);
@@ -587,14 +651,92 @@ __global__ void __launch_bounds__(256) melspec_kernel(const float* __restrict__ 
         }
         __syncthreads();
     }
-    for (int k = threadIdx.x; k < nbins; k += 256) mag[k] = sqrtf(z[k].x * z[k].x + z[k].y * z[k].y);   // power = 1
-    __syncthreads();
-    for (int m = threadIdx.x; m < n_mels; m += 256) {
-        const int2 bd = bands[m];
-        float acc = 0.f;
-        for (int k = bd.x; k < bd.y; ++k) acc += mag[k] * __ldg(fb + (size_t)k * n_mels + m);
-        out[out_bnd ? ((size_t)b * frames + f) * n_mels + m : ((size_t)b * n_mels + m) * frames + f] = logf(fmaxf(acc, 1e-5f));
+    mel_finish<PLAIN>(p, z, mag, b, f);
+}
+
+// forward DFT of R points in registers, e^{-2 pi i q r / R}
+__device__ __forceinline__ float2 c_add(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float2 c_sub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
+__device__ __forceinline__ float2 c_mul(float2 a, float2 w) { return make_float2(a.x * w.x - a.y * w.y, a.x * w.y + a.y * w.x); }
+__device__ __forceinline__ float2 c_mul_mi(float2 a) { return make_float2(a.y, -a.x); }   // -i a, exact
+template <int R> __device__ __forceinline__ void dft_small(float2* v);
+template <> __device__ __forceinline__ void dft_small<2>(float2* v) {
+    const float2 a = v[0], b = v[1];
+    v[0] = c_add(a, b); v[1] = c_sub(a, b);
+}
+template <> __device__ __forceinline__ void dft_small<4>(float2* v) {
+    const float2 t0 = c_add(v[0], v[2]), t1 = c_sub(v[0], v[2]), t2 = c_add(v[1], v[3]), t3 = c_mul_mi(c_sub(v[1], v[3]));
+    v[0] = c_add(t0, t2); v[2] = c_sub(t0, t2); v[1] = c_add(t1, t3); v[3] = c_sub(t1, t3);
+}
+template <> __device__ __forceinline__ void dft_small<3>(float2* v) {
+    constexpr float S1 = 0.866025403784438647f;   // sin(2 pi / 3)
+    const float2 s = c_add(v[1], v[2]), d = c_sub(v[1], v[2]);
+    const float2 t = make_float2(v[0].x - 0.5f * s.x, v[0].y - 0.5f * s.y);
+    const float2 u = make_float2(S1 * d.y, -S1 * d.x);   // -i sin(2 pi / 3) (v1 - v2)
+    v[0] = c_add(v[0], s); v[1] = c_add(t, u); v[2] = c_sub(t, u);
+}
+template <> __device__ __forceinline__ void dft_small<5>(float2* v) {
+    constexpr float C1 = 0.309016994374947424f, C2 = -0.809016994374947424f;   // cos(2 pi / 5), cos(4 pi / 5)
+    constexpr float S1 = 0.951056516295153572f, S2 = 0.587785252292473129f;    // sin(2 pi / 5), sin(4 pi / 5)
+    const float2 b1 = c_add(v[1], v[4]), b2 = c_add(v[2], v[3]), d1 = c_sub(v[1], v[4]), d2 = c_sub(v[2], v[3]);
+    const float2 t1 = make_float2(v[0].x + C1 * b1.x + C2 * b2.x, v[0].y + C1 * b1.y + C2 * b2.y);
+    const float2 t2 = make_float2(v[0].x + C2 * b1.x + C1 * b2.x, v[0].y + C2 * b1.y + C1 * b2.y);
+    const float2 u1 = c_mul_mi(make_float2(S1 * d1.x + S2 * d2.x, S1 * d1.y + S2 * d2.y));
+    const float2 u2 = c_mul_mi(make_float2(S2 * d1.x - S1 * d2.x, S2 * d1.y - S1 * d2.y));
+    v[0] = c_add(v[0], c_add(b1, b2));
+    v[1] = c_add(t1, u1); v[4] = c_sub(t1, u1); v[2] = c_add(t2, u2); v[3] = c_sub(t2, u2);
+}
+
+// one Stockham stage of radix R after Ns points of every sub-transform are done: butterfly j reads in[j + q n/R] (q < R), turns
+// input q by e^{-2 pi i q k / (Ns R)} (k = j mod Ns) and writes out[(j - k) R + k + r Ns]
+template <int R>
+__device__ __forceinline__ void stockham_stage(const float2* __restrict__ in, float2* __restrict__ out, const float2* __restrict__ tw, int n, int Ns) {
+    const int m = n / R, tstep = n / (Ns * R);
+    for (int j = threadIdx.x; j < m; j += 256) {
+        const int k = j % Ns;
+        float2 v[R];
+#pragma unroll
+        for (int q = 0; q < R; ++q) v[q] = in[j + q * m];
+#pragma unroll
+        for (int q = 1; q < R; ++q) v[q] = c_mul(v[q], tw[q * k * tstep]);
+        dft_small<R>(v);
+        const int o = (j - k) * R + k;
+#pragma unroll
+        for (int r = 0; r < R; ++r) out[o + r * Ns] = v[r];
     }
+}
+
+template <bool PLAIN>
+__global__ void __launch_bounds__(256) melspec_mixed_kernel(const MelParams p) {
+    extern __shared__ float2 zsm[];
+    const int n_fft = p.n_fft;
+    float2* z0 = zsm;                      // [2 n_fft]: Stockham ping-pong, stage s reads z0 + (s & 1) n_fft
+    float2* tw = zsm + 2 * n_fft;          // [n_fft] twiddles e^{-2 pi i k / n_fft}
+    const int f = blockIdx.x, b = blockIdx.y;
+    const int nw = mel_frame_len(p, f, b);
+    if (nw < 0) return;
+    for (int n = threadIdx.x; n < n_fft; n += 256) {
+        z0[n] = make_float2(mel_sample<PLAIN>(p, b, nw, f, n), 0.f);
+        float sn, cs;
+        sincospif(-2.f * (float)n / (float)n_fft, &sn, &cs);
+        tw[n] = make_float2(cs, sn);
+    }
+    __syncthreads();
+    int Ns = 1;
+    for (int s = 0; s < p.nstages; ++s) {
+        const float2* in = z0 + (s & 1) * n_fft;
+        float2* out = z0 + ((s & 1) ^ 1) * n_fft;
+        switch (p.radix[s]) {
+            case 4: stockham_stage<4>(in, out, tw, n_fft, Ns); break;
+            case 2: stockham_stage<2>(in, out, tw, n_fft, Ns); break;
+            case 3: stockham_stage<3>(in, out, tw, n_fft, Ns); break;
+            default: stockham_stage<5>(in, out, tw, n_fft, Ns); break;
+        }
+        Ns *= p.radix[s];
+        __syncthreads();
+    }
+    const int last = p.nstages & 1;
+    mel_finish<PLAIN>(p, z0 + last * n_fft, reinterpret_cast<float*>(z0 + (last ^ 1) * n_fft), b, f);   // |X|^p in the free buffer
 }
 
 }  // namespace b200
@@ -711,21 +853,68 @@ extern "C" int b200_cfg_combine(const float* pred, const float* null_pred, doubl
     cfg_apply_kernel<<<dim3(gx < 1 ? 1 : gx, B), 256, 0, st>>>(pred, null_pred, ws_red, out, per_sample, cfg_strength, remove_parallel, keep_parallel_frac);
     return check_launch("cfg_apply_kernel");
 }
+// n_fft = 2^a 3^b 5^c -> radices in stage order (4s first, then a leftover 2, 3s, 5s); 0 stages when n_fft is not 5-smooth
+static int mel_factor(int n, int* radix) {
+    int s = 0;
+    while (n % 4 == 0 && s < MEL_MAX_STAGES) { radix[s++] = 4; n /= 4; }
+    for (int r : {2, 3, 5})
+        while (n % r == 0 && s < MEL_MAX_STAGES) { radix[s++] = r; n /= r; }
+    return n == 1 ? s : 0;
+}
+extern "C" int b200_melspec_ex(const b200_melspec_args* a, b200_stream_t stream) {
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    B200_REQUIRE(a && a->wave && a->window && a->fb && a->out && a->ws_bands && a->B > 0 && a->B <= 65535, "melspec: bad arguments");
+    const int n_fft = a->n_fft;
+    MelParams p{};
+    p.nstages = n_fft >= 64 && n_fft <= 4096 ? mel_factor(n_fft, p.radix) : 0;
+    B200_REQUIRE(p.nstages > 0, "melspec: n_fft must be in [64, 4096] with no prime factor other than 2, 3 and 5 (got %d)", n_fft);
+    B200_REQUIRE(a->hop > 0 && a->n_mels > 0, "melspec: hop and n_mels must be positive");
+    B200_REQUIRE(a->win_length >= 1 && a->win_length <= n_fft, "melspec: win_length must be in [1, n_fft] (got %d)", a->win_length);
+    B200_REQUIRE(a->power > 0.f && a->norm_scale > 0.f, "melspec: power and norm_scale must be positive");
+    B200_REQUIRE(a->center ? a->nw > n_fft / 2 : a->nw >= n_fft,
+                 "melspec: the wave must be longer than n_fft/2 with center (reflect padding), at least n_fft long without");
+    B200_REQUIRE((reinterpret_cast<uintptr_t>(a->ws_bands) & 7) == 0, "melspec: ws_bands must be 8-byte aligned");
+    const int pad = a->center ? n_fft / 2 : 0;
+    p.wave = a->wave; p.window = a->window; p.fb = a->fb; p.bands = reinterpret_cast<const int2*>(a->ws_bands); p.out = a->out;
+    p.wave_lens = a->wave_lens;
+    p.nw_max = a->nw; p.n_fft = n_fft; p.hop = a->hop; p.n_mels = a->n_mels; p.out_bnd = a->out_bnd;
+    p.frames = 1 + (a->nw + 2 * pad - n_fft) / a->hop;
+    p.win_off = (n_fft - a->win_length) / 2; p.win_len = a->win_length; p.center = a->center ? 1 : 0;
+    p.power = a->power; p.scale = a->norm_scale;
+    while ((1 << p.log2n) < n_fft) ++p.log2n;
+    mel_bands_kernel<<<(a->n_mels + 127) / 128, 128, 0, st>>>(a->fb, n_fft / 2 + 1, a->n_mels, reinterpret_cast<int2*>(a->ws_bands));
+    if (int rc = check_launch("mel_bands_kernel")) return rc;
+    const bool plain = p.win_len == n_fft && p.center && p.power == 1.f && p.scale == 1.f;
+    const dim3 grid(p.frames, a->B);
+    if ((n_fft & (n_fft - 1)) == 0) {
+        const size_t smem = (size_t)n_fft * 8 + (size_t)(n_fft / 2) * 8 + (size_t)(n_fft / 2 + 1) * 4;   // <= 52 KB at 4096
+        static DeviceOnce once, once_p;
+        if (plain) {
+            B200_REQUIRE(set_max_smem_once(once_p, melspec_kernel<true>, 64 * 1024) == cudaSuccess, "melspec: cudaFuncSetAttribute failed");
+            melspec_kernel<true><<<grid, 256, smem, st>>>(p);
+        } else {
+            B200_REQUIRE(set_max_smem_once(once, melspec_kernel<false>, 64 * 1024) == cudaSuccess, "melspec: cudaFuncSetAttribute failed");
+            melspec_kernel<false><<<grid, 256, smem, st>>>(p);
+        }
+        return check_launch("melspec_kernel");
+    }
+    // two buffers and the twiddles: <= 97 200 B at 4050, the largest 5-smooth size, so the opt-in above 48 KB is needed (H100: 227 KB)
+    const size_t smem = (size_t)n_fft * 3 * 8;
+    static DeviceOnce once, once_p;
+    if (plain) {
+        B200_REQUIRE(set_max_smem_once(once_p, melspec_mixed_kernel<true>, 3 * 8 * 4096) == cudaSuccess, "melspec: cudaFuncSetAttribute failed");
+        melspec_mixed_kernel<true><<<grid, 256, smem, st>>>(p);
+    } else {
+        B200_REQUIRE(set_max_smem_once(once, melspec_mixed_kernel<false>, 3 * 8 * 4096) == cudaSuccess, "melspec: cudaFuncSetAttribute failed");
+        melspec_mixed_kernel<false><<<grid, 256, smem, st>>>(p);
+    }
+    return check_launch("melspec_mixed_kernel");
+}
 extern "C" int b200_melspec(const float* wave, const float* window, const float* fb, float* out, int32_t B, int32_t nw, int32_t n_fft,
                             int32_t hop, int32_t n_mels, int32_t* ws_bands, const int32_t* wave_lens, int32_t out_bnd, b200_stream_t stream) {
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    B200_REQUIRE(wave && window && fb && out && ws_bands && B > 0 && B <= 65535, "melspec: bad arguments");
-    B200_REQUIRE(n_fft >= 64 && (n_fft & (n_fft - 1)) == 0 && n_fft <= 4096 && hop > 0 && nw > n_fft / 2, "melspec: n_fft must be a power of two <= 4096 and the wave longer than n_fft/2");
-    B200_REQUIRE(n_mels > 0 && (reinterpret_cast<uintptr_t>(ws_bands) & 7) == 0, "melspec: ws_bands must be 8-byte aligned");
-    const int frames = 1 + nw / hop;
-    int log2n = 0;
-    while ((1 << log2n) < n_fft) ++log2n;
-    int2* bands = reinterpret_cast<int2*>(ws_bands);
-    mel_bands_kernel<<<(n_mels + 127) / 128, 128, 0, st>>>(fb, n_fft / 2 + 1, n_mels, bands);
-    if (int rc = check_launch("mel_bands_kernel")) return rc;
-    const size_t smem = (size_t)n_fft * 8 + (size_t)(n_fft / 2) * 8 + (size_t)(n_fft / 2 + 1) * 4;
-    static DeviceOnce once;
-    B200_REQUIRE(set_max_smem_once(once, melspec_kernel, 64 * 1024) == cudaSuccess, "melspec: cudaFuncSetAttribute failed");
-    melspec_kernel<<<dim3(frames, B), 256, smem, st>>>(wave, window, fb, bands, out, nw, n_fft, log2n, hop, n_mels, frames, wave_lens, out_bnd);
-    return check_launch("melspec_kernel");
+    b200_melspec_args a{};
+    a.wave = wave; a.window = window; a.fb = fb; a.out = out; a.B = B; a.nw = nw; a.n_fft = n_fft; a.hop = hop; a.n_mels = n_mels;
+    a.ws_bands = ws_bands; a.wave_lens = wave_lens; a.out_bnd = out_bnd;
+    a.win_length = n_fft; a.center = 1; a.power = 1.f; a.norm_scale = 1.f;
+    return b200_melspec_ex(&a, stream);
 }

@@ -785,26 +785,27 @@ class Transformer(_PackOwner):
 
 
 class _Spectrogram(Module):
-    def __init__(self, n_fft):
+    def __init__(self, win_length):
         super().__init__()
-        self.register_buffer('window', torch.hann_window(n_fft, periodic=True))
+        self.register_buffer('window', torch.hann_window(win_length, periodic=True))   # [win_length], unpadded, as torchaudio keeps it
 
 
 class _MelScale(Module):
-    def __init__(self, n_freqs, n_mels, sample_rate):
+    def __init__(self, n_freqs, n_mels, sample_rate, norm=None):
         super().__init__()
-        self.register_buffer('fb', mel_filterbank(n_freqs, n_mels, sample_rate))
+        self.register_buffer('fb', mel_filterbank(n_freqs, n_mels, sample_rate, norm=norm))
 
 
 class _MelSTFT(Module):
-    def __init__(self, n_fft, n_mels, sample_rate):
+    def __init__(self, n_fft, win_length, n_mels, sample_rate, norm=None):
         super().__init__()
-        self.spectrogram = _Spectrogram(n_fft)
-        self.mel_scale = _MelScale(n_fft // 2 + 1, n_mels, sample_rate)
+        self.spectrogram = _Spectrogram(win_length)
+        self.mel_scale = _MelScale(n_fft // 2 + 1, n_mels, sample_rate, norm)
 
 
-def mel_filterbank(n_freqs, n_mels, sample_rate, f_min=0.0, f_max=None):
-    """HTK mel filterbank, norm=None — what torchaudio.transforms.MelSpectrogram builds for the reference (:265-275)."""
+def mel_filterbank(n_freqs, n_mels, sample_rate, f_min=0.0, f_max=None, norm=None):
+    """HTK mel filterbank — what torchaudio.transforms.MelSpectrogram builds for the reference (:265-275); norm='slaney' scales
+    filter i by 2 / (f[i+2] - f[i]) (torchaudio's melscale_fbanks), still on the HTK scale."""
     f_max = f_max if f_max is not None else sample_rate / 2
     hz2mel = lambda f: 2595.0 * math.log10(1.0 + f / 700.0)
     all_freqs = torch.linspace(0, sample_rate // 2, n_freqs)
@@ -812,20 +813,62 @@ def mel_filterbank(n_freqs, n_mels, sample_rate, f_min=0.0, f_max=None):
     f_pts = 700.0 * (10 ** (m_pts / 2595.0) - 1.0)
     f_diff = f_pts[1:] - f_pts[:-1]
     slopes = f_pts[None, :] - all_freqs[:, None]
-    return torch.clamp(torch.minimum(-slopes[:, :-2] / f_diff[:-1], slopes[:, 2:] / f_diff[1:]), min=0.0)
+    fb = torch.clamp(torch.minimum(-slopes[:, :-2] / f_diff[:-1], slopes[:, 2:] / f_diff[1:]), min=0.0)
+    if norm == 'slaney':
+        fb *= (2.0 / (f_pts[2:n_mels + 2] - f_pts[:n_mels]))[None]
+    return fb
+
+
+MEL_NFFT_MIN, MEL_NFFT_MAX = 64, 4096
+
+
+def _five_smooth(n):
+    for p in (2, 3, 5):
+        while n % p == 0:
+            n //= p
+    return n == 1
 
 
 class MelSpec(Module):
+    """The reference's MelSpec (e2_tts.py:248-290) with its full signature: torchaudio's MelSpectrogram semantics for win_length
+    (a periodic Hann window of win_length <= n_fft taps, centred in the frame), center (reflect padding by n_fft // 2, or valid
+    frames only), power > 0, normalize (True / 'window': divide X by sqrt(sum(window^2)); 'frame_length': by sqrt(n_fft)) and
+    norm (None or 'slaney'), for any filter_length in [64, 4096] with no prime factor other than 2, 3 and 5."""
+
     def __init__(self, filter_length=1024, hop_length=256, win_length=1024, n_mel_channels=100, sampling_rate=24_000,
                  normalize=False, power=1, norm=None, center=True):
         super().__init__()
-        if (win_length, normalize, power, norm, center) != (filter_length, False, 1, None, True):
-            _unsupported('mel_spec_kwargs', dict(win_length=win_length, normalize=normalize, power=power, norm=norm, center=center),
-                         'e2_tts.py:249-260')
+        win_length = filter_length if win_length is None else win_length
+        if not (MEL_NFFT_MIN <= filter_length <= MEL_NFFT_MAX and _five_smooth(filter_length)):
+            _unsupported('mel_spec_kwargs[\'filter_length\']', filter_length,
+                         f'e2_tts.py:251 (the FFT kernels take n_fft in [{MEL_NFFT_MIN}, {MEL_NFFT_MAX}] with prime factors 2, 3 and 5 only)')
+        if power is None:
+            _unsupported('mel_spec_kwargs[\'power\']', power, 'e2_tts.py:257 (power=None is a complex spectrum, which the reference then takes the log of)')
+        if not power > 0:
+            raise ValueError(f'mel_spec_kwargs power must be positive (got {power!r})')
+        if not 1 <= win_length <= filter_length:
+            raise ValueError(f'mel_spec_kwargs win_length must be in [1, filter_length={filter_length}] (got {win_length}), as torch.stft requires')
+        if normalize not in (False, True, 'window', 'frame_length'):
+            raise ValueError(f"mel_spec_kwargs normalize must be a bool, 'window' or 'frame_length' (got {normalize!r})")
+        if norm not in (None, 'slaney'):
+            raise ValueError(f"mel_spec_kwargs norm must be None or 'slaney' (got {norm!r})")
         self.n_mel_channels, self.sampling_rate = n_mel_channels, sampling_rate
-        self.n_fft, self.hop = filter_length, hop_length
-        self.mel_stft = _MelSTFT(filter_length, n_mel_channels, sampling_rate)
+        self.n_fft, self.hop, self.win_length = filter_length, hop_length, win_length
+        self.center, self.power = bool(center), float(power)
+        self.mel_stft = _MelSTFT(filter_length, win_length, n_mel_channels, sampling_rate, norm)
+        window = self.mel_stft.spectrogram.window.double()
+        self.norm_scale = {False: 1.0, 'frame_length': filter_length ** -0.5}.get(normalize, float(window.square().sum().rsqrt()))
         self.register_buffer('dummy', torch.tensor(0), persistent=False)
+
+    def frames(self, n):
+        """frames of n samples (int or tensor): 1 + n // hop centred (even n_fft), 1 + (n - n_fft) // hop without centring"""
+        return ops.melspec_frames(n, self.n_fft, self.hop, self.center)
+
+    def _melspec(self, waves, **kw):
+        if waves.shape[1] < (self.n_fft // 2 + 1 if self.center else self.n_fft):
+            raise ValueError(f'MelSpec: {waves.shape[1]} samples are too few for one frame of n_fft={self.n_fft} (center={self.center})')
+        return ops.melspec(waves.to(F32).contiguous(), self.mel_stft.spectrogram.window, self.mel_stft.mel_scale.fb, self.n_fft, self.hop,
+                           center=self.center, power=self.power, norm_scale=self.norm_scale, **kw)
 
     def forward(self, inp):
         if inp.ndim == 3:
@@ -833,7 +876,7 @@ class MelSpec(Module):
         assert inp.ndim == 2
         if self.dummy.device != inp.device:
             self.to(inp.device)
-        return ops.melspec(inp.to(F32).contiguous(), self.mel_stft.spectrogram.window, self.mel_stft.mel_scale.fb, self.n_fft, self.hop)
+        return self._melspec(inp)
 
     def collate(self, waves, lens=None):
         """On-device data path (SURVEY §8f row 3): what the reference does per item on CPU workers — `MelSpec` in HFDataset.__getitem__
@@ -842,8 +885,8 @@ class MelSpec(Module):
         waves: list of 1-D fp32 tensors at `sampling_rate` (resampling is the dataset's job) or a zero-padded [B, nw_max] tensor with
         `lens` (samples per sequence). Returns dict(mel [B, n_frames_max, n_mels] fp32, mel_lengths [B] int64) — pass as
         `model(batch['mel'], text=..., lens=batch['mel_lengths'])`. A length past the padded wave counts as the padded length;
-        an item of at most n_fft/2 samples is too short for the reflect padding (the reference's MelSpec raises on it): its
-        frames are zeros and its mel_lengths entry is 0."""
+        an item too short for one frame — at most n_fft/2 samples centred (too short for the reflect padding: the reference's
+        MelSpec raises on it), fewer than n_fft without centring — has zero frames and its mel_lengths entry is 0."""
         if isinstance(waves, (list, tuple)):
             dev = self.dummy.device if self.dummy.device.type == 'cuda' else waves[0].device
             lens = torch.tensor([w.shape[-1] for w in waves], dtype=torch.int32)
@@ -858,11 +901,11 @@ class MelSpec(Module):
             lens = lens.to(device=waves.device, dtype=torch.int32)
         if self.dummy.device != waves.device:
             self.to(waves.device)
-        mel = ops.melspec(waves.to(F32).contiguous(), self.mel_stft.spectrogram.window, self.mel_stft.mel_scale.fb, self.n_fft, self.hop,
-                          wave_lens=lens.contiguous(), out_bnd=True)
+        mel = self._melspec(waves, wave_lens=lens.contiguous(), out_bnd=True)
         lens = lens.long().clamp(max=waves.shape[1])      # the kernel clamps the same way
-        mel_lengths = torch.where(lens > self.n_fft // 2, 1 + lens // self.hop, 0)
-        n_max = int(1 + waves.shape[1] // self.hop)
+        long_enough = lens > self.n_fft // 2 if self.center else lens >= self.n_fft
+        mel_lengths = torch.where(long_enough, self.frames(lens), 0)
+        n_max = int(self.frames(waves.shape[1]))
         return dict(mel=mel[:, :n_max], mel_lengths=mel_lengths)
 
 

@@ -1018,13 +1018,23 @@ def cfg_combine(pred, null_pred, strength, remove_parallel, keep_frac):
     return out
 
 
-def melspec(wave, window, fb, n_fft, hop, wave_lens=None, out_bnd=False):
+def melspec_frames(nw, n_fft, hop, center=True):
+    """frames of a wave of nw samples: reflect-padded by n_fft // 2 on both sides (center) or valid frames only (torch.stft)"""
+    pad = n_fft // 2 if center else 0
+    return 1 + (nw + 2 * pad - n_fft) // hop
+
+
+def melspec(wave, window, fb, n_fft, hop, wave_lens=None, out_bnd=False, center=True, power=1.0, norm_scale=1.0):
     """MelSpec front-end (e2_tts.py:248-290): fp32 [B, nw] -> [B, n_mels, frames] (or [B, frames, n_mels] with out_bnd); wave_lens
-    (int32 [B]) makes it the on-device collate of a zero-padded ragged batch (trainer.py:61-82)."""
+    (int32 [B]) makes it the on-device collate of a zero-padded ragged batch (trainer.py:61-82). window: the unpadded window of
+    win_length <= n_fft taps; center, power and norm_scale as b200_melspec_ex documents them."""
     B, nw = wave.shape
     n_mels = fb.shape[1]
-    frames = 1 + nw // hop
+    frames = melspec_frames(nw, n_fft, hop, center)
     out = torch.empty((B, frames, n_mels) if out_bnd else (B, n_mels, frames), device=wave.device, dtype=F32)
     bands = torch.empty(2 * n_mels, device=wave.device, dtype=torch.int32)
-    lib.call('b200_melspec', wave, _c(window), _c(fb), out, B, nw, n_fft, hop, n_mels, bands, wave_lens, int(out_bnd), _stream())
+    a = lib.make_args('b200_melspec_args', wave=wave, window=_c(window), fb=_c(fb), out=out, B=B, nw=nw, n_fft=n_fft, hop=hop,
+                      n_mels=n_mels, ws_bands=bands, wave_lens=wave_lens, out_bnd=int(out_bnd), win_length=window.shape[0],
+                      center=int(center), power=float(power), norm_scale=float(norm_scale))
+    lib.call('b200_melspec_ex', a, _stream())
     return out

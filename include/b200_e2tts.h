@@ -378,15 +378,36 @@ int b200_axpy(const float* y, const float* f, float a, float* out, int64_t n, b2
  * out = pred + (orth + par * keep) * strength per sample over all n*d elements. ws_red: 2*B doubles. */
 int b200_cfg_combine(const float* pred, const float* null_pred, double* ws_red, float* out, int32_t B, int64_t per_sample,
                      float cfg_strength, int32_t remove_parallel, float keep_parallel_frac, b200_stream_t stream);
-/* MelSpec (e2_tts.py:248-290): wave fp32 [B, nw] -> log-mel fp32 [B, n_mels, 1 + nw/hop]; window [n_fft], fb [n_fft/2+1, n_mels].
- * Shared-memory radix-2 FFT per frame + band-limited filterbank; ws_bands: caller workspace of 2 * n_mels int32 (8-byte aligned),
- * filled by the call with each filter's non-zero bin range.
+/* MelSpec (e2_tts.py:248-290, torchaudio MelSpectrogram with the reference's mel_spec_kwargs) -> log(clamp(mel, 1e-5)):
+ * wave fp32 [B, nw] -> log-mel fp32 [B, n_mels, frames]; window fp32 [win_length] (the periodic Hann window, unpadded: its taps sit
+ * at (n_fft - win_length)/2 .. of each n_fft frame, zeros elsewhere, as torch.stft pads it); fb fp32 [n_fft/2+1, n_mels] (HTK or
+ * Slaney-scaled: any filterbank works, only its non-zero band per filter is read).
+ *   center != 0: reflect-padded by n_fft/2 on both sides, frames = 1 + (nw + 2 (n_fft/2) - n_fft) / hop (= 1 + nw/hop for even
+ *                n_fft); needs nw > n_fft/2.
+ *   center == 0: valid frames only, frames = 1 + (nw - n_fft) / hop; needs nw >= n_fft.
+ *   bin k: (|X_k| * norm_scale)^power (power 1: |X_k| exactly; normalize=True / 'window': norm_scale = 1/sqrt(sum window^2);
+ *          'frame_length': 1/sqrt(n_fft); none: 1).
+ * Refused before any launch: n_fft outside [64, 4096] or with a prime factor other than 2, 3 and 5; power <= 0 (a complex spectrum,
+ * power=None, is not a log-mel); win_length outside [1, n_fft]; norm_scale <= 0. Power-of-two n_fft runs a radix-2 FFT, the others
+ * a mixed-radix (4/2/3/5) Stockham FFT, both in shared memory.
+ * ws_bands: caller workspace of 2 * n_mels int32 (8-byte aligned), filled by the call with each filter's non-zero bin range.
  * On-device collate (trainer.py:61-82 collate_fn + :101-131 HFDataset.__getitem__, SURVEY §8f row 3): wave_lens (optional int32 [B]) =
- * samples per sequence of a zero-padded ragged batch (a length past nw counts as nw) — sequence b yields 1 + wave_lens[b]/hop frames
- * (reflect-padded at its own end), the remaining frames are the collate's zero padding. A sequence of wave_lens[b] <= n_fft/2 samples
- * is too short to reflect-pad (the reference's MelSpec raises on it): all its frames are written as zeros. out_bnd != 0 writes
- * [B, frames, n_mels] (the layout E2TTS.forward consumes, trainer.py:253 rearrange 'b d n -> b n d') instead of the reference
- * MelSpec's [B, n_mels, frames]. */
+ * samples per sequence of a zero-padded ragged batch (a length past nw counts as nw) — sequence b yields the frame count above for
+ * its own length (reflect-padded at its own end when centred), the remaining frames are the collate's zero padding. A sequence
+ * too short for one frame (wave_lens[b] <= n_fft/2 centred — the reference's MelSpec raises on it — or < n_fft without centring) has
+ * all its frames written as zeros. out_bnd != 0 writes [B, frames, n_mels] (the layout E2TTS.forward consumes, trainer.py:253
+ * rearrange 'b d n -> b n d') instead of the reference MelSpec's [B, n_mels, frames]. */
+typedef struct {
+    const float *wave, *window, *fb; float* out;
+    int32_t B, nw, n_fft, hop, n_mels;
+    int32_t* ws_bands; const int32_t* wave_lens; int32_t out_bnd;
+    int32_t win_length;   /* taps of `window`, 1..n_fft */
+    int32_t center;
+    float power;          /* > 0 */
+    float norm_scale;     /* > 0; 1 = not normalised */
+} b200_melspec_args;
+int b200_melspec_ex(const b200_melspec_args* a, b200_stream_t stream);
+/* The defaults of b200_melspec_ex (win_length = n_fft, center, power 1, norm_scale 1): same code, same bits. */
 int b200_melspec(const float* wave, const float* window, const float* fb, float* out, int32_t B, int32_t nw, int32_t n_fft,
                  int32_t hop, int32_t n_mels, int32_t* ws_bands, const int32_t* wave_lens, int32_t out_bnd, b200_stream_t stream);
 
