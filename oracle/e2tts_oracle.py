@@ -38,13 +38,30 @@ import torch.nn.functional as F
 # --------------------------------------------------------------------------------------------------
 # config
 
+# x-transformers' Attention defaults for a key missing from attn_kwargs, and the reference's attn_kwargs (e2_tts.py:548-551)
+XT_DEFAULTS = dict(gate_value_heads=False, softclamp_logits=False, logit_softclamp_value=50.)
+REF_ATTN_KWARGS = dict(gate_value_heads=True, softclamp_logits=True)
+
+
+def act_of(ff_kwargs):
+    """the GLU activation of these ff_kwargs, x-transformers' precedence: relu_squared, then swish, then the exact erf GELU"""
+    if ff_kwargs.get('relu_squared'):
+        return lambda g: F.relu(g) ** 2
+    if ff_kwargs.get('swish'):
+        return F.silu
+    return F.gelu
+
 
 @dataclass
 class TransformerCfg:
+    """Transformer's keyword arguments (e2_tts.py:518-552) besides dropout / max_seq_len. A switch that is set must find its weights
+    in the state dict: a missing key is a KeyError, never "off"."""
     dim: int
     depth: int = 8
     heads: int = 8
     dim_head: int = 64
+    text_heads: int | None = None
+    text_dim_head: int | None = None
     ff_mult: float = 4
     text_ff_mult: float | None = None
     dim_text: int | None = None
@@ -54,13 +71,24 @@ class TransformerCfg:
     kernel_size: int = 31
     num_registers: int = 32
     num_residual_streams: int = 4
-    softclamp: float = 50.0
+    attn_fourier_embed_input: bool = False
+    attn_kwargs: dict | None = None    # None: the reference's REF_ATTN_KWARGS; {}: x-transformers' defaults (no gate, no clamp)
+    ff_kwargs: dict | None = None
 
     def __post_init__(self):
         self.dim_text = self.dim_text or self.dim // 2  # :566
+        self.text_heads = self.text_heads or self.heads  # :569
+        self.text_dim_head = self.text_dim_head or self.dim_head  # :570
         self.text_ff_mult = self.text_ff_mult or self.ff_mult  # :571 (feedforward reads its width from the weights)
         self.text_depth = self.text_depth or self.depth  # :572
         assert 1 <= self.text_depth <= self.depth  # :574
+        attn = {**XT_DEFAULTS, **(REF_ATTN_KWARGS if self.attn_kwargs is None else self.attn_kwargs)}
+        self.softclamp = float(attn['logit_softclamp_value']) if attn['softclamp_logits'] else None
+        # keyword arguments of the attention / feed-forward leaves, whose defaults are the reference's (head gate on; GELU, no multiplier,
+        # output bias): only a switch set away from them is passed, so the default model calls the leaves as they always were called
+        self.attn_kw = {} if attn['gate_value_heads'] else dict(gate=False)
+        ff = self.ff_kwargs or {}
+        self.ff_kw = dict(act=act_of(ff), mult_bias=bool(ff.get('glu_mult_bias')), bias=not ff.get('no_bias')) if ff else {}
 
 
 # --------------------------------------------------------------------------------------------------
@@ -146,8 +174,9 @@ def apply_rotary(t, freqs):  # A.3 on (b,h,n,dh); rotate_half on interleaved pai
     return t * freqs.cos() + rot * freqs.sin()
 
 
-def attention(sd, p, x, mask, freqs, value_residual, heads, dim_head, softclamp):
-    """A.4; returns (out, orig_values). `p` = key prefix of the Attention module."""
+def attention(sd, p, x, mask, freqs, value_residual, heads, dim_head, softclamp, gate=True):
+    """A.4; returns (out, orig_values). `p` = key prefix of the Attention module, softclamp None = no logit soft-clamp, gate = the
+    value-head gate (gate_value_heads)."""
     b, n, _ = x.shape
     split = lambda t: t.reshape(b, n, heads, dim_head).permute(0, 2, 1, 3)
     q, k, v = (split(x @ sd[p + f'.to_{c}.weight'].t()) for c in 'qkv')
@@ -158,23 +187,31 @@ def attention(sd, p, x, mask, freqs, value_residual, heads, dim_head, softclamp)
         v = v * mix + value_residual * (1.0 - mix)
     q, k = apply_rotary(q, freqs), apply_rotary(k, freqs)
     sim = torch.einsum('bhid,bhjd->bhij', q, k) * dim_head ** -0.5
-    sim = torch.tanh(sim / softclamp) * softclamp
+    if softclamp is not None:
+        sim = torch.tanh(sim / softclamp) * softclamp
     if mask is not None:
         sim = sim.masked_fill(~mask[:, None, None, :], -torch.finfo(sim.dtype).max)
     attn = drop(p + '.attn_dropout', torch.softmax(sim.float(), dim=-1).to(sim.dtype))
     out = torch.einsum('bhij,bhjd->bhid', attn, v)
-    gate = torch.sigmoid(x @ sd[p + '.to_v_head_gate.weight'].t() + sd[p + '.to_v_head_gate.bias'])
-    out = out * gate.permute(0, 2, 1)[..., None]
+    if gate:
+        g = torch.sigmoid(x @ sd[p + '.to_v_head_gate.weight'].t() + sd[p + '.to_v_head_gate.bias'])
+        out = out * g.permute(0, 2, 1)[..., None]
     out = out.permute(0, 2, 1, 3).reshape(b, n, heads * dim_head) @ sd[p + '.to_out.weight'].t()
     if mask is not None:
         out = out * mask[..., None]
     return out, orig_v
 
 
-def feedforward(sd, p, x):  # A.2 GEGLU (exact erf GELU), nn.Dropout between the GLU and the output Linear
+def feedforward(sd, p, x, act=F.gelu, mult_bias=False, bias=True):
+    """A.2 GLU with activation `act`, the optional multiplier (glu_mult_bias) and output bias (not no_bias); nn.Dropout between the GLU
+    and the output Linear"""
     h = x @ sd[p + '.ff.0.proj.weight'].t() + sd[p + '.ff.0.proj.bias']
     u, g = h.chunk(2, dim=-1)
-    return drop(p + '.ff.1', u * F.gelu(g)) @ sd[p + '.ff.2.weight'].t() + sd[p + '.ff.2.bias']
+    hid = u * act(g)
+    if mult_bias:
+        hid = hid * sd[p + '.ff.0.mult_bias']
+    y = drop(p + '.ff.1', hid) @ sd[p + '.ff.2.weight'].t()
+    return y + sd[p + '.ff.2.bias'] if bias else y
 
 
 def depthwise_conv(sd, p, x, mask):  # :312-328
@@ -189,6 +226,8 @@ def depthwise_conv(sd, p, x, mask):  # :312-328
 
 
 def hyper_width(sd, p, res, S):  # A.5 width connection on (b, n, S, d)
+    if S == 1:  # num_residual_streams=1, hyper-connections `Residual`: the stream is the branch input and the residual
+        return res[..., 0, :], res, None
     d = res.shape[-1]
     normed = F.normalize(res, dim=-1) * d ** 0.5 * (sd[p + '.norm.gamma'] + 1.0)
     alpha = torch.tanh(normed @ sd[p + '.dynamic_alpha_fn']) * sd[p + '.dynamic_alpha_scale'] + sd[p + '.static_alpha']
@@ -198,6 +237,8 @@ def hyper_width(sd, p, res, S):  # A.5 width connection on (b, n, S, d)
 
 
 def hyper_depth(rest, beta, y):  # A.5 depth connection
+    if beta is None:  # `Residual`: branch output + residual (the CUDA path adds the branch in fp32 and stores only the sum)
+        return _rs(y[..., None, :] + rest)
     return _rs(_rs(y)[..., None, :] * beta[..., None] + rest)
 
 
@@ -237,7 +278,8 @@ def transformer_forward(sd, cfg: TransformerCfg, x, times=None, mask=None, text_
         four = torch.cat((times[:, None], fr.sin(), fr.cos()), dim=-1)  # :363
         cond = F.silu(four @ sd[P + '.time_cond_mlp.1.weight'].t() + sd[P + '.time_cond_mlp.1.bias'])
 
-    freqs = rotary_freqs(npr, cfg.dim_head, dev)  # :793 (text uses the same dim_head, :798)
+    freqs = rotary_freqs(npr, cfg.dim_head, dev)  # :793
+    text_freqs = freqs if cfg.text_dim_head == cfg.dim_head else rotary_freqs(npr, cfg.text_dim_head, dev)  # :600, :798
 
     has_text = text_embed is not None
     if has_text:
@@ -258,6 +300,9 @@ def transformer_forward(sd, cfg: TransformerCfg, x, times=None, mask=None, text_
             return h * g[:, None, :]
         return h
 
+    def ff(prefix_key, h):  # FeedForward(**ff_kwargs) :646, :692
+        return feedforward(sd, prefix_key, h, **cfg.ff_kw)
+
     skips = []
     attn_first, text_attn_first = None, None
     for i in range(L):
@@ -268,12 +313,12 @@ def transformer_forward(sd, cfg: TransformerCfg, x, times=None, mask=None, text_
             br, rest, beta = hyper_width(sd, hp + '.1.0', ts, S)
             ts = hyper_depth(rest, beta, depthwise_conv(sd, tp + '.0', _rs(br), mask))
             br, rest, beta = hyper_width(sd, hp + '.1.1', ts, S)
-            out, vals = attention(sd, tp + '.2', _rs(rmsnorm(br, sd[tp + '.1.g'])), mask, freqs, text_attn_first,
-                                  cfg.heads, cfg.dim_head, cfg.softclamp)
+            out, vals = attention(sd, tp + '.2', _rs(rmsnorm(br, sd[tp + '.1.g'])), mask, text_freqs, text_attn_first,
+                                  cfg.text_heads, cfg.text_dim_head, cfg.softclamp, **cfg.attn_kw)
             ts = hyper_depth(rest, beta, out)
             text_attn_first = vals if text_attn_first is None else text_attn_first
             br, rest, beta = hyper_width(sd, hp + '.1.2', ts, S)
-            ts = hyper_depth(rest, beta, feedforward(sd, tp + '.4', _rs(rmsnorm(br, sd[tp + '.3.g']))))
+            ts = hyper_depth(rest, beta, ff(tp + '.4', _rs(rmsnorm(br, sd[tp + '.3.g']))))
             at = torch.cat((xs, ts), dim=-1)  # :508-513 on every stream
             xs_new = _rs(xs + at @ sd[tp + '.5.text_to_audio.weight'].t())
             if (tp + '.5.audio_to_text.weight') in sd:
@@ -290,14 +335,15 @@ def transformer_forward(sd, cfg: TransformerCfg, x, times=None, mask=None, text_
         xs = hyper_depth(rest, beta, depthwise_conv(sd, sp + '.1', _rs(br), mask))
         br, rest, beta = hyper_width(sd, hp + '.0.1', xs, S)  # :906-916
         a_in = norm(sp + '.2', br)
-        if (sp + '.4.linear.weight') in sd:  # attn_input_fourier_embed :909 (Transformer(attn_fourier_embed_input=True), :545-546, :639)
+        # attn_input_fourier_embed :909 (:545-546, :639); its weights in the state dict turn it on as well, like the E2TTS-level switches
+        if cfg.attn_fourier_embed_input or (sp + '.4.linear.weight') in sd:
             a_in = linear_fourier_embed(sd, sp + '.4', a_in)
         out, vals = attention(sd, sp + '.3', a_in, mask, freqs, attn_first,
-                              cfg.heads, cfg.dim_head, cfg.softclamp)
+                              cfg.heads, cfg.dim_head, cfg.softclamp, **cfg.attn_kw)
         xs = hyper_depth(rest, beta, post(sp + '.5', out))
         attn_first = vals if attn_first is None else attn_first
         br, rest, beta = hyper_width(sd, hp + '.0.2', xs, S)  # :936-939
-        xs = hyper_depth(rest, beta, post(sp + '.8', feedforward(sd, sp + '.7', norm(sp + '.6', br))))
+        xs = hyper_depth(rest, beta, post(sp + '.8', ff(sp + '.7', norm(sp + '.6', br))))
 
     assert not skips
     out = xs[:, R:].sum(dim=2)  # :943-947 drop registers, reduce streams
@@ -489,7 +535,9 @@ def randomize_zero_init(sd, seed=1234, scale=0.05, dyn_scale=0.5):
     vacuous. This perturbs every all-zero float tensor (and the constant gate biases) in place,
     deterministically, and returns sd. dyn_scale = value of the hyper-connections' dynamic_alpha/beta_scale (reference init
     0.01): 0.5 makes the stream mixing strongly input dependent, which is what a 2-layer fixture wants, but across 8 layers it
-    amplifies bf16 rounding of the residual streams ~10x (the fp32 oracle with STAGE_ROUND moves its own prediction by 12 %)."""
+    amplifies bf16 rounding of the residual streams ~10x (the fp32 oracle with STAGE_ROUND moves its own prediction by 12 %).
+    The GLU multipliers (ff_kwargs glu_mult_bias, initialised to ones, which the loop leaves alone and which are invisible at 1) are
+    drawn afterwards from a generator of their own, so the weights of a model without them do not depend on their presence."""
     g = torch.Generator().manual_seed(seed)
     for k in sorted(sd.keys()):
         v = sd[k]
@@ -503,4 +551,8 @@ def randomize_zero_init(sd, seed=1234, scale=0.05, dyn_scale=0.5):
             v.copy_(torch.randn(v.shape, generator=g) * scale)
         elif k.endswith('dynamic_alpha_scale') or k.endswith('dynamic_beta_scale'):
             v.fill_(dyn_scale)
+    g = torch.Generator().manual_seed(seed + 500)
+    for k in sorted(sd.keys()):
+        if k.endswith('.ff.0.mult_bias'):
+            sd[k].copy_(1.0 + 0.5 * torch.randn(sd[k].shape, generator=g))
     return sd

@@ -3,10 +3,9 @@ text_depth < depth, dim_text != dim // 2, ff_mult / text_ff_mult != 4 (one of th
 abs_pos_emb=False and kernel_size != 31, stored from the original e2_tts.py by tools/make_geometry_golden.py. Shared by
 tests/test_geometry_vs_reference.py (oracle against the original's stored outputs) and tests/test_gpu_geometry.py.
 
-Every knob is a field of the oracle's TransformerCfg, so `cfg(tkw)` is the whole oracle configuration of a case. `knobs` names the
-knobs a case's negative control reverts, one at a time, to the reference's default (test_geometry_vs_reference.py): the oracle must
-then miss the stored outputs."""
-from oracle import e2tts_oracle as O
+Every knob is a field of the oracle's TransformerCfg, so TransformerCfg(**tkw) is the whole oracle configuration of a case. `knobs`
+names the knobs a case's negative control reverts, one at a time, to the reference's default (test_geometry_vs_reference.py): the
+oracle must then miss the stored outputs."""
 from oracle import reference_cases as RC
 
 # the reference's defaults of the knobs (e2_tts.py:524-541); dim_text, text_ff_mult and text_depth follow dim, ff_mult and depth
@@ -41,11 +40,6 @@ for _c in GEOMETRY_CASES.values():
 # text, duration, steps, cfg_strength; y0 = first draw of generator 3000 + seed
 GEOMETRY_SAMPLE = dict(seed=107, tkw=dict(dim=128, depth=4, heads=2, text_depth=2, num_registers=8, kernel_size=5), cond=(2, 20),
                        lens=[20, 13], text=['Hello', 'Goodbye then'], duration=[40, 33], steps=4, cfg_strength=1.0)
-
-
-def cfg(tkw, **kw):
-    """oracle configuration of transformer kwargs `tkw`"""
-    return O.TransformerCfg(**tkw, **kw)
 
 
 def reverted(c, knob):

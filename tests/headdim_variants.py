@@ -3,15 +3,8 @@
 tools/make_headdim_golden.py. Shared by tests/test_headdim_vs_reference.py (oracle against the original's stored outputs) and the
 GPU tests of the same geometry.
 
-The oracle of oracle/e2tts_oracle.py gives both streams the audio stream's heads, head dim and rotary table (the reference's defaults,
-e2_tts.py:569-570). `headdim_oracle(tkw)` runs it, for the duration of a `with` block, with the text attention of `tkw` — its own
-text_heads, text_dim_head and RotaryEmbedding(text_dim_head) (:600, :798, :875) — and with what a case adds besides the geometry
-(num_residual_streams=1, attn_kwargs); `cfg(tkw)` is the oracle configuration of the rest."""
-import contextlib
-
-from oracle import e2tts_oracle as O
-from attn_variants import variant_oracle
-from residual_variants import plain_residual_oracle
+The oracle takes the same kwargs as configuration (oracle/e2tts_oracle.py TransformerCfg: text_heads, text_dim_head and the text
+stream's own RotaryEmbedding(text_dim_head), :600, :798, :875)."""
 
 # forward + backward cases of the original: class, seed, transformer kwargs, (batch, frames), lens, text, drop_text_cond
 HEADDIM_CASES = {
@@ -37,42 +30,3 @@ for _c in HEADDIM_CASES.values():
 # generator 3000 + seed
 HEADDIM_SAMPLE = dict(seed=88, tkw=dict(dim=128, depth=2, heads=1, dim_head=128, text_heads=2, text_dim_head=64), cond=(2, 20),
                       text=['Hello', 'Goodbye then'], duration=[40, 33], steps=4, cfg_strength=1.0)
-
-
-ORACLE_EXTRA = ('attn_kwargs', 'text_heads', 'text_dim_head')   # transformer kwargs headdim_oracle applies
-
-
-def cfg(tkw, **kw):
-    """oracle configuration of transformer kwargs `tkw` (the keys of ORACLE_EXTRA are applied by headdim_oracle)"""
-    return O.TransformerCfg(**{k: v for k, v in tkw.items() if k not in ORACLE_EXTRA}, **kw)
-
-
-@contextlib.contextmanager
-def text_geometry_oracle(heads, dim_head, text_heads, text_dim_head):
-    """the oracle's text attention (key prefix `<transformer>.layers.<i>.1.2`) with its own head count, head dim and rotary table"""
-    inner = O.attention
-
-    def attention(sd, p, x, mask, freqs, value_residual, h, dh, softclamp):
-        if p.endswith('.1.2'):
-            h, dh = text_heads, text_dim_head
-            freqs = O.rotary_freqs(x.shape[1], dh, x.device)
-        return inner(sd, p, x, mask, freqs, value_residual, h, dh, softclamp)
-    O.attention = attention
-    try:
-        yield
-    finally:
-        O.attention = inner
-
-
-@contextlib.contextmanager
-def headdim_oracle(tkw):
-    """inside the block the oracle computes the backbone of transformer kwargs `tkw`: text attention geometry, plain residual and
-    attn_kwargs as given"""
-    heads, dim_head = tkw.get('heads', 8), tkw.get('dim_head', 64)
-    with contextlib.ExitStack() as stack:
-        if tkw.get('num_residual_streams', 4) == 1:
-            stack.enter_context(plain_residual_oracle())
-        if 'attn_kwargs' in tkw:
-            stack.enter_context(variant_oracle(tkw['attn_kwargs']))
-        stack.enter_context(text_geometry_oracle(heads, dim_head, tkw.get('text_heads') or heads, tkw.get('text_dim_head') or dim_head))
-        yield

@@ -6,6 +6,7 @@ import random
 import torch
 
 from conftest import rel_l2
+from dropout_ref import with_dropout
 from kernel_checks import dev
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
@@ -21,11 +22,10 @@ def check(name, got, want, tol):
     assert e < tol, f'{name}: rel-L2 {e:.4g} >= {tol}'
 
 
-def whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, model_kw=None, e2tts_kw=None, drop_text_cond=False, dyn_scale=0.05,
-                grads=True):
+def whole_model(pkg, tkw, B, N, lens, seed, tol_pred=3e-2, e2tts_kw=None, drop_text_cond=False, dyn_scale=0.05, grads=True):
     torch.manual_seed(seed)
     random.seed(seed)   # the hyper-connections draw their initial stream with python's randrange: the same case on every run
-    model = pkg.E2TTS(transformer=dict(dropout=0., max_seq_len=N, **tkw, **(model_kw or {})), use_vocos=False, **(e2tts_kw or {}))
+    model = pkg.E2TTS(transformer=dict(dropout=0., max_seq_len=N, **tkw), use_vocos=False, **(e2tts_kw or {}))
     # dyn_scale 0.05 (5x the reference's init of the hyper-connections' dynamic scales): with the 0.5 of the 2-layer fixtures a depth-8
     # stack amplifies bf16 rounding of the residual streams ~10x — the fp32 oracle with its OWN stage outputs rounded to bf16
     # (O.STAGE_ROUND) then moves its prediction by 12.6 %, exactly what the kernels showed. The probe below
@@ -113,3 +113,39 @@ def check_grads(sd, rec, rel=2e-4, floor=1e-7):
         assert float((g[RC.sample_index(g.numel())] - r['values'].double()).abs().max()) <= tol, k
         assert abs(float(g.abs().max()) - r['max']) <= tol, k
         assert abs(float(g.norm()) - r['norm']) <= 5 * rel * r['norm'] + floor, k
+
+
+def oracle_case(c, rec, sd=None, hook=None):
+    """The oracle on a stored case of the original: `c` holds cls, seed, tkw (the Transformer kwargs) and, where they are not the
+    defaults, kw (the E2TTS kwargs), lens and drop (drop_text_cond); `rec` is its record (tests/golden/reference/). Weights `sd` (default:
+    the case's seeded weights, taking gradients), inputs rebuilt from the seed, the original's draws injected, O.DROPOUT = hook; the
+    loss is backpropagated when it takes a gradient. Returns (sd, loss, prediction or None for a DurationPredictor)."""
+    cls = c.get('cls', 'E2TTS')
+    if sd is None:
+        sd = grad_sd(RC.state_dict(cls, c['seed'], c['tkw'], **c.get('kw', {})))
+    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
+    lens = torch.tensor(c['lens']) if c.get('lens') else None
+    text = O.list_str_to_tensor(c['text'])
+    if cls == 'E2TTS':
+        o = with_dropout(hook, O.e2tts_forward, sd, O.TransformerCfg(**c['tkw']), mel, text, lens=lens, drop_text_cond=c.get('drop', False),
+                         x0=RC.randn(mel.shape, c['seed'] + 2000), times=rec['times'], span_mask=rec['span_mask'])
+        loss, pred = o['loss'], o['pred']
+    else:
+        torch.manual_seed(c['seed'])
+        rand_frac = mel.new_zeros(mel.shape[0]).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
+        loss = with_dropout(hook, O.duration_forward, sd, O.TransformerCfg(cond_on_time=False, **c['tkw']), mel, text, lens=lens,
+                            rand_frac=rand_frac)
+        pred = None
+    if loss.requires_grad:
+        loss.backward()
+    return sd, loss, pred
+
+
+def check_case(c, rec, sd, loss, pred):
+    """oracle_case's results against the record: prediction sample rel-L2 < 1e-4 and its norm within 1e-4, loss within 1e-5, gradient
+    samples within check_grads at the case's grad_tol (default: the 2-layer E2TTS fixtures' bound, a DurationPredictor's looser one)"""
+    if pred is not None:
+        assert RC.compact_rel_l2(pred, rec['pred']) < 1e-4
+        assert abs(float(pred.detach().double().norm()) - rec['pred']['norm']) <= 1e-4 * rec['pred']['norm']
+    assert abs(float(loss.detach()) - rec['loss']) <= 1e-5 * abs(rec['loss'])
+    check_grads(sd, rec['grads'], *c.get('grad_tol', (2e-4, 1e-7) if c.get('cls', 'E2TTS') == 'E2TTS' else (5e-4, 1e-6)))

@@ -1,15 +1,8 @@
-"""Test infrastructure for Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True):
-the cases stored from the original e2_tts.py by tools/make_residual_golden.py, and a context that turns the oracle of
-oracle/e2tts_oracle.py into that backbone.
-
-With one stream the reference's hyper-connection modules are `Residual` (oracle/ref_leaves/hyper_connections.py): the width
+"""Cases of Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True), stored from the
+original e2_tts.py by tools/make_residual_golden.py. The oracle of oracle/e2tts_oracle.py runs that backbone when its config has one
+stream: with one stream the reference's hyper-connection modules are `Residual` (oracle/ref_leaves/hyper_connections.py), the width
 connection hands the stream itself to the branch and keeps it as the residual, the depth connection is `branch_out + residual`, and
-expand / reduce are identities. The oracle holds its streams as (b, n, S, d), so with S = 1 swapping its two hyper-connection leaves is
-all it takes; the stage rounding of the conditioning probe (O.STAGE_ROUND) stays on the residual sum, which the CUDA path stores in
-bf16 (the branch output itself is added in fp32 inside the producing kernel and never stored)."""
-import contextlib
-
-from oracle import e2tts_oracle as O
+expand / reduce are identities."""
 
 KW1 = dict(dim=128, depth=2, heads=2, num_residual_streams=1)
 
@@ -24,22 +17,3 @@ RESIDUAL1_CASES = {
 }
 # E2TTS.sample: weights seed, cond (batch, frames), text, duration, steps, cfg_strength; y0 = first draw of generator 3000 + seed
 RESIDUAL1_SAMPLE = dict(seed=70, cond=(2, 20), text=['Hello', 'Goodbye then'], duration=[40, 33], steps=4, cfg_strength=1.0)
-
-
-def _width(sd, p, res, S):
-    return res[..., 0, :], res, None
-
-
-def _depth(rest, beta, y):
-    return O._rs(y[..., None, :] + rest)
-
-
-@contextlib.contextmanager
-def plain_residual_oracle():
-    """Inside the block the oracle computes the num_residual_streams=1 backbone (use it with TransformerCfg(num_residual_streams=1))."""
-    saved = O.hyper_width, O.hyper_depth
-    O.hyper_width, O.hyper_depth = _width, _depth
-    try:
-        yield
-    finally:
-        O.hyper_width, O.hyper_depth = saved

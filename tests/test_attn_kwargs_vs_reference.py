@@ -1,12 +1,11 @@
 """CPU: the x-transformers `attn_kwargs` of Transformer (e2_tts.py:548-551) besides the reference's default — no head gate, no logit
-soft-clamp, another clamp value. The oracle of tests/attn_variants.py against what the original e2_tts.py computed on those settings
+soft-clamp, another clamp value. The oracle with the same attn_kwargs against what the original e2_tts.py computed on those settings
 (tests/golden/reference/attn_kwargs_*.pt, tools/make_attn_kwargs_golden.py), the package's parameter layout against the original's,
 the switches that still raise, and the C-ABI validation of the unclamped / no-gate fields."""
 import pytest
-import torch
 
-from attn_variants import ATTN_KWARGS_CASES, clamp_of, variant_oracle
-from model_checks import check_grads, grad_sd
+from attn_variants import ATTN_KWARGS_CASES
+from model_checks import check_case, oracle_case
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
 
@@ -20,29 +19,9 @@ def _tkw(c):
 @pytest.mark.parametrize('name', list(ATTN_KWARGS_CASES))
 def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
-    c = ATTN_KWARGS_CASES[name]
+    c = dict(ATTN_KWARGS_CASES[name], tkw=_tkw(ATTN_KWARGS_CASES[name]))
     g = RC.load('attn_kwargs_' + name)
-    sd = grad_sd(RC.state_dict(c['cls'], c['seed'], _tkw(c)))
-    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
-    lens = torch.tensor(c['lens'])
-    text = O.list_str_to_tensor(c['text'])
-    with variant_oracle(c['attn_kwargs']):
-        if c['cls'] == 'E2TTS':
-            x0 = RC.randn(mel.shape, c['seed'] + 2000)
-            o = O.e2tts_forward(sd, O.TransformerCfg(**RC.KW), mel, text, lens=lens, x0=x0, times=g['times'], span_mask=g['span_mask'])
-            loss = o['loss']
-            assert RC.compact_rel_l2(o['pred'], g['pred']) < 1e-4
-            assert abs(float(o['pred'].detach().double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
-        else:
-            torch.manual_seed(c['seed'])
-            rand_frac = mel.new_zeros(mel.shape[0]).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
-            loss = O.duration_forward(sd, O.TransformerCfg(cond_on_time=False, **RC.KW), mel, text, lens=lens, rand_frac=rand_frac)
-    assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
-    loss.backward()
-    if c['cls'] == 'E2TTS':
-        check_grads(sd, g['grads'])
-    else:
-        check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+    check_case(c, g, *oracle_case(c, g))
 
 
 @pytest.mark.parametrize('name', list(ATTN_KWARGS_CASES))
@@ -70,7 +49,7 @@ def test_state_dict_matches_reference(name):
 def test_attn_kwargs_parse(attn_kwargs, gate, clamp):
     """a missing key takes x-transformers' default; the reference's default dict keeps the module constant clamp"""
     t = pkg.Transformer(dim=128, depth=2, heads=2, attn_kwargs=attn_kwargs)
-    assert t.softclamp == clamp == clamp_of(attn_kwargs)
+    assert t.softclamp == clamp == O.TransformerCfg(dim=128, attn_kwargs=attn_kwargs).softclamp
     if attn_kwargs.get('gate_value_heads') and attn_kwargs.get('softclamp_logits') and clamp == 50.0:
         assert t.softclamp == pkg.modules.SOFTCLAMP
     attn = t.layers[1][0][3]

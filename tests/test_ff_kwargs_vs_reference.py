@@ -1,13 +1,15 @@
 """CPU: the x-transformers `ff_kwargs` of Transformer (e2_tts.py:552) — SwiGLU, ReLU^2 GLU, the GLU multiplicative bias and the output
-Linear without bias. The oracle of tests/ff_variants.py against what the original e2_tts.py computed on those settings
-(tests/golden/reference/ff_kwargs_*.pt, tools/make_ff_kwargs_golden.py), the package's parameter layout against the original's, the
-parsing of the keywords (precedence, explicit defaults, refusals), and the C-ABI validation of the GLU activation fields."""
+Linear without bias. The oracle with the same ff_kwargs against what the original e2_tts.py computed on those settings
+(tests/golden/reference/ff_kwargs_*.pt, tools/make_ff_kwargs_golden.py), a negative control per switch family (ff_kwargs, attn_kwargs,
+text geometry), the package's parameter layout against the original's, the parsing of the keywords (precedence, explicit defaults,
+refusals), and the C-ABI validation of the GLU activation fields."""
 import pytest
 import torch
 
-from ff_variants import FF_KWARGS_CASES, XTFeedForward, case_oracle, cfg, state_dict
-from model_checks import check_grads, grad_sd
-from oracle import e2tts_oracle as O
+from attn_variants import ATTN_KWARGS_CASES
+from ff_variants import FF_KWARGS_CASES, XTFeedForward
+from headdim_variants import HEADDIM_CASES
+from model_checks import check_case, oracle_case
 from oracle import reference_cases as RC
 from oracle.ref_leaves.x_transformers.x_transformers import FeedForward as LeafFeedForward
 
@@ -23,41 +25,40 @@ def _tkw(c):
 @pytest.mark.parametrize('name', list(FF_KWARGS_CASES))
 def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples (mult_bias included) within the bounds of tests/test_oracle_vs_reference.py"""
-    c = FF_KWARGS_CASES[name]
+    c = dict(FF_KWARGS_CASES[name], tkw=_tkw(FF_KWARGS_CASES[name]))
     g = RC.load('ff_kwargs_' + name)
-    sd = grad_sd(state_dict(c))
-    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
-    lens = torch.tensor(c['lens'])
-    text = O.list_str_to_tensor(c['text'])
-    with case_oracle(c):
-        if c['cls'] == 'E2TTS':
-            x0 = RC.randn(mel.shape, c['seed'] + 2000)
-            o = O.e2tts_forward(sd, cfg(c), mel, text, lens=lens, x0=x0, times=g['times'], span_mask=g['span_mask'])
-            loss = o['loss']
-            assert RC.compact_rel_l2(o['pred'], g['pred']) < 1e-4
-            assert abs(float(o['pred'].detach().double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
-        else:
-            torch.manual_seed(c['seed'])
-            rand_frac = mel.new_zeros(mel.shape[0]).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
-            loss = O.duration_forward(sd, cfg(c, cond_on_time=False), mel, text, lens=lens, rand_frac=rand_frac)
-    assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
-    loss.backward()
-    if c['cls'] == 'E2TTS':
-        check_grads(sd, g['grads'])
-    else:
-        check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+    check_case(c, g, *oracle_case(c, g))
     if c['ff_kwargs'].get('glu_mult_bias'):
         assert any(k.endswith('.ff.0.mult_bias') and v is not None for k, v in g['grads'].items())
 
 
+# one stored case per switch family, by record name, with its whole Transformer kwargs, and the least the oracle without the switch
+# misses its prediction by (rel-L2; the cases pass at 1e-4)
+SEES = {
+    'ff_kwargs_swish': (dict(FF_KWARGS_CASES['swish'], tkw=_tkw(FF_KWARGS_CASES['swish'])), 1e-2),
+    'attn_kwargs_clamp30': (dict(ATTN_KWARGS_CASES['clamp30'], tkw=dict(RC.KW, attn_kwargs=ATTN_KWARGS_CASES['clamp30']['attn_kwargs'])),
+                            1e-2),
+    # text geometry 1 x 128, as wide as the audio's 2 x 64, so the default text geometry runs on the same weights; the text stream
+    # reaches the prediction through the cross-conditions only, and 2 x 64 moves it by 8.7e-3
+    'headdim_mixed_a64_t128': (HEADDIM_CASES['mixed_a64_t128'], 5e-3),
+}
+
+
 def test_oracle_sees_the_variant():
-    """the stored outputs tell the variants apart: the default GELU feed-forward misses the SwiGLU golden's prediction bound"""
-    c = FF_KWARGS_CASES['swish']
-    g = RC.load('ff_kwargs_swish')
-    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
-    o = O.e2tts_forward(state_dict(c), cfg(c), mel, O.list_str_to_tensor(c['text']), lens=torch.tensor(c['lens']),
-                        x0=RC.randn(mel.shape, c['seed'] + 2000), times=g['times'], span_mask=g['span_mask'])
-    assert RC.compact_rel_l2(o['pred'], g['pred']) > 1e-2
+    """the stored outputs tell the variants apart, one switch family at a time: the oracle configured with the defaults of everything
+    but the audio geometry, on the case's own weights plus the default model's for what the case lacks (clamp30's head gates: its clamp
+    value alone moves the prediction by ~3e-6), misses the case's prediction, so a test that built the model with a switch and the
+    oracle without it fails"""
+    for record, (c, bound) in SEES.items():
+        g = RC.load(record)
+        default = {k: v for k, v in c['tkw'].items() if k in ('dim', 'depth', 'heads', 'dim_head')}
+        sd = RC.state_dict(c['cls'], c['seed'], c['tkw'])
+        for k, v in RC.state_dict(c['cls'], c['seed'], default).items():
+            sd.setdefault(k, v)
+        _, _, pred = oracle_case(dict(c, tkw=default), g, sd=sd)
+        e = RC.compact_rel_l2(pred, g['pred'])
+        print(f'{record}: the default config misses by {e:.3g}')
+        assert e > bound, record
 
 
 @pytest.mark.parametrize('name', list(FF_KWARGS_CASES))

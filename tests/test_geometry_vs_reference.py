@@ -5,41 +5,19 @@ parameter layout against the original's, and the geometries that raise."""
 import pytest
 import torch
 
-from geometry_variants import GEOMETRY_CASES, GEOMETRY_SAMPLE, cfg, reverted
-from model_checks import check_grads, grad_sd
+from geometry_variants import GEOMETRY_CASES, GEOMETRY_SAMPLE, reverted
+from model_checks import check_case, oracle_case
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
 
 import e2_tts_pytorch_b200 as pkg
 
 
-def run_oracle(c, g, tkw, sd):
-    """(loss, prediction or None) of the oracle on case `c`'s inputs and the stored draws of its record `g`"""
-    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
-    lens = torch.tensor(c['lens'])
-    text = O.list_str_to_tensor(c['text'])
-    if c['cls'] == 'E2TTS':
-        x0 = RC.randn(mel.shape, c['seed'] + 2000)
-        o = O.e2tts_forward(sd, cfg(tkw), mel, text, lens=lens, x0=x0, times=g['times'], span_mask=g['span_mask'], drop_text_cond=c['drop'])
-        return o['loss'], o['pred']
-    torch.manual_seed(c['seed'])
-    rand_frac = mel.new_zeros(mel.shape[0]).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
-    return O.duration_forward(sd, cfg(tkw, cond_on_time=False), mel, text, lens=lens, rand_frac=rand_frac), None
-
-
 @pytest.mark.parametrize('name', list(GEOMETRY_CASES))
 def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
-    c = GEOMETRY_CASES[name]
-    g = RC.load('geometry_' + name)
-    sd = grad_sd(RC.state_dict(c['cls'], c['seed'], c['tkw']))
-    loss, pred = run_oracle(c, g, c['tkw'], sd)
-    if pred is not None:
-        assert RC.compact_rel_l2(pred, g['pred']) < 1e-4
-        assert abs(float(pred.detach().double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
-    assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
-    loss.backward()
-    check_grads(sd, g['grads'], *c['grad_tol'])
+    c, g = GEOMETRY_CASES[name], RC.load('geometry_' + name)
+    check_case(c, g, *oracle_case(c, g))
     depth, text_depth = c['tkw']['depth'], c['tkw'].get('text_depth', c['tkw']['depth'])
     last = f'transformer.layers.{text_depth - 1}.1.'
     if c['drop']:   # the text stream is skipped: its parameters get no gradient
@@ -57,7 +35,7 @@ def test_knob_reverted_misses_reference(name, knob):
     g = RC.load('geometry_' + name)
     tkw, sd = reverted(c, knob)
     with torch.no_grad():
-        loss, pred = run_oracle(c, g, tkw, sd)
+        _, loss, pred = oracle_case(dict(c, tkw=tkw), g, sd=sd)
     if pred is not None:
         assert RC.compact_rel_l2(pred, g['pred']) > 1e-2
     else:
@@ -70,7 +48,8 @@ def test_sample_vs_reference():
     g = RC.load('geometry_sample')
     cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
     with torch.no_grad():
-        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), cfg(s['tkw']), cond, O.list_str_to_tensor(s['text']),
+        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), O.TransformerCfg(**s['tkw']), cond,
+                             O.list_str_to_tensor(s['text']),
                              duration=torch.tensor(s['duration']), lens=torch.tensor(s['lens']), y0=RC.randn(g['shape'], 3000 + s['seed']),
                              steps=s['steps'], cfg_strength=s['cfg_strength'])
     assert tuple(got.shape) == g['shape'] == (2, max(s['duration']), 100)

@@ -9,7 +9,6 @@ import pytest
 import torch
 
 from attn_ref import attn_bwd, attn_fwd, autograd64, dropout_keep, host_maskbits, restate, unclamped_inputs
-from attn_variants import variant_oracle
 from conftest import rel_l2
 from kernel_checks import BF16, F32, F64, Rv, agree, check_b, check_e, check_f, dev, h64, nans, pkg, stream
 from model_checks import small_model, whole_model
@@ -202,7 +201,6 @@ def test_attention_node_variants(pkg, gate, clamp):
     """ops.Attention at the cfg2 widths (d512, 8 heads) without gate and/or clamp: og and v equal the composition of b200_qkv_post and
     the attention kernels it wraps (E), and its parameter gradients agree with float64 autograd of the x-transformers attention to
     bf16 accuracy (cosine >= 0.999)"""
-    from attn_variants import attention as xt_attention
     ops = pkg.ops
     B, Np, H, Din = 2, 160, 8, 512
     T, I = B * Np, H * 64
@@ -230,7 +228,7 @@ def test_attention_node_variants(pkg, gate, clamp):
         sd['a.to_v_head_gate.bias'] = h64(bg).requires_grad_()
     x64 = h64(xn).view(B, Np, Din).requires_grad_()
     freqs = O.rotary_freqs(Np, 64, 'cpu').to(F64)
-    ref, _ = xt_attention(sd, 'a', x64, mask.cpu().bool(), freqs, None, H, 64, clamp)
+    ref, _ = O.attention(sd, 'a', x64, mask.cpu().bool(), freqs, None, H, 64, clamp, gate)
     ref = ref * mask.cpu()[..., None]
     (ref * h64(dog).view(B, Np, I)).sum().backward()
     ok = mask.cpu().bool().view(-1)
@@ -252,8 +250,7 @@ def test_e2tts_cfg2_shape_attn_kwargs_vs_oracle(pkg, setting):
     """BASELINE cfg2's model (d512, depth 8, 8 heads, N = 1024, ragged B = 2) with these attn_kwargs: conditioning probe < 1.5 %, loss
     within 1e-2, prediction rel-L2 within 3e-2, every gradient cosine >= 0.99 (the bounds of tests/test_gpu_parity_full.py)"""
     kw = ATTN_SETTINGS[setting]
-    with variant_oracle(kw):
-        whole_model(pkg, dict(dim=512, depth=8, heads=8), B=2, N=1024, lens=[1024, 800], seed=40, model_kw=dict(attn_kwargs=kw))
+    whole_model(pkg, dict(dim=512, depth=8, heads=8, attn_kwargs=kw), B=2, N=1024, lens=[1024, 800], seed=40)
 
 
 def test_sample_32_steps_plain_attention_vs_oracle(pkg):
@@ -264,9 +261,8 @@ def test_sample_32_steps_plain_attention_vs_oracle(pkg):
     y0 = torch.randn(2, 64, 100)
     with pkg.inject_randomness(y0=y0.to(dev())):
         out = model.sample(cond.to(dev()), text=text, duration=64, steps=32, cfg_strength=1.0, return_raw_output=True)
-    with variant_oracle(dict()):
-        want = O.e2tts_sample(sd, O.TransformerCfg(dim=128, depth=2, heads=2), cond, O.list_str_to_tensor(text), duration=64, y0=y0,
-                              steps=32, cfg_strength=1.0)
+    want = O.e2tts_sample(sd, O.TransformerCfg(dim=128, depth=2, heads=2, attn_kwargs=dict()), cond, O.list_str_to_tensor(text),
+                          duration=64, y0=y0, steps=32, cfg_strength=1.0)
     assert out.shape == want.shape
     assert rel_l2(out.cpu(), want) < 5e-2
 
@@ -311,9 +307,8 @@ def test_duration_predictor_plain_attention_vs_oracle(pkg):
         loss = model(mel.to(dev()), text=text, lens=lens.to(dev()))
     loss.backward()
     osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    with variant_oracle(dict()):
-        ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, dim=128, depth=2, heads=2), mel, O.list_str_to_tensor(text),
-                                 lens=lens, rand_frac=rand_frac)
+    ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, dim=128, depth=2, heads=2, attn_kwargs=dict()), mel,
+                             O.list_str_to_tensor(text), lens=lens, rand_frac=rand_frac)
     ref.backward()
     assert abs(float(loss) - float(ref)) <= 1e-2 * abs(float(ref))
     total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())

@@ -16,7 +16,6 @@ import torch
 
 from conftest import rel_l2
 from dropout_ref import KernelMasks, SeedRecorder, splitmix64, with_dropout
-from headdim_variants import cfg, headdim_oracle
 from kernel_checks import F64, dev, pkg  # noqa: F401  (pytest fixture)
 from model_checks import cos
 from oracle import e2tts_oracle as O
@@ -126,13 +125,13 @@ def oracle(c, sd, x, masks, grad=True, probe=False):
         return cap['y']
     O.transformer_forward = transformer_forward
     try:
-        with headdim_oracle(c['tkw']), torch.set_grad_enabled(grad):
+        with torch.set_grad_enabled(grad):
             if c['cls'] == 'E2TTS':
-                o = with_dropout(masks, O.e2tts_forward, osd, cfg(c['tkw']), mel, text, x0=x['x0'].to(dt), times=x['times'].to(dt),
-                                 span_mask=x['span'], lens=lens)
+                o = with_dropout(masks, O.e2tts_forward, osd, O.TransformerCfg(**c['tkw']), mel, text, x0=x['x0'].to(dt),
+                                 times=x['times'].to(dt), span_mask=x['span'], lens=lens)
                 loss, pred = o['loss'], o['pred']
             else:
-                loss = with_dropout(masks, O.duration_forward, osd, cfg(c['tkw'], cond_on_time=False), mel, text, lens=lens,
+                loss = with_dropout(masks, O.duration_forward, osd, O.TransformerCfg(cond_on_time=False, **c['tkw']), mel, text, lens=lens,
                                     rand_frac=x['rand_frac'].to(dt))
                 pred = cap['y']
         if grad:

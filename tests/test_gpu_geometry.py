@@ -15,7 +15,7 @@ import pytest
 import torch
 
 from conftest import rel_l2
-from geometry_variants import GEOMETRY_CASES, GEOMETRY_SAMPLE, cfg
+from geometry_variants import GEOMETRY_CASES, GEOMETRY_SAMPLE
 from hyper_conv_ref import S, check_hc_case, hc_fwd_launch
 from kernel_checks import dev, pkg, sms  # noqa: F401
 from model_checks import cos, small_model, whole_model
@@ -116,7 +116,8 @@ def test_duration_predictor_geometry_vs_oracle(pkg):
         loss = model(mel.to(dev()), text=text, lens=lens.to(dev()))
     loss.backward()
     osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    ref = O.duration_forward(osd, cfg(tkw, cond_on_time=False), mel, O.list_str_to_tensor(text), lens=lens, rand_frac=rand_frac)
+    ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, **tkw), mel, O.list_str_to_tensor(text), lens=lens,
+                             rand_frac=rand_frac)
     ref.backward()
     assert abs(float(loss) - float(ref)) <= 1e-2 * abs(float(ref))
     total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())
@@ -142,7 +143,7 @@ def test_sample_ragged_duration_vs_oracle(pkg):
     with pkg.inject_randomness(y0=y0.to(dev())):
         out = model.sample(cond.to(dev()), text=s['text'], lens=lens.to(dev()), duration=duration.to(dev()), steps=s['steps'],
                            cfg_strength=s['cfg_strength'], return_raw_output=True)
-    want = O.e2tts_sample(sd, cfg(s['tkw']), cond, O.list_str_to_tensor(s['text']), duration=duration, lens=lens, y0=y0,
+    want = O.e2tts_sample(sd, O.TransformerCfg(**s['tkw']), cond, O.list_str_to_tensor(s['text']), duration=duration, lens=lens, y0=y0,
                           steps=s['steps'], cfg_strength=s['cfg_strength'])
     assert out.shape == want.shape == (2, max(s['duration']), 100)
     assert rel_l2(out.cpu(), want) < 5e-2

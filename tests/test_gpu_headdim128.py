@@ -13,13 +13,10 @@ import pytest
 import torch
 
 from attn_ref import attn_bwd, attn_fwd, autograd64, d128_inputs, dropout_keep, host_maskbits, restate
-from attn_variants import variant_oracle
 from conftest import rel_l2
-from headdim_variants import cfg, headdim_oracle
 from kernel_checks import BF16, F32, F64, U, Rv, agree, check_b, check_e, check_f, dev, gamma, h64, nans, pkg, stream
 from model_checks import cos, small_model, whole_model
 from oracle import e2tts_oracle as O
-from residual_variants import plain_residual_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -297,17 +294,14 @@ def test_e2tts_d512_depth8_heads4x128_vs_oracle(pkg):
 
 def test_e2tts_mixed_geometry_vs_oracle(pkg):
     """audio 8 x 64, text 2 x 128: two rotary tables, two qkv packings"""
-    text = dict(text_heads=2, text_dim_head=128)
-    with headdim_oracle(dict(heads=8, dim_head=64, **text)):
-        whole_model(pkg, dict(dim=512, depth=2, heads=8, dim_head=64), B=2, N=224, lens=[224, 170], seed=41, model_kw=text)
+    whole_model(pkg, dict(dim=512, depth=2, heads=8, dim_head=64, text_heads=2, text_dim_head=128), B=2, N=224, lens=[224, 170], seed=41)
 
 
 def test_e2tts_plain_residual_unclamped_d128_vs_oracle(pkg):
     """dim_head 128 with num_residual_streams=1 and attn_kwargs=dict() (no clamp, no head gate), at cfg2's shape like the 64-wide
     tests of these switches"""
-    with plain_residual_oracle(), variant_oracle(dict()):
-        whole_model(pkg, dict(dim=512, depth=8, heads=4, dim_head=128, num_residual_streams=1), B=2, N=1024, lens=[1024, 800], seed=40,
-                     model_kw=dict(attn_kwargs=dict()))
+    whole_model(pkg, dict(dim=512, depth=8, heads=4, dim_head=128, num_residual_streams=1, attn_kwargs=dict()), B=2, N=1024,
+                lens=[1024, 800], seed=40)
 
 
 SMALL = dict(dim=128, depth=2, heads=1, dim_head=128, text_heads=2, text_dim_head=64)
@@ -321,8 +315,7 @@ def test_sample_32_steps_d128_vs_oracle(pkg):
     y0 = torch.randn(2, 64, 100)
     with pkg.inject_randomness(y0=y0.to(dev())):
         out = model.sample(cond.to(dev()), text=text, duration=64, steps=32, cfg_strength=1.0, return_raw_output=True)
-    with headdim_oracle(SMALL):
-        want = O.e2tts_sample(sd, cfg(SMALL), cond, O.list_str_to_tensor(text), duration=64, y0=y0, steps=32, cfg_strength=1.0)
+    want = O.e2tts_sample(sd, O.TransformerCfg(**SMALL), cond, O.list_str_to_tensor(text), duration=64, y0=y0, steps=32, cfg_strength=1.0)
     assert out.shape == want.shape
     assert rel_l2(out.cpu(), want) < 5e-2
 
@@ -338,8 +331,8 @@ def test_duration_predictor_d128_vs_oracle(pkg):
         loss = model(mel.to(dev()), text=text, lens=lens.to(dev()))
     loss.backward()
     osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    with headdim_oracle(SMALL):
-        ref = O.duration_forward(osd, cfg(SMALL, cond_on_time=False), mel, O.list_str_to_tensor(text), lens=lens, rand_frac=rand_frac)
+    ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, **SMALL), mel, O.list_str_to_tensor(text), lens=lens,
+                             rand_frac=rand_frac)
     ref.backward()
     assert abs(float(loss) - float(ref)) <= 1e-2 * abs(float(ref))
     total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())

@@ -229,7 +229,7 @@ def test_e2tts_attn_fourier_embed_input_vs_oracle(pkg):
     """SURVEY §8f row 4, first variant: Transformer(attn_fourier_embed_input=True) (e2_tts.py:545-546; LinearFourierEmbed :368-386 on the
     attention input, :909) — wgmma GEMM + b200_fourier_feat_* against the oracle, which tests/test_oracle_vs_reference.py pins to the
     reference's own code with the switch on. Loss, prediction and every parameter gradient incl. `layers.{i}.0.4.linear.weight`."""
-    whole_model(pkg, dict(dim=256, depth=2, heads=4), B=2, N=224, lens=[224, 170], seed=60, model_kw=dict(attn_fourier_embed_input=True))
+    whole_model(pkg, dict(dim=256, depth=2, heads=4, attn_fourier_embed_input=True), B=2, N=224, lens=[224, 170], seed=60)
 
 
 def test_e2tts_concat_cond_vs_oracle(pkg):

@@ -6,14 +6,13 @@ Kernels, element-wise against float64 with NaN-filled outputs (the method of ker
 Bit-exact properties: masked rows of the residual convolution keep x (and pass dy); its pre-activation equals the plain launch's;
 the branch norm's forward equals the final norm's with one stream and no registers.
 Nodes at the config-2 widths (ops.BranchNorm, ops.DwConv / OutProj / FeedForward with a residual): the residual's gradient is dy
-itself. Model: the cfg2-shape E2TTS against the fp32 oracle of tests/residual_variants.py, DurationPredictor, 32-step sample(), a
+itself. Model: the cfg2-shape E2TTS against the fp32 oracle with one stream, DurationPredictor, 32-step sample(), a
 graphed training step, and no hyper-connection entry point launched."""
 import pytest
 import torch
 
 from conftest import rel_l2
 from oracle import e2tts_oracle as O
-from residual_variants import plain_residual_oracle
 from hyper_conv_ref import CV_TN, cdiv, dw_mask, dw_ref, model_mask
 from kernel_checks import BF16, F64, U, U16, check_b, check_e, check_f, dev, gamma, gen, h64, nans, pkg, stream
 from model_checks import small_model, whole_model
@@ -295,8 +294,7 @@ def test_nodes_with_residual(pkg):
 def test_e2tts_cfg2_shape_plain_residual_vs_oracle(pkg):
     """BASELINE cfg2's model (d512, depth 8, 8 heads, N = 1024, ragged B = 2) with num_residual_streams=1: conditioning probe < 1.5 %,
     loss within 1e-2, prediction rel-L2 within 3e-2, every gradient cosine >= 0.99 (the bounds of tests/model_checks.py)"""
-    with plain_residual_oracle():
-        whole_model(pkg, dict(dim=512, depth=8, heads=8, num_residual_streams=1), B=2, N=1024, lens=[1024, 800], seed=40)
+    whole_model(pkg, dict(dim=512, depth=8, heads=8, num_residual_streams=1), B=2, N=1024, lens=[1024, 800], seed=40)
 
 
 SMALL = dict(dim=128, depth=2, heads=2, num_residual_streams=1)
@@ -310,9 +308,7 @@ def test_sample_32_steps_plain_residual_vs_oracle(pkg):
     y0 = torch.randn(2, 64, 100)
     with pkg.inject_randomness(y0=y0.to(dev())):
         out = model.sample(cond.to(dev()), text=text, duration=64, steps=32, cfg_strength=1.0, return_raw_output=True)
-    with plain_residual_oracle():
-        want = O.e2tts_sample(sd, O.TransformerCfg(dim=128, depth=2, heads=2, num_residual_streams=1), cond, O.list_str_to_tensor(text),
-                              duration=64, y0=y0, steps=32, cfg_strength=1.0)
+    want = O.e2tts_sample(sd, O.TransformerCfg(**SMALL), cond, O.list_str_to_tensor(text), duration=64, y0=y0, steps=32, cfg_strength=1.0)
     assert out.shape == want.shape
     assert rel_l2(out.cpu(), want) < 5e-2
 
@@ -365,9 +361,8 @@ def test_duration_predictor_plain_residual_vs_oracle(pkg):
         loss = model(mel.to(dev()), text=text, lens=lens.to(dev()))
     loss.backward()
     osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    with plain_residual_oracle():
-        ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, dim=128, depth=2, heads=2, num_residual_streams=1), mel,
-                                 O.list_str_to_tensor(text), lens=lens, rand_frac=rand_frac)
+    ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, **SMALL), mel, O.list_str_to_tensor(text), lens=lens,
+                             rand_frac=rand_frac)
     ref.backward()
     assert abs(float(loss) - float(ref)) <= 1e-2 * abs(float(ref))
     total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())

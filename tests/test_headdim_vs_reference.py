@@ -1,12 +1,12 @@
 """CPU: the attention geometry knobs of Transformer (e2_tts.py:527-531) — 128-wide heads (dim_head, text_dim_head) and a text stream
-with its own head count (text_heads). The oracle of tests/headdim_variants.py against what the original e2_tts.py computed with them
+with its own head count (text_heads). The oracle with the same geometry against what the original e2_tts.py computed with them
 (tests/golden/reference/headdim_*.pt, tools/make_headdim_golden.py), the package's parameter layout against the original's, the head
 dims that still raise, and the C-ABI validation of dim_head."""
 import pytest
 import torch
 
-from headdim_variants import HEADDIM_CASES, HEADDIM_SAMPLE, cfg, headdim_oracle
-from model_checks import check_grads, grad_sd
+from headdim_variants import HEADDIM_CASES, HEADDIM_SAMPLE
+from model_checks import check_case, oracle_case
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
 
@@ -16,30 +16,8 @@ import e2_tts_pytorch_b200 as pkg
 @pytest.mark.parametrize('name', list(HEADDIM_CASES))
 def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
-    c = HEADDIM_CASES[name]
-    g = RC.load('headdim_' + name)
-    sd = grad_sd(RC.state_dict(c['cls'], c['seed'], c['tkw']))
-    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
-    lens = torch.tensor(c['lens'])
-    text = O.list_str_to_tensor(c['text'])
-    with headdim_oracle(c['tkw']):
-        if c['cls'] == 'E2TTS':
-            x0 = RC.randn(mel.shape, c['seed'] + 2000)
-            o = O.e2tts_forward(sd, cfg(c['tkw']), mel, text, lens=lens, x0=x0, times=g['times'], span_mask=g['span_mask'],
-                                drop_text_cond=c['drop'])
-            loss = o['loss']
-            assert RC.compact_rel_l2(o['pred'], g['pred']) < 1e-4
-            assert abs(float(o['pred'].detach().double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
-        else:
-            torch.manual_seed(c['seed'])
-            rand_frac = mel.new_zeros(mel.shape[0]).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
-            loss = O.duration_forward(sd, cfg(c['tkw'], cond_on_time=False), mel, text, lens=lens, rand_frac=rand_frac)
-    assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
-    loss.backward()
-    if c['cls'] == 'E2TTS':
-        check_grads(sd, g['grads'])
-    else:
-        check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+    c, g = HEADDIM_CASES[name], RC.load('headdim_' + name)
+    check_case(c, g, *oracle_case(c, g))
     if c['drop']:   # the text stream is skipped: its parameters get no gradient
         assert g['grads']['transformer.layers.0.1.2.to_q.weight'] is None
 
@@ -48,8 +26,9 @@ def test_sample_vs_reference():
     s = HEADDIM_SAMPLE
     g = RC.load('headdim_sample')
     cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
-    with torch.no_grad(), headdim_oracle(s['tkw']):
-        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), cfg(s['tkw']), cond, O.list_str_to_tensor(s['text']),
+    with torch.no_grad():
+        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), O.TransformerCfg(**s['tkw']), cond,
+                             O.list_str_to_tensor(s['text']),
                              duration=torch.tensor(s['duration']), y0=RC.randn(g['shape'], 3000 + s['seed']), steps=s['steps'],
                              cfg_strength=s['cfg_strength'])
     assert tuple(got.shape) == g['shape']

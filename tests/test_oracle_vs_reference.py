@@ -7,25 +7,14 @@ import pytest
 import torch
 
 from oracle import e2tts_oracle as O
-from model_checks import check_grads, grad_sd
+from model_checks import check_case, check_grads, grad_sd, oracle_case
 from oracle import reference_cases as RC
 
 
 def _forward_case(name):
-    c = RC.FORWARD_CASES[name]
-    g = RC.load('forward_' + name)
-    sd = grad_sd(RC.state_dict('E2TTS', c['seed'], c['tkw'], **c['kw']))
-    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
-    x0 = RC.randn(mel.shape, c['seed'] + 2000)
-    lens_t = torch.tensor(c['lens']) if c['lens'] else None
-    cfg = O.TransformerCfg(dim=c['tkw']['dim'], depth=c['tkw']['depth'], heads=c['tkw']['heads'])
-    o = O.e2tts_forward(sd, cfg, mel, O.list_str_to_tensor(c['text']), lens=lens_t, drop_text_cond=c['drop'], x0=x0, times=g['times'],
-                        span_mask=g['span_mask'])
-    o['loss'].backward()
-    assert abs(float(o['loss'].detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
-    assert RC.compact_rel_l2(o['pred'], g['pred']) < 1e-4
-    assert abs(float(o['pred'].double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
-    check_grads(sd, g['grads'])
+    c, g = RC.FORWARD_CASES[name], RC.load('forward_' + name)
+    sd, loss, pred = oracle_case(c, g)
+    check_case(c, g, sd, loss, pred)
     return sd
 
 

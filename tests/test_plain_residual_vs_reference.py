@@ -1,49 +1,25 @@
-"""CPU: Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True). The oracle of
-tests/residual_variants.py against what the original e2_tts.py computed with that setting (tests/golden/reference/residual1_*.pt,
+"""CPU: Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True). The oracle with
+one stream against what the original e2_tts.py computed with that setting (tests/golden/reference/residual1_*.pt,
 tools/make_residual_golden.py), the package's parameter layout against the original's, the stream counts that still raise, and the
 C-ABI validation of the branch-norm and residual-convolution fields."""
 import pytest
 import torch
 
-from model_checks import check_grads, grad_sd
+from model_checks import check_case, oracle_case
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
-from residual_variants import RESIDUAL1_CASES, RESIDUAL1_SAMPLE, plain_residual_oracle
+from residual_variants import RESIDUAL1_CASES, RESIDUAL1_SAMPLE
 
 import e2_tts_pytorch_b200 as pkg
-
-
-def _cfg(c, **kw):
-    return O.TransformerCfg(**c['tkw'], **kw)
 
 
 @pytest.mark.parametrize('name', list(RESIDUAL1_CASES))
 def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
-    c = RESIDUAL1_CASES[name]
-    g = RC.load('residual1_' + name)
-    sd = grad_sd(RC.state_dict(c['cls'], c['seed'], c['tkw']))
+    c, g = RESIDUAL1_CASES[name], RC.load('residual1_' + name)
+    sd, loss, pred = oracle_case(c, g)
     assert not any('.hyper_conns.' in k for k in sd)
-    mel = RC.randn((c['mel'][0], c['mel'][1], 100), c['seed'] + 1000)
-    lens = torch.tensor(c['lens'])
-    text = O.list_str_to_tensor(c['text'])
-    with plain_residual_oracle():
-        if c['cls'] == 'E2TTS':
-            x0 = RC.randn(mel.shape, c['seed'] + 2000)
-            o = O.e2tts_forward(sd, _cfg(c), mel, text, lens=lens, x0=x0, times=g['times'], span_mask=g['span_mask'], drop_text_cond=c['drop'])
-            loss = o['loss']
-            assert RC.compact_rel_l2(o['pred'], g['pred']) < 1e-4
-            assert abs(float(o['pred'].detach().double().norm()) - g['pred']['norm']) <= 1e-4 * g['pred']['norm']
-        else:
-            torch.manual_seed(c['seed'])
-            rand_frac = mel.new_zeros(mel.shape[0]).uniform_(0, 1)   # the draw of e2_tts.py:1082 under the same seed
-            loss = O.duration_forward(sd, _cfg(c, cond_on_time=False), mel, text, lens=lens, rand_frac=rand_frac)
-    assert abs(float(loss.detach()) - g['loss']) <= 1e-5 * abs(g['loss'])
-    loss.backward()
-    if c['cls'] == 'E2TTS':
-        check_grads(sd, g['grads'])
-    else:
-        check_grads(sd, g['grads'], rel=5e-4, floor=1e-6)
+    check_case(c, g, sd, loss, pred)
     if c.get('drop'):   # the text stream is skipped: its parameters get no gradient
         assert g['grads']['transformer.layers.0.1.2.to_q.weight'] is None
 
@@ -53,7 +29,7 @@ def test_sample_vs_reference():
     g = RC.load('residual1_sample')
     tkw = RESIDUAL1_CASES['depth2']['tkw']
     cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
-    with torch.no_grad(), plain_residual_oracle():
+    with torch.no_grad():
         got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], tkw), O.TransformerCfg(**tkw), cond, O.list_str_to_tensor(s['text']),
                              duration=torch.tensor(s['duration']), y0=RC.randn(g['shape'], 3000 + s['seed']), steps=s['steps'],
                              cfg_strength=s['cfg_strength'])

@@ -14,7 +14,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
-from ff_variants import FF_KWARGS_CASES, XTFeedForward, state_dict  # noqa: E402
+from ff_variants import FF_KWARGS_CASES, XTFeedForward  # noqa: E402
 from oracle import reference_cases as RC  # noqa: E402
 from oracle.load_reference import load_reference, run_reference_forward  # noqa: E402
 
@@ -29,7 +29,7 @@ def main():
         lens = torch.tensor(c['lens'])
         if c['cls'] == 'E2TTS':
             model = ref.E2TTS(transformer=dict(dropout=0., max_seq_len=128, **tkw), use_vocos=False)
-            model.load_state_dict(state_dict(c))
+            model.load_state_dict(RC.state_dict(c['cls'], c['seed'], tkw))
             torch.manual_seed(c['seed'])
             ref.torch = RC.noise(torch, c['seed'] + 2000)   # x0 = the first draw of that generator
             try:
@@ -40,7 +40,7 @@ def main():
             obj = dict(loss=float(out.loss.detach()), pred=RC.compact(out.pred_flow), times=rec['times'], span_mask=rec['span_mask'])
         else:
             model = ref.DurationPredictor(transformer=dict(dropout=0., max_seq_len=128, **tkw))
-            model.load_state_dict(state_dict(c))
+            model.load_state_dict(RC.state_dict(c['cls'], c['seed'], tkw))
             torch.manual_seed(c['seed'])
             loss = model(mel, text=c['text'], lens=lens)
             loss.backward()
