@@ -8,8 +8,10 @@
 //                             register accumulators, then the fused epilogue (bias / AdaLN gate / row mask / residual / GEGLU(+dropout))
 //                             on the accumulator fragments. Plain bf16 outputs are written 64 x 64 at a time into a 128B-swizzled smem
 //                             staging slice (two per warpgroup, alternating) and leave as TMA tile stores (bulk async groups), so the
-//                             warpgroup moves on to the next slice while the previous one drains; GEGLU outputs leave as bf16x2 stores
-//                             from the fragments, fp32 split-K partials through vector atomics.
+//                             warpgroup moves on to the next slice while the previous one drains. A residual slice is TMA-loaded into
+//                             the staging buffer its output slice will occupy (the tile's first two while its last k-blocks still run),
+//                             and the epilogue adds it from shared memory in place. GEGLU outputs leave as bf16x2 stores from the
+//                             fragments, fp32 split-K partials through vector atomics.
 // While a consumer warpgroup runs its epilogue the producer is already filling the ring with the next tile's operands.
 // Operands may be K-major or MN-major (transposed storage) so that the backward contractions
 // dX = dY*W and dW = dY^T*X read activations exactly as they lie in HBM — no transposes are materialised.
@@ -24,6 +26,7 @@ constexpr int BM = 128;
 constexpr int BK = 64;              // 64 bf16 = one 128-byte swizzle atom
 constexpr int kGemmThreads = 384;   // warpgroup 0 TMA, warpgroups 1..2 MMA + epilogue
 constexpr int A_STAGE_BYTES = BM * BK * 2;
+constexpr int kSliceBytes = 64 * 64 * 2;   // one 64 x 64 bf16 output slice, 128B-swizzled (the TMA box layout)
 
 struct GemmParams {
     int M, N, K;
@@ -39,6 +42,7 @@ struct GemmParams {
     const unsigned long long* seed_dev;   // optional device addend of the seed (CUDA-graph replays)
     int atomic_out;
     int tma_store;   // bf16 output through the smem staging slices and TMA stores (tmD)
+    int resid_tma;   // tma_store with a 16-byte aligned residual: its slices are TMA-loaded into the staging buffers (tmR)
     const float* glu_mult;   // optional [N/2] multiplier of the hidden units (x-transformers GLU mult_bias), hidden-unit order
 };
 
@@ -53,9 +57,9 @@ struct GemmSmem {
     static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
     static constexpr int kStages = (STAGE_BYTES <= 32768) ? 6 : 4;
     static constexpr int TILE_BYTES = kStages * STAGE_BYTES;
-    static constexpr int SLICE_BYTES = 64 * 64 * 2;              // one 64 x 64 bf16 output slice, 128B-swizzled
-    static constexpr int STG_BYTES = 2 * 2 * SLICE_BYTES;        // two slices per consumer warpgroup: 32 KB
-    static constexpr int BAR_BYTES = 128;
+    static constexpr int STG_BYTES = 2 * 2 * kSliceBytes;        // two slices per consumer warpgroup: 32 KB
+    static constexpr int BAR_BYTES = 128;                        // full / empty per stage, + one residual barrier per staging slice
+    static_assert((2 * kStages + 4) * 8 <= BAR_BYTES, "GEMM mbarriers exceed their shared-memory slot");
     static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + 1024;  // + slack for manual 1024B alignment
     static_assert(TOTAL <= 227 * 1024, "GEMM shared memory exceeds the 227 KB a block may use");
 };
@@ -105,6 +109,37 @@ __device__ __forceinline__ float2 glu_act2(float2 g) {
     if constexpr (ACT == GLU_GELU) return gelu_erf2(g);
     else if constexpr (ACT == GLU_SILU) return silu2(g);
     else return relu2_2(g);
+}
+
+// Output staging: each consumer warpgroup owns two 64 x 64 bf16 slices in shared memory (kSliceBytes each, 128B-swizzled: the TMA box
+// layout) and fills them alternately; the warpgroup's n-th slice uses buffer n & 1. A thread writes its fragment rows r, r + 8 and, per
+// 8-column group jj of the slice, the 4 bytes at column 8 jj + 2 (lane % 4) to 16-byte chunk (jj ^ (r & 7)) of the row — the TMA's 128B swizzle,
+// and conflict-free: the 8 rows of a warp store land in 8 different chunks (r & 7 == lane / 4 for both rows). slice_addr gives that
+// address; toff = (16 wq + lane / 4) * 128 + 4 (lane % 4), swz = (lane / 4) << 4.
+__device__ __forceinline__ uint32_t slice_addr(uint32_t buf, uint32_t toff, uint32_t swz, int i, int jj) {
+    return buf + toff + (uint32_t)i * 8 * 128 + (((uint32_t)jj << 4) ^ swz);
+}
+// Waits until the buffer of slice n is free (the store issued from it two slices ago has read it); returns its shared address.
+__device__ __forceinline__ uint32_t slice_acquire(uint8_t* my_stg, uint32_t n, int cw, int t) {
+    if (t == 0) bulk_wait_group_read<1>();
+    named_bar_sync(1 + cw, 128);
+    return smem_u32(my_stg + (n & 1) * kSliceBytes);
+}
+// TMA-loads the residual's 64 x 64 slice at (column c0, row c1) into staging buffer b; completes on that buffer's barrier. The
+// whole box counts: the TMA zero-fills what lies outside the tensor.
+__device__ __forceinline__ void resid_load(const CUtensorMap* m, uint8_t* my_stg, uint64_t* my_rbar, uint32_t b, int c0, int c1) {
+    mbar_arrive_expect_tx(&my_rbar[b], kSliceBytes);
+    tma_load_2d(my_stg + b * kSliceBytes, m, &my_rbar[b], c0, c1);
+}
+// Orders the warpgroup's generic-proxy writes of slice n before the TMA (async proxy) reads them, then one thread stores the slice at
+// (column c0, row c1) of `m`; rows and columns outside the tensor are clipped.
+__device__ __forceinline__ void slice_store(const CUtensorMap* m, uint8_t* my_stg, uint32_t n, int cw, int t, int c0, int c1) {
+    fence_proxy_async();
+    named_bar_sync(1 + cw, 128);
+    if (t == 0) {
+        tma_store_2d(m, my_stg + (n & 1) * kSliceBytes, c0, c1);
+        bulk_commit_group();
+    }
 }
 
 // GLU epilogue on the accumulator fragments: every 128 packed columns hold [0,64) = u, [64,128) = gate of the same 64 hidden units, so a
@@ -160,6 +195,59 @@ __device__ __forceinline__ void glu_epilogue(const GemmParams& p, float (&acc)[M
 }
 
 
+// The tile's 64 x 64 output slices from the finished fragments, each through the warpgroup's next staging buffer and a TMA store.
+// RESID: the buffer already holds the slice's residual, TMA-loaded by resid_load (the first two of a tile from the mainloop, the
+// others here, one slice ahead); each pair is added in fp32 from the address it is written back to.
+template <bool RESID, int BN, int MH>
+__device__ __forceinline__ void store_slices(const GemmParams& p, float (&acc)[MH][BN / 2], const CUtensorMap* tmD, const CUtensorMap* tmR,
+                                             uint8_t* my_stg, uint64_t* my_rbar, uint32_t& nslice, int tm, int tn, int cw, int wq, int lane,
+                                             int t) {
+    const uint32_t swz = (uint32_t)(lane >> 2) << 4;
+    const uint32_t toff = (uint32_t)(wq * 16 + (lane >> 2)) * 128 + 4 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < MH; ++h) {
+        const int rowb = tm * BM * MH + (cw * MH + h) * 64;
+#pragma unroll
+        for (int s = 0; s < BN / 64; ++s) {
+            const int colb = tn * BN + s * 64;
+            if (colb >= p.N) break;                  // uniform across the warpgroup
+            uint32_t buf;
+            if constexpr (RESID) {
+                // the buffer holds this slice's residual once its barrier completes (each buffer's barrier completes once per two
+                // slices of the warpgroup); it was free when the load was issued
+                buf = smem_u32(my_stg + (nslice & 1) * kSliceBytes);
+                mbar_wait(&my_rbar[nslice & 1], (nslice >> 1) & 1);
+            } else {
+                buf = slice_acquire(my_stg, nslice, cw, t);
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {
+                    const int j = s * 8 + jj;
+                    const uint32_t a = slice_addr(buf, toff, swz, i, jj);
+                    float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
+                    if constexpr (RESID) {
+                        const uint32_t r = ld_shared_u32(a);
+                        v0 += bf16_lo(r); v1 += bf16_hi(r);
+                    }
+                    st_shared_u32(a, pack_bf16(v0, v1));
+                }
+            }
+            slice_store(tmD, my_stg, nslice, cw, t, colb, rowb);
+            if constexpr (RESID) {
+                // the slice two further uses this buffer: 128 columns on (BN = 256), or these columns of the next m64 block (MH = 2)
+                const bool more = MH == 1 ? (s + 2 < BN / 64 && colb + 128 < p.N) : (h + 1 < MH && tn * BN + 64 < p.N);
+                if (t == 0 && more) {
+                    bulk_wait_group_read<0>();       // the store just issued has read this buffer
+                    resid_load(tmR, my_stg, my_rbar, nslice & 1, MH == 1 ? colb + 128 : colb, MH == 1 ? rowb : rowb + 64);
+                }
+            }
+            ++nslice;
+        }
+    }
+}
+
 // One bf16 pair / fp32 pair of the output: columns (col, col + 1) of `row`; col is even.
 __device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col, float v0, float v1) {
     const bool two = col + 1 < p.N;
@@ -183,7 +271,8 @@ __device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col
 template <int BN, bool A_MN, bool B_MN, int MH>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
-                  const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD, const GemmParams p) {
+                  const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
+                  const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
     using S = GemmSmem<BN, MH>;
     constexpr int kStages = S::kStages;
     constexpr int BMT = BM * MH;   // rows of the CTA tile
@@ -196,6 +285,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint8_t* stg = smem + S::TILE_BYTES;   // output staging slices: [warpgroup][2][64 x 128 B]
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES + S::STG_BYTES);
     uint64_t* empty_bar = full_bar + kStages;
+    uint64_t* resid_bar = empty_bar + kStages;   // [warpgroup][2]: the residual slice TMA-loaded into that staging buffer has landed
 
     const int wg = threadIdx.x >> 7;
 
@@ -204,10 +294,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         tma_prefetch_desc(&tmA2);
         tma_prefetch_desc(&tmB);
         if (p.tma_store) tma_prefetch_desc(&tmD);
+        if (p.resid_tma) tma_prefetch_desc(&tmR);
         for (int i = 0; i < kStages; ++i) {
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 2);   // one arrival per consumer warpgroup
         }
+        for (int i = 0; i < 4; ++i) mbar_init(&resid_bar[i], 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -265,7 +357,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     constexpr uint32_t a_adv = A_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;   // per k16 step, in 16-B units
     constexpr uint32_t b_adv = B_MN ? (16 * 128) >> 4 : (16 * 2) >> 4;
     float acc[MH][NACC];
-    uint8_t* my_stg = stg + cw * 2 * S::SLICE_BYTES;
+    uint8_t* my_stg = stg + cw * 2 * kSliceBytes;
+    uint64_t* my_rbar = resid_bar + cw * 2;
     uint32_t nslice = 0;                       // staging slices this warpgroup has filled so far (buffer = nslice & 1)
     int stage = 0;
     uint32_t phase = 0;
@@ -276,6 +369,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int sp = rest / p.tiles_n;
         const int kb0 = sp * p.kb_per_split;
         const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+        // resid_tma: each residual slice is TMA-loaded into the staging buffer its output slice will use and completes on that buffer's
+        // barrier. The tile's first two go out two k-blocks before its mainloop ends, once the previous tile's stores have left both
+        // buffers; the third and fourth as soon as the store of the first and second has left its buffer.
+        const int kb_resid = max(kb0, kb1 - 2);
         int prev = -1;
         for (int kb = kb0; kb < kb1; ++kb) {
             mbar_wait(&full_bar[stage], phase);
@@ -295,6 +392,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 }
             }
             wgmma_commit();
+            if (p.resid_tma && kb == kb_resid && t == 0) {
+                const int r0 = tm * BMT + cw * MH * 64;
+                bulk_wait_group_read<0>();
+                resid_load(&tmR, my_stg, my_rbar, nslice & 1, tn * BN, r0);
+                if (tn * BN + 64 < p.N) resid_load(&tmR, my_stg, my_rbar, (nslice + 1) & 1, tn * BN + 64, r0);
+                else if (MH == 2) resid_load(&tmR, my_stg, my_rbar, (nslice + 1) & 1, tn * BN, r0 + 64);
+            }
             wgmma_wait<1>();   // the MMAs of the previous k-block have retired: its smem slot may be refilled
 #pragma unroll
             for (int h = 0; h < MH; ++h) fence_regs(acc[h]);
@@ -313,10 +417,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int cq = 2 * (lane & 3);
         if (p.tma_store) {
             // first the element-wise epilogue in place on the fragments (rows >= M and columns >= N are left as they are: the TMA
-            // store clips them), then 64 x 64 slices: the thread's rows r, r + 8 and, per 8-column group jj of the slice, the 4 bytes
-            // at column 8 jj + cq, written to 16-byte chunk (jj ^ (r & 7)) of the row — the TMA's 128B swizzle, and conflict-free:
-            // the 8 rows of a warp store land in 8 different chunks. r & 7 == lane / 4 for both rows.
-            if (p.bias || p.colscale || p.rowmask || p.resid) {
+            // store clips them), then the 64 x 64 slices; a TMA-loaded residual is added there, read from the address the output
+            // pair is written back to. The order stays bias -> AdaLN gate -> row mask -> + residual.
+            const bool resid_ldg = p.resid && !p.resid_tma;
+            if (p.bias || p.colscale || p.rowmask || resid_ldg) {
 #pragma unroll
                 for (int h = 0; h < MH; ++h) {
 #pragma unroll
@@ -325,7 +429,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         if (row >= p.M) continue;
                         const bool masked = p.rowmask && p.rowmask[row] == 0;
                         const float* cs = p.colscale ? p.colscale + (long long)(row / p.rows_per_batch) * p.N : nullptr;
-                        const __nv_bfloat16* rp = p.resid ? reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr : nullptr;
+                        const __nv_bfloat16* rp = resid_ldg ? reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr : nullptr;
 #pragma unroll
                         for (int j = 0; j < BN / 8; ++j) {
                             const int col = tn * BN + 8 * j + cq;
@@ -349,35 +453,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                 }
             }
-            const uint32_t swz = (uint32_t)(lane >> 2) << 4;
-            const uint32_t toff = (uint32_t)(wq * 16 + (lane >> 2)) * 128 + 2 * cq;
-#pragma unroll
-            for (int h = 0; h < MH; ++h) {
-                const int rowb = tm * BMT + (cw * MH + h) * 64;
-#pragma unroll
-                for (int s = 0; s < BN / 64; ++s) {
-                    const int colb = tn * BN + s * 64;
-                    if (colb >= p.N) break;                  // uniform across the warpgroup
-                    const uint32_t buf = smem_u32(my_stg + (nslice & 1) * S::SLICE_BYTES);
-                    if (t == 0) bulk_wait_group_read<1>();   // the store issued from this buffer two slices ago has read it
-                    named_bar_sync(1 + cw, 128);
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-#pragma unroll
-                        for (int jj = 0; jj < 8; ++jj) {
-                            const int j = s * 8 + jj;
-                            st_shared_u32(buf + toff + i * 8 * 128 + (((uint32_t)jj << 4) ^ swz), pack_bf16(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]));
-                        }
-                    }
-                    fence_proxy_async();                     // the generic-proxy smem writes, before the TMA (async proxy) reads them
-                    named_bar_sync(1 + cw, 128);
-                    if (t == 0) {
-                        tma_store_2d(&tmD, my_stg + (nslice & 1) * S::SLICE_BYTES, colb, rowb);   // rows >= M, columns >= N are clipped
-                        bulk_commit_group();
-                    }
-                    ++nslice;
-                }
-            }
+            // a copy of the slice loop per case keeps the plain path free of per-element residual branches
+            if (p.resid_tma) store_slices<true, BN, MH>(p, acc, &tmD, &tmR, my_stg, my_rbar, nslice, tm, tn, cw, wq, lane, t);
+            else store_slices<false, BN, MH>(p, acc, &tmD, &tmR, my_stg, my_rbar, nslice, tm, tn, cw, wq, lane, t);
         } else if (!p.geglu) {
 #pragma unroll
             for (int h = 0; h < MH; ++h) {
@@ -479,7 +557,7 @@ static int make_map_uncached(CUtensorMap* m, const void* ptr, int64_t inner, int
 }
 
 template <int BN, bool A_MN, bool B_MN, int MH>
-static int launch_gemm(const CUtensorMap (&tm)[4], const GemmParams& p, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap (&tm)[5], const GemmParams& p, cudaStream_t st) {
     using S = GemmSmem<BN, MH>;
     auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, MH>;
     static DeviceOnce once;   // one flag per template instantiation and device
@@ -488,7 +566,7 @@ static int launch_gemm(const CUtensorMap (&tm)[4], const GemmParams& p, cudaStre
         B200_REQUIRE(e == cudaSuccess, "gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
     const int grid = p.num_work < num_sms() ? p.num_work : num_sms();
-    kern<<<grid, kGemmThreads, S::TOTAL, st>>>(tm[0], tm[1], tm[2], tm[3], p);
+    kern<<<grid, kGemmThreads, S::TOTAL, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], p);
     return check_launch("gemm_wgmma_kernel");
 }
 
@@ -557,8 +635,8 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     if (!a->d_fp32) B200_REQUIRE((a->ldd % 8) == 0, "gemm: bf16 output pitch must be a multiple of 8");
     if (a->resid) B200_REQUIRE((a->ldr % 8) == 0, "gemm: residual pitch must be a multiple of 8");
 
-    CUtensorMap tm[4];
-    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2], &tD = tm[3];
+    CUtensorMap tm[5];
+    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2], &tD = tm[3], &tR = tm[4];
     int rc;
     const int64_t KA = a->A2 ? a->K1 : a->K;
     if (!a_mn) rc = make_map(&tA, a->A, KA, a->M, a->lda, BM);
@@ -575,13 +653,14 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     else rc = make_map(&tB, a->B, a->N, a->K, a->ldb, BK);
     if (rc) return rc;
     if (!a->d_fp32) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D) & 3) == 0, "gemm: bf16 output must be 4-byte aligned");
-    // TMA tile stores need a 16-byte aligned base (the pitch is a multiple of 16 bytes already); other bf16 outputs store from the fragments
-    p.tma_store = !a->d_fp32 && !a->geglu && (reinterpret_cast<uintptr_t>(a->D) & 15) == 0;
-    if (p.tma_store) {
-        if ((rc = make_map(&tD, a->D, a->N, a->M, a->ldd, 64))) return rc;
-    } else {
-        tD = tB;   // unused
-    }
+    // TMA tile stores and loads need 16-byte aligned bases (every pitch is a multiple of 16 bytes already); other bf16 outputs store
+    // from the fragments, and other residuals are read from global memory next to them
+    const auto a16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    p.tma_store = !a->d_fp32 && !a->geglu && a16(a->D);
+    p.resid_tma = p.tma_store && a->resid && a16(a->resid);
+    tD = tR = tB;   // unused unless set below
+    if (p.tma_store && (rc = make_map(&tD, a->D, a->N, a->M, a->ldd, 64))) return rc;
+    if (p.resid_tma && (rc = make_map(&tR, a->resid, a->N, a->M, a->ldr, 64))) return rc;
     if (a->geglu && a->D2) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D2) & 3) == 0, "gemm: GEGLU pre-activation buffer must be 4-byte aligned");
     if (a->resid) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->resid) & 3) == 0, "gemm: residual must be 4-byte aligned");
 

@@ -109,6 +109,11 @@ template <int N>
 __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 // named barriers (ids 1..15; __syncthreads owns id 0): bar.sync waits until `n` threads of the CTA have reached barrier `id`
 __device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 // counts the calling threads towards barrier `id` without waiting: the producer side of a producer / consumer hand-off
 __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
