@@ -47,6 +47,7 @@ struct GemmParams {
 };
 
 constexpr int GLU_GELU = 1, GLU_SILU = 2, GLU_RELU2 = 3;
+constexpr int ACT_GELU = 1;   // b200_gemm_args.act: plain exact-erf GELU of (z + bias), no GLU
 
 // Tiles: (BM * MH) x BN. MH == 2 gives each consumer warpgroup 128 rows (two m64 MMAs per k-step share one B tile); BN == 256 gives it
 // one m64n256 MMA per k-step. Both halve the smem -> tensor-core bytes per FLOP of the 128 x 128 tile; 128 fp32 accumulators per thread.
@@ -268,7 +269,9 @@ __device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col
     }
 }
 
-template <int BN, bool A_MN, bool B_MN, int MH>
+// ACT = ACT_GELU: GELU(z + bias) ahead of the rest of the epilogue (b200_gemm_args.act; instantiated for K-major A and B only).
+// ACT = 0 compiles to the instructions the kernel had before it took the parameter.
+template <int BN, bool A_MN, bool B_MN, int MH, int ACT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                   const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
@@ -420,7 +423,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             // store clips them), then the 64 x 64 slices; a TMA-loaded residual is added there, read from the address the output
             // pair is written back to. The order stays bias -> AdaLN gate -> row mask -> + residual.
             const bool resid_ldg = p.resid && !p.resid_tma;
-            if (p.bias || p.colscale || p.rowmask || resid_ldg) {
+            if (ACT || p.bias || p.colscale || p.rowmask || resid_ldg) {
 #pragma unroll
                 for (int h = 0; h < MH; ++h) {
 #pragma unroll
@@ -437,6 +440,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                             const bool two = col + 1 < p.N;
                             float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
                             if (p.bias) { v0 += __ldg(p.bias + col); if (two) v1 += __ldg(p.bias + col + 1); }
+                            if constexpr (ACT == ACT_GELU) { const float2 g = gelu_erf2(make_float2(v0, v1)); v0 = g.x; v1 = g.y; }
                             if (cs) { v0 *= __ldg(cs + col); if (two) v1 *= __ldg(cs + col + 1); }
                             if (masked) { v0 = 0.f; v1 = 0.f; }
                             if (rp) {
@@ -473,6 +477,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         const bool two = col + 1 < p.N;
                         float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
                         if (p.bias) { v0 += __ldg(p.bias + col); if (two) v1 += __ldg(p.bias + col + 1); }
+                        if constexpr (ACT == ACT_GELU) { const float2 g = gelu_erf2(make_float2(v0, v1)); v0 = g.x; v1 = g.y; }
                         if (cs) { v0 *= __ldg(cs + col); if (two) v1 *= __ldg(cs + col + 1); }
                         if (masked) { v0 = 0.f; v1 = 0.f; }
                         if (rp) {
@@ -556,10 +561,10 @@ static int make_map_uncached(CUtensorMap* m, const void* ptr, int64_t inner, int
     return 0;
 }
 
-template <int BN, bool A_MN, bool B_MN, int MH>
+template <int BN, bool A_MN, bool B_MN, int MH, int ACT = 0>
 static int launch_gemm(const CUtensorMap (&tm)[5], const GemmParams& p, cudaStream_t st) {
     using S = GemmSmem<BN, MH>;
-    auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, MH>;
+    auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, MH, ACT>;
     static DeviceOnce once;   // one flag per template instantiation and device
     {
         cudaError_t e = set_max_smem_once(once, kern, S::TOTAL);
@@ -632,6 +637,12 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
         B200_REQUIRE((a->ldd % 8) == 0 && (!a->D2 || (a->ldd2 % 8) == 0), "gemm: GEGLU output pitch must be a multiple of 8");
         B200_REQUIRE(!a->bias || (reinterpret_cast<uintptr_t>(a->bias) & 15) == 0, "gemm: GEGLU bias must be 16-byte aligned");
     }
+    B200_REQUIRE(a->act == 0 || a->act == ACT_GELU, "gemm: act=%d is not an activation code (0 none, 1 GELU)", (int)a->act);
+    if (a->act) {
+        B200_REQUIRE(!a->geglu && a->split_k >= 0 && a->split_k <= 1 && !a->d_fp32, "gemm: act needs a bf16 output without GLU or split-K");
+        B200_REQUIRE(!a_mn && !b_mn, "gemm: act is built for K-major operands only");
+        B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D) & 15) == 0, "gemm: act needs a 16-byte aligned output (TMA tile stores)");
+    }
     if (!a->d_fp32) B200_REQUIRE((a->ldd % 8) == 0, "gemm: bf16 output pitch must be a multiple of 8");
     if (a->resid) B200_REQUIRE((a->ldr % 8) == 0, "gemm: residual pitch must be a multiple of 8");
 
@@ -669,6 +680,11 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
         if (trace)
             fprintf(stderr, "GEMMTRACE %d %d %d amn=%d bmn=%d split=%d geglu=%d two=%d mh=%d epi=%d%d%d%d\n", p.M, p.N, p.K, (int)a_mn, (int)b_mn, split,
                     p.geglu, a->A2 != nullptr, wide ? 3 : MH, p.bias != nullptr, p.colscale != nullptr, p.rowmask != nullptr, p.resid != nullptr);
+    }
+    if (a->act) {
+        if (wide) return launch_gemm<256, false, false, 1, ACT_GELU>(tm, p, st);
+        if (MH == 2) return launch_gemm<128, false, false, 2, ACT_GELU>(tm, p, st);
+        return launch_gemm<128, false, false, 1, ACT_GELU>(tm, p, st);
     }
     if (wide) {
         if (!a_mn && !b_mn) return launch_gemm<256, false, false, 1>(tm, p, st);

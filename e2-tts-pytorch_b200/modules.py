@@ -1068,9 +1068,14 @@ class E2TTS(_PackOwner):
         self.embed_text = text_embed_klass(dim_text, num_embeds=text_num_embeds, **char_embed_kwargs)
         self.register_buffer('zero', torch.tensor(0.), persistent=False)
         self.velocity_consistency_weight = velocity_consistency_weight
-        # Vocos is a separate pretrained network fetched from the HF hub (e2_tts.py:1244): out of scope (SURVEY §2 row 10).
+        # Vocos (e2_tts.py:1244) is loaded from local files only: a checkpoint directory or a repo id already in the local HF cache.
+        # When neither resolves, vocos stays None and sample() refuses to decode (nothing is downloaded).
         self.vocos = None
         self._use_vocos_requested = use_vocos
+        if use_vocos:
+            from .vocos import Vocos, resolve_local
+            if resolve_local(pretrained_vocos_path) is not None:
+                self.vocos = Vocos.from_pretrained(pretrained_vocos_path)
 
     @property
     def device(self):
@@ -1135,10 +1140,12 @@ class E2TTS(_PackOwner):
                vocoder=None, return_raw_output=None, save_to_filename=None):
         """e2_tts.py:1332-1466. Fixed-grid ODE on t = linspace(0, 1, steps) (torchdiffeq semantics, SURVEY A.7)."""
         self.eval()
-        if not (exists(return_raw_output) and return_raw_output) and not exists(vocoder) and (self._use_vocos_requested or exists(save_to_filename)):
+        no_vocos = self._use_vocos_requested and not exists(self.vocos)
+        if not (exists(return_raw_output) and return_raw_output) and not exists(vocoder) and (no_vocos or exists(save_to_filename)):
             # fail BEFORE the ODE loop (124 transformer passes at the defaults), not after it
             raise NotImplementedError('Vocos decoding / audio saving needs the pretrained vocoder from the HF hub and is out of scope '
-                                      '(SURVEY.md §2 row 10): call sample(..., return_raw_output=True), pass `vocoder=`, or build E2TTS(use_vocos=False)')
+                                      '(SURVEY.md §2 row 10): call sample(..., return_raw_output=True), pass `vocoder=`, build '
+                                      'E2TTS(use_vocos=False), or pass a local `pretrained_vocos_path`')
         if cond.ndim == 2:
             cond = self.mel_spec(cond).transpose(1, 2)
             assert cond.shape[-1] == self.num_channels
@@ -1189,7 +1196,12 @@ class E2TTS(_PackOwner):
         if exists(return_raw_output) and return_raw_output:
             return out
         if exists(vocoder):
+            assert not exists(self.vocos), '`use_vocos` should not be turned on if you are passing in a custom `vocoder` on sampling'
             return vocoder(out.transpose(1, 2))
+        if exists(self.vocos):   # :1440-1451, the whole ragged batch in one decode: item b is out[b, :duration[b]]
+            audio = self.vocos.decode_padded(out, duration, db_to_amp=True)
+            hop = self.vocos.hop_length
+            return [audio[b, :int(n) * hop] for b, n in enumerate(duration.tolist())]
         return out
 
     @_on_module_device

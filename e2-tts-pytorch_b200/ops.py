@@ -62,9 +62,10 @@ def _zeros(shape, device):
 
 def gemm(A, B, M, N, K, *, lda=None, ldb=None, A2=None, lda2=0, K1=0, a_mn=False, b_mn=False, out=None, ldd=None,
          out_fp32=False, D2=None, ldd2=0, bias=None, colscale=None, rows_per_batch=0, rowmask=None, resid=None, ldr=0,
-         geglu=False, dropout_p=0.0, seed=0, split_k=1, force_tile=0, seed_dev=None, glu_mult=None):
+         geglu=False, dropout_p=0.0, seed=0, split_k=1, force_tile=0, seed_dev=None, glu_mult=None, act=0):
     """D[M,N] = epilogue(sum_k A[m,k] B[n,k]) on the wgmma GEMM (include/b200_e2tts.h: b200_gemm). geglu: the GLU activation code
-    (GLU_GELU, GLU_SILU, GLU_RELU2; True is GELU), glu_mult: fp32 [N/2] multiplier of the hidden units."""
+    (GLU_GELU, GLU_SILU, GLU_RELU2; True is GELU), glu_mult: fp32 [N/2] multiplier of the hidden units. act: ACT_GELU applies the
+    exact-erf GELU to (z + bias) without a GLU."""
     dev = A.device
     n_out = N // 2 if geglu else N
     if ldd is None:
@@ -75,17 +76,18 @@ def gemm(A, B, M, N, K, *, lda=None, ldb=None, A2=None, lda2=0, K1=0, a_mn=False
         A, lda if lda is not None else (M if a_mn else K), A2, lda2, K1,
         B, ldb if ldb is not None else (N if b_mn else K), M, N, K, int(a_mn), int(b_mn),
         out, ldd, int(out_fp32), D2, ldd2, bias, colscale, rows_per_batch,
-        rowmask, resid, ldr, int(geglu), float(dropout_p), int(seed), int(split_k), int(force_tile), seed_dev, glu_mult))
+        rowmask, resid, ldr, int(geglu), float(dropout_p), int(seed), int(split_k), int(force_tile), seed_dev, glu_mult, int(act)))
     lib.call('b200_gemm', args, _stream())
     return out
 
 
 _GEMM_FIELDS = ('A', 'lda', 'A2', 'lda2', 'K1', 'B', 'ldb', 'M', 'N', 'K', 'a_mn_major', 'b_mn_major', 'D', 'ldd', 'd_fp32', 'D2', 'ldd2',
                 'bias', 'colscale', 'rows_per_batch', 'rowmask', 'resid', 'ldr', 'geglu', 'dropout_p', 'seed', 'split_k', 'force_tile', 'seed_dev',
-                'glu_mult')
+                'glu_mult', 'act')
 
 # GLU activation codes of b200_gemm's GLU epilogue and b200_glu_bwd (x-transformers FeedForward: default, swish=True, relu_squared=True)
 GLU_GELU, GLU_SILU, GLU_RELU2 = 1, 2, 3
+ACT_GELU = 1   # b200_gemm_args.act
 
 
 def grad_weight(dY, X, T, n_out, n_in, *, ldy=None, ldx=None, out=None, ldd=None):
@@ -1038,3 +1040,34 @@ def melspec(wave, window, fb, n_fft, hop, wave_lens=None, out_bnd=False, center=
                       center=int(center), power=float(power), norm_scale=float(norm_scale))
     lib.call('b200_melspec_ex', a, _stream())
     return out
+
+
+# ---------------------------------------------------------------------------------------------------------- Vocos decoder (inference)
+
+
+def vocos_im2col(mel, lens, lda, db_to_amp=False):
+    """mel fp32 [B, T, C], lens int32 [B] -> bf16 [B * T, lda]: the k-7 embed Conv1d's operand (b200_vocos_im2col)."""
+    B, T, C = mel.shape
+    out = torch.empty((B * T, lda), device=mel.device, dtype=BF16)
+    lib.call('b200_vocos_im2col', _c(mel), lens, out, B, T, C, lda, int(bool(db_to_amp)), _stream())
+    return out
+
+
+def vocos_ln(x, lens, weight, bias, eps, B, T, D, conv_w=None, conv_b=None):
+    """LayerNorm of bf16 rows [B * T, D] (b200_vocos_ln), after the masked depthwise k-7 conv when conv_w is given
+    (b200_vocos_dwconv_ln); rows past an item's length are zeros."""
+    y = torch.empty((B * T, D), device=x.device, dtype=BF16)
+    a = lib.make_args('b200_vocos_ln_args', x=x, lens=lens, conv_w=conv_w, conv_b=conv_b, ln_w=weight, ln_b=bias, y=y, B=B, T=T, D=D,
+                      eps=float(eps))
+    lib.call('b200_vocos_dwconv_ln' if conv_w is not None else 'b200_vocos_ln', a, _stream())
+    return y
+
+
+def vocos_istft(spec, window, lens, B, T, n_fft, hop):
+    """ISTFTHead('same') after its Linear: spec fp32 [B * T, n_fft + 2] -> audio fp32 [B, T * hop] (b200_vocos_istft)."""
+    frames = torch.empty((B * T, n_fft), device=spec.device, dtype=F32)
+    audio = torch.empty((B, T * hop), device=spec.device, dtype=F32)
+    a = lib.make_args('b200_vocos_istft_args', spec=spec, window=window, lens=lens, frames=frames, audio=audio, B=B, T=T, n_fft=n_fft,
+                      hop=hop)
+    lib.call('b200_vocos_istft', a, _stream())
+    return audio

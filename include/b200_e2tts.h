@@ -72,6 +72,9 @@ typedef struct {
                            * 3 = 128 x 256 CTA tiles (one m64n256 MMA per warpgroup and k-step); auto picks 3 for M >= 512, N >= 256 */
     const uint64_t* seed_dev;   /* optional DEVICE word added to `seed` when the kernel runs (see "dropout seeds" below); NULL = none */
     const float* glu_mult;      /* optional GLU hidden-unit multiplier (see geglu above); NULL = none */
+    int32_t act;                /* 0: none; 1: exact-erf GELU of (z + bias) ahead of the rest of the epilogue (Vocos ConvNeXt pwconv1 ->
+                                 * nn.GELU, vocos/modules.py ConvNeXtBlock), the GLU epilogue's GELU polynomial. Needs K-major A and B, a
+                                 * bf16 16-byte aligned D (TMA tile stores); refused with geglu, split_k > 1 or d_fp32. */
 } b200_gemm_args;
 int b200_gemm(const b200_gemm_args* a, b200_stream_t stream);
 
@@ -411,6 +414,44 @@ int b200_melspec_ex(const b200_melspec_args* a, b200_stream_t stream);
 int b200_melspec(const float* wave, const float* window, const float* fb, float* out, int32_t B, int32_t nw, int32_t n_fft,
                  int32_t hop, int32_t n_mels, int32_t* ws_bands, const int32_t* wave_lens, int32_t out_bnd, b200_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Vocos mel decoder (the reference's E2TTS(use_vocos=True): Vocos.from_pretrained e2_tts.py:1244, decode of each sampled mel
+ * :1440-1451; published vocos package: VocosBackbone with ConvNeXt blocks, ISTFTHead with 'same' padding). Inference only.
+ * A ragged batch is held as rows [B * T] (T = the longest item, row b * T + t = frame t of item b) with lens[b] frames per item
+ * (int32 [B], 1 <= lens[b] <= T); every kernel treats item b as if it were decoded alone.
+ *
+ * im2col of the backbone's embed Conv1d(C -> dim, k 7, pad 3): mel fp32 [B, T, C] -> A bf16 [B * T, lda], column c * 7 + j =
+ *   mel[b, t + j - 3, c], 0 outside [0, lens[b]) and on rows t >= lens[b]; columns 7C .. lda-1 are 0 (lda % 8 == 0, >= 7C). The embed
+ *   is then one b200_gemm against the Conv1d weight viewed [dim, 7C]. db_to_amp != 0: each value is 10^(x / 20) (torchaudio
+ *   DB_to_amplitude(x, ref=1, power=0.5), e2_tts.py:1444), formed in double and rounded to fp32, before the bf16 rounding. */
+int b200_vocos_im2col(const float* mel, const int32_t* lens, void* A, int32_t B, int32_t T, int32_t C, int32_t lda, int32_t db_to_amp,
+                      b200_stream_t stream);
+/* LayerNorm over D channels (nn.LayerNorm(dim, eps) of the backbone: `norm`, `final_layer_norm`, each block's `norm`), bf16 x / y
+ * [B * T, D] with fp32 math, D a multiple of 64 up to 1024; rows t >= lens[b] are written as zeros and never read.
+ * b200_vocos_dwconv_ln first applies the block's masked depthwise Conv1d(k 7, pad 3) + bias (conv_w fp32 [D, 7], conv_b [D]), zero-
+ * padded at the item's own ends; b200_vocos_ln is the LayerNorm alone (conv_w, conv_b unused). y must not alias x. */
+typedef struct {
+    const void* x; const int32_t* lens;
+    const float *conv_w, *conv_b, *ln_w, *ln_b;
+    void* y;
+    int32_t B, T, D; float eps;
+} b200_vocos_ln_args;
+int b200_vocos_dwconv_ln(const b200_vocos_ln_args* a, b200_stream_t stream);
+int b200_vocos_ln(const b200_vocos_ln_args* a, b200_stream_t stream);
+/* ISTFTHead('same') after its Linear (vocos/heads.py ISTFTHead.forward + vocos/spectral_ops.py ISTFT): spec fp32 [B * T, n_fft + 2] =
+ * [log-magnitude (n_fft/2 + 1) | phase (n_fft/2 + 1)]; S = min(exp(mag), 1e2) (cos p + i sin p); per frame irfft(S, n_fft) (the
+ * imaginary parts of bins 0 and n_fft/2 are dropped) times window fp32 [n_fft], written to the caller's workspace frames fp32
+ * [B * T, n_fft]; then each output sample sums its frames in increasing frame order (no atomics: deterministic), with the
+ * overlap-added window^2 envelope of the item's own frames, trimmed by (n_fft - hop) / 2 at both ends: audio fp32 [B, T * hop],
+ * item b holding lens[b] * hop samples and exact zeros after them. Refused: n_fft not a power of two in [64, 4096], hop outside
+ * [1, n_fft], (n_fft - hop) odd. Lengths are read on the device and clamped to [0, T] (the host wrapper refuses lengths < 1
+ * before any launch). Two launches. */
+typedef struct {
+    const float* spec; const float* window; const int32_t* lens;
+    float* frames; float* audio;
+    int32_t B, T, n_fft, hop;
+} b200_vocos_istft_args;
+int b200_vocos_istft(const b200_vocos_istft_args* a, b200_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Around the forward/backward step (SURVEY §8e, §8f row 1): multi-tensor gradient gather for ONE ncclAllReduce per step, global
