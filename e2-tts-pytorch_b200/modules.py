@@ -9,6 +9,7 @@ import contextlib
 import copy
 import ctypes
 import math
+import numbers
 import random as pyrandom
 from collections import namedtuple
 from functools import partial
@@ -859,6 +860,7 @@ class MelSpec(Module):
         window = self.mel_stft.spectrogram.window.double()
         self.norm_scale = {False: 1.0, 'frame_length': filter_length ** -0.5}.get(normalize, float(window.square().sum().rsqrt()))
         self.register_buffer('dummy', torch.tensor(0), persistent=False)
+        self._resample_table = None     # ops.ResampleTable of every rate pair collate() has met; its taps: buffer `resample_taps`
 
     def frames(self, n):
         """frames of n samples (int or tensor): 1 + n // hop centred (even n_fft), 1 + (n - n_fft) // hop without centring"""
@@ -878,15 +880,27 @@ class MelSpec(Module):
             self.to(inp.device)
         return self._melspec(inp)
 
-    def collate(self, waves, lens=None):
-        """On-device data path (SURVEY §8f row 3): what the reference does per item on CPU workers — `MelSpec` in HFDataset.__getitem__
-        (trainer.py:101-131) — and per batch in `collate_fn` (:61-82: zero-pad the mels to the longest, lengths) plus the trainer's
-        `rearrange(batch['mel'], 'b d n -> b n d')` (:253), as ONE kernel launch over the ragged batch.
-        waves: list of 1-D fp32 tensors at `sampling_rate` (resampling is the dataset's job) or a zero-padded [B, nw_max] tensor with
-        `lens` (samples per sequence). Returns dict(mel [B, n_frames_max, n_mels] fp32, mel_lengths [B] int64) — pass as
+    def collate(self, waves, lens=None, sample_rates=None):
+        """On-device data path (SURVEY §8f row 3): what the reference does per item on CPU workers — the resampling and `MelSpec` of
+        HFDataset.__getitem__ (trainer.py:101-131) — and per batch in `collate_fn` (:61-82: zero-pad the mels to the longest,
+        lengths) plus the trainer's `rearrange(batch['mel'], 'b d n -> b n d')` (:253), as at most two kernel launches over the
+        ragged batch.
+        waves: list of 1-D fp32 tensors or a zero-padded [B, nw_max] tensor with `lens` (samples per sequence).
+        sample_rates: None (every item is at `sampling_rate`), an int, or a per-item list / 1-D tensor of positive integer rates.
+        Items at another rate are resampled to `sampling_rate` first, as the dataset's torchaudio.transforms.Resample(rate,
+        sampling_rate) does (same fp32 taps, same output length), all rates in one launch (ops.resample); items already at
+        `sampling_rate` pass through unchanged, and a batch with no other rate takes no resampling launch at all.
+        Returns dict(mel [B, n_frames_max, n_mels] fp32, mel_lengths [B] int64) — pass as
         `model(batch['mel'], text=..., lens=batch['mel_lengths'])`. A length past the padded wave counts as the padded length;
         an item too short for one frame — at most n_fft/2 samples centred (too short for the reflect padding: the reference's
-        MelSpec raises on it), fewer than n_fft without centring — has zero frames and its mel_lengths entry is 0."""
+        MelSpec raises on it), fewer than n_fft without centring — has zero frames and its mel_lengths entry is 0.
+        n_frames_max is that of the longest resampled item with a list, and that of the padded width resampled at the slowest
+        conversion present with a padded tensor."""
+        B = len(waves) if isinstance(waves, (list, tuple)) else waves.shape[0]
+        rates = self._collate_rates(sample_rates, B)
+        if rates is not None and all(r == self.sampling_rate for r in rates):
+            rates = None
+        host_lens = [w.shape[-1] for w in waves] if isinstance(waves, (list, tuple)) else None
         if isinstance(waves, (list, tuple)):
             dev = self.dummy.device if self.dummy.device.type == 'cuda' else waves[0].device
             lens = torch.tensor([w.shape[-1] for w in waves], dtype=torch.int32)
@@ -901,12 +915,59 @@ class MelSpec(Module):
             lens = lens.to(device=waves.device, dtype=torch.int32)
         if self.dummy.device != waves.device:
             self.to(waves.device)
+        if rates is not None:
+            waves, lens = self._resample(waves.to(F32).contiguous(), lens.contiguous(), rates, host_lens)
         mel = self._melspec(waves, wave_lens=lens.contiguous(), out_bnd=True)
         lens = lens.long().clamp(max=waves.shape[1])      # the kernel clamps the same way
         long_enough = lens > self.n_fft // 2 if self.center else lens >= self.n_fft
         mel_lengths = torch.where(long_enough, self.frames(lens), 0)
         n_max = int(self.frames(waves.shape[1]))
         return dict(mel=mel[:, :n_max], mel_lengths=mel_lengths)
+
+    @staticmethod
+    def _collate_rates(sample_rates, B):
+        """sample_rates -> a list of B ints, or None; what torchaudio refuses (a non-integer rate) or cannot mean (a rate <= 0) is a
+        ValueError"""
+        if sample_rates is None:
+            return None
+        if hasattr(sample_rates, 'ndim') and hasattr(sample_rates, 'tolist'):     # a tensor or a numpy array
+            if sample_rates.ndim > 1:
+                raise ValueError(f'sample_rates must be an int or a 1-D list / tensor of rates (got shape {tuple(sample_rates.shape)})')
+            sample_rates = sample_rates.tolist()
+        rates = list(sample_rates) if isinstance(sample_rates, (list, tuple)) else [sample_rates] * B
+        if len(rates) != B:
+            raise ValueError(f'sample_rates has {len(rates)} entries for a batch of {B}')
+        out = []
+        for r in rates:
+            if isinstance(r, bool) or not isinstance(r, numbers.Real) or not math.isfinite(r) or int(r) != r or r <= 0:
+                raise ValueError(f'sample rates must be positive integers (got {r!r}), as torchaudio.transforms.Resample requires')
+            out.append(int(r))
+        return out
+
+    def _rate_table(self, rates, device):
+        """the ops.ResampleTable of every rate pair met so far, rebuilt (host tap tables, one upload) when `rates` bring a new one;
+        its data is the non-persistent buffer `resample_taps`, so it follows .to() and stays out of the state_dict"""
+        pairs = {(r, self.sampling_rate) for r in rates if r != self.sampling_rate}
+        table = self._resample_table
+        if table is None or not pairs <= set(table.index):
+            table = self._resample_table = ops.ResampleTable(sorted(pairs | set(table.index if table else ())), device=device)
+            self.register_buffer('resample_taps', table.data, persistent=False)
+        table.data = self.resample_taps
+        return table
+
+    def _resample(self, waves, lens, rates, host_lens):
+        """one b200_resample launch to `sampling_rate` over the batch (items at that rate pass through) -> (waves [B, nr], lens)"""
+        target = self.sampling_rate
+        table = self._rate_table(rates, waves.device)
+        nw = waves.shape[1]
+        if host_lens is not None:
+            nr = max(ops.resample_length(n, r, target) if r != target else n for n, r in zip(host_lens, rates))
+        else:
+            nr = max(ops.resample_length(nw, r, target) if r != target else nw for r in set(rates))
+        idx = torch.tensor([table.index[(r, target)] if r != target else -1 for r in rates], dtype=torch.int32)
+        if waves.is_cuda:
+            idx = idx.pin_memory().to(waves.device, non_blocking=True)
+        return ops.resample(waves, lens, idx, table, nr)
 
 
 # ----------------------------------------------------------------------------------------------------------------------

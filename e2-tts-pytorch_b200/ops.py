@@ -8,6 +8,8 @@ inputs (so autograd / DDP see per-parameter gradients) next to their packed bf16
 """
 from __future__ import annotations
 
+import math
+
 import torch
 from torch.autograd import Function
 from torch.autograd.function import once_differentiable
@@ -1040,6 +1042,103 @@ def melspec(wave, window, fb, n_fft, hop, wave_lens=None, out_bnd=False, center=
                       center=int(center), power=float(power), norm_scale=float(norm_scale))
     lib.call('b200_melspec_ex', a, _stream())
     return out
+
+
+# ------------------------------------------------------------------------------------------------ resampling (trainer.py:116-118)
+# torchaudio.transforms.Resample(orig, new) with the defaults the reference's HFDataset uses: sinc_interp_hann, lowpass_filter_width 6,
+# rolloff 0.99, taps built in float64 and cached as float32.
+RESAMPLE_LOWPASS_WIDTH, RESAMPLE_ROLLOFF = 6, 0.99
+
+
+def resample_pair(orig, new):
+    """(orig', new'): the rates reduced by their gcd, as torchaudio reduces them"""
+    g = math.gcd(orig, new)
+    return orig // g, new // g
+
+
+def resample_length(n, orig, new):
+    """torchaudio's output length for n samples: ceil(torch.as_tensor(new' n / orig')), a float32 ceil (one short of the exact
+    ceiling at some lengths), never more than the new' (n // orig' + 1) samples its strided convolution produces"""
+    o, w = resample_pair(orig, new)
+    return min(int(torch.ceil(torch.as_tensor(w * n / o))), w * (n // o + 1))
+
+
+def resample_taps(orig, new):
+    """The banded form of torchaudio's fp32 tap table for orig -> new: (orig', new', width, first int32 [new'], count int32 [new'],
+    taps fp32 [sum count]). Phase k of the full table [new', 2 width + orig'] is zero outside columns first[k] .. first[k] + count[k]
+    - 1. The values are torchaudio's construction (_get_sinc_resample_kernel with dtype=None: the phase offsets -k / new' divided in
+    float32, everything else in float64, rounded once to float32), evaluated only on the columns around each phase's centre: every
+    other column has its time clamped to +-lowpass_filter_width, where the tap is 0 in fp32, and that is checked here."""
+    o, n = resample_pair(orig, new)
+    lw, base = RESAMPLE_LOWPASS_WIDTH, min(o, n) * RESAMPLE_ROLLOFF
+    width = math.ceil(lw * o / base)
+    cols_total = 2 * width + o
+    span = math.ceil(lw * o / base) + 2
+    centre = torch.arange(n, dtype=torch.float64) * o / n + width        # column where phase k's time is 0
+    m = (centre - span).floor().long().clamp(min=0)[:, None] + torch.arange(2 * span + 2)
+    inside = m < cols_total
+    t = torch.arange(0, -n, -1)[:, None] / n + (m - width).to(torch.float64) / o
+    t *= base
+    t = t.clamp_(-lw, lw)
+    window = torch.cos(t * math.pi / lw / 2) ** 2
+    t *= math.pi
+    taps = torch.where(t == 0, torch.tensor(1.0).to(t), t.sin() / t)
+    taps *= window * (base / o)
+    taps = torch.where(inside, taps.to(torch.float32), 0.0)
+    nz = taps != 0
+    if bool((nz[:, 0] & (m[:, 0] > 0)).any() or (nz[:, -1] & (m[:, -1] < cols_total - 1)).any()):
+        raise RuntimeError(f'resample_taps({orig}, {new}): a non-zero tap at the edge of the evaluated columns')
+    col = torch.arange(m.shape[1])
+    lo = torch.where(nz, col, m.shape[1]).min(1).values
+    hi = torch.where(nz, col, -1).max(1).values
+    first = m.gather(1, lo[:, None])[:, 0]
+    count = hi - lo + 1
+    keep = (col >= lo[:, None]) & (col <= hi[:, None])
+    return o, n, width, first.to(torch.int32), count.to(torch.int32), taps[keep].contiguous()
+
+
+RESAMPLE_PAIR_WORDS = 6    # per rate pair: orig', new', width, phase offset, tap offset, taps; per phase: first tap, count, tap offset
+
+
+class ResampleTable:
+    """The rate pairs of one b200_resample launch packed into one int32 tensor (taps as their fp32 bits): [pairs | phases | taps],
+    in the layout include/b200_e2tts.h documents. `index[(orig, new)]` is the pair's slot (the b200_resample pair_idx value)."""
+
+    def __init__(self, pairs, device=None):
+        self.index, words, phases, taps = {}, [], [], []
+        n_phases = n_taps = 0
+        self.max_pair_words = 0
+        for p in pairs:
+            o, n, width, first, count, t = resample_taps(*p)
+            self.index[p] = len(words)
+            words.append([o, n, width, n_phases, n_taps, t.numel()])
+            off = torch.cumsum(count, 0, dtype=torch.int32) - count
+            phases.append(torch.stack([first, count, off], 1).flatten())
+            taps.append(t.view(torch.int32))
+            self.max_pair_words = max(self.max_pair_words, 3 * n + t.numel())
+            n_phases += n
+            n_taps += t.numel()
+        self.n_pairs, self.n_phases, self.n_taps = len(words), n_phases, n_taps
+        head = torch.tensor(words, dtype=torch.int32).flatten()
+        self.data = torch.cat([head, *phases, *taps]).to(device)
+
+    def pointers(self):
+        base = self.data.data_ptr()
+        return base, base + 4 * RESAMPLE_PAIR_WORDS * self.n_pairs, base + 4 * (RESAMPLE_PAIR_WORDS * self.n_pairs + 3 * self.n_phases)
+
+
+def resample(wave, wave_lens, pair_idx, table, nr):
+    """b200_resample (trainer.py:116-118, torchaudio.transforms.Resample per item): fp32 [B, nw] with wave_lens int32 [B] -> (fp32
+    [B, nr], out_lens int32 [B]). pair_idx int32 [B]: the item's slot in `table` (a ResampleTable on the wave's device), or -1 to
+    pass the item through. Samples at or past wave_lens[b] count as zero and are never read; out[b, j] = +0 for j >= out_lens[b]."""
+    B, nw = wave.shape
+    out = torch.empty((B, nr), device=wave.device, dtype=F32)
+    out_lens = torch.empty(B, device=wave.device, dtype=torch.int32)
+    pairs, phases, taps = table.pointers()
+    a = lib.make_args('b200_resample_args', wave=_c(wave), wave_lens=wave_lens, pair_idx=pair_idx, pairs=pairs, phases=phases, taps=taps,
+                      out=out, out_lens=out_lens, B=B, nw=nw, nr=nr, n_pairs=table.n_pairs, max_pair_words=table.max_pair_words)
+    lib.call('b200_resample', a, _stream())
+    return out, out_lens
 
 
 # ---------------------------------------------------------------------------------------------------------- Vocos decoder (inference)

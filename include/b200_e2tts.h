@@ -414,6 +414,33 @@ int b200_melspec_ex(const b200_melspec_args* a, b200_stream_t stream);
 int b200_melspec(const float* wave, const float* window, const float* fb, float* out, int32_t B, int32_t nw, int32_t n_fft,
                  int32_t hop, int32_t n_mels, int32_t* ws_bands, const int32_t* wave_lens, int32_t out_bnd, b200_stream_t stream);
 
+/* Resampling ahead of the mel (trainer.py:116-118: HFDataset.__getitem__ builds torchaudio.transforms.Resample(sample_rate, target)
+ * for every item whose rate is not the target and applies it in fp32): a ragged batch of mixed rates in ONE launch.
+ * wave fp32 [B, nw] with wave_lens int32 [B] (clamped to [0, nw]; samples at or past an item's length count as zero and are never
+ * read); pair_idx int32 [B]: the item's rate pair in the table below, or < 0 to pass the item through unchanged (equal rates).
+ * Rate pair p (orig', new': the rates reduced by their gcd; width: torchaudio's ceil(6 orig' / (0.99 min(orig', new')))):
+ *   out[b, j] = sum_i taps[i] * x[s + i] over the band of phase k = j mod new', s = (j div new') orig' - width + first[k], the taps
+ *   summed in increasing i by one fma chain (a fixed order: an item gives the same bits alone or in any batch);
+ *   out_lens[b] = min(ceilf((float)((double)(new' L) / orig')), new' (L div orig' + 1), nr) for L = wave_lens[b] (torchaudio's
+ *   length: its ceil runs in float32); a passed-through item has out_lens[b] = min(L, nr) and out[b, j] = x[j], bit for bit.
+ *   out[b, j] = +0 for out_lens[b] <= j < nr. A pair_idx >= n_pairs gives out_lens[b] = 0.
+ * The table is the banded form of torchaudio's fp32 taps (sinc_interp_hann, lowpass_filter_width 6, rolloff 0.99): per phase only
+ * the contiguous run of non-zero taps, in three caller-built device arrays:
+ *   pairs  int32 [n_pairs * 6]: orig', new', width, first phase (index into phases / 3), first tap (index into taps), taps of the pair;
+ *   phases int32 [3 per phase]: first non-zero column of the phase's row in torchaudio's [new', 2 width + orig'] table, count, offset
+ *          of its taps from the pair's first tap;
+ *   taps   fp32: each pair's bands, phase after phase.
+ * max_pair_words >= 3 new' + taps of every pair: when it is at most 12288 (48 KB) each block stages its item's pair in shared
+ *   memory, otherwise the taps are read from global memory.
+ * Refused before any launch: B < 1, nw < 0, nr < 0, n_pairs < 0, max_pair_words < 0, a missing pointer. */
+typedef struct {
+    const float* wave; const int32_t* wave_lens; const int32_t* pair_idx;
+    const int32_t *pairs, *phases; const float* taps;
+    float* out; int32_t* out_lens;
+    int32_t B, nw, nr, n_pairs, max_pair_words;
+} b200_resample_args;
+int b200_resample(const b200_resample_args* a, b200_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------------
  * Vocos mel decoder (the reference's E2TTS(use_vocos=True): Vocos.from_pretrained e2_tts.py:1244, decode of each sampled mel
  * :1440-1451; published vocos package: VocosBackbone with ConvNeXt blocks, ISTFTHead with 'same' padding). Inference only.
