@@ -21,7 +21,7 @@ import torch.nn.functional as F
 from torch import nn
 from torch.nn import Module, ModuleList
 
-from . import lib, ops
+from . import lib, ode, ops
 
 LossBreakdown = namedtuple('LossBreakdown', ['flow', 'velocity_consistency'])  # e2_tts.py:71
 E2TTSReturn = namedtuple('E2TTS', ['loss', 'cond', 'pred_flow', 'pred_data', 'loss_breakdown'])  # e2_tts.py:73
@@ -80,6 +80,62 @@ def _unsupported(name, value, ref):
     raise NotImplementedError(
         f'{name}={value!r} is a non-default research switch of the reference ({ref}) for which no CUDA kernel is built; '
         f'there is no fallback path (SURVEY.md §2 row 8)')
+
+
+_ODE_REF = 'e2_tts.py:1122-1126'
+# torchdiffeq methods without a solver here, and why
+_ODE_REFUSED = {
+    'dopri8': "its 13-stage tableau is not restated",
+    'heun2': "only some torchdiffeq versions have it", 'heun3': "only some torchdiffeq versions have it",
+    'explicit_adams': "a multistep method", 'implicit_adams': "a multistep method", 'fixed_adams': "a multistep method",
+    'scipy_solver': "a host solver",
+}
+
+
+def _real(v):
+    return isinstance(v, numbers.Real) and not isinstance(v, bool)
+
+
+def _parse_odeint_kwargs(kw):
+    """E2TTS(odeint_kwargs) -> dict(method, rtol, atol, options) for E2TTS.sample. 'midpoint' and 'euler' run the fixed-grid loop and
+    take the other keys as they always did (ignored); a dict without 'method' keeps that midpoint loop. 'rk4' and the adaptive
+    methods of ode.py take `atol` / `rtol` as Python floats (torchdiffeq's defaults 1e-9 / 1e-7 when missing) and `options` with only
+    first_step, safety, ifactor, dfactor and max_num_steps (ignored by 'rk4', as torchdiffeq's fixed-grid solvers ignore them).
+    Everything else raises NotImplementedError naming the key."""
+    method = kw.get('method', 'midpoint')
+    if method in ('midpoint', 'euler'):
+        return dict(method=method)
+    if method != 'rk4' and method not in ode.ADAPTIVE_METHODS:
+        why = _ODE_REFUSED.get(method, 'not a torchdiffeq method this package solves') if isinstance(method, str) else 'not a method name'
+        _unsupported("odeint_kwargs['method']", method, f'{_ODE_REF}; {why}')
+    for key in kw:
+        if key not in ('method', 'atol', 'rtol', 'options'):
+            _unsupported(f'odeint_kwargs[{key!r}]', kw[key], _ODE_REF)
+    out = dict(method=method)
+    for key in ('rtol', 'atol'):
+        v = kw.get(key, ode.DEFAULT_TOL[key])
+        if not _real(v):
+            _unsupported(f'odeint_kwargs[{key!r}]', v, f'{_ODE_REF}; a tolerance is a Python float here, not a tensor')
+        if not (math.isfinite(v) and v >= 0):
+            raise ValueError(f'odeint_kwargs[{key!r}]={v!r}: want a finite tolerance >= 0')
+        out[key] = float(v)
+    options = kw.get('options') or {}
+    if not isinstance(options, dict):
+        _unsupported("odeint_kwargs['options']", options, _ODE_REF)
+    for key, v in options.items():
+        if key not in ode.DEFAULT_OPTIONS:
+            _unsupported(f'odeint_kwargs[\'options\'][{key!r}]', v, _ODE_REF)
+        if key == 'max_num_steps':
+            if not isinstance(v, numbers.Integral) or isinstance(v, bool) or v < 1:
+                raise ValueError(f"odeint_kwargs['options']['max_num_steps']={v!r}: want an int >= 1")
+        elif key == 'first_step' and v is None:
+            continue
+        elif not _real(v):
+            _unsupported(f'odeint_kwargs[\'options\'][{key!r}]', v, f'{_ODE_REF}; a Python float here, not a tensor')
+        elif not (math.isfinite(v) and v > 0):
+            raise ValueError(f"odeint_kwargs['options'][{key!r}]={v!r}: want a finite value > 0")
+    out['options'] = {k: (int(v) if k == 'max_num_steps' else v if v is None else float(v)) for k, v in options.items()}
+    return out
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -1096,8 +1152,7 @@ class E2TTS(_PackOwner):
         super().__init__()
         if num_freq_tokens != 1:
             _unsupported('num_freq_tokens', num_freq_tokens, 'e2_tts.py:1130')
-        if odeint_kwargs.get('method', 'midpoint') not in ('midpoint', 'euler'):
-            _unsupported('odeint_kwargs', odeint_kwargs, 'e2_tts.py:1122-1126 (fixed-grid midpoint/euler only)')
+        _parse_odeint_kwargs(odeint_kwargs)
         self.num_freq_tokens, self.has_freq_axis = 1, False
         if isinstance(transformer, dict):
             transformer = dict(transformer)
@@ -1199,7 +1254,9 @@ class E2TTS(_PackOwner):
     @_on_module_device
     def sample(self, cond, *, text=None, lens=None, duration=None, steps=32, cfg_strength=1., cfg_null_model=None, max_duration=4096,
                vocoder=None, return_raw_output=None, save_to_filename=None):
-        """e2_tts.py:1332-1466. Fixed-grid ODE on t = linspace(0, 1, steps) (torchdiffeq semantics, SURVEY A.7)."""
+        """e2_tts.py:1332-1466. The ODE on t = linspace(0, 1, steps) with the torchdiffeq method of `odeint_kwargs` (SURVEY A.7): the
+        fixed-grid midpoint / euler loop below, or rk4 and the adaptive Runge–Kutta methods of ode.py."""
+        ode_kw = _parse_odeint_kwargs(self.odeint_kwargs)   # odeint_kwargs is a plain attribute: checked again before any work
         self.eval()
         no_vocos = self._use_vocos_requested and not exists(self.vocos)
         if not (exists(return_raw_output) and return_raw_output) and not exists(vocoder) and (no_vocos or exists(save_to_filename)):
@@ -1240,19 +1297,22 @@ class E2TTS(_PackOwner):
         y = _rng.draw('y0', lambda: torch.randn_like(cond))
         ts_host = torch.linspace(0, 1, steps)          # fixed grid (torchdiffeq semantics); step sizes stay host floats: no device sync per step
         ts = ts_host.to(dev)
-        method = self.odeint_kwargs.get('method', 'midpoint')
+        method = ode_kw.pop('method')
         # weights are fixed for the whole solve: pack each model's operands once (fresh), not once per function evaluation
         freeze_null = cfg_null_model._pack()[0].freeze() if exists(cfg_null_model) else contextlib.nullcontext()
         with self._pack()[0].freeze(), freeze_null:
             fn_eval = fn   # (one function evaluation as a CUDA graph was measured: -1 % at cfg5, but re-capturing per call costs the e2e path 19 %)
-            for i in range(steps - 1):
-                t0, dt = ts[i], float(ts_host[i + 1] - ts_host[i])
-                if method == 'euler':
-                    y = ops.axpy(y, fn_eval(t0, y), dt)
-                else:
-                    half = 0.5 * dt
-                    ymid = ops.axpy(y, fn_eval(t0, y), half)
-                    y = ops.axpy(y, fn_eval(t0 + half, ymid), dt)
+            if method not in ('midpoint', 'euler'):   # rk4 and the adaptive Runge–Kutta methods
+                y = ode.odeint(fn_eval, y, steps, method, **ode_kw)
+            else:
+                for i in range(steps - 1):
+                    t0, dt = ts[i], float(ts_host[i + 1] - ts_host[i])
+                    if method == 'euler':
+                        y = ops.axpy(y, fn_eval(t0, y), dt)
+                    else:
+                        half = 0.5 * dt
+                        ymid = ops.axpy(y, fn_eval(t0, y), half)
+                        y = ops.axpy(y, fn_eval(t0 + half, ymid), dt)
         out = torch.where(cond_mask, cond, y)
         if exists(return_raw_output) and return_raw_output:
             return out

@@ -1022,6 +1022,54 @@ def cfg_combine(pred, null_pred, strength, remove_parallel, keep_frac):
     return out
 
 
+ODE_MAX_SOURCES = 7
+
+
+def _ode_sources(ks, ws, prefix):
+    """k0..k{S-1} and their fp32 weights as keyword arguments of the b200_ode_* structs"""
+    if not 1 <= len(ks) == len(ws) <= ODE_MAX_SOURCES:
+        raise ValueError(f'{len(ks)} sources with {len(ws)} weights: want 1..{ODE_MAX_SOURCES} of each')
+    kw = {f'k{j}': _c(k) for j, k in enumerate(ks)}
+    kw.update({f'{prefix}{j}': float(w) for j, w in enumerate(ws)})
+    return kw, len(ks)
+
+
+def ode_combine(y0, ks, ws, out=None):
+    """y0 + sum_j ws[j] * ks[j] (fp32): stage inputs and updates of the Runge–Kutta methods of E2TTS.sample (SURVEY A.7)."""
+    out = torch.empty_like(y0) if out is None else out
+    kw, S = _ode_sources(ks, ws, 'w')
+    lib.call('b200_ode_combine', lib.make_args('b200_ode_combine_args', y0=_c(y0), S=S, out=out, n=y0.numel(), **kw), _stream())
+    return out
+
+
+def ode_step_error(y0, ks, err_w, y1, atol, rtol, ws, ratio, sol_w=None):
+    """The error ratio rms((sum_j err_w[j] ks[j]) / (atol + rtol max(|y0|, |y1|))) of one adaptive step into `ratio` (fp32 [1]);
+    with `sol_w`, y1 = y0 + sum_j sol_w[j] ks[j] is written first. ws: fp64 workspace of the reduction."""
+    kw, S = _ode_sources(ks, err_w, 'e')
+    kw.update({f's{j}': float(w) for j, w in enumerate(sol_w or ())})
+    lib.call('b200_ode_step_error', lib.make_args('b200_ode_step_error_args', y0=_c(y0), S=S, y1=y1, write_y1=int(sol_w is not None),
+                                                  atol=float(atol), rtol=float(rtol), ws=ws, ws_len=ws.numel(), ratio=ratio,
+                                                  n=y0.numel(), **kw), _stream())
+    return ratio
+
+
+def ode_scaled_norms(y0, a, b, c, atol, rtol, ws, out):
+    """out[0] = rms(a / scale) (a may be None), out[1] = rms((b - c) / scale) (c None: rms(b / scale)), scale = atol + |y0| rtol:
+    the norms of the initial step size. ws: fp64 workspace of 2 * ws_len doubles, out: fp32 [2]."""
+    lib.call('b200_ode_scaled_norms', lib.make_args('b200_ode_norms_args', y0=_c(y0), a=_c(a), b=_c(b), c=_c(c), atol=float(atol),
+                                                    rtol=float(rtol), ws=ws, ws_len=ws.numel() // 2, out=out, n=y0.numel()), _stream())
+    return out
+
+
+def ode_dense_output(y0, y1, ks, mid_w, dt, x, out=None):
+    """The quartic dense output of an accepted step at x = (t - t0) / (t1 - t0), with y_mid = y0 + sum_j mid_w[j] ks[j]."""
+    out = torch.empty_like(y0) if out is None else out
+    kw, S = _ode_sources(ks, mid_w, 'm')
+    lib.call('b200_ode_dense_output', lib.make_args('b200_ode_dense_args', y0=_c(y0), y1=_c(y1), S=S, dt=float(dt), x=float(x), out=out,
+                                                    n=y0.numel(), **kw), _stream())
+    return out
+
+
 def melspec_frames(nw, n_fft, hop, center=True):
     """frames of a wave of nw samples: reflect-padded by n_fft // 2 on both sides (center) or valid frames only (torch.stft)"""
     pad = n_fft // 2 if center else 0

@@ -377,6 +377,81 @@ int b200_masked_mean_bwd(const float* dout, const uint8_t* mask, void* dx, int32
 
 /* Fixed-grid ODE update out = y + a * f (torchdiffeq midpoint/euler as called at e2_tts.py:1421; SURVEY A.7). */
 int b200_axpy(const float* y, const float* f, float a, float* out, int64_t n, b200_stream_t stream);
+/* ------------------------------------------------------------------------------------------------
+ * Runge–Kutta solver passes of E2TTS.sample for odeint_kwargs methods 'rk4', 'dopri5', 'bosh3', 'fehlberg2' and 'adaptive_heun'
+ * (the odeint call at e2_tts.py:1421 with odeint_kwargs :1122-1126; torchdiffeq 0.2.x restated in SURVEY A.7). The ODE state is
+ * the whole padded [B, max_duration, C] fp32 tensor of n elements; k0..k{S-1} are function evaluations (stage derivatives) of the
+ * same size; the weights (tableau entry times the step size, rounded to fp32) are formed on the host. Memory-bound fp32 passes,
+ * float4-vectorised when every pointer is 16-byte aligned, scalar otherwise and for the n % 4 tail. S is 1..7 (dopri5 has 7 stages).
+ *
+ * Reductions (step_error, norms) accumulate fp32 quotients squared in fp64: each block writes its partial sum to ws, one more block
+ * adds the partials in a fixed order and writes the root mean square as fp32. The grid is min(ceil(n / 1024), ws_len) blocks
+ * whatever the device, so the result is bit-identical from run to run; an n larger than the grid covers is wrapped by a grid-stride
+ * loop. */
+
+/* out = y0 + sum_j w_j k_j (the sum is formed first, then added to y0: torchdiffeq's y0 + k.matmul(beta * dt)). Replaces the stage
+ * inputs of _runge_kutta_step (rk_common.py, `yi = y0 + k[..., :i + 1].matmul(beta_i * dt)`), its `y1` of a tableau without
+ * first-same-as-last, and rk4_alt_step_func's update (fixed_grid.py / misc: (k1 + 3 (k2 + k3) + k4) dt / 8). out may alias y0. */
+typedef struct {
+    const float* y0;
+    const float *k0, *k1, *k2, *k3, *k4, *k5, *k6;
+    float w0, w1, w2, w3, w4, w5, w6;
+    int32_t S;
+    float* out;
+    int64_t n;
+} b200_ode_combine_args;
+int b200_ode_combine(const b200_ode_combine_args* a, b200_stream_t stream);
+
+/* The error estimate and its norm of one adaptive step (_adaptive_step, rk_common.py: `y1_error = k.matmul(dt * c_error)`,
+ * `error_tol = atol + rtol * max(|y0|, |y1|)`, `error_ratio = rms_norm(y1_error / error_tol)`) in one pass:
+ *   write_y1 != 0: y1 = y0 + sum_j s_j k_j is computed and stored (a tableau without first-same-as-last);
+ *   write_y1 == 0: y1 is read (dopri5 / bosh3: the last stage input is the solution).
+ * ratio[0] = sqrt(mean((sum_j e_j k_j / tol)^2)) in fp32. ws: ws_len doubles (1..65535). atol, rtol: finite, >= 0. */
+typedef struct {
+    const float* y0;
+    const float *k0, *k1, *k2, *k3, *k4, *k5, *k6;
+    float e0, e1, e2, e3, e4, e5, e6;
+    float s0, s1, s2, s3, s4, s5, s6;
+    int32_t S;
+    float* y1;
+    int32_t write_y1;
+    float atol, rtol;
+    double* ws;
+    int32_t ws_len;
+    float* ratio;
+    int64_t n;
+} b200_ode_step_error_args;
+int b200_ode_step_error(const b200_ode_step_error_args* a, b200_stream_t stream);
+
+/* The scaled norms of the initial step size (_select_initial_step, misc.py): scale = atol + |y0| rtol,
+ *   out[0] = rms(a / scale) when a is non-null (d0 with a = y0),
+ *   out[1] = rms((b - c) / scale), or rms(b / scale) when c is NULL (d1 with b = f0; d2 * h0 with b = f(t0 + h0, y0 + h0 f0), c = f0).
+ * ws: 2 * ws_len doubles (ws_len 1..65535). atol, rtol: finite, >= 0. */
+typedef struct {
+    const float *y0, *a, *b, *c;
+    float atol, rtol;
+    double* ws;
+    int32_t ws_len;
+    float* out;
+    int64_t n;
+} b200_ode_norms_args;
+int b200_ode_scaled_norms(const b200_ode_norms_args* a, b200_stream_t stream);
+
+/* Dense output of the last accepted step at x = (t - t0) / (t1 - t0) (RKAdaptiveStepsizeODESolver._interp_fit + interp.py
+ * _interp_fit / _interp_evaluate): y_mid = y0 + sum_j m_j k_j (m_j = dt c_mid_j), f0 = k0, f1 = k{S-1}, the quartic
+ * e + x d + x^2 c + x^3 b + x^4 a with e = y0, d = dt f0, c = dt (f1 - 4 f0) - 11 y0 - 5 y1 + 16 y_mid,
+ * b = dt (5 f0 - 3 f1) + 18 y0 + 14 y1 - 32 y_mid, a = 2 dt (f1 - f0) - 8 (y1 + y0) + 16 y_mid, all in fp32, without storing them. */
+typedef struct {
+    const float *y0, *y1;
+    const float *k0, *k1, *k2, *k3, *k4, *k5, *k6;
+    float m0, m1, m2, m3, m4, m5, m6;
+    int32_t S;
+    float dt, x;
+    float* out;
+    int64_t n;
+} b200_ode_dense_args;
+int b200_ode_dense_output(const b200_ode_dense_args* a, b200_stream_t stream);
+
 /* Classifier-free guidance with the APG orthogonal projection in fp64 (e2_tts.py:1323-1330, project :113-124):
  * out = pred + (orth + par * keep) * strength per sample over all n*d elements. ws_red: 2*B doubles. */
 int b200_cfg_combine(const float* pred, const float* null_pred, double* ws_red, float* out, int32_t B, int64_t per_sample,
