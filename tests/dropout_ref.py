@@ -1,11 +1,11 @@
 """Dropout with known masks, for holding training steps with dropout on to the oracle of oracle/e2tts_oracle.py through its
 `O.DROPOUT` hook (called as DROPOUT(name, x) on the attention probabilities, name `<prefix>.attn_dropout`, and on the GEGLU hidden,
 name `<prefix>.ff.1`: the qualified names of the reference's nn.Dropout modules). Shared by tests/test_dropout_vs_reference.py,
-tools/make_dropout_golden.py and tests/test_gpu_dropout_step.py.
+oracle/make_reference_golden.py and tests/test_gpu_dropout_step.py.
 
 Two mask recipes:
   * hashed (CPU): the kept set of a dropout module depends only on its qualified name, the input shape and the case seed (a
-    torch.Generator seeded with zlib.crc32 of the three), kept elements scaled by 1 / (1 - p). tools/make_dropout_golden.py puts it in
+    torch.Generator seeded with zlib.crc32 of the three), kept elements scaled by 1 / (1 - p). oracle/make_reference_golden.py puts it in
     place of every nn.Dropout of the original e2_tts.py; `HashedDropout` gives the oracle the same masks.
   * the kernels' own (GPU): `SeedRecorder` records the host seed and the device seed word of every ops.Attention / ops.FeedForward
     call of a forward, keyed by the dropout module it belongs to (through the identity of the to_q / ff.0.proj weight it receives).

@@ -1,6 +1,6 @@
 """Cases of the reference's model-shape knobs besides the defaults (Transformer, e2_tts.py:518-552): depth past 8 (six skip levels),
 text_depth < depth, dim_text != dim // 2, ff_mult / text_ff_mult != 4 (one of them non-integer), num_registers != 32 (0 included),
-abs_pos_emb=False and kernel_size != 31, stored from the original e2_tts.py by tools/make_geometry_golden.py. Shared by
+abs_pos_emb=False and kernel_size != 31, stored from the original e2_tts.py by oracle/make_reference_golden.py. Shared by
 tests/test_geometry_vs_reference.py (oracle against the original's stored outputs) and tests/test_gpu_geometry.py.
 
 Every knob is a field of the oracle's TransformerCfg, so TransformerCfg(**tkw) is the whole oracle configuration of a case. `knobs`

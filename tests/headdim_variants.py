@@ -1,6 +1,6 @@
 """Cases of the reference's attention geometry knobs besides the defaults (e2_tts.py:527-531, defaults :569-570): 128-wide heads
 (dim_head, text_dim_head) and a text stream with its own head count (text_heads), stored from the original e2_tts.py by
-tools/make_headdim_golden.py. Shared by tests/test_headdim_vs_reference.py (oracle against the original's stored outputs) and the
+oracle/make_reference_golden.py. Shared by tests/test_headdim_vs_reference.py (oracle against the original's stored outputs) and the
 GPU tests of the same geometry.
 
 The oracle takes the same kwargs as configuration (oracle/e2tts_oracle.py TransformerCfg: text_heads, text_dim_head and the text

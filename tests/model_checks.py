@@ -1,6 +1,6 @@
 """Whole-model checks shared by the test modules: the GPU model against the fp32 oracle (oracle/e2tts_oracle.py) computed on the host,
-the small seeded models of the sampling / duration / graphed-step tests, and the oracle's gradients against the original's stored
-samples (tests/golden/reference/)."""
+the small seeded models of the sampling / duration / graphed-step tests and those checks, and the oracle against the original's stored
+outputs, gradient samples and parameter shapes (tests/golden/reference/)."""
 import random
 
 import torch
@@ -92,6 +92,94 @@ def small_model(pkg, seed, cls='E2TTS', **transformer_kw):
     return model.to(dev()), sd
 
 
+def sample_vs_oracle(pkg, seed, tkw, cond=(2, 24), text=('Hello', 'Goodbye'), duration=64, lens=None, steps=32, cfg_strength=1.0):
+    """E2TTS.sample of small_model(pkg, seed, **tkw) against the oracle's fixed-grid ODE on the same weights: cond (batch, frames) and
+    then y0 drawn under seed + 1, y0 as long as the longest duration (an int, or a tensor of one per batch element, as `lens`). Same
+    shape, rel-L2 < 5e-2. Returns the GPU sample."""
+    model, sd = small_model(pkg, seed, **tkw)
+    torch.manual_seed(seed + 1)
+    cond = torch.randn(*cond, 100)
+    y0 = torch.randn(cond.shape[0], int(torch.as_tensor(duration).max()), 100)
+    on_dev = lambda t: t.to(dev()) if torch.is_tensor(t) else t   # noqa: E731
+    with pkg.inject_randomness(y0=y0.to(dev())):
+        out = model.sample(cond.to(dev()), text=list(text), lens=on_dev(lens), duration=on_dev(duration), steps=steps,
+                           cfg_strength=cfg_strength, return_raw_output=True)
+    want = O.e2tts_sample(sd, O.TransformerCfg(**tkw), cond, O.list_str_to_tensor(list(text)), duration=duration, lens=lens, y0=y0,
+                          steps=steps, cfg_strength=cfg_strength)
+    assert out.shape == want.shape
+    e = rel_l2(out.cpu(), want)
+    print(f'{steps}-step sample {tkw}: rel-L2 {e:.4g}')
+    assert e < 5e-2
+    return out
+
+
+def duration_vs_oracle(pkg, seed, tkw):
+    """DurationPredictor small_model(pkg, seed, **tkw) in training mode on three ragged items drawn after it, with the prefix fractions
+    pinned, against the oracle: loss within 1e-2; a parameter the oracle leaves without a gradient gets none (or an all-zero one); every
+    other gradient present, with cosine >= 0.99 wherever it is not negligible next to the whole gradient"""
+    model, sd = small_model(pkg, seed, 'DurationPredictor', **tkw)
+    model.train()
+    mel = torch.randn(3, 72, 100)
+    lens = torch.tensor([72, 50, 31])
+    text = ['abc', 'hello world', 'x']
+    rand_frac = torch.tensor([0.3, 0.6, 0.9])
+    with pkg.inject_randomness(duration_rand_frac=rand_frac.to(dev())):
+        loss = model(mel.to(dev()), text=text, lens=lens.to(dev()))
+    loss.backward()
+    osd = grad_sd(sd)
+    ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, **tkw), mel, O.list_str_to_tensor(text), lens=lens,
+                             rand_frac=rand_frac)
+    ref.backward()
+    print(f'duration predictor {tkw}: loss {float(loss):.6f} (oracle {float(ref):.6f})')
+    assert abs(float(loss) - float(ref)) <= 1e-2 * abs(float(ref))
+    total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())
+    for k, p in model.named_parameters():
+        gr = osd[k].grad
+        if gr is None:
+            assert p.grad is None or float(p.grad.abs().max()) == 0.0, f'{k} should be unused'
+            continue
+        assert p.grad is not None, k
+        if float(gr.norm()) < 1e-4 * total:
+            continue
+        assert cos(p.grad.cpu(), gr) >= 0.99, k
+
+
+def step_inputs(pkg, B=2, N=96, span=(20, 70)):
+    """(mel, text ids, inject_randomness kwargs) of one training step on the GPU: mel, x0 and times drawn in that order from torch's
+    global generator, frames span[0]:span[1] of every item masked, the text kept"""
+    mel = torch.randn(B, N, 100, device=dev())
+    text = pkg.list_str_to_tensor(['Hello', 'Goodbye']).to(dev())
+    x0, times = torch.randn(B, N, 100, device=dev()), torch.rand(B, device=dev())
+    span_mask = torch.zeros(B, N, dtype=torch.bool, device=dev())
+    span_mask[:, span[0]:span[1]] = True
+    return mel, text, dict(x0=x0, times=times, span_mask=span_mask, drop_text_cond=False)
+
+
+def graphed_matches_eager(pkg, model, mel, text, rnd):
+    """One eager step of `model` (training mode, text never dropped) with the randomness `rnd` pinned, then a GraphedTrainStep on the
+    same inputs: loss within 1e-3 |loss| + 1e-5, the same parameters with a gradient, each within rel-L2 2e-3 of the eager one (fp32
+    atomics reorder between runs). Returns (the step, its loss)."""
+    model.train()
+    model.cond_drop_prob = 0.0
+    with pkg.inject_randomness(**rnd):
+        out = model(mel, text=text)
+        out.loss.backward()
+        want_loss = float(out.loss)
+        want = {n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None}
+        for p in model.parameters():
+            p.grad = None
+        del out   # an alive eager graph keeps its AccumulateGrad nodes (bound to the default stream) and would drag stream 0 into the capture
+        step = pkg.GraphedTrainStep(model, mel, text=text)
+        got_loss = float(step())
+    torch.cuda.synchronize()
+    assert abs(got_loss - want_loss) <= 1e-3 * abs(want_loss) + 1e-5, (got_loss, want_loss)
+    got = {n: p.grad for n, p in model.named_parameters() if p.grad is not None}
+    assert set(got) == set(want)
+    for n in want:
+        assert rel_l2(got[n].float().cpu(), want[n].float().cpu()) < 2e-3 or float(want[n].norm()) == 0, n
+    return step, got_loss
+
+
 def grad_sd(sd):
     return {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
 
@@ -149,3 +237,26 @@ def check_case(c, rec, sd, loss, pred):
         assert abs(float(pred.detach().double().norm()) - rec['pred']['norm']) <= 1e-4 * rec['pred']['norm']
     assert abs(float(loss.detach()) - rec['loss']) <= 1e-5 * abs(rec['loss'])
     check_grads(sd, rec['grads'], *c.get('grad_tol', (2e-4, 1e-7) if c.get('cls', 'E2TTS') == 'E2TTS' else (5e-4, 1e-6)))
+
+
+def state_dict_vs_reference(c, rec):
+    """keys and shapes of the package's model of stored case `c` (cls, tkw) equal the original's (`rec['shapes']`), so its checkpoints
+    load; returns them"""
+    import e2_tts_pytorch_b200 as pkg
+    t = dict(dropout=0., max_seq_len=128, **c['tkw'])
+    m = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
+    got = {k: tuple(v.shape) for k, v in m.state_dict().items()}
+    assert got == rec['shapes']
+    return got
+
+
+def sample_vs_reference(s, rec, lens=None):
+    """the oracle's E2TTS.sample on stored sample case `s` (seed, tkw, cond (batch, frames), text, duration, steps, cfg_strength) with the
+    prompt lengths `lens`, from the y0 the original drew (generator 3000 + seed), against its record: same shape, rel-L2 < 1e-4"""
+    cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
+    with torch.no_grad():
+        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), O.TransformerCfg(**s['tkw']), cond,
+                             O.list_str_to_tensor(s['text']), duration=torch.tensor(s['duration']), lens=lens,
+                             y0=RC.randn(rec['shape'], 3000 + s['seed']), steps=s['steps'], cfg_strength=s['cfg_strength'])
+    assert tuple(got.shape) == rec['shape']
+    assert RC.compact_rel_l2(got, rec['out']) < 1e-4

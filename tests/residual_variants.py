@@ -1,5 +1,5 @@
 """Cases of Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True), stored from the
-original e2_tts.py by tools/make_residual_golden.py. The oracle of oracle/e2tts_oracle.py runs that backbone when its config has one
+original e2_tts.py by oracle/make_reference_golden.py. The oracle of oracle/e2tts_oracle.py runs that backbone when its config has one
 stream: with one stream the reference's hyper-connection modules are `Residual` (oracle/ref_leaves/hyper_connections.py), the width
 connection hands the stream itself to the branch and keeps it as the residual, the depth connection is `branch_out + residual`, and
 expand / reduce are identities."""
@@ -15,5 +15,6 @@ RESIDUAL1_CASES = {
                          drop=True),
     'duration': dict(cls='DurationPredictor', seed=68, tkw=KW1, mel=(3, 72), lens=[72, 50, 31], text=['abc', 'hello world', 'x']),
 }
-# E2TTS.sample: weights seed, cond (batch, frames), text, duration, steps, cfg_strength; y0 = first draw of generator 3000 + seed
-RESIDUAL1_SAMPLE = dict(seed=70, cond=(2, 20), text=['Hello', 'Goodbye then'], duration=[40, 33], steps=4, cfg_strength=1.0)
+# E2TTS.sample: weights seed, transformer kwargs, cond (batch, frames), text, duration, steps, cfg_strength; y0 = first draw of
+# generator 3000 + seed
+RESIDUAL1_SAMPLE = dict(seed=70, tkw=KW1, cond=(2, 20), text=['Hello', 'Goodbye then'], duration=[40, 33], steps=4, cfg_strength=1.0)

@@ -1,26 +1,21 @@
 """CPU: the x-transformers `attn_kwargs` of Transformer (e2_tts.py:548-551) besides the reference's default — no head gate, no logit
 soft-clamp, another clamp value. The oracle with the same attn_kwargs against what the original e2_tts.py computed on those settings
-(tests/golden/reference/attn_kwargs_*.pt, tools/make_attn_kwargs_golden.py), the package's parameter layout against the original's,
+(tests/golden/reference/attn_kwargs_*.pt, oracle/make_reference_golden.py), the package's parameter layout against the original's,
 the switches that still raise, and the C-ABI validation of the unclamped / no-gate fields."""
 import pytest
 
 from attn_variants import ATTN_KWARGS_CASES
-from model_checks import check_case, oracle_case
+from model_checks import check_case, oracle_case, state_dict_vs_reference
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
 
 import e2_tts_pytorch_b200 as pkg
 
 
-def _tkw(c):
-    return dict(RC.KW, attn_kwargs=c['attn_kwargs'])
-
-
 @pytest.mark.parametrize('name', list(ATTN_KWARGS_CASES))
 def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples within the bounds of tests/test_oracle_vs_reference.py"""
-    c = dict(ATTN_KWARGS_CASES[name], tkw=_tkw(ATTN_KWARGS_CASES[name]))
-    g = RC.load('attn_kwargs_' + name)
+    c, g = ATTN_KWARGS_CASES[name], RC.load('attn_kwargs_' + name)
     check_case(c, g, *oracle_case(c, g))
 
 
@@ -28,12 +23,8 @@ def test_oracle_vs_reference(name):
 def test_state_dict_matches_reference(name):
     """keys and shapes of the original's model with the same attn_kwargs: its checkpoints load"""
     c = ATTN_KWARGS_CASES[name]
-    want = RC.load('attn_kwargs_' + name)['shapes']
-    t = dict(dropout=0., max_seq_len=128, **_tkw(c))
-    m = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
-    got = {k: tuple(v.shape) for k, v in m.state_dict().items()}
-    assert got == want
-    has_gate = {**dict(gate_value_heads=False), **c['attn_kwargs']}['gate_value_heads']
+    got = state_dict_vs_reference(c, RC.load('attn_kwargs_' + name))
+    has_gate = c['tkw']['attn_kwargs'].get('gate_value_heads', False)
     assert any(k.endswith('to_v_head_gate.weight') for k in got) == has_gate
 
 

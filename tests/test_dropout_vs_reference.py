@@ -1,4 +1,4 @@
-"""CPU: the oracle's dropout hook (O.DROPOUT) against the original e2_tts.py trained with dropout on. tools/make_dropout_golden.py ran
+"""CPU: the oracle's dropout hook (O.DROPOUT) against the original e2_tts.py trained with dropout on. oracle/make_reference_golden.py ran
 the original with dropout = 0.25, every nn.Dropout replaced by a seeded mask of its qualified name (tests/dropout_ref.py), on an E2TTS
 of depth 2 with ragged lengths, with the text dropped, with num_residual_streams=1, with 2 x 128 audio heads and 1 x 64 text heads,
 and on a DurationPredictor (tests/golden/reference/dropout_*.pt). The oracle, given the same masks through the hook, must match its

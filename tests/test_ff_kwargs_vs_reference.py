@@ -1,6 +1,6 @@
 """CPU: the x-transformers `ff_kwargs` of Transformer (e2_tts.py:552) — SwiGLU, ReLU^2 GLU, the GLU multiplicative bias and the output
 Linear without bias. The oracle with the same ff_kwargs against what the original e2_tts.py computed on those settings
-(tests/golden/reference/ff_kwargs_*.pt, tools/make_ff_kwargs_golden.py), a negative control per switch family (ff_kwargs, attn_kwargs,
+(tests/golden/reference/ff_kwargs_*.pt, oracle/make_reference_golden.py), a negative control per switch family (ff_kwargs, attn_kwargs,
 text geometry), the package's parameter layout against the original's, the parsing of the keywords (precedence, explicit defaults,
 refusals), and the C-ABI validation of the GLU activation fields."""
 import pytest
@@ -9,7 +9,7 @@ import torch
 from attn_variants import ATTN_KWARGS_CASES
 from ff_variants import FF_KWARGS_CASES, XTFeedForward
 from headdim_variants import HEADDIM_CASES
-from model_checks import check_case, oracle_case
+from model_checks import check_case, oracle_case, state_dict_vs_reference
 from oracle import reference_cases as RC
 from oracle.ref_leaves.x_transformers.x_transformers import FeedForward as LeafFeedForward
 
@@ -18,26 +18,20 @@ import e2_tts_pytorch_b200 as pkg
 GLU_GELU, GLU_SILU, GLU_RELU2 = pkg.ops.GLU_GELU, pkg.ops.GLU_SILU, pkg.ops.GLU_RELU2
 
 
-def _tkw(c):
-    return dict(c['tkw'], ff_kwargs=c['ff_kwargs'])
-
-
 @pytest.mark.parametrize('name', list(FF_KWARGS_CASES))
 def test_oracle_vs_reference(name):
     """loss, prediction and gradient samples (mult_bias included) within the bounds of tests/test_oracle_vs_reference.py"""
-    c = dict(FF_KWARGS_CASES[name], tkw=_tkw(FF_KWARGS_CASES[name]))
-    g = RC.load('ff_kwargs_' + name)
+    c, g = FF_KWARGS_CASES[name], RC.load('ff_kwargs_' + name)
     check_case(c, g, *oracle_case(c, g))
-    if c['ff_kwargs'].get('glu_mult_bias'):
+    if c['tkw']['ff_kwargs'].get('glu_mult_bias'):
         assert any(k.endswith('.ff.0.mult_bias') and v is not None for k, v in g['grads'].items())
 
 
 # one stored case per switch family, by record name, with its whole Transformer kwargs, and the least the oracle without the switch
 # misses its prediction by (rel-L2; the cases pass at 1e-4)
 SEES = {
-    'ff_kwargs_swish': (dict(FF_KWARGS_CASES['swish'], tkw=_tkw(FF_KWARGS_CASES['swish'])), 1e-2),
-    'attn_kwargs_clamp30': (dict(ATTN_KWARGS_CASES['clamp30'], tkw=dict(RC.KW, attn_kwargs=ATTN_KWARGS_CASES['clamp30']['attn_kwargs'])),
-                            1e-2),
+    'ff_kwargs_swish': (FF_KWARGS_CASES['swish'], 1e-2),
+    'attn_kwargs_clamp30': (ATTN_KWARGS_CASES['clamp30'], 1e-2),
     # text geometry 1 x 128, as wide as the audio's 2 x 64, so the default text geometry runs on the same weights; the text stream
     # reaches the prediction through the cross-conditions only, and 2 x 64 moves it by 8.7e-3
     'headdim_mixed_a64_t128': (HEADDIM_CASES['mixed_a64_t128'], 5e-3),
@@ -65,12 +59,8 @@ def test_oracle_sees_the_variant():
 def test_state_dict_matches_reference(name):
     """keys and shapes of the original's model with the same ff_kwargs (ff.0.mult_bias present, ff.2.bias absent where asked)"""
     c = FF_KWARGS_CASES[name]
-    want = RC.load('ff_kwargs_' + name)['shapes']
-    t = dict(dropout=0., max_seq_len=128, **_tkw(c))
-    m = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
-    got = {k: tuple(v.shape) for k, v in m.state_dict().items()}
-    assert got == want
-    kw = c['ff_kwargs']
+    got = state_dict_vs_reference(c, RC.load('ff_kwargs_' + name))
+    kw = c['tkw']['ff_kwargs']
     n_ff = sum(k.endswith('.ff.0.proj.weight') for k in got)
     assert n_ff == 2 * c['tkw']['depth']   # audio and text feed-forward of every layer
     assert sum(k.endswith('.ff.0.mult_bias') for k in got) == (n_ff if kw.get('glu_mult_bias') else 0)

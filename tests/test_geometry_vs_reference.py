@@ -1,12 +1,12 @@
 """CPU: the model-shape knobs of Transformer (e2_tts.py:518-552) — depth 12, text_depth < depth, dim_text != dim // 2, ff_mult and
 text_ff_mult != 4, num_registers 0 / 8 / 16, abs_pos_emb=False, kernel_size 1 / 5 / 7. The oracle against what the original e2_tts.py
-computed with them (tests/golden/reference/geometry_*.pt, tools/make_geometry_golden.py), one negative control per knob, the package's
+computed with them (tests/golden/reference/geometry_*.pt, oracle/make_reference_golden.py), one negative control per knob, the package's
 parameter layout against the original's, and the geometries that raise."""
 import pytest
 import torch
 
 from geometry_variants import GEOMETRY_CASES, GEOMETRY_SAMPLE, reverted
-from model_checks import check_case, oracle_case
+from model_checks import check_case, oracle_case, sample_vs_reference, state_dict_vs_reference
 from oracle import e2tts_oracle as O
 from oracle import reference_cases as RC
 
@@ -44,27 +44,15 @@ def test_knob_reverted_misses_reference(name, knob):
 
 def test_sample_vs_reference():
     """4 midpoint steps, a per-element duration and a ragged prompt"""
-    s = GEOMETRY_SAMPLE
-    g = RC.load('geometry_sample')
-    cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
-    with torch.no_grad():
-        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), O.TransformerCfg(**s['tkw']), cond,
-                             O.list_str_to_tensor(s['text']),
-                             duration=torch.tensor(s['duration']), lens=torch.tensor(s['lens']), y0=RC.randn(g['shape'], 3000 + s['seed']),
-                             steps=s['steps'], cfg_strength=s['cfg_strength'])
-    assert tuple(got.shape) == g['shape'] == (2, max(s['duration']), 100)
-    assert RC.compact_rel_l2(got, g['out']) < 1e-4
+    s, g = GEOMETRY_SAMPLE, RC.load('geometry_sample')
+    sample_vs_reference(s, g, lens=torch.tensor(s['lens']))
+    assert g['shape'] == (2, max(s['duration']), 100)
 
 
 @pytest.mark.parametrize('name', list(GEOMETRY_CASES))
 def test_state_dict_matches_reference(name):
     """keys and shapes of the original's model with the same geometry: its checkpoints load"""
-    c = GEOMETRY_CASES[name]
-    want = RC.load('geometry_' + name)['shapes']
-    t = dict(dropout=0., max_seq_len=128, **c['tkw'])
-    m = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
-    got = {k: tuple(v.shape) for k, v in m.state_dict().items()}
-    assert got == want
+    state_dict_vs_reference(GEOMETRY_CASES[name], RC.load('geometry_' + name))
 
 
 def test_geometry_is_recorded():

@@ -18,8 +18,7 @@ from conftest import rel_l2
 from geometry_variants import GEOMETRY_CASES, GEOMETRY_SAMPLE
 from hyper_conv_ref import S, check_hc_case, hc_fwd_launch
 from kernel_checks import dev, pkg, sms  # noqa: F401
-from model_checks import cos, small_model, whole_model
-from oracle import e2tts_oracle as O
+from model_checks import duration_vs_oracle, graphed_matches_eager, sample_vs_oracle, small_model, step_inputs, whole_model
 
 pytestmark = pytest.mark.gpu
 
@@ -105,60 +104,24 @@ def test_e2tts_no_registers_vs_oracle(pkg, N):
 
 def test_duration_predictor_geometry_vs_oracle(pkg):
     """DurationPredictor with text_depth < depth and dim_text != dim // 2 (the reference-pinned 'duration' case's geometry)"""
-    tkw = GEOMETRY_CASES['duration']['tkw']
-    model, sd = small_model(pkg, 140, 'DurationPredictor', **tkw)
-    model.train()
-    mel = torch.randn(3, 72, 100)
-    lens = torch.tensor([72, 50, 31])
-    text = ['abc', 'hello world', 'x']
-    rand_frac = torch.tensor([0.3, 0.6, 0.9])
-    with pkg.inject_randomness(duration_rand_frac=rand_frac.to(dev())):
-        loss = model(mel.to(dev()), text=text, lens=lens.to(dev()))
-    loss.backward()
-    osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, **tkw), mel, O.list_str_to_tensor(text), lens=lens,
-                             rand_frac=rand_frac)
-    ref.backward()
-    assert abs(float(loss) - float(ref)) <= 1e-2 * abs(float(ref))
-    total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())
-    for k, p in model.named_parameters():
-        gr = osd[k].grad
-        if gr is None:
-            assert p.grad is None or float(p.grad.abs().max()) == 0.0, f'{k} should be unused'
-            continue
-        if float(gr.norm()) < 1e-4 * total:
-            continue
-        assert cos(p.grad.cpu(), gr) >= 0.99, k
+    duration_vs_oracle(pkg, 140, GEOMETRY_CASES['duration']['tkw'])
 
 
 def test_sample_ragged_duration_vs_oracle(pkg):
     """E2TTS.sample with a per-element duration and ragged prompt lengths, at the sample case's geometry (text_depth 2 of 4, 8
     registers, kernel 5)"""
     s = GEOMETRY_SAMPLE
-    model, sd = small_model(pkg, 141, **s['tkw'])
-    torch.manual_seed(142)
-    cond = torch.randn(s['cond'][0], s['cond'][1], 100)
-    y0 = torch.randn(s['cond'][0], max(s['duration']), 100)
-    lens, duration = torch.tensor(s['lens']), torch.tensor(s['duration'])
-    with pkg.inject_randomness(y0=y0.to(dev())):
-        out = model.sample(cond.to(dev()), text=s['text'], lens=lens.to(dev()), duration=duration.to(dev()), steps=s['steps'],
-                           cfg_strength=s['cfg_strength'], return_raw_output=True)
-    want = O.e2tts_sample(sd, O.TransformerCfg(**s['tkw']), cond, O.list_str_to_tensor(s['text']), duration=duration, lens=lens, y0=y0,
-                          steps=s['steps'], cfg_strength=s['cfg_strength'])
-    assert out.shape == want.shape == (2, max(s['duration']), 100)
-    assert rel_l2(out.cpu(), want) < 5e-2
+    out = sample_vs_oracle(pkg, 141, s['tkw'], cond=s['cond'], text=s['text'], duration=torch.tensor(s['duration']),
+                           lens=torch.tensor(s['lens']), steps=s['steps'], cfg_strength=s['cfg_strength'])
+    assert out.shape == (2, max(s['duration']), 100)
 
 
 TEXT_DEPTH = dict(dim=128, depth=6, heads=2, text_depth=3, dim_text=128, num_registers=16)
 
 
-def _step(pkg, model, B, N, seed):
+def _step(pkg, B, N, seed):
     torch.manual_seed(seed)
-    mel = torch.randn(B, N, 100, device=dev())
-    x0, times = torch.randn(B, N, 100, device=dev()), torch.rand(B, device=dev())
-    span = torch.zeros(B, N, dtype=torch.bool, device=dev())
-    span[:, N // 5:N - N // 6] = True
-    return mel, pkg.list_str_to_tensor(['Hello', 'Goodbye']).to(dev()), dict(x0=x0, times=times, span_mask=span, drop_text_cond=False)
+    return step_inputs(pkg, B, N, span=(N // 5, N - N // 6))
 
 
 def test_text_depth_schedules_agree_without_dropout(pkg, monkeypatch):
@@ -168,7 +131,7 @@ def test_text_depth_schedules_agree_without_dropout(pkg, monkeypatch):
     model, _ = small_model(pkg, 150, **TEXT_DEPTH)
     model.train()
     B, N = 2, 96
-    mel, text, rnd = _step(pkg, model, B, N, 151)
+    mel, text, rnd = _step(pkg, B, N, 151)
     lens = torch.tensor([96, 70], device=dev())
 
     def run():
@@ -195,23 +158,4 @@ def test_text_depth_schedules_agree_without_dropout(pkg, monkeypatch):
 def test_graphed_step_matches_eager_text_depth(pkg):
     """GraphedTrainStep replays the eager step's gradients with text_depth < depth"""
     model, _ = small_model(pkg, 152, **TEXT_DEPTH)
-    model.train()
-    model.cond_drop_prob = 0.0
-    B, N = 2, 96
-    mel, text, rnd = _step(pkg, model, B, N, 153)
-    with pkg.inject_randomness(**rnd):
-        out = model(mel, text=text)
-        out.loss.backward()
-        want = {n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None}
-        for p in model.parameters():
-            p.grad = None
-        del out
-        step = pkg.GraphedTrainStep(model, mel, text=text)
-        step()
-    torch.cuda.synchronize()
-    for n, p in model.named_parameters():
-        if n in want:
-            assert p.grad is not None, n
-            assert rel_l2(p.grad.float().cpu(), want[n].float().cpu()) < 2e-3 or float(want[n].norm()) == 0, n
-        else:
-            assert p.grad is None or float(p.grad.abs().max()) == 0.0, n
+    graphed_matches_eager(pkg, model, *_step(pkg, 2, 96, 153))

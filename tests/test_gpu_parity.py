@@ -14,7 +14,7 @@ import torch.nn.functional as F
 
 from conftest import GOLDEN, rel_l2
 from kernel_checks import dev, pkg
-from model_checks import cos
+from model_checks import cos, graphed_matches_eager, step_inputs
 from oracle import e2tts_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -427,30 +427,9 @@ def test_graphed_train_step_matches_eager_step(pkg):
     torch.manual_seed(0)
     B, N = 2, 96
     model = pkg.E2TTS(transformer=dict(dim=128, depth=2, heads=2, dropout=0.0), use_vocos=False).to(dev())
-    model.train()
-    model.cond_drop_prob = 0.0
-    mel = torch.randn(B, N, 100, device=dev())
-    text = pkg.list_str_to_tensor(['Hello', 'Goodbye']).to(dev())
-    x0 = torch.randn(B, N, 100, device=dev())
-    times = torch.rand(B, device=dev())
-    span = torch.zeros(B, N, dtype=torch.bool, device=dev())
-    span[:, 20:70] = True
-    with pkg.inject_randomness(x0=x0, times=times, span_mask=span, drop_text_cond=False):
-        out = model(mel, text=text)
-        out.loss.backward()
-        want_loss = float(out.loss)
-        want = {n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None}
-        for p in model.parameters():
-            p.grad = None
-        del out   # an alive eager graph keeps its AccumulateGrad nodes (bound to the default stream) and would drag stream 0 into the capture
-        step = pkg.GraphedTrainStep(model, mel, text=text)
-        got_loss = float(step())
+    mel, text, rnd = step_inputs(pkg, B, N)
+    step, got_loss = graphed_matches_eager(pkg, model, mel, text, rnd)
     assert step.launches_per_step > 50
-    assert abs(got_loss - want_loss) <= 1e-3 * abs(want_loss) + 1e-5, (got_loss, want_loss)
-    got = {n: p.grad for n, p in model.named_parameters() if p.grad is not None}
-    assert set(got) == set(want)
-    worst = max(rel_l2(got[n].float().cpu(), want[n].float().cpu()) for n in want if float(want[n].norm()) > 0)
-    assert worst < 2e-3, f'graphed vs eager gradients: worst rel-L2 {worst:.3g}'   # fp32 atomics reorder between runs
     # a new batch flows through the static input; the loss changes
     got2 = float(step(torch.randn(B, N, 100, device=dev())))
     assert got2 == got2 and got2 != got_loss
@@ -458,7 +437,7 @@ def test_graphed_train_step_matches_eager_step(pkg):
     model_d = pkg.E2TTS(transformer=dict(dim=128, depth=2, heads=2, dropout=0.3), use_vocos=False).to(dev())
     model_d.train()
     model_d.cond_drop_prob = 0.0
-    with pkg.inject_randomness(x0=x0, times=times, span_mask=span, drop_text_cond=False):
+    with pkg.inject_randomness(**rnd):
         step_d = pkg.GraphedTrainStep(model_d, mel, text=text)
         l1, l2 = float(step_d()), float(step_d())
     assert l1 == l1 and l2 == l2 and l1 != l2, (l1, l2)

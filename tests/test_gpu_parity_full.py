@@ -10,7 +10,7 @@ import torch.nn.functional as F
 from attn_ref import dropout_keep
 from conftest import rel_l2
 from kernel_checks import dev, pkg
-from model_checks import check, cos, small_model, whole_model
+from model_checks import check, cos, sample_vs_oracle, small_model, whole_model
 from oracle import e2tts_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -252,17 +252,7 @@ SMALL = dict(dim=128, depth=2, heads=2)
 
 
 def test_sample_32_steps_vs_oracle(pkg):
-    model, sd = small_model(pkg, 60, **SMALL)
-    cfg = O.TransformerCfg(**SMALL)
-    torch.manual_seed(61)
-    cond = torch.randn(2, 24, 100)
-    text = ['Hello', 'Goodbye']
-    y0 = torch.randn(2, 64, 100)
-    with pkg.inject_randomness(y0=y0.to(dev())):
-        out = model.sample(cond.to(dev()), text=text, duration=64, steps=32, cfg_strength=1.0, return_raw_output=True)
-    want = O.e2tts_sample(sd, cfg, cond, O.list_str_to_tensor(text), duration=64, y0=y0, steps=32, cfg_strength=1.0)
-    assert out.shape == want.shape
-    assert rel_l2(out.cpu(), want) < 5e-2
+    sample_vs_oracle(pkg, 60, SMALL)
 
 
 def test_sample_euler_and_null_model(pkg):

@@ -12,10 +12,9 @@ import pytest
 import torch
 
 from conftest import rel_l2
-from oracle import e2tts_oracle as O
 from hyper_conv_ref import CV_TN, cdiv, dw_mask, dw_ref, model_mask
 from kernel_checks import BF16, F64, U, U16, check_b, check_e, check_f, dev, gamma, gen, h64, nans, pkg, stream
-from model_checks import small_model, whole_model
+from model_checks import duration_vs_oracle, graphed_matches_eager, sample_vs_oracle, small_model, step_inputs, whole_model
 
 pytestmark = pytest.mark.gpu
 
@@ -301,29 +300,13 @@ SMALL = dict(dim=128, depth=2, heads=2, num_residual_streams=1)
 
 
 def test_sample_32_steps_plain_residual_vs_oracle(pkg):
-    model, sd = small_model(pkg, 70, **SMALL)
-    torch.manual_seed(71)
-    cond = torch.randn(2, 24, 100)
-    text = ['Hello', 'Goodbye']
-    y0 = torch.randn(2, 64, 100)
-    with pkg.inject_randomness(y0=y0.to(dev())):
-        out = model.sample(cond.to(dev()), text=text, duration=64, steps=32, cfg_strength=1.0, return_raw_output=True)
-    want = O.e2tts_sample(sd, O.TransformerCfg(**SMALL), cond, O.list_str_to_tensor(text), duration=64, y0=y0, steps=32, cfg_strength=1.0)
-    assert out.shape == want.shape
-    assert rel_l2(out.cpu(), want) < 5e-2
+    sample_vs_oracle(pkg, 70, SMALL)
 
 
 def test_graphed_step_matches_eager_and_launches_no_hyper_connection(pkg, monkeypatch):
     """GraphedTrainStep replays the eager step's gradients; neither launches a hyper-connection entry point"""
     model, _ = small_model(pkg, 3, **SMALL)
-    model.train()
-    model.cond_drop_prob = 0.0
-    B, N = 2, 96
-    mel = torch.randn(B, N, 100, device=dev())
-    text = pkg.list_str_to_tensor(['Hello', 'Goodbye']).to(dev())
-    x0, times = torch.randn(B, N, 100, device=dev()), torch.rand(B, device=dev())
-    span = torch.zeros(B, N, dtype=torch.bool, device=dev())
-    span[:, 20:70] = True
+    mel, text, rnd = step_inputs(pkg)
     called = set()
     real_call = pkg.lib.call
 
@@ -331,44 +314,11 @@ def test_graphed_step_matches_eager_and_launches_no_hyper_connection(pkg, monkey
         called.add(name)
         return real_call(name, *a)
     monkeypatch.setattr(pkg.lib, 'call', recording_call)
-    with pkg.inject_randomness(x0=x0, times=times, span_mask=span, drop_text_cond=False):
-        out = model(mel, text=text)
-        out.loss.backward()
-        want = {n: p.grad.detach().clone() for n, p in model.named_parameters() if p.grad is not None}
-        for p in model.parameters():
-            p.grad = None
-        del out
-        step = pkg.GraphedTrainStep(model, mel, text=text)
-        step()
-    torch.cuda.synchronize()
+    graphed_matches_eager(pkg, model, mel, text, rnd)
     assert not any(n.startswith('b200_hc_') for n in called), sorted(n for n in called if n.startswith('b200_hc_'))
     assert {'b200_final_norm_fwd', 'b200_final_norm_bwd', 'b200_dwconv_fwd', 'b200_dwconv_bwd', 'b200_rowgate_resid_bwd'} <= called
-    for n, p in model.named_parameters():
-        if n in want:
-            assert p.grad is not None, n
-            assert rel_l2(p.grad.float().cpu(), want[n].float().cpu()) < 2e-3 or float(want[n].norm()) == 0, n
 
 
 def test_duration_predictor_plain_residual_vs_oracle(pkg):
     """DurationPredictor(num_residual_streams=1): loss within 1e-2 of the oracle, gradient cosines >= 0.99"""
-    model, sd = small_model(pkg, 41, 'DurationPredictor', **SMALL)
-    model.train()
-    mel = torch.randn(3, 72, 100)
-    lens = torch.tensor([72, 50, 31])
-    text = ['abc', 'hello world', 'x']
-    rand_frac = torch.tensor([0.3, 0.6, 0.9])
-    with pkg.inject_randomness(duration_rand_frac=rand_frac.to(dev())):
-        loss = model(mel.to(dev()), text=text, lens=lens.to(dev()))
-    loss.backward()
-    osd = {k: v.clone().requires_grad_(v.is_floating_point()) for k, v in sd.items()}
-    ref = O.duration_forward(osd, O.TransformerCfg(cond_on_time=False, **SMALL), mel, O.list_str_to_tensor(text), lens=lens,
-                             rand_frac=rand_frac)
-    ref.backward()
-    assert abs(float(loss) - float(ref)) <= 1e-2 * abs(float(ref))
-    total = float(torch.cat([v.grad.flatten() for v in osd.values() if v.grad is not None]).norm())
-    for k, p in model.named_parameters():
-        gr = osd[k].grad
-        if gr is None or float(gr.norm()) < 1e-4 * total:
-            continue
-        got = p.grad.double().cpu().flatten()
-        assert float(got @ gr.double().flatten() / (got.norm() * gr.double().norm())) >= 0.99, k
+    duration_vs_oracle(pkg, 41, SMALL)

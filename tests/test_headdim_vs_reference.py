@@ -1,13 +1,11 @@
 """CPU: the attention geometry knobs of Transformer (e2_tts.py:527-531) — 128-wide heads (dim_head, text_dim_head) and a text stream
 with its own head count (text_heads). The oracle with the same geometry against what the original e2_tts.py computed with them
-(tests/golden/reference/headdim_*.pt, tools/make_headdim_golden.py), the package's parameter layout against the original's, the head
+(tests/golden/reference/headdim_*.pt, oracle/make_reference_golden.py), the package's parameter layout against the original's, the head
 dims that still raise, and the C-ABI validation of dim_head."""
 import pytest
-import torch
 
 from headdim_variants import HEADDIM_CASES, HEADDIM_SAMPLE
-from model_checks import check_case, oracle_case
-from oracle import e2tts_oracle as O
+from model_checks import check_case, oracle_case, sample_vs_reference, state_dict_vs_reference
 from oracle import reference_cases as RC
 
 import e2_tts_pytorch_b200 as pkg
@@ -23,27 +21,13 @@ def test_oracle_vs_reference(name):
 
 
 def test_sample_vs_reference():
-    s = HEADDIM_SAMPLE
-    g = RC.load('headdim_sample')
-    cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
-    with torch.no_grad():
-        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], s['tkw']), O.TransformerCfg(**s['tkw']), cond,
-                             O.list_str_to_tensor(s['text']),
-                             duration=torch.tensor(s['duration']), y0=RC.randn(g['shape'], 3000 + s['seed']), steps=s['steps'],
-                             cfg_strength=s['cfg_strength'])
-    assert tuple(got.shape) == g['shape']
-    assert RC.compact_rel_l2(got, g['out']) < 1e-4
+    sample_vs_reference(HEADDIM_SAMPLE, RC.load('headdim_sample'))
 
 
 @pytest.mark.parametrize('name', list(HEADDIM_CASES))
 def test_state_dict_matches_reference(name):
     """keys and shapes of the original's model with the same geometry: its checkpoints load"""
-    c = HEADDIM_CASES[name]
-    want = RC.load('headdim_' + name)['shapes']
-    t = dict(dropout=0., max_seq_len=128, **c['tkw'])
-    m = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
-    got = {k: tuple(v.shape) for k, v in m.state_dict().items()}
-    assert got == want
+    state_dict_vs_reference(HEADDIM_CASES[name], RC.load('headdim_' + name))
 
 
 def test_geometry_is_recorded():

@@ -1,12 +1,10 @@
 """CPU: Transformer(num_residual_streams=1), the plain residual backbone (e2_tts.py:547, :607 with disable=True). The oracle with
 one stream against what the original e2_tts.py computed with that setting (tests/golden/reference/residual1_*.pt,
-tools/make_residual_golden.py), the package's parameter layout against the original's, the stream counts that still raise, and the
+oracle/make_reference_golden.py), the package's parameter layout against the original's, the stream counts that still raise, and the
 C-ABI validation of the branch-norm and residual-convolution fields."""
 import pytest
-import torch
 
-from model_checks import check_case, oracle_case
-from oracle import e2tts_oracle as O
+from model_checks import check_case, oracle_case, sample_vs_reference, state_dict_vs_reference
 from oracle import reference_cases as RC
 from residual_variants import RESIDUAL1_CASES, RESIDUAL1_SAMPLE
 
@@ -25,27 +23,13 @@ def test_oracle_vs_reference(name):
 
 
 def test_sample_vs_reference():
-    s = RESIDUAL1_SAMPLE
-    g = RC.load('residual1_sample')
-    tkw = RESIDUAL1_CASES['depth2']['tkw']
-    cond = RC.randn((s['cond'][0], s['cond'][1], 100), s['seed'] + 1000)
-    with torch.no_grad():
-        got = O.e2tts_sample(RC.state_dict('E2TTS', s['seed'], tkw), O.TransformerCfg(**tkw), cond, O.list_str_to_tensor(s['text']),
-                             duration=torch.tensor(s['duration']), y0=RC.randn(g['shape'], 3000 + s['seed']), steps=s['steps'],
-                             cfg_strength=s['cfg_strength'])
-    assert tuple(got.shape) == g['shape']
-    assert RC.compact_rel_l2(got, g['out']) < 1e-4
+    sample_vs_reference(RESIDUAL1_SAMPLE, RC.load('residual1_sample'))
 
 
 @pytest.mark.parametrize('name', list(RESIDUAL1_CASES))
 def test_state_dict_matches_reference(name):
     """keys and shapes of the original's model: no hyper_conns entries, so its checkpoints load"""
-    c = RESIDUAL1_CASES[name]
-    want = RC.load('residual1_' + name)['shapes']
-    t = dict(dropout=0., max_seq_len=128, **c['tkw'])
-    m = pkg.E2TTS(transformer=t, use_vocos=False) if c['cls'] == 'E2TTS' else pkg.DurationPredictor(transformer=t)
-    got = {k: tuple(v.shape) for k, v in m.state_dict().items()}
-    assert got == want
+    state_dict_vs_reference(RESIDUAL1_CASES[name], RC.load('residual1_' + name))
 
 
 def test_plain_residual_makes_no_randrange_draw():
