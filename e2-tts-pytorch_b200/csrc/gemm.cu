@@ -664,10 +664,12 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     else rc = make_map(&tB, a->B, a->N, a->K, a->ldb, BK);
     if (rc) return rc;
     if (!a->d_fp32) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D) & 3) == 0, "gemm: bf16 output must be 4-byte aligned");
-    // TMA tile stores and loads need 16-byte aligned bases (every pitch is a multiple of 16 bytes already); other bf16 outputs store
-    // from the fragments, and other residuals are read from global memory next to them
+    // TMA tile stores and loads need 16-byte aligned bases (every pitch is a multiple of 16 bytes already), and the stores rows of
+    // whole 16-byte units: a tile store does not clip the last partial unit of a row at column N, so with N % 8 != 0 it would write
+    // the tile's columns past N into the output's padding. Other bf16 outputs store from the fragments, and other residuals are read
+    // from global memory next to them.
     const auto a16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-    p.tma_store = !a->d_fp32 && !a->geglu && a16(a->D);
+    p.tma_store = !a->d_fp32 && !a->geglu && a16(a->D) && (p.N % 8) == 0;
     p.resid_tma = p.tma_store && a->resid && a16(a->resid);
     tD = tR = tB;   // unused unless set below
     if (p.tma_store && (rc = make_map(&tD, a->D, a->N, a->M, a->ldd, 64))) return rc;

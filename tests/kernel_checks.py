@@ -226,6 +226,69 @@ def ref64(A, B):
     return a @ b.t(), gamma(A.shape[1]) * (a.abs() @ b.abs().t())
 
 
+def operands(M, N, K, seed, scale=1.0):
+    """bf16 A [M, K] and B [N, K] (B scaled), drawn on the device"""
+    g = torch.Generator(device=dev()).manual_seed(seed)
+    A = torch.randn(M, K, device=dev(), generator=g).to(BF16)
+    B = (torch.randn(N, K, device=dev(), generator=g) * scale).to(BF16)
+    return A, B
+
+
+def nan_out(M, ld, fp32=False):
+    return torch.full((M, ld), float('nan'), device=dev(), dtype=F32 if fp32 else BF16)
+
+
+# ------------------------------------------------------------------------------- restated host selection of the GEMM (b200_gemm)
+def item_shape(M, N, force_tile=0):
+    """(rows, cols) of one CTA tile"""
+    wide = force_tile == 3 or (force_tile == 0 and M >= 512 and N >= 256)
+    if wide:
+        return 128, 256
+    return (128 if force_tile == 1 else (256 if (force_tile == 2 or M >= 256) else 128)), 128
+
+
+def work_items(M, N, K, force_tile=0, split_k=1):
+    """(work items, splits, k-blocks per split)"""
+    r, c = item_shape(M, N, force_tile)
+    tiles = -(-M // r) * -(-N // c)
+    kb = -(-K // 64)
+    split = split_k if split_k > 1 else 1
+    if split_k < 0:
+        units = sms()
+        s_fill = (units + tiles // 2) // tiles
+        while s_fill > 1 and tiles * s_fill > units:
+            s_fill -= 1
+        split = max(1, min(max(s_fill, 1), max(kb // 8, 1), 64))
+    split = min(split, kb)
+    per = -(-kb // split)
+    split = -(-kb // per)
+    return tiles * split, split, per
+
+
+def cta_tiles(M, N, K, force_tile=0):
+    """Per CTA of the persistent launch (no split-K), the tiles it runs in order: (tm, tn, slices), with `slices` the 64 x 64 output
+    slices each consumer warpgroup stages for that tile. Work item w = blockIdx.x + i * grid, grid = min(items, SMs); tm = w % tiles_m,
+    tn = w // tiles_m. A warpgroup's slice counter runs on across its CTA's tiles and picks the staging buffer (and residual barrier)
+    by its parity."""
+    r, c = item_shape(M, N, force_tile)
+    tiles_m = -(-M // r)
+    items = work_items(M, N, K, force_tile)[0]
+    grid = min(items, sms())
+    per_col = lambda tn: -(-min(c, N - tn * c) // 64) * (r // 128)
+    return [[(w % tiles_m, w // tiles_m, per_col(w // tiles_m)) for w in range(b, items, grid)] for b in range(grid)]
+
+
+def odd_starts(ctas):
+    """number of tiles that begin on an odd slice count of their warpgroup (the staging buffer 1 and the barrier phase that go with it)"""
+    n = 0
+    for tiles in ctas:
+        done = 0
+        for _, _, s in tiles:
+            n += done & 1
+            done += s
+    return n
+
+
 def assert_close(name, got, ref, bound):
     got = got.to(F64)
     err = (got - ref).abs()

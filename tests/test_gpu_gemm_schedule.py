@@ -7,57 +7,21 @@ float64: the cfg2 shapes are too large for the host). Bounds:
   (k-blocks, wgmma k16 steps, split-K atomics) is within gamma_K * sum_k |a_k b_k| of the exact value (Higham, Accuracy and
   Stability of Numerical Algorithms, 2nd ed., eq. (3.5)); fp32 epilogue operations (bias, gate, residual add) round once each.
   bf16 outputs: one round-to-nearest of that fp32 value: + 2^-8 |value| (bf16 unit roundoff).
-The tile and split-K selections are restated below from b200_gemm so that each case can assert which side of a threshold it is on.
+The tile and split-K selections are restated in kernel_checks (item_shape, work_items) so that each case can assert which side of a
+threshold it is on.
 """
 import math
 
 import pytest
 import torch
 
-from kernel_checks import BF16, F32, F64, U, U16, assert_close, check_bf16, dev, drop_mask, pkg, ref64, sms
+from kernel_checks import (BF16, F32, F64, U, U16, assert_close, check_bf16, dev, drop_mask, item_shape, nan_out, operands, pkg, ref64,
+                           sms, work_items)
 
 pytestmark = pytest.mark.gpu
 
 
-# ---------------------------------------------------------------------------------------------- restated host selection (b200_gemm)
-def item_shape(M, N, force_tile=0):
-    """(rows, cols) of one CTA tile"""
-    wide = force_tile == 3 or (force_tile == 0 and M >= 512 and N >= 256)
-    if wide:
-        return 128, 256
-    return (128 if force_tile == 1 else (256 if (force_tile == 2 or M >= 256) else 128)), 128
-
-
-def work_items(M, N, K, force_tile=0, split_k=1):
-    """(work items, splits, k-blocks per split)"""
-    r, c = item_shape(M, N, force_tile)
-    tiles = -(-M // r) * -(-N // c)
-    kb = -(-K // 64)
-    split = split_k if split_k > 1 else 1
-    if split_k < 0:
-        units = sms()
-        s_fill = (units + tiles // 2) // tiles
-        while s_fill > 1 and tiles * s_fill > units:
-            s_fill -= 1
-        split = max(1, min(max(s_fill, 1), max(kb // 8, 1), 64))
-    split = min(split, kb)
-    per = -(-kb // split)
-    split = -(-kb // per)
-    return tiles * split, split, per
-
-
-# ---------------------------------------------------------------------------------------------- operands and checks
-def operands(M, N, K, seed, scale=1.0):
-    g = torch.Generator(device=dev()).manual_seed(seed)
-    A = torch.randn(M, K, device=dev(), generator=g).to(BF16)
-    B = (torch.randn(N, K, device=dev(), generator=g) * scale).to(BF16)
-    return A, B
-
-
-def nan_out(M, ld, fp32=False):
-    return torch.full((M, ld), float('nan'), device=dev(), dtype=F32 if fp32 else BF16)
-
-
+# ---------------------------------------------------------------------------------------------- checks
 def run_plain(pkg, M, N, K, seed, force_tile=0, b_mn=False, a_mn=False):
     A, B = operands(M, N, K, seed)
     ref, acc = ref64(A, B)
