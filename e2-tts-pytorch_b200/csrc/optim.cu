@@ -1,6 +1,7 @@
 // Multi-tensor kernels for the step AROUND the forward/backward hot path (SURVEY §8f row 1, §8e):
 //   flat_gather  : every parameter gradient -> one contiguous fp32 buffer (x 1/world), ONE launch, so the data-parallel exchange is a
 //                  single ncclAllReduce over one buffer instead of DDP's bucket copies + hooks (trainer.py:155-162, :270)
+//   flat_accumulate : the same walk, adding (x scale) into the buffer instead of overwriting it: gradient accumulation over micro-batches
 //   sumsq        : global gradient norm^2 of that buffer (clip_grad_norm_, trainer.py:272-273)
 //   adopt_step   : gradient clip + Adopt update (adam-atan2-pytorch `Adopt`, trainer.py:183, :275) + EMA of the parameters
 //                  (ema-pytorch `EMA.update`, trainer.py:279) in ONE pass: 5 reads + 4 writes of fp32 per parameter
@@ -29,6 +30,26 @@ __global__ void __launch_bounds__(256) flat_gather_kernel(const b200_chunk* __re
         reinterpret_cast<float4*>(dst)[i] = v;
     }
     for (int i = n4 * 4 + threadIdx.x; i < c.n; i += 256) dst[i] = __ldg(src + i) * scale;
+}
+
+// accumulate: flat[flat_offset + i] = fmaf(scale, ptr[i], flat[flat_offset + i]) — the gather's twin for gradient accumulation over
+// micro-batches. A NULL ptr leaves its slot as it is, and `used` is only ever set (the OR of the presence flags over the calls).
+__global__ void __launch_bounds__(256) flat_accumulate_kernel(const b200_chunk* __restrict__ chunks, float* __restrict__ flat, float scale,
+                                                              float* __restrict__ used) {
+    const b200_chunk c = chunks[blockIdx.x];
+    const float* __restrict__ src = reinterpret_cast<const float*>(c.ptr);
+    if (src == nullptr) return;
+    float* __restrict__ dst = flat + c.flat_offset;
+    if (used && threadIdx.x == 0) used[c.pidx] = 1.f;
+    const bool vec = ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(dst)) & 15) == 0;
+    const int n4 = vec ? c.n >> 2 : 0;
+    for (int i = threadIdx.x; i < n4; i += 256) {
+        const float4 g = __ldg(reinterpret_cast<const float4*>(src) + i);
+        float4 a = reinterpret_cast<const float4*>(dst)[i];
+        a.x = fmaf(scale, g.x, a.x); a.y = fmaf(scale, g.y, a.y); a.z = fmaf(scale, g.z, a.z); a.w = fmaf(scale, g.w, a.w);
+        reinterpret_cast<float4*>(dst)[i] = a;
+    }
+    for (int i = n4 * 4 + threadIdx.x; i < c.n; i += 256) dst[i] = fmaf(scale, __ldg(src + i), dst[i]);
 }
 
 // sumsq: the block partials go to a static device array and the last block to finish adds them in block order, so the norm is
@@ -162,6 +183,12 @@ extern "C" int b200_flat_gather(const b200_chunk* chunks_dev, int32_t n_chunks, 
     B200_REQUIRE(chunks_dev && flat && n_chunks > 0, "flat_gather: null pointer / empty table");
     flat_gather_kernel<<<n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(chunks_dev, flat, scale, used);
     return check_launch("flat_gather_kernel");
+}
+
+extern "C" int b200_flat_accumulate(const b200_chunk* chunks_dev, int32_t n_chunks, float* flat, float scale, float* used, b200_stream_t stream) {
+    B200_REQUIRE(chunks_dev && flat && n_chunks > 0, "flat_accumulate: null pointer / empty table");
+    flat_accumulate_kernel<<<n_chunks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(chunks_dev, flat, scale, used);
+    return check_launch("flat_accumulate_kernel");
 }
 
 extern "C" int b200_flat_scatter(const b200_chunk* chunks_dev, int32_t n_chunks, const float* flat, b200_stream_t stream) {

@@ -21,10 +21,15 @@ branch: it would be frozen either way).
 """
 from __future__ import annotations
 
+import random
+import time
+
 import torch
 
 from . import lib
 from .optim import GradSync, broadcast_module
+
+MAX_BATCH = 64   # b200_small_linear's row limit (csrc/small.cu): the per-item conditioning GEMMs take at most 64 items
 
 
 class _Loss:
@@ -32,14 +37,44 @@ class _Loss:
         self.loss = loss
 
 
+def _refuse_ddp_wrapper(model, who):
+    if hasattr(model, 'module') and not hasattr(model, 'transformer'):
+        raise ValueError(f'{who}: pass the bare E2TTS module, not a DistributedDataParallel wrapper '
+                         '(gradients are averaged by one flat all-reduce after the replay)')
+
+
+def _world(process_group):
+    import torch.distributed as dist
+    return dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
+
+
+def _new_seed_word(model, dev):
+    """the device seed word: every dropout seed of the step is `host seed + *seed_dev` (frozen host part, stepping device part)"""
+    seed_dev = torch.randint(0, 2 ** 62, (1,), dtype=torch.int64).to(dev)
+    model.transformer._seed_dev = seed_dev
+    return seed_dev
+
+
+def _train_pass(model, seed_dev, mel, text, lens):
+    """one forward + backward as captured: the seed word steps first, then the model's own training objective"""
+    lib.call('b200_seed_advance', seed_dev, torch.cuda.current_stream().cuda_stream)
+    out = model(mel, text=text, lens=lens)
+    if torch.is_tensor(out):       # DurationPredictor.forward returns the scalar loss itself (e2_tts.py:1113)
+        out = _Loss(out)
+    out.loss.backward()
+    return out
+
+
+def _clear_grads(model):
+    for p in model.parameters():
+        p.grad = None
+
+
 class GraphedTrainStep:
     def __init__(self, model, mel, *, text=None, lens=None, warmup=3, process_group=None, flat_grads=None):
         """model: an E2TTS or a DurationPredictor (NOT wrapped in DistributedDataParallel — the exchange is done here). flat_grads: True forces the flat
         gradient buffer even on one rank (for the fused optimiser); default = only when world_size > 1."""
-        import torch.distributed as dist
-        if hasattr(model, 'module') and not hasattr(model, 'transformer'):
-            raise ValueError('GraphedTrainStep: pass the bare E2TTS module, not a DistributedDataParallel wrapper '
-                             '(gradients are averaged by one flat all-reduce after the replay)')
+        _refuse_ddp_wrapper(model, 'GraphedTrainStep')
         if model.training and 0.0 < float(getattr(model, 'cond_drop_prob', 0.0)) < 1.0:
             raise ValueError('GraphedTrainStep: cond_drop_prob must be 0 or 1 (the text-drop branch is decided on the host)')
         if not mel.is_cuda:
@@ -49,14 +84,12 @@ class GraphedTrainStep:
         self.mel = mel.clone()
         self.text = text.clone() if torch.is_tensor(text) else (model.tokenizer(text).to(dev) if isinstance(text, list) else None)
         self.lens = lens.clone() if torch.is_tensor(lens) else None
-        world = dist.get_world_size(process_group) if dist.is_available() and dist.is_initialized() else 1
+        world = _world(process_group)
         if world > 1:
             broadcast_module(model, 0, process_group)    # replicas must start identical (DDP does this when it wraps the module)
         use_flat = (world > 1) if flat_grads is None else bool(flat_grads) or world > 1
         self.grad_sync = GradSync(list(model.parameters()), process_group) if use_flat else None
-        # the device seed word: every dropout seed of the step is `host seed + *seed_dev` (frozen host part, stepping device part)
-        self._seed_dev = torch.randint(0, 2 ** 62, (1,), dtype=torch.int64).to(dev)
-        model.transformer._seed_dev = self._seed_dev
+        self._seed_dev = _new_seed_word(model, dev)
         cur = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(dev)
         side.wait_stream(cur)
@@ -87,16 +120,10 @@ class GraphedTrainStep:
             self.grad_sync.attach()
 
     def _eager(self):
-        lib.call('b200_seed_advance', self._seed_dev, torch.cuda.current_stream().cuda_stream)
-        out = self.model(self.mel, text=self.text, lens=self.lens)
-        if torch.is_tensor(out):       # DurationPredictor.forward returns the scalar loss itself (e2_tts.py:1113)
-            out = _Loss(out)
-        out.loss.backward()
-        return out
+        return _train_pass(self.model, self._seed_dev, self.mel, self.text, self.lens)
 
     def _clear_grads(self):
-        for p in self.model.parameters():
-            p.grad = None
+        _clear_grads(self.model)
 
     def __call__(self, mel=None, *, text=None, lens=None):
         """Run one step on a new batch of the captured shapes; returns the (device) loss tensor of that step (this rank's)."""
@@ -115,3 +142,223 @@ class GraphedTrainStep:
                 if p.grad is not g:
                     p.grad = g
         return self.out.loss
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# ragged batches: one graph per (length bucket, text mode), all in one memory pool, with gradient accumulation
+
+
+class BucketPlan:
+    """The host side of BucketedTrainStep, no GPU needed: which bucket a batch of `n` frames goes to, how its text ids are padded,
+    and every refusal that must come before a launch."""
+
+    def __init__(self, buckets, batch_size, max_seq_len, interpolated_text=False):
+        b = sorted({int(x) for x in buckets})
+        if not b or b[0] < 1:
+            raise ValueError(f'BucketedTrainStep: buckets must be positive frame counts, got {tuple(buckets)}')
+        if b[-1] > max_seq_len:
+            raise ValueError(f'BucketedTrainStep: bucket {b[-1]} exceeds the transformer\'s max_seq_len ({max_seq_len})')
+        if not 1 <= int(batch_size) <= MAX_BATCH:
+            raise ValueError(f'BucketedTrainStep: batch_size {batch_size} is outside 1..{MAX_BATCH} (b200_small_linear takes at most '
+                             f'{MAX_BATCH} items per launch)')
+        self.buckets, self.batch_size, self.interpolated_text = tuple(b), int(batch_size), bool(interpolated_text)
+
+    def bucket(self, n):
+        """the smallest bucket >= n"""
+        for nb in self.buckets:
+            if n <= nb:
+                return nb
+        raise ValueError(f'BucketedTrainStep: a batch of {n} frames exceeds the largest bucket ({self.buckets[-1]})')
+
+    def check(self, batch, n, text_width=None):
+        """-> the bucket of a [batch, n, channels] mel with text ids `text_width` columns wide (None: no text); raises ValueError"""
+        if batch != self.batch_size:
+            raise ValueError(f'BucketedTrainStep: batch of {batch} items, the graphs were captured for batch_size={self.batch_size}')
+        nb = self.bucket(n)
+        if self.interpolated_text and text_width is not None and text_width > nb:
+            raise ValueError(f'BucketedTrainStep: {text_width} text ids do not fit bucket {nb}: with interpolated_text the text is '
+                             'spread over the frames, so it cannot be cut')
+        return nb
+
+    @staticmethod
+    def pad_text(ids, nb, out=None):
+        """(b, nt) ids with -1 padding -> (b, nb): padded with -1 or cut to nb columns — CharacterEmbed cuts and pads to the
+        sequence length itself (e2_tts.py:407-412), so its rows are unchanged"""
+        if out is None:
+            out = torch.empty(ids.shape[0], nb, dtype=torch.int64, device=ids.device)
+        w = min(ids.shape[1], nb)
+        out[:, :w].copy_(ids[:, :w], non_blocking=True)
+        out[:, w:].fill_(-1)
+        return out
+
+
+def text_modes(model):
+    """the text-drop decisions a call can reach, as (drop,) flags: E2TTS in training mode draws the reference's coin
+    `random() < cond_drop_prob` (e2_tts.py:1261), so 0 < p < 1 reaches both, p <= 0 only the text and p >= 1 only the dropped one;
+    an E2TTS in eval mode or a DurationPredictor always uses the text"""
+    p = float(getattr(model, 'cond_drop_prob', 0.0))
+    if not (hasattr(model, 'cond_drop_prob') and model.training):
+        return (False,)
+    if p <= 0.0:
+        return (False,)
+    if p >= 1.0:
+        return (True,)
+    return (False, True)
+
+
+def draw_text_drop(model, has_text):
+    """the text-drop decision of one call: exactly one python `random.random()` for an E2TTS in training mode (as
+    transformer_with_pred_head draws it, whether or not text is given); no text at all means the dropped graph"""
+    drop = hasattr(model, 'cond_drop_prob') and model.training and random.random() < model.cond_drop_prob
+    return bool(drop) or not has_text
+
+
+class _KeepPythonRandom:
+    """restores python's `random` state on exit: warm-ups and captures run the model's own coin, which must not shift the user's"""
+
+    def __enter__(self):
+        self.state = random.getstate()
+
+    def __exit__(self, *a):
+        random.setstate(self.state)
+
+
+class BucketedTrainStep:
+    """CUDA-graphed training steps on ragged batches with gradient accumulation (trainer.py:61-82 pads each batch to its longest clip,
+    :142/:160/:250 accumulate `grad_accumulation_steps` micro-batches). GraphedTrainStep is the fixed-shape, k = 1 special case.
+
+        steps = BucketedTrainStep(model, batch_size=16, buckets=(256, 512, 768, 1024, 1408), grad_accumulation_steps=4)
+        for batch in loader:
+            loss = steps(batch['mel'], text=batch['text'], lens=batch['lens'])
+            if steps.sync_gradients:
+                opt.step(steps.grad_sync.flat)
+
+    * A batch of n frames replays the graph of the smallest bucket N_b >= n: mel is zero-padded to N_b, `lens` defaults to n (the
+      reference's full(seq_len)) and is kept as given otherwise, text ids are padded with -1 / cut to N_b columns. Frames at or past
+      `lens` are masked keys, zeroed ahead of both convolutions and outside the loss span, so the padding changes no loss or gradient;
+      only the noise the CUDA generator draws differs (it is drawn at the padded shape).
+    * The text-drop coin is drawn per call on the host (one `random.random()`, as the reference) and picks the text or the
+      text-dropped graph of the bucket; only the modes cond_drop_prob can reach are captured.
+    * Every graph ends with b200_flat_accumulate (x 1 / (k * world)) into one GradSync buffer: the first call of a window clears it,
+      the k-th does ONE all-reduce, attaches p.grad as views of it and sets `sync_gradients`. Between windows p.grad holds the
+      previous window's views; feed the optimiser only when `sync_gradients` is set.
+    * All graphs share one memory pool (captured largest bucket first) and one dropout seed word. Nothing a caller reads lives in
+      the pool: the loss is copied into a buffer of its own and the gradients are consumed by the in-graph accumulate.
+    FusedAdoptEMA runs one EMA update per optimiser step (ema-pytorch's EMA.update runs per micro-batch in trainer.py:279)."""
+
+    def __init__(self, model, batch_size, buckets, *, grad_accumulation_steps=1, process_group=None, warmup=3):
+        _refuse_ddp_wrapper(model, 'BucketedTrainStep')
+        if float(getattr(model, 'velocity_consistency_weight', 0.0)) > 0.0:
+            raise ValueError('BucketedTrainStep: velocity consistency is not graphed (the reference trainer feeds it the EMA model '
+                             'each step, trainer.py:259-268); use the eager step')
+        k = int(grad_accumulation_steps)
+        if k < 1:
+            raise ValueError(f'BucketedTrainStep: grad_accumulation_steps must be >= 1, got {grad_accumulation_steps}')
+        from .modules import InterpolatedCharacterEmbed
+        self.plan = BucketPlan(buckets, batch_size, model.transformer.max_seq_len,
+                               isinstance(getattr(model, 'embed_text', None), InterpolatedCharacterEmbed))
+        dev = next(model.parameters()).device
+        if dev.type != 'cuda':
+            raise ValueError('BucketedTrainStep: the model must live on the GPU')
+        self.model, self.grad_accumulation_steps = model, k
+        self.modes = text_modes(model)
+        world = _world(process_group)
+        if world > 1:
+            broadcast_module(model, 0, process_group)    # replicas must start identical (DDP does this when it wraps the module)
+        self.grad_sync = GradSync(list(model.parameters()), process_group)
+        self._scale = 1.0 / (k * world)
+        self._seed_dev = _new_seed_word(model, dev)
+        self._e2tts = hasattr(model, 'cond_drop_prob')
+        B, C = self.plan.batch_size, model.num_channels
+        order = sorted(self.plan.buckets, reverse=True)   # largest first: it sizes the zero pool and the caches before the small ones
+        # static inputs and loss outputs, all outside the graph pool
+        self._mel = {nb: torch.zeros(B, nb, C, device=dev) for nb in order}
+        self._lens = {nb: torch.full((B,), nb, device=dev, dtype=torch.int64) for nb in order}
+        self._text = {}
+        for nb in order:
+            t = torch.full((B, nb), -1, device=dev, dtype=torch.int64)
+            t[:, :max(1, nb // 4)] = ord('a')
+            self._text[nb] = t
+        self._loss = {(nb, d): torch.zeros((), device=dev) for nb in order for d in self.modes}
+        self.graphs, self._tables = {}, {}
+        cdp = getattr(model, 'cond_drop_prob', None)
+        t0 = time.perf_counter()
+        with _KeepPythonRandom():
+            try:
+                cur = torch.cuda.current_stream(dev)
+                side = torch.cuda.Stream(dev)
+                side.wait_stream(cur)
+                with torch.cuda.stream(side):   # warm-up off the capture stream: lazy initialisation, caches, packed weights, rotary tables
+                    for nb in order:
+                        for drop in self.modes:
+                            for _ in range(max(1, warmup)):
+                                self._pass(nb, drop)
+                                _clear_grads(model)
+                    if world > 1:
+                        self.grad_sync.all_reduce()    # NCCL communicator / channel setup outside the timed path
+                cur.wait_stream(side)
+                torch.cuda.synchronize(dev)
+                torch.cuda.empty_cache()
+                self.pool = torch.cuda.graph_pool_handle()
+                n0 = lib.launch_count()
+                for nb in order:
+                    for drop in self.modes:
+                        _clear_grads(model)      # no graph's backward may add into another graph's gradient tensors
+                        table = self.grad_sync.new_table()
+                        g = torch.cuda.CUDAGraph()
+                        with torch.cuda.graph(g, pool=self.pool):
+                            out = self._pass(nb, drop)
+                            self._loss[nb, drop].copy_(out.loss.reshape(()))
+                            grads = self.grad_sync.accumulate(table, self._scale)   # recorded against the (still empty) table
+                        self.grad_sync.fill_table(table, grads)
+                        del out, grads
+                        _clear_grads(model)
+                        self.graphs[nb, drop], self._tables[nb, drop] = g, table
+                self.launches_per_step = (lib.launch_count() - n0) // len(self.graphs)
+            finally:
+                if cdp is not None:
+                    model.cond_drop_prob = cdp
+        torch.cuda.synchronize(dev)
+        self.capture_seconds = time.perf_counter() - t0   # warm-ups + captures
+        self.grad_sync.zero()
+        self._micro = 0
+        self.sync_gradients = False
+
+    def _pass(self, nb, drop):
+        if self._e2tts:    # pin the coin inside the capture; python's random state is restored by the caller
+            self.model.cond_drop_prob = 1.0 if drop else 0.0
+        text = None if (drop and self._e2tts) else self._text[nb]
+        return _train_pass(self.model, self._seed_dev, self._mel[nb], text, self._lens[nb])
+
+    def __call__(self, mel, *, text=None, lens=None):
+        """One micro-step on a [batch_size, n, channels] mel (n <= the largest bucket), text ids [batch_size, nt] or a list of
+        strings, optional lens [batch_size]. Returns this micro-batch's (unscaled) loss on the device."""
+        if isinstance(text, list):
+            from .modules import list_str_to_tensor
+            text = (self.model.tokenizer(text) if self._e2tts else list_str_to_tensor(text)).to(mel.device)
+        B, n = int(mel.shape[0]), int(mel.shape[1])
+        nb = self.plan.check(B, n, None if text is None else int(text.shape[1]))
+        if text is None and True not in self.modes:
+            raise ValueError('BucketedTrainStep: text=None needs the text-dropped graph, which is only captured for an E2TTS in '
+                             'training mode with cond_drop_prob > 0')
+        drop = draw_text_drop(self.model, text is not None)
+        if self._micro == 0:
+            self.grad_sync.zero()
+        m = self._mel[nb]
+        m[:, :n].copy_(mel, non_blocking=True)
+        if n < nb:
+            m[:, n:].zero_()
+        if lens is None:
+            self._lens[nb].fill_(n)
+        else:
+            self._lens[nb].copy_(lens, non_blocking=True)
+        if text is not None and not drop:
+            self.plan.pad_text(text, nb, out=self._text[nb])
+        self.graphs[nb, drop].replay()
+        self._micro += 1
+        self.sync_gradients = self._micro == self.grad_accumulation_steps
+        if self.sync_gradients:
+            self._micro = 0
+            self.grad_sync.all_reduce()
+            self.grad_sync.attach()
+        return self._loss[nb, drop].clone()

@@ -5,6 +5,7 @@ Reference call sites (e2_tts_pytorch/trainer.py of the original project): DDP gr
 :279. Here they are three launches over flat fp32 buffers:
 
     GradSync()      b200_flat_gather  every p.grad (x 1/world) -> ONE contiguous buffer, then ONE ncclAllReduce (no bucket hooks)
+    .accumulate()   b200_flat_accumulate  buffer += p.grad x 1/(steps*world) per micro-batch (grad_accumulation_steps, :142/:160/:250)
     FusedAdoptEMA   b200_sumsq        global gradient norm^2 of that buffer
                     b200_adopt_step   clip + Adopt + EMA in one pass
 
@@ -124,6 +125,23 @@ class GradSync:
                 raise RuntimeError('GradSync.gather: p.grad already is the flat view (gather twice without a backward in between?)')
         lib.call('b200_flat_gather', table if table is not None else lay.table(grads), lay.n_chunks, self.flat, 1.0 / self.world, self.used, _stream())
         return grads
+
+    def accumulate(self, table=None, scale=1.0):
+        """The accumulating twin of gather(): flat += scale * p.grad (one fmaf per element), `used` ORed with this micro-step's
+        presence flags; a parameter without a gradient keeps its slot. scale = 1 / (steps * world) for accelerate's `loss / steps`
+        plus DDP's average. Clear the buffer with zero() at the start of each accumulation window. Same `table` rule as gather()."""
+        lay = self.layout
+        grads = [p.grad for p in lay.params]
+        for g, v in zip(grads, self.grad_views):
+            if g is not None and g.data_ptr() == v.data_ptr():
+                raise RuntimeError('GradSync.accumulate: p.grad is the flat view itself (attach() ran without a backward in between?)')
+        lib.call('b200_flat_accumulate', table if table is not None else lay.table(grads), lay.n_chunks, self.flat, float(scale), self.used,
+                 _stream())
+        return grads
+
+    def zero(self):
+        """Clear the gradients and the `used` flags (one memset over the shared buffer)."""
+        self._buf.zero_()
 
     def new_table(self):
         return torch.zeros(self.layout.n_chunks * _CHUNK_DT.itemsize, device=self.layout.device, dtype=torch.uint8)

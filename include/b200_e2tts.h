@@ -568,6 +568,12 @@ typedef struct { void* ptr; int64_t flat_offset; int32_t n; int32_t pidx; /* ind
  * used (optional, fp32 [n_params]): used[pidx] = 1 if the parameter had a gradient else 0 — summed by the same all-reduce when it
  * lies right behind the gradients, it tells the optimiser which parameters no rank touched (torch optimisers skip grad=None). */
 int b200_flat_gather(const b200_chunk* chunks_dev, int32_t n_chunks, float* flat, float scale, float* used, b200_stream_t stream);
+/* Gradient accumulation over micro-batches (trainer.py grad_accumulation_steps): flat[flat_offset + i] = fmaf(scale, ptr[i],
+ * flat[flat_offset + i]), ONE fp32 rounding per element. A NULL ptr (no gradient on this micro-step) leaves its slot untouched;
+ * used[pidx] (optional) is set to 1 where ptr is non-NULL and never cleared, so over the micro-steps it is the OR of the presence
+ * flags (torch: p.grad is None only if no micro-step produced one). The 4-element padding between parameters is never written.
+ * No allocation, no host sync: capturable. scale = 1 / (steps * world_size) gives accelerate's loss / steps and DDP's average. */
+int b200_flat_accumulate(const b200_chunk* chunks_dev, int32_t n_chunks, float* flat, float scale, float* used, b200_stream_t stream);
 /* ptr[i] = flat[flat_offset + i] (e.g. EMA weights into a module's parameters) */
 int b200_flat_scatter(const b200_chunk* chunks_dev, int32_t n_chunks, const float* flat, b200_stream_t stream);
 /* *out = sum x[i]^2 (out: ONE device float, overwritten): torch.nn.utils.clip_grad_norm_'s total norm, trainer.py:272-273.
