@@ -10,8 +10,11 @@
 //                             staging slice (two per warpgroup, alternating) and leave as TMA tile stores (bulk async groups), so the
 //                             warpgroup moves on to the next slice while the previous one drains. A residual slice is TMA-loaded into
 //                             the staging buffer its output slice will occupy (the tile's first two while its last k-blocks still run),
-//                             and the epilogue adds it from shared memory in place. GEGLU outputs leave as bf16x2 stores from the
-//                             fragments, fp32 split-K partials through vector atomics.
+//                             and the epilogue adds it from shared memory in place. GLU outputs of K-major operands take the same
+//                             slices: per 64 rows and 128 packed columns, u + bias and gate + bias leave as two pre-activation
+//                             slices and h, computed from the bf16 values just staged, as a third; the producer stages the tile's
+//                             bias and glu_mult in shared memory. Outputs without 16-byte aligned bases store bf16x2 pairs from the fragments, fp32 split-K
+//                             partials go through vector atomics.
 // While a consumer warpgroup runs its epilogue the producer is already filling the ring with the next tile's operands.
 // Operands may be K-major or MN-major (transposed storage) so that the backward contractions
 // dX = dY*W and dW = dY^T*X read activations exactly as they lie in HBM — no transposes are materialised.
@@ -44,6 +47,7 @@ struct GemmParams {
     int tma_store;   // bf16 output through the smem staging slices and TMA stores (tmD)
     int resid_tma;   // tma_store with a 16-byte aligned residual: its slices are TMA-loaded into the staging buffers (tmR)
     const float* glu_mult;   // optional [N/2] multiplier of the hidden units (x-transformers GLU mult_bias), hidden-unit order
+    int glu_tma;     // GLU outputs through the staging slices and TMA stores (h: tmD, pre-activations: tmD2); bias / glu_mult staged per tile
 };
 
 constexpr int GLU_GELU = 1, GLU_SILU = 2, GLU_RELU2 = 3;
@@ -59,9 +63,10 @@ struct GemmSmem {
     static constexpr int kStages = (STAGE_BYTES <= 32768) ? 6 : 4;
     static constexpr int TILE_BYTES = kStages * STAGE_BYTES;
     static constexpr int STG_BYTES = 2 * 2 * kSliceBytes;        // two slices per consumer warpgroup: 32 KB
-    static constexpr int BAR_BYTES = 128;                        // full / empty per stage, + one residual barrier per staging slice
-    static_assert((2 * kStages + 4) * 8 <= BAR_BYTES, "GEMM mbarriers exceed their shared-memory slot");
-    static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + 1024;  // + slack for manual 1024B alignment
+    static constexpr int BAR_BYTES = 256;   // full / empty per stage, one residual barrier per staging slice, GLU operands full / empty
+    static_assert((2 * kStages + 4 + 2) * 8 <= BAR_BYTES, "GEMM mbarriers exceed their shared-memory slot");
+    static constexpr int OPS_BYTES = BN * 4 + BN / 2 * 4;        // GLU tile operands: packed bias [BN] and glu_mult [BN / 2], fp32
+    static constexpr int TOTAL = TILE_BYTES + STG_BYTES + BAR_BYTES + OPS_BYTES + 1024;  // + slack for manual 1024B alignment
     static_assert(TOTAL <= 227 * 1024, "GEMM shared memory exceeds the 227 KB a block may use");
 };
 
@@ -119,6 +124,13 @@ __device__ __forceinline__ float2 glu_act2(float2 g) {
 // address; toff = (16 wq + lane / 4) * 128 + 4 (lane % 4), swz = (lane / 4) << 4.
 __device__ __forceinline__ uint32_t slice_addr(uint32_t buf, uint32_t toff, uint32_t swz, int i, int jj) {
     return buf + toff + (uint32_t)i * 8 * 128 + (((uint32_t)jj << 4) ^ swz);
+}
+// toff of the GLU epilogue, from the lane index read inside it: computed once ahead of the tile loop, it would hold a register
+// through the mainloop, and the 128 x 256 tile spills it.
+__device__ __forceinline__ uint32_t slice_toff(int wq) {
+    uint32_t l;
+    asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));
+    return (uint32_t)(wq * 16 + (l >> 2)) * 128 + 4 * (l & 3);
 }
 // Waits until the buffer of slice n is free (the store issued from it two slices ago has read it); returns its shared address.
 __device__ __forceinline__ uint32_t slice_acquire(uint8_t* my_stg, uint32_t n, int cw, int t) {
@@ -249,6 +261,74 @@ __device__ __forceinline__ void store_slices(const GemmParams& p, float (&acc)[M
     }
 }
 
+// GLU epilogue through the staging slices. Per 64-row band and 128-packed-column group, three 64 x 64 slices leave by TMA store:
+// u + bias to D2 at packed column colg, gate + bias to D2 at colg + 64, then h to D at hidden column colg / 2. Hidden unit c of the
+// group sits at the same slice position as its u and gate, so h is computed pair by pair from the bf16 u and gate the thread itself
+// wrote to the two buffers (the rounded values the backward pass recomputes from) and written over u once u's store has read it.
+// sbias / smult: the tile's packed bias and glu_mult slice, staged in shared memory by the producer; the dropout hashes are made in
+// the h loop, one pair at a time. Bit-identical to glu_epilogue.
+template <int ACT, int BN, int MH>
+__device__ __forceinline__ void glu_store_slices(const GemmParams& p, float (&acc)[MH][BN / 2], const CUtensorMap* tmD, const CUtensorMap* tmD2,
+                                                 uint8_t* my_stg, const float* sbias, const float* smult, uint32_t& nslice, int tm, int tn,
+                                                 int cw, int wq, int lane, int t) {
+    const uint32_t swz = (uint32_t)(lane >> 2) << 4;
+    const uint32_t toff = slice_toff(wq);
+    const int cq = 2 * (lane & 3);
+    const bool do_drop = p.dropout_p > 0.f;
+    const float keep_scale = do_drop ? 65536.f / (65536.f - (float)(uint32_t)(p.dropout_p * 65536.f)) : 1.f;
+    const uint32_t seedmix = do_drop ? seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull)) : 0u;
+    const uint32_t thr32 = drop_thresh32((uint32_t)(p.dropout_p * 65536.f));
+#pragma unroll
+    for (int h = 0; h < MH; ++h) {
+        const int rowb = tm * BM * MH + (cw * MH + h) * 64;
+#pragma unroll
+        for (int sub = 0; sub < BN / 128; ++sub) {
+            const int colg = tn * BN + sub * 128;   // first packed column of the group (N % 128 == 0)
+            if (colg >= p.N) break;                  // uniform across the warpgroup
+            // u (half 0), then gate (half 1): + bias, rounded to bf16, out to D2
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+                const uint32_t buf = slice_acquire(my_stg, nslice, cw, t);
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                    for (int jj = 0; jj < 8; ++jj) {
+                        const int j = sub * 16 + half * 8 + jj;
+                        float2 v = make_float2(acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]);
+                        if (p.bias) v = fadd2(v, *reinterpret_cast<const float2*>(sbias + 8 * j + cq));
+                        st_shared_u32(slice_addr(buf, toff, swz, i, jj), pack_bf16(v.x, v.y));
+                    }
+                }
+                slice_store(tmD2, my_stg, nslice, cw, t, colg + 64 * half, rowb);
+                ++nslice;
+            }
+            // h into u's buffer: its store was issued two slices ago, the gate store one ago
+            const uint32_t bu = slice_acquire(my_stg, nslice, cw, t);
+            const uint32_t bg = smem_u32(my_stg + ((nslice + 1) & 1) * kSliceBytes);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int row = rowb + wq * 16 + (lane >> 2) + 8 * i;
+#pragma unroll
+                for (int jj = 0; jj < 8; ++jj) {
+                    const int hl = sub * 64 + 8 * jj + cq;   // hidden-unit column within the tile
+                    const uint32_t a = slice_addr(bu, toff, swz, i, jj);
+                    const uint32_t wu = ld_shared_u32(a), wgt = ld_shared_u32(slice_addr(bg, toff, swz, i, jj));
+                    float2 h2 = fmul2(make_float2(bf16_lo(wu), bf16_hi(wu)), glu_act2<ACT>(make_float2(bf16_lo(wgt), bf16_hi(wgt))));
+                    if (p.glu_mult) h2 = fmul2(h2, *reinterpret_cast<const float2*>(smult + hl));
+                    if (do_drop) {
+                        const int hcol = tn * (BN / 2) + hl;
+                        const DropWords hsh = drop_words(seedmix, (uint32_t)(((unsigned long long)row * (unsigned long long)(p.N / 2) + hcol) >> 1));
+                        h2 = fmul2(h2, make_float2(hsh.a >= thr32 ? keep_scale : 0.f, hsh.b >= thr32 ? keep_scale : 0.f));
+                    }
+                    st_shared_u32(a, pack_bf16(h2.x, h2.y));
+                }
+            }
+            slice_store(tmD, my_stg, nslice, cw, t, colg / 2, rowb);
+            ++nslice;
+        }
+    }
+}
+
 // One bf16 pair / fp32 pair of the output: columns (col, col + 1) of `row`; col is even.
 __device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col, float v0, float v1) {
     const bool two = col + 1 < p.N;
@@ -275,7 +355,7 @@ template <int BN, bool A_MN, bool B_MN, int MH, int ACT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
                   const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
-                  const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
+                  const __grid_constant__ CUtensorMap tmR, const __grid_constant__ CUtensorMap tmD2, const GemmParams p) {
     using S = GemmSmem<BN, MH>;
     constexpr int kStages = S::kStages;
     constexpr int BMT = BM * MH;   // rows of the CTA tile
@@ -289,6 +369,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::TILE_BYTES + S::STG_BYTES);
     uint64_t* empty_bar = full_bar + kStages;
     uint64_t* resid_bar = empty_bar + kStages;   // [warpgroup][2]: the residual slice TMA-loaded into that staging buffer has landed
+    uint64_t* ops_full = resid_bar + 4;          // glu_tma: the tile's bias / glu_mult have landed in sops
+    uint64_t* ops_empty = ops_full + 1;          // glu_tma: both consumer warpgroups are done reading them (one arrival each)
+    float* sops = reinterpret_cast<float*>(smem + S::TILE_BYTES + S::STG_BYTES + S::BAR_BYTES);   // [BN] bias, then [BN / 2] glu_mult
+    // the GLU TMA path is built into the K-major kernels only (the model's FF-in); the others keep their instructions as they were
+    constexpr bool kGluTma = !A_MN && !B_MN;
+    const bool glu_ops = kGluTma && p.glu_tma && (p.bias || p.glu_mult);
 
     const int wg = threadIdx.x >> 7;
 
@@ -298,11 +384,17 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         tma_prefetch_desc(&tmB);
         if (p.tma_store) tma_prefetch_desc(&tmD);
         if (p.resid_tma) tma_prefetch_desc(&tmR);
+        if (kGluTma && p.glu_tma) {
+            tma_prefetch_desc(&tmD);
+            tma_prefetch_desc(&tmD2);
+        }
         for (int i = 0; i < kStages; ++i) {
             mbar_init(&full_bar[i], 1);
             mbar_init(&empty_bar[i], 2);   // one arrival per consumer warpgroup
         }
         for (int i = 0; i < 4; ++i) mbar_init(&resid_bar[i], 1);
+        mbar_init(ops_full, 1);
+        mbar_init(ops_empty, 2);
         fence_barrier_init();
     }
     __syncthreads();
@@ -313,7 +405,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             // ------------------------------------------------------------ TMA producer
             int stage = 0;
             uint32_t phase = 0;
-            for (int w = blockIdx.x; w < p.num_work; w += gridDim.x) {
+            uint32_t ntile = 0;
+            for (int w = blockIdx.x; w < p.num_work; w += gridDim.x, ++ntile) {
                 const int tm = w % p.tiles_m;
                 const int rest = w / p.tiles_m;
                 const int tn = rest % p.tiles_n;
@@ -345,6 +438,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     }
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
+                if (glu_ops) {
+                    // after the tile's operands, so the ring is refilled ahead of the previous tile's epilogue; the next tile's
+                    // k-blocks wait for ring slots that the consumers free only after that epilogue anyway
+                    const int nb = min(BN, p.N - brow);   // packed columns of the tile (a multiple of 128)
+                    mbar_wait(ops_empty, (ntile & 1) ^ 1);
+                    mbar_arrive_expect_tx(ops_full, (p.bias ? nb * 4 : 0) + (p.glu_mult ? nb * 2 : 0));
+                    if (p.bias) bulk_load_1d(sops, p.bias + brow, nb * 4, ops_full);
+                    if (p.glu_mult) bulk_load_1d(sops + BN, p.glu_mult + brow / 2, nb * 2, ops_full);
+                }
             }
         }
         return;
@@ -365,7 +467,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint32_t nslice = 0;                       // staging slices this warpgroup has filled so far (buffer = nslice & 1)
     int stage = 0;
     uint32_t phase = 0;
-    for (int w = blockIdx.x; w < p.num_work; w += gridDim.x) {
+    uint32_t ntile = 0;
+    for (int w = blockIdx.x; w < p.num_work; w += gridDim.x, ++ntile) {
         const int tm = w % p.tiles_m;
         const int rest = w / p.tiles_m;
         const int tn = rest % p.tiles_n;
@@ -460,6 +563,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             // a copy of the slice loop per case keeps the plain path free of per-element residual branches
             if (p.resid_tma) store_slices<true, BN, MH>(p, acc, &tmD, &tmR, my_stg, my_rbar, nslice, tm, tn, cw, wq, lane, t);
             else store_slices<false, BN, MH>(p, acc, &tmD, &tmR, my_stg, my_rbar, nslice, tm, tn, cw, wq, lane, t);
+        } else if (kGluTma && p.glu_tma) {
+            if constexpr (kGluTma) {
+                if (glu_ops) mbar_wait(ops_full, ntile & 1);
+                if (p.geglu == GLU_GELU) glu_store_slices<GLU_GELU, BN, MH>(p, acc, &tmD, &tmD2, my_stg, sops, sops + BN, nslice, tm, tn, cw, wq, lane, t);
+                else if (p.geglu == GLU_SILU) glu_store_slices<GLU_SILU, BN, MH>(p, acc, &tmD, &tmD2, my_stg, sops, sops + BN, nslice, tm, tn, cw, wq, lane, t);
+                else glu_store_slices<GLU_RELU2, BN, MH>(p, acc, &tmD, &tmD2, my_stg, sops, sops + BN, nslice, tm, tn, cw, wq, lane, t);
+                // the last slice_store's barrier is behind every read of sops by this warpgroup
+                if (glu_ops && t == 0) mbar_arrive(ops_empty);
+            }
         } else if (!p.geglu) {
 #pragma unroll
             for (int h = 0; h < MH; ++h) {
@@ -522,8 +634,8 @@ static PFN_encodeTiled get_encode_fn() {
 }
 
 // 2-D bf16 tensor map: `inner` contiguous elements, `outer` rows of pitch `ld` elements; box = box_inner x box_outer with the swizzle
-// whose span equals the box's row bytes (64 elements / 128B swizzle for operand tiles and plain output tiles, 32 elements / 64B
-// swizzle for the GEGLU output pieces).
+// whose span equals the box's row bytes: 64 elements / 128B swizzle for the operand tiles and every output, pre-activation and
+// residual slice (the only box width in use; 32 elements would take the 64B swizzle).
 // A descriptor is a pure function of (pointer, extents, pitch, box): the caching allocator hands the same addresses back every
 // training step, so a small per-thread direct-mapped cache removes ~1500 driver encode calls per step from the host critical path.
 struct MapKey { const void* ptr; int64_t inner, outer, ld; int box, box_inner; };
@@ -562,7 +674,7 @@ static int make_map_uncached(CUtensorMap* m, const void* ptr, int64_t inner, int
 }
 
 template <int BN, bool A_MN, bool B_MN, int MH, int ACT = 0>
-static int launch_gemm(const CUtensorMap (&tm)[5], const GemmParams& p, cudaStream_t st) {
+static int launch_gemm(const CUtensorMap (&tm)[6], const GemmParams& p, cudaStream_t st) {
     using S = GemmSmem<BN, MH>;
     auto kern = gemm_wgmma_kernel<BN, A_MN, B_MN, MH, ACT>;
     static DeviceOnce once;   // one flag per template instantiation and device
@@ -571,7 +683,7 @@ static int launch_gemm(const CUtensorMap (&tm)[5], const GemmParams& p, cudaStre
         B200_REQUIRE(e == cudaSuccess, "gemm: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
     const int grid = p.num_work < num_sms() ? p.num_work : num_sms();
-    kern<<<grid, kGemmThreads, S::TOTAL, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], p);
+    kern<<<grid, kGemmThreads, S::TOTAL, st>>>(tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
     return check_launch("gemm_wgmma_kernel");
 }
 
@@ -646,8 +758,8 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     if (!a->d_fp32) B200_REQUIRE((a->ldd % 8) == 0, "gemm: bf16 output pitch must be a multiple of 8");
     if (a->resid) B200_REQUIRE((a->ldr % 8) == 0, "gemm: residual pitch must be a multiple of 8");
 
-    CUtensorMap tm[5];
-    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2], &tD = tm[3], &tR = tm[4];
+    CUtensorMap tm[6];
+    CUtensorMap &tA = tm[0], &tA2 = tm[1], &tB = tm[2], &tD = tm[3], &tR = tm[4], &tD2 = tm[5];
     int rc;
     const int64_t KA = a->A2 ? a->K1 : a->K;
     if (!a_mn) rc = make_map(&tA, a->A, KA, a->M, a->lda, BM);
@@ -669,19 +781,26 @@ extern "C" int b200_gemm(const b200_gemm_args* a, b200_stream_t stream) {
     // the tile's columns past N into the output's padding. Other bf16 outputs store from the fragments, and other residuals are read
     // from global memory next to them.
     const auto a16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+    // GLU outputs take the same path when both operands are K-major and h, the pre-activations and glu_mult have 16-byte aligned
+    // bases (the producer bulk-copies the tile's bias and glu_mult into shared memory; the bias is 16-byte aligned already). N % 128 == 0 and the pitches are
+    // multiples of 8 for every GLU problem.
     p.tma_store = !a->d_fp32 && !a->geglu && a16(a->D) && (p.N % 8) == 0;
     p.resid_tma = p.tma_store && a->resid && a16(a->resid);
-    tD = tR = tB;   // unused unless set below
+    p.glu_tma = a->geglu && !a_mn && !b_mn && a->D2 && a16(a->D) && a16(a->D2) && (!a->glu_mult || a16(a->glu_mult));
+    tD = tR = tD2 = tB;   // unused unless set below
     if (p.tma_store && (rc = make_map(&tD, a->D, a->N, a->M, a->ldd, 64))) return rc;
     if (p.resid_tma && (rc = make_map(&tR, a->resid, a->N, a->M, a->ldr, 64))) return rc;
+    if (p.glu_tma && (rc = make_map(&tD, a->D, a->N / 2, a->M, a->ldd, 64))) return rc;
+    if (p.glu_tma && (rc = make_map(&tD2, a->D2, a->N, a->M, a->ldd2, 64))) return rc;
     if (a->geglu && a->D2) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->D2) & 3) == 0, "gemm: GEGLU pre-activation buffer must be 4-byte aligned");
     if (a->resid) B200_REQUIRE((reinterpret_cast<uintptr_t>(a->resid) & 3) == 0, "gemm: residual must be 4-byte aligned");
 
     {
         static const bool trace = getenv("B200_GEMM_TRACE") != nullptr;   // developer aid: log every problem shape
         if (trace)
-            fprintf(stderr, "GEMMTRACE %d %d %d amn=%d bmn=%d split=%d geglu=%d two=%d mh=%d epi=%d%d%d%d\n", p.M, p.N, p.K, (int)a_mn, (int)b_mn, split,
-                    p.geglu, a->A2 != nullptr, wide ? 3 : MH, p.bias != nullptr, p.colscale != nullptr, p.rowmask != nullptr, p.resid != nullptr);
+            fprintf(stderr, "GEMMTRACE %d %d %d amn=%d bmn=%d split=%d geglu=%d two=%d mh=%d epi=%d%d%d%d store=%s\n", p.M, p.N, p.K, (int)a_mn,
+                    (int)b_mn, split, p.geglu, a->A2 != nullptr, wide ? 3 : MH, p.bias != nullptr, p.colscale != nullptr, p.rowmask != nullptr,
+                    p.resid != nullptr, (p.tma_store || p.glu_tma) ? "tma" : "frag");
     }
     if (a->act) {
         if (wide) return launch_gemm<256, false, false, 1, ACT_GELU>(tm, p, st);
