@@ -496,6 +496,7 @@ class Transformer(_PackOwner):
         max_seq_len=8192, kernel_size=31, dropout=0.1, num_registers=32, scale_residual=False, attn_laser=False,
         attn_laser_softclamp_value=15., attn_fourier_embed_input=False, attn_fourier_embed_input_frac=0.25, num_residual_streams=4,
         attn_kwargs: dict = dict(gate_value_heads=True, softclamp_logits=True), ff_kwargs: dict = dict(),
+        checkpoint_activations: bool = False,
     ):
         super().__init__()
         assert depth % 2 == 0, 'depth needs to be even'
@@ -538,6 +539,10 @@ class Transformer(_PackOwner):
         self.has_freq_axis = False
         self.dropout = dropout
         self.num_streams = num_residual_streams
+        # Activation checkpointing (not a reference switch): a training forward under autograd keeps only each layer's boundary tensors
+        # and recomputes the layer's sub-blocks in the backward (_run_layers, ops.Segment) — less memory for about one more forward
+        # of the stack. The right choice depends on batch and clip length, so it is the user's; a plain attribute, read every forward.
+        self.checkpoint_activations = bool(checkpoint_activations)
 
         self.num_registers = num_registers
         self.registers = nn.Parameter(torch.zeros(num_registers, dim))
@@ -721,7 +726,7 @@ class Transformer(_PackOwner):
             y = ops.DwConv.apply(br, conv.dw_conv1d[0].weight, conv.dw_conv1d[0].bias, mask_u8, B, Np, plain)
             return depth(rest, y, beta)
 
-        def sub_attn(res, hcm, gain, mode, attn, pk, vf, colscale, lfe=None):
+        def sub_attn(res, hcm, gain, mode, attn, pk, vf, colscale, seed, lfe=None):
             br, rest, beta = width(res, hcm, gain, mode)
             if lfe is not None:   # attn_input_fourier_embed (:909): between the attention norm (fused into the width kernel) and the attention
                 br = ops.FourierLinear.apply(br, lfe.linear.weight, pk['lfe'], *lfe.split_dims)
@@ -730,23 +735,54 @@ class Transformer(_PackOwner):
             og, v = ops.Attention.apply(br, attn.to_q.weight, attn.to_k.weight, attn.to_v.weight, gate.weight if gate is not None else None,
                                         gate.bias if gate is not None else None, mix[0].weight if mix is not None else None,
                                         mix[0].bias if mix is not None else None, vf if mix is not None else None,
-                                        pk['qkv'], cs, sn, mask_u8, B, Np, attn.heads, p_drop, next_seed(), self.softclamp, self._seed_dev, mbits,
+                                        pk['qkv'], cs, sn, mask_u8, B, Np, attn.heads, p_drop, seed, self.softclamp, self._seed_dev, mbits,
                                         attn.dim_head)
             y = ops.OutProj.apply(og, attn.to_out.weight, pk['out'], colscale, mask_u8, B, Np, rest if plain else None)
             return depth(rest, y, beta), (v if vf is None else vf)
 
-        def sub_ff(res, hcm, gain, mode, ff, pk, colscale):
+        def sub_ff(res, hcm, gain, mode, ff, pk, colscale, seed):
             br, rest, beta = width(res, hcm, gain, mode)
             y = ops.FeedForward.apply(br, ff.ff[0].proj.weight, ff.ff[0].proj.bias, ff.ff[2].weight, ff.ff[2].bias,
-                                      pk['w1'], pk['b1'], pk['w2'], colscale, B, Np, p_drop, next_seed(), self._seed_dev,
+                                      pk['w1'], pk['b1'], pk['w2'], colscale, B, Np, p_drop, seed, self._seed_dev,
                                       rest if plain else None, ff.act, ff.ff[0].mult_bias)
             return close(depth(rest, y, beta))
 
-        def text_block(i, ts, tvf):  # the three text sub-blocks of layer i (:853-882)
-            text, thc, pk = self.layers[i][1], self.hyper_conns[i][1], P[i]['t']
+        def text_subblocks(i, ts, tvf, gains, seeds, pk):  # the three text sub-blocks of layer i (:853-882; no gains: plain RMSNorms)
+            text, thc = self.layers[i][1], self.hyper_conns[i][1]
             ts = sub_conv(ts, thc[0], text[0])
-            ts, tvf = sub_attn(ts, thc[1], text[1].g, 1, text[2], pk, tvf, None)
-            return sub_ff(ts, thc[2], text[3].g, 1, text[4], pk, None), tvf
+            ts, tvf = sub_attn(ts, thc[1], text[1].g, 1, text[2], pk, tvf, None, seeds[0])
+            return sub_ff(ts, thc[2], text[3].g, 1, text[4], pk, None, seeds[1]), tvf
+
+        def audio_subblocks(i, xs, vf, gains4, seeds, pk):  # the three audio sub-blocks of layer i (:900-939)
+            speech, shc = self.layers[i][0], self.hyper_conns[i][0]
+            g_an, g_az, g_fn, g_fz = gains4
+            mode = 2 if self.cond_on_time else 1
+            xs = sub_conv(xs, shc[0], speech[1])  # :900-902
+            xs, vf = sub_attn(xs, shc[1], g_an, mode, speech[3], pk, vf, g_az, seeds[0],
+                              speech[4] if isinstance(speech[4], LinearFourierEmbed) else None)  # :906-916
+            return sub_ff(xs, shc[2], g_fn, mode, speech[7], pk, g_fz, seeds[1]), vf  # :936-939
+
+        # Transformer(checkpoint_activations=True) under autograd: each layer's audio sub-blocks and each text block are one
+        # ops.Segment, which keeps only its inputs and runs the sub-blocks again in the backward. The seeds are drawn here, in the
+        # order of the plain path, and handed in, so the recompute draws the dropout masks of the forward.
+        ckpt = self.checkpoint_activations and self.training and torch.is_grad_enabled()
+
+        def segment(subblocks, i, res, vf, gains, seeds, pk):
+            """subblocks(i, res, vf, gains, seeds, pk) -> (closed stream tensor, values), plain or as one ops.Segment"""
+            if not ckpt:
+                return subblocks(i, res, vf, gains, seeds, pk)
+            keys, first = tuple(pk), vf is None
+
+            def run(res, vf, *rest):
+                gains, w = rest[:len(rest) - len(keys)], rest[len(rest) - len(keys):]
+                out, v = subblocks(i, res, vf, gains, seeds, dict(zip(keys, w)))
+                return (out, v) if first else (out,)
+            outs = ops.Segment.apply(run, res, vf, *gains, *pk.values())
+            return outs[0], (outs[1] if first else vf)
+
+        def text_block(i, ts, tvf):
+            seeds = next_seed(), next_seed()
+            return segment(text_subblocks, i, ts, tvf, (), seeds, P[i]['t'])
 
         # The text sub-blocks of layer i+1 depend on the cross-conditioning of layer i only, not on layer i's audio sub-blocks
         # (:853-939): enqueue them on a second stream so that the half-width text kernels (K = dt GEMMs, D = dt token kernels)
@@ -785,16 +821,9 @@ class Transformer(_PackOwner):
                 skips.append(xs)
             else:
                 xs = ops.SkipProj.apply(xs, skips.pop(), speech[0].weight, pk['skip'])
-            if self.cond_on_time:
-                g_an, g_az, g_fn, g_fz = gains[4 * i:4 * i + 4]
-                mode = 2
-            else:
-                g_an, g_az, g_fn, g_fz = speech[2].g, None, speech[6].g, None
-                mode = 1
-            xs = sub_conv(xs, shc[0], speech[1])  # :900-902
-            xs, v_first = sub_attn(xs, shc[1], g_an, mode, speech[3], pk['a'], v_first, g_az,
-                                   speech[4] if isinstance(speech[4], LinearFourierEmbed) else None)  # :906-916
-            xs = sub_ff(xs, shc[2], g_fn, mode, speech[7], pk['a'], g_fz)  # :936-939
+            gains4 = tuple(gains[4 * i:4 * i + 4]) if self.cond_on_time else (speech[2].g, None, speech[6].g, None)
+            seeds = next_seed(), next_seed()
+            xs, v_first = segment(audio_subblocks, i, xs, v_first, gains4, seeds, pk['a'])
         assert not skips
         return xs
 

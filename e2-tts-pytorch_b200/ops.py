@@ -661,6 +661,41 @@ class SkipProj(Function):
         return dx.view(T, S, D), dskip.view(T, S, D), dW, None
 
 
+# ---------------------------------------------------------------------------------------------------- activation checkpointing
+def _leaves(tensors, needs_grad):
+    return [t.detach().requires_grad_(g) if t is not None else None for t, g in zip(tensors, needs_grad)]
+
+
+class Segment(Function):
+    """One checkpointed segment of Transformer(checkpoint_activations=True): `run(*inputs)` runs one layer's audio sub-blocks, or one
+    text block, through the nodes above and returns the tensors it makes (the closed stream tensor, and the values when it is the
+    first layer). The inputs are the stream tensor, v_first (or None), the gains and the packed weight handles; `run` draws no seed,
+    packs nothing and takes no zero-pool slab, so calling it twice on the same inputs launches the same kernels on the same operands.
+    forward: runs it in grad mode, as the plain path does (the nodes pick the same kernel variants: width statistics, convolution
+    pre-activations), drops that graph and keeps only the inputs. backward: runs it again on the stream the forward ran on (autograd
+    runs this node there) and backpropagates the incoming gradients through the recomputed graph: parameter gradients accumulate into
+    .grad, the inputs' gradients are returned."""
+
+    @staticmethod
+    def forward(ctx, run, *inputs):
+        ctx.set_materialize_grads(False)   # an output nobody reads (the last text block's values) passes no zero-filled gradient
+        ctx.run = run
+        ctx.save_for_backward(*inputs)
+        with torch.enable_grad():
+            outs = run(*_leaves(inputs, ctx.needs_input_grad[1:]))
+        return tuple(o.detach() for o in outs)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        inputs = _leaves(ctx.saved_tensors, ctx.needs_input_grad[1:])
+        with torch.enable_grad():
+            outs = ctx.run(*inputs)
+        pairs = [(o, g) for o, g in zip(outs, grads) if g is not None and o.requires_grad]
+        if pairs:
+            torch.autograd.backward([o for o, _ in pairs], [g for _, g in pairs])
+        return (None, *[x.grad if x is not None and x.requires_grad else None for x in inputs])
+
+
 # ---------------------------------------------------------------------------------------------------- stem / head
 class StemLinear(Function):
     """proj_in(x) + cond_proj_in(cond) as ONE K = 2*Cp GEMM over the packed [w | cond] operand (e2_tts.py:1267-1277);
