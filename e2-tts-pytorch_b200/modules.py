@@ -1058,10 +1058,38 @@ class MelSpec(Module):
 # ----------------------------------------------------------------------------------------------------------------------
 
 
-class _HLGaussRegression(Module):  # A.6, regression mode
-    def __init__(self, dim):
+class _HLGaussHead(Module):
+    """hl-gauss-pytorch HLGaussLayer(dim, hl_gauss_loss, use_regression, regress_activation=Softplus()) (A.6; e2_tts.py:1035-1040):
+    the regression head Linear(dim, 1) -> Softplus with the MSE loss, or with use_regression=False the classification head
+    Linear(dim, num_bins) with the HL-Gauss loss. `hl_gauss_loss` is checked in both modes, as the reference builds its HLGaussLoss
+    either way; the loss holds no parameters or buffers, so the state_dict is `to_pred.0.weight` / `.bias` in both."""
+
+    def __init__(self, dim, hl_gauss_loss=None, use_regression=True):
         super().__init__()
-        self.to_pred = nn.Sequential(nn.Linear(dim, 1), nn.Softplus())
+        if not use_regression and hl_gauss_loss is None:
+            raise ValueError('DurationPredictor: use_regression=False needs `hl_gauss_loss` (hl-gauss-pytorch HLGaussLayer asserts it)')
+        self.spec = ops.HLGaussSpec(**hl_gauss_loss) if hl_gauss_loss is not None else None
+        self.use_regression = bool(use_regression)
+        if self.use_regression:
+            self.to_pred = nn.Sequential(nn.Linear(dim, 1), nn.Softplus())
+        else:
+            if self.spec.num_bins > ops.HL_GAUSS_MAX_BINS:
+                _unsupported('hl_gauss_loss num_bins', self.spec.num_bins,
+                             f'e2_tts.py:966 (the HL-Gauss loss kernel takes at most {ops.HL_GAUSS_MAX_BINS} bins)')
+            self.to_pred = nn.Sequential(nn.Linear(dim, self.spec.num_bins))
+
+    def forward(self, pooled, target=None):
+        """pooled fp32 [B, dim] -> the prediction [B] (target None) or the loss against target [B]"""
+        lin = self.to_pred[0]
+        if self.use_regression:
+            pred = ops.SmallLinear.apply(pooled, lin.weight, lin.bias, 4, 1, False).squeeze(-1)
+            if target is None:
+                return pred
+            return F.mse_loss(pred, target)  # (B,) scalar glue, :1111
+        logits = ops.SmallLinear.apply(pooled, lin.weight, lin.bias, 0, 1, False)
+        if target is None:
+            return ops.hl_gauss_predict(logits, self.spec)
+        return ops.HLGaussLoss.apply(logits, target, self.spec)
 
 
 def _resolve_tokenizer(tokenizer, text_num_embeds):
@@ -1084,8 +1112,6 @@ class DurationPredictor(_PackOwner):
         super().__init__()
         if num_freq_tokens != 1:
             _unsupported('num_freq_tokens', num_freq_tokens, 'e2_tts.py:965')
-        if hl_gauss_loss is not None or not use_regression:
-            _unsupported('hl_gauss_loss', hl_gauss_loss, 'e2_tts.py:966-967 (only the regression head is used by the reference defaults)')
         self.num_freq_tokens, self.has_freq_axis = 1, False
         if isinstance(transformer, dict):
             transformer = dict(transformer)
@@ -1099,7 +1125,7 @@ class DurationPredictor(_PackOwner):
         self.proj_in = nn.Linear(self.num_channels, self.dim)
         self.tokenizer, text_num_embeds = _resolve_tokenizer(tokenizer, text_num_embeds)
         self.embed_text = CharacterEmbed(transformer.dim_text, num_embeds=text_num_embeds, **char_embed_kwargs)
-        self.hl_gauss_layer = _HLGaussRegression(self.dim)
+        self.hl_gauss_layer = _HLGaussHead(self.dim, hl_gauss_loss, use_regression)   # :1035-1040
 
     def _add_weights(self, pack):
         w = dict(tr=self.transformer._add_weights(pack), proj_in=pack.buffer(self.dim, (self.num_channels + 7) // 8 * 8))
@@ -1134,11 +1160,9 @@ class DurationPredictor(_PackOwner):
         tr = self.transformer
         y = tr._forward_from_h(w['tr'], h, B, N, None, mask, text_ids=ids, text_embed_module=self.embed_text)
         pooled = ops.MaskedMean.apply(y, mask.to(torch.uint8).contiguous(), B, N)
-        lin = self.hl_gauss_layer.to_pred[0]
-        pred = ops.SmallLinear.apply(pooled, lin.weight, lin.bias, 4, 1, False).squeeze(-1)
         if not return_loss:
-            return pred
-        return F.mse_loss(pred, lens.float())  # (B,) scalar glue, :1111
+            return self.hl_gauss_layer(pooled)   # :1107
+        return self.hl_gauss_layer(pooled, lens.float())   # :1111
 
 
 class _RngOverride:

@@ -989,6 +989,69 @@ class MaskedMean(Function):
         return dx, None, None, None
 
 
+HL_GAUSS_MAX_BINS = 4096   # b200_hl_gauss_fwd holds one item's bins in a CTA's shared memory
+
+
+class HLGaussSpec:
+    """hl-gauss-pytorch HLGaussLoss(min_value, max_value, num_bins, sigma=None, sigma_to_bin_ratio=2., clamp_to_range=False)
+    (SURVEY A.6): the keywords of DurationPredictor(hl_gauss_loss=dict(...)), checked as the package checks them (num_bins > 1,
+    min_value < max_value); sigma defaults to sigma_to_bin_ratio * bin size. The default ratio is not pinned by a reference test."""
+
+    def __init__(self, min_value, max_value, num_bins, sigma=None, sigma_to_bin_ratio=2., clamp_to_range=False):
+        if isinstance(num_bins, bool) or int(num_bins) != num_bins or num_bins <= 1:
+            raise ValueError(f'hl_gauss_loss: num_bins must be an integer > 1 (got {num_bins!r})')
+        if not float(min_value) < float(max_value):
+            raise ValueError(f'hl_gauss_loss: min_value must be below max_value (got {min_value!r}, {max_value!r})')
+        self.min_value, self.max_value, self.num_bins = float(min_value), float(max_value), int(num_bins)
+        bin_size = (self.max_value - self.min_value) / self.num_bins
+        self.sigma = float(sigma if sigma is not None else bin_size * sigma_to_bin_ratio)
+        if not (math.isfinite(self.sigma) and self.sigma > 0):
+            raise ValueError(f'hl_gauss_loss: sigma must be positive (got {self.sigma!r})')
+        self.clamp_to_range = bool(clamp_to_range)
+
+    def args(self, shape, **kw):
+        B, nb = shape
+        return lib.make_args('b200_hl_gauss_args', B=B, num_bins=nb, min_value=self.min_value, max_value=self.max_value,
+                             sigma=self.sigma, clamp_to_range=int(self.clamp_to_range), **kw)
+
+
+class HLGaussLoss(Function):
+    """hl-gauss-pytorch HLGaussLoss(logits, target) (SURVEY A.6; e2_tts.py:1111): the batch-mean cross-entropy of fp32 logits
+    [B, num_bins] against the Gaussian histograms of `target` [B], one b200_hl_gauss_fwd launch; backward (dloss / B) (softmax - p)."""
+
+    @staticmethod
+    def forward(ctx, logits, target, spec):
+        logits = _c(logits)
+        B = logits.shape[0]
+        dev = logits.device
+        loss = torch.empty((), device=dev, dtype=F32)
+        ce = torch.empty(B, device=dev, dtype=F32)
+        diff = torch.empty_like(logits)
+        count = torch.zeros(1, device=dev, dtype=torch.int32)
+        a = spec.args(logits.shape, logits=logits, target=_c(target.to(F32)), ce=ce, loss=loss, diff=diff, ws_count=count)
+        lib.call('b200_hl_gauss_fwd', a, _stream())
+        ctx.save_for_backward(diff)
+        ctx.spec = spec
+        return loss
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dloss):
+        (diff,) = ctx.saved_tensors
+        dlogits = torch.empty_like(diff)
+        a = ctx.spec.args(diff.shape, diff=diff, dloss=_c(dloss.to(F32)), dlogits=dlogits)
+        lib.call('b200_hl_gauss_bwd', a, _stream())
+        return dlogits, None, None
+
+
+def hl_gauss_predict(logits, spec):
+    """hl-gauss-pytorch HLGaussLoss(logits) (e2_tts.py:1107): sum_i softmax(logits)_i centre_i per item, fp32 [B]; no gradient"""
+    logits = _c(logits.detach())
+    pred = torch.empty(logits.shape[0], device=logits.device, dtype=F32)
+    lib.call('b200_hl_gauss_fwd', spec.args(logits.shape, logits=logits, pred=pred), _stream())
+    return pred
+
+
 def stem_prepare(B, N, C, Cp, *, x1=None, x0=None, times=None, span=None, x_in=None, cond_in=None, want_cond=False, concat=False):
     """Flow-matching input stage (e2_tts.py:1519-1543): builds the bf16 GEMM operand [w | cond] (2*Cp columns); concat=True lays it out
     as cat(cond, w) for the single proj_in of E2TTS(concat_cond=True) (:1263-1265)."""

@@ -371,6 +371,29 @@ typedef struct {
 int b200_dwconv_fwd(const b200_dwconv_args* a, b200_stream_t stream);
 int b200_dwconv_bwd(const b200_dwconv_args* a, b200_stream_t stream);
 
+/* HL-Gauss classification head of DurationPredictor(hl_gauss_loss=..., use_regression=False) (e2_tts.py:966-967 ctor arguments,
+ * :1035-1040 HLGaussLayer, :1107 prediction, :1111 loss against lens.float(); hl-gauss-pytorch HLGaussLoss, SURVEY A.6) on fp32
+ * logits [B, num_bins] (b200_small_linear, identity activation). One CTA per item; 1 <= B <= 64, 2 <= num_bins <= 4096.
+ *   Edges s_j = min + j (max - min) / num_bins (s_N = max), centres (s_i + s_{i+1}) / 2, x_j = (s_j - y) / (sqrt(2) sigma) with
+ *   y = target[b], clamped to [min, max] when clamp_to_range. Masses erf(x_{i+1}) - erf(x_i), taken through erfc where both lie on
+ *   one side of 0; p = mass / (erf(x_N) - erf(x_0)), NaN where that fp32 difference of erf values is 0, as the reference's.
+ * fwd, target != NULL (training): ce[b] = -sum_i p_i log_softmax(l)_i (max-shifted), diff [B, num_bins] = softmax - p (saved for the
+ *   backward), *loss = mean_b ce[b], summed in item order by the last CTA (no float atomics: the same bits on every launch).
+ *   ws_count: one zeroed 32-bit word, left zero again by the call (the last CTA is found by atomicInc wrapping at B - 1).
+ * fwd, target == NULL (prediction): pred[b] = sum_i softmax(l)_i centre_i.
+ * bwd: dlogits = (*dloss / B) * diff; dloss is read on the device (graph-capturable). */
+typedef struct {
+    const float *logits, *target;
+    float *pred, *ce, *loss, *diff;
+    uint32_t* ws_count;
+    const float* dloss; float* dlogits;
+    int32_t B, num_bins;
+    float min_value, max_value, sigma;
+    int32_t clamp_to_range;
+} b200_hl_gauss_args;
+int b200_hl_gauss_fwd(const b200_hl_gauss_args* a, b200_stream_t stream);
+int b200_hl_gauss_bwd(const b200_hl_gauss_args* a, b200_stream_t stream);
+
 /* Masked mean over the sequence (maybe_masked_mean e2_tts.py:212-224): x bf16 [B,N,D] -> out fp32 [B,D]; bwd. */
 int b200_masked_mean_fwd(const void* x, const uint8_t* mask, float* out, int32_t B, int32_t N, int32_t D, b200_stream_t stream);
 int b200_masked_mean_bwd(const float* dout, const uint8_t* mask, void* dx, int32_t B, int32_t N, int32_t D, b200_stream_t stream);
