@@ -143,7 +143,7 @@ attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
     // fragment rows of this thread: r0 and r0 + 8 of the warpgroup's 64; columns 8 j + cq + {0, 1}
     const int r0 = cw * 64 + wq * 16 + (lane >> 2);
     const unsigned int* mb = p.maskbits + (size_t)b * p.mask_words;
-    const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
+    const uint32_t seedmix = drop_seed_word(p.seed, p.seed_dev);
     unsigned long long drop_row[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) drop_row[i] = ((unsigned long long)bh * p.Np + (unsigned long long)(q0 + r0 + 8 * i)) * (unsigned long long)p.drop_stride;
@@ -546,7 +546,7 @@ attn_bwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
         key[i] = k0 + kr0 + 8 * i;
         kok[i] = key[i] < p.Np && ((p.maskbits[(size_t)b * p.mask_words + (key[i] >> 5)] >> (key[i] & 31)) & 1u);
     }
-    const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
+    const uint32_t seedmix = drop_seed_word(p.seed, p.seed_dev);
     const bool kodd = (lane >> 2) & 1;
     const bool active = k0 + cw * 64 < p.Np;   // a warpgroup whose 64 keys all lie at or past Np keeps only the barrier protocol
     const uint64_t kdesc = make_smem_desc_sw128(smem_u32(sK + cw * TILE8), 16, 1024);        // K-major A of S^T
@@ -842,7 +842,7 @@ attn_bwd_d128_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid
         key[i] = k0 + kr0 + 8 * i;
         kok[i] = key[i] < p.Np && ((p.maskbits[(size_t)b * p.mask_words + (key[i] >> 5)] >> (key[i] & 31)) & 1u);
     }
-    const uint32_t seedmix = seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull));
+    const uint32_t seedmix = drop_seed_word(p.seed, p.seed_dev);
     const bool kodd = (lane >> 2) & 1;
     // S^T (warpgroup 0): A = K, B = Q_i; dP^T (warpgroup 1): A = V, B = dO_i — both K-major over the 128 head dims
     const uint64_t adesc = make_smem_desc_sw128(smem_u32(cw == 0 ? sK : sV), 16, 1024);
@@ -999,6 +999,43 @@ static int make_dq_map(CUtensorMap* m, float* dq, int BH, int Np, int dh) {
     return 0;
 }
 
+// The argument rules and parameter fields b200_attn_fwd and b200_attn_bwd share (their argument and parameter structs name them
+// alike): dim_head, shape, logit clamp, dropout; then the key-validity bitmask, unless the caller has built it. `who` prefixes
+// every refusal.
+template <class Args, class P>
+static int attn_setup(const Args* a, P& p, const char* who, cudaStream_t st) {
+    B200_REQUIRE(a->dim_head == 64 || a->dim_head == 128, "%s: dim_head must be 64 or 128 (got %d)", who, a->dim_head);
+    B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "%s: bad shape", who);
+    if (a->unclamped) {
+        B200_REQUIRE(a->softclamp == 0.f, "%s: unclamped attention needs softclamp == 0 (got %g)", who, a->softclamp);
+    } else {
+        B200_REQUIRE(a->softclamp > 0.f, "%s: softclamp value must be > 0, or set unclamped for attention without the logit soft-clamp", who);
+    }
+    B200_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, "%s: dropout must be in [0,1)", who);
+    B200_REQUIRE(a->softclamp <= 64.f, "%s: softclamp %g > 64: the clamped wgmma kernel exponentiates the clamped logits without a "
+                 "running maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", who, a->softclamp);
+    p.B = a->B; p.H = a->H; p.Np = a->Np;
+    if (a->unclamped) {
+        p.clamp = 0.f; p.scale_over_clamp = 0.f;
+    } else {
+        p.clamp = a->softclamp; p.scale_over_clamp = a->scale / a->softclamp;
+    }
+    p.scale = a->scale; p.scale_log2e = a->scale * LOG2E_F;
+    p.dropout_p = a->dropout_p;
+    p.drop_thresh = drop_thresh16(a->dropout_p);
+    p.keep_scale = drop_keep_scale(p.drop_thresh);
+    p.seed = a->seed; p.seed_dev = reinterpret_cast<const unsigned long long*>(a->seed_dev);
+    p.drop_stride = (a->Np + 1) & ~1;
+    p.mask_words = ((a->Np + TKV - 1) / TKV) * 4;
+    p.maskbits = reinterpret_cast<const unsigned int*>(a->ws_maskbits);
+    if (!a->maskbits_ready) {
+        attn_maskbits_kernel<<<(a->B * p.mask_words + 127) / 128, 128, 0, st>>>(a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits),
+                                                                             a->B, a->Np, p.mask_words);
+        return check_launch("attn_maskbits_kernel");
+    }
+    return 0;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -1019,38 +1056,10 @@ extern "C" int b200_attn_maskbits(const uint8_t* keymask, void* ws_maskbits, int
 extern "C" int b200_attn_fwd(const b200_attn_fwd_args* a, b200_stream_t stream) {
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B200_REQUIRE(a && a->q && a->k && a->v && a->o && a->og && a->lse && a->ws_maskbits, "attn_fwd: null pointer");
-    B200_REQUIRE(a->dim_head == 64 || a->dim_head == 128, "attn_fwd: dim_head must be 64 or 128 (got %d)", a->dim_head);
-    B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_fwd: bad shape");
-    if (a->unclamped) {
-        B200_REQUIRE(a->softclamp == 0.f, "attn_fwd: unclamped attention needs softclamp == 0 (got %g)", a->softclamp);
-    } else {
-        B200_REQUIRE(a->softclamp > 0.f, "attn_fwd: softclamp value must be > 0, or set unclamped for attention without the logit soft-clamp");
-    }
-    B200_REQUIRE(a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_fwd: dropout must be in [0,1)");
-    B200_REQUIRE(a->softclamp <= 64.f, "attn_fwd: softclamp %g > 64: the clamped wgmma kernel exponentiates the clamped logits without a "
-                 "running maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
     AttnTcP p{};
+    if (int rc = attn_setup(a, p, "attn_fwd", st)) return rc;
     p.nkv = (a->Np + TKV - 1) / TKV;
-    p.mask_words = p.nkv * 4;
-    p.maskbits = reinterpret_cast<const unsigned int*>(a->ws_maskbits);
-    if (!a->maskbits_ready) {
-        const int total = a->B * p.mask_words;
-        attn_maskbits_kernel<<<(total + 127) / 128, 128, 0, st>>>(a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits), a->B, a->Np, p.mask_words);
-        if (int rc = check_launch("attn_maskbits_kernel")) return rc;
-    }
     p.gate = a->gate; p.o = (__nv_bfloat16*)a->o; p.og = (__nv_bfloat16*)a->og; p.lse = a->lse;
-    p.B = a->B; p.H = a->H; p.Np = a->Np;
-    if (a->unclamped) {
-        p.clamp = 0.f; p.scale_over_clamp = 0.f;
-    } else {
-        p.clamp = a->softclamp; p.scale_over_clamp = a->scale / a->softclamp;
-    }
-    p.scale = a->scale; p.scale_log2e = a->scale * LOG2E_F;
-    p.dropout_p = a->dropout_p;
-    p.drop_thresh = (unsigned int)(a->dropout_p * 65536.f);
-    p.keep_scale = 65536.f / (65536.f - (float)p.drop_thresh);
-    p.seed = a->seed; p.seed_dev = reinterpret_cast<const unsigned long long*>(a->seed_dev);
-    p.drop_stride = (a->Np + 1) & ~1;
     CUtensorMap tq, tk, tv;
     const long long rows = (long long)a->B * a->H * a->Np;
     const int dh = a->dim_head, na = dh / 64;
@@ -1070,14 +1079,8 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     B200_REQUIRE(a && a->q && a->k && a->v && a->o && a->d_og && a->lse && a->ws_dO && a->ws_delta && a->dq && a->dk && a->dv && a->ws_maskbits,
                  "attn_bwd: null pointer");
-    B200_REQUIRE(a->dim_head == 64 || a->dim_head == 128, "attn_bwd: dim_head must be 64 or 128 (got %d)", a->dim_head);
-    B200_REQUIRE(a->B > 0 && a->H > 0 && a->Np > 0 && a->B <= 65535 && a->H <= 65535, "attn_bwd: bad shape");
-    if (a->unclamped) {
-        B200_REQUIRE(a->softclamp == 0.f, "attn_bwd: unclamped attention needs softclamp == 0 (got %g)", a->softclamp);
-    }
-    B200_REQUIRE((a->unclamped || a->softclamp > 0.f) && a->dropout_p >= 0.f && a->dropout_p < 1.f, "attn_bwd: bad softclamp / dropout");
-    B200_REQUIRE(a->softclamp <= 64.f, "attn_bwd: softclamp %g > 64: the clamped wgmma kernel exponentiates the clamped logits without a "
-                 "running maximum, which needs exp(+-softclamp) well inside fp32 / bf16 range (the reference uses 50)", a->softclamp);
+    AttnBwdTcP p{};
+    if (int rc = attn_setup(a, p, "attn_bwd", st)) return rc;
     const AttnPrepP pp{a->gate, (const __nv_bfloat16*)a->o, a->B, a->H, a->Np, (const __nv_bfloat16*)a->d_og, a->d_gate,
                        (__nv_bfloat16*)a->ws_dO, a->ws_delta};
     const int dh = a->dim_head;
@@ -1085,32 +1088,12 @@ extern "C" int b200_attn_bwd(const b200_attn_bwd_args* a, b200_stream_t stream) 
     if (dh == 64) attn_bwd_prep_kernel<64><<<(unsigned)((prep_threads + 255) / 256), 256, 0, st>>>(pp);
     else attn_bwd_prep_kernel<128><<<(unsigned)((prep_threads + 255) / 256), 256, 0, st>>>(pp);
     if (int rc = check_launch("attn_bwd_prep_kernel")) return rc;
-    AttnBwdTcP p{};
     p.nq = (a->Np + TQB - 1) / TQB;
-    p.mask_words = ((a->Np + TKV - 1) / TKV) * 4;
-    p.maskbits = reinterpret_cast<const unsigned int*>(a->ws_maskbits);
-    if (!a->maskbits_ready) {
-        const int total = a->B * p.mask_words;
-        attn_maskbits_kernel<<<(total + 127) / 128, 128, 0, st>>>(a->keymask, reinterpret_cast<unsigned int*>(a->ws_maskbits), a->B, a->Np, p.mask_words);
-        if (int rc = check_launch("attn_maskbits_kernel")) return rc;
-    }
     const size_t nelem = (size_t)a->B * a->H * a->Np * dh;
     cudaError_t e = cudaMemsetAsync(a->dq, 0, nelem * sizeof(float), st);
     B200_REQUIRE(e == cudaSuccess, "attn_bwd: memset: %s", cudaGetErrorString(e));
     p.lse = a->lse; p.delta = a->ws_delta;
     p.dk = (__nv_bfloat16*)a->dk; p.dv = (__nv_bfloat16*)a->dv;
-    p.B = a->B; p.H = a->H; p.Np = a->Np;
-    p.scale = a->scale; p.scale_log2e = a->scale * LOG2E_F;
-    if (a->unclamped) {
-        p.clamp = 0.f; p.scale_over_clamp = 0.f;
-    } else {
-        p.clamp = a->softclamp; p.scale_over_clamp = a->scale / a->softclamp;
-    }
-    p.dropout_p = a->dropout_p;
-    p.drop_thresh = (unsigned int)(a->dropout_p * 65536.f);
-    p.keep_scale = 65536.f / (65536.f - (float)p.drop_thresh);
-    p.drop_stride = (a->Np + 1) & ~1;
-    p.seed = a->seed; p.seed_dev = reinterpret_cast<const unsigned long long*>(a->seed_dev);
     CUtensorMap tq, tk, tv, tdo, tdq;
     const long long rows = (long long)a->B * a->H * a->Np;
     const int kv_rows = dh == 64 ? TKV : 64;   // keys per CTA

@@ -350,9 +350,9 @@ __global__ void __launch_bounds__(256) glu_bwd_kernel(const __nv_bfloat16* dh, c
     const int nchunk = inner >> 3;
     const int cl = threadIdx.x & 31, rl = threadIdx.x >> 5;
     const int c = blockIdx.x * 32 + cl;
-    const uint32_t thr = (uint32_t)(dropout_p * 65536.f);
-    const float ks = dropout_p > 0.f ? 65536.f / (65536.f - (float)thr) : 1.f;
-    const uint32_t seedmix = seed_mix32(seed + (seed_dev ? __ldg(seed_dev) : 0ull));
+    const uint32_t thr = drop_thresh16(dropout_p);
+    const float ks = dropout_p > 0.f ? drop_keep_scale(thr) : 1.f;
+    const uint32_t seedmix = drop_seed_word(seed, seed_dev);
     float su[8] = {0, 0, 0, 0, 0, 0, 0, 0}, sg[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     float sm[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // MULT only
     if (c < nchunk) {
@@ -370,7 +370,7 @@ __global__ void __launch_bounds__(256) glu_bwd_kernel(const __nv_bfloat16* dh, c
             unpack8(*reinterpret_cast<const uint4*>(ug + pu), u);
             unpack8(*reinterpret_cast<const uint4*>(ug + pu + 64), g);
             if (dropout_p > 0.f) {   // same pair hash as the GLU epilogue of the forward GEMM
-                const uint32_t pbase = (uint32_t)(((unsigned long long)row * (unsigned long long)inner + hcol) >> 1);
+                const uint32_t pbase = glu_drop_pair(row, inner, hcol);
 #pragma unroll
                 for (int j = 0; j < 8; j += 2) {
                     const DropWords hsh = drop_words(seedmix, pbase + (j >> 1));

@@ -5,16 +5,19 @@
 // Structure (one persistent CTA per SM, 384 threads, warp-specialised):
 //   warpgroup 0, one thread : TMA producer — cp.async.bulk.tensor 2-D tiles (128B swizzle) into a kStages smem ring
 //   warpgroups 1, 2         : MMA + epilogue — each owns 64 * MH rows of the CTA tile: wgmma.m64nBNk16 from the smem ring into
-//                             register accumulators, then the fused epilogue (bias / AdaLN gate / row mask / residual / GEGLU(+dropout))
-//                             on the accumulator fragments. Plain bf16 outputs are written 64 x 64 at a time into a 128B-swizzled smem
-//                             staging slice (two per warpgroup, alternating) and leave as TMA tile stores (bulk async groups), so the
-//                             warpgroup moves on to the next slice while the previous one drains. A residual slice is TMA-loaded into
-//                             the staging buffer its output slice will occupy (the tile's first two while its last k-blocks still run),
-//                             and the epilogue adds it from shared memory in place. GLU outputs of K-major operands take the same
-//                             slices: per 64 rows and 128 packed columns, u + bias and gate + bias leave as two pre-activation
-//                             slices and h, computed from the bf16 values just staged, as a third; the producer stages the tile's
-//                             bias and glu_mult in shared memory. Outputs without 16-byte aligned bases store bf16x2 pairs from the fragments, fp32 split-K
-//                             partials go through vector atomics.
+//                             register accumulators, then the fused epilogue on the accumulator fragments. It decides twice: GLU or
+//                             not, then TMA slices or fragment stores. A non-GLU output gets one element-wise pass in place
+//                             (epilogue_pass: bias / act / AdaLN gate / row mask / residual from global memory), a GLU output takes
+//                             h from one routine (glu_h_pair: activation, glu_mult, dropout), and either leaves by the same two paths:
+//                             - TMA: 64 x 64 at a time through a 128B-swizzled smem staging slice (two per warpgroup, alternating) and
+//                               a TMA tile store (bulk async groups), so the warpgroup moves on while the previous slice drains. A
+//                               residual slice is TMA-loaded into the staging buffer its output slice will occupy (the tile's first
+//                               two while its last k-blocks still run) and added there. GLU (K-major operands only): per 64 rows and
+//                               128 packed columns, u + bias and gate + bias leave as two pre-activation slices and h, computed from
+//                               the bf16 values just staged, as a third; the producer stages the tile's bias and glu_mult in smem.
+//                             - fragments: bf16x2 / fp32 pairs stored from registers, fp32 split-K partials through vector atomics —
+//                               for outputs without 16-byte aligned bases, N % 8 != 0, fp32, MN-major GLU and GLU without D2. The
+//                               fragment GLU path is also the reference the TMA one is tested against, bit for bit.
 // While a consumer warpgroup runs its epilogue the producer is already filling the ring with the next tile's operands.
 // Operands may be K-major or MN-major (transposed storage) so that the backward contractions
 // dX = dY*W and dW = dY^T*X read activations exactly as they lie in HBM — no transposes are materialised.
@@ -155,22 +158,50 @@ __device__ __forceinline__ void slice_store(const CUtensorMap* m, uint8_t* my_st
     }
 }
 
+// Fragment of an m64nBN accumulator: thread (wq, lane) holds rows 16 wq + lane / 4 (+ 8) and, for every 8-column group j,
+// columns 8 j + 2 (lane % 4) + {0, 1}: acc[h][4 j + 2 i + c] = (row + 8 i, column + c) of the warpgroup's m64 block h.
+__device__ __forceinline__ int frag_row(int tm, int cw, int wq, int lane, int MH, int h, int i) {
+    return tm * BM * MH + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
+}
+
+// GLU dropout state, built once per epilogue: P(drop) = thr32 / 2^32 on the hash words of the hidden-unit pairs of an [M, N / 2]
+// hidden tensor; kept units are scaled by keep_scale. (The threshold is converted once per use: one shared conversion makes the
+// 128 x 256 MN-major kernels spill.)
+struct GluDrop { bool on; float keep_scale; uint32_t seed, thr32; };
+__device__ __forceinline__ GluDrop glu_drop(const GemmParams& p) {
+    const bool on = p.dropout_p > 0.f;
+    return GluDrop{on, on ? drop_keep_scale(drop_thresh16(p.dropout_p)) : 1.f, on ? drop_seed_word(p.seed, p.seed_dev) : 0u,
+                   drop_thresh32(drop_thresh16(p.dropout_p))};
+}
+
+// One packed pair of hidden units (hcol, hcol + 1) of `row`: h = u * act(gate) (* glu_mult) (* dropout keep / (1 - p)), bf16, from the
+// bf16 pre-activation words (the rounded values the backward pass recomputes from). mult_pair() loads the glu_mult pair, when `mult`;
+// pair() gives the dropout pair index (glu_drop_pair). Both are evaluated only inside their branches: loaded or computed ahead of
+// them, they hold registers that make the GEMM kernels spill.
+template <int ACT, class MultPair, class PairIdx>
+__device__ __forceinline__ uint32_t glu_h_pair(uint32_t wu, uint32_t wgt, bool mult, MultPair mult_pair, const GluDrop& dr, PairIdx pair) {
+    float2 h2 = fmul2(make_float2(bf16_lo(wu), bf16_hi(wu)), glu_act2<ACT>(make_float2(bf16_lo(wgt), bf16_hi(wgt))));
+    if (mult) h2 = fmul2(h2, mult_pair());
+    if (dr.on) {
+        const DropWords hsh = drop_words(dr.seed, pair());
+        h2 = fmul2(h2, make_float2(hsh.a >= dr.thr32 ? dr.keep_scale : 0.f, hsh.b >= dr.thr32 ? dr.keep_scale : 0.f));
+    }
+    return pack_bf16(h2.x, h2.y);
+}
+
 // GLU epilogue on the accumulator fragments: every 128 packed columns hold [0,64) = u, [64,128) = gate of the same 64 hidden units, so a
-// thread holds both halves of each of its hidden units (fragment groups j and j + 8 of the 128-column group).
-// h = u * act(gate) (* glu_mult) (* dropout keep / (1 - p)), bf16; D2 <- the bf16 pre-activations.
+// thread holds both halves of each of its hidden units (fragment groups j and j + 8 of the 128-column group). D2 <- the bf16
+// pre-activations, D <- h. The reference the TMA path (glu_store_slices) is tested against, and the path of MN-major operands and of
+// calls whose h, pre-activation or glu_mult base is not 16-byte aligned or that give no D2.
 template <int ACT, int BN, int MH>
 __device__ __forceinline__ void glu_epilogue(const GemmParams& p, float (&acc)[MH][BN / 2], int tm, int tn, int cw, int wq, int lane) {
-    constexpr int BMT = BM * MH;
     const int cq = 2 * (lane & 3);
-    const bool do_drop = p.dropout_p > 0.f;
-    const float keep_scale = do_drop ? 65536.f / (65536.f - (float)(uint32_t)(p.dropout_p * 65536.f)) : 1.f;
-    const uint32_t seedmix = do_drop ? seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull)) : 0u;
-    const uint32_t thr32 = drop_thresh32((uint32_t)(p.dropout_p * 65536.f));
+    const GluDrop dr = glu_drop(p);
 #pragma unroll
     for (int h = 0; h < MH; ++h) {
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
+            const int row = frag_row(tm, cw, wq, lane, MH, h, i);
             if (row >= p.M) continue;
 #pragma unroll
             for (int sub = 0; sub < BN / 128; ++sub) {
@@ -192,15 +223,9 @@ __device__ __forceinline__ void glu_epilogue(const GemmParams& p, float (&acc)[M
                         *reinterpret_cast<uint32_t*>(d2) = wu;
                         *reinterpret_cast<uint32_t*>(d2 + 64) = wgt;
                     }
-                    // the backward pass recomputes from the bf16-rounded pre-activations: use them here too
-                    float2 h2 = fmul2(make_float2(bf16_lo(wu), bf16_hi(wu)), glu_act2<ACT>(make_float2(bf16_lo(wgt), bf16_hi(wgt))));
-                    if (p.glu_mult) h2 = fmul2(h2, make_float2(__ldg(p.glu_mult + hcol), __ldg(p.glu_mult + hcol + 1)));
-                    if (do_drop) {
-                        // hidden-unit pairs (2k, 2k+1) of one row share a 32-bit hash; N/2 is even, so (row * N/2 + hcol) >> 1 pairs them
-                        const DropWords hsh = drop_words(seedmix, (uint32_t)(((unsigned long long)row * (unsigned long long)(p.N / 2) + hcol) >> 1));
-                        h2 = fmul2(h2, make_float2(hsh.a >= thr32 ? keep_scale : 0.f, hsh.b >= thr32 ? keep_scale : 0.f));
-                    }
-                    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + hcol) = pack_bf16(h2.x, h2.y);
+                    const auto m = [&] { return make_float2(__ldg(p.glu_mult + hcol), __ldg(p.glu_mult + hcol + 1)); };
+                    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + hcol) =
+                        glu_h_pair<ACT>(wu, wgt, p.glu_mult, m, dr, [&] { return glu_drop_pair(row, p.N / 2, hcol); });
                 }
             }
         }
@@ -266,7 +291,7 @@ __device__ __forceinline__ void store_slices(const GemmParams& p, float (&acc)[M
 // group sits at the same slice position as its u and gate, so h is computed pair by pair from the bf16 u and gate the thread itself
 // wrote to the two buffers (the rounded values the backward pass recomputes from) and written over u once u's store has read it.
 // sbias / smult: the tile's packed bias and glu_mult slice, staged in shared memory by the producer; the dropout hashes are made in
-// the h loop, one pair at a time. Bit-identical to glu_epilogue.
+// the h loop, one pair at a time. Bit-identical to glu_epilogue: both take h from glu_h_pair.
 template <int ACT, int BN, int MH>
 __device__ __forceinline__ void glu_store_slices(const GemmParams& p, float (&acc)[MH][BN / 2], const CUtensorMap* tmD, const CUtensorMap* tmD2,
                                                  uint8_t* my_stg, const float* sbias, const float* smult, uint32_t& nslice, int tm, int tn,
@@ -274,10 +299,7 @@ __device__ __forceinline__ void glu_store_slices(const GemmParams& p, float (&ac
     const uint32_t swz = (uint32_t)(lane >> 2) << 4;
     const uint32_t toff = slice_toff(wq);
     const int cq = 2 * (lane & 3);
-    const bool do_drop = p.dropout_p > 0.f;
-    const float keep_scale = do_drop ? 65536.f / (65536.f - (float)(uint32_t)(p.dropout_p * 65536.f)) : 1.f;
-    const uint32_t seedmix = do_drop ? seed_mix32(p.seed + (p.seed_dev ? __ldg(p.seed_dev) : 0ull)) : 0u;
-    const uint32_t thr32 = drop_thresh32((uint32_t)(p.dropout_p * 65536.f));
+    const GluDrop dr = glu_drop(p);
 #pragma unroll
     for (int h = 0; h < MH; ++h) {
         const int rowb = tm * BM * MH + (cw * MH + h) * 64;
@@ -313,14 +335,8 @@ __device__ __forceinline__ void glu_store_slices(const GemmParams& p, float (&ac
                     const int hl = sub * 64 + 8 * jj + cq;   // hidden-unit column within the tile
                     const uint32_t a = slice_addr(bu, toff, swz, i, jj);
                     const uint32_t wu = ld_shared_u32(a), wgt = ld_shared_u32(slice_addr(bg, toff, swz, i, jj));
-                    float2 h2 = fmul2(make_float2(bf16_lo(wu), bf16_hi(wu)), glu_act2<ACT>(make_float2(bf16_lo(wgt), bf16_hi(wgt))));
-                    if (p.glu_mult) h2 = fmul2(h2, *reinterpret_cast<const float2*>(smult + hl));
-                    if (do_drop) {
-                        const int hcol = tn * (BN / 2) + hl;
-                        const DropWords hsh = drop_words(seedmix, (uint32_t)(((unsigned long long)row * (unsigned long long)(p.N / 2) + hcol) >> 1));
-                        h2 = fmul2(h2, make_float2(hsh.a >= thr32 ? keep_scale : 0.f, hsh.b >= thr32 ? keep_scale : 0.f));
-                    }
-                    st_shared_u32(a, pack_bf16(h2.x, h2.y));
+                    const auto m = [&] { return *reinterpret_cast<const float2*>(smult + hl); };
+                    st_shared_u32(a, glu_h_pair<ACT>(wu, wgt, p.glu_mult, m, dr, [&] { return glu_drop_pair(row, p.N / 2, tn * (BN / 2) + hl); }));
                 }
             }
             slice_store(tmD, my_stg, nslice, cw, t, colg / 2, rowb);
@@ -347,6 +363,77 @@ __device__ __forceinline__ void store_pair(const GemmParams& p, int row, int col
         if (two) *reinterpret_cast<uint32_t*>(dp) = pack_bf16(v0, v1);   // ldd % 8 == 0 and col even: 4-byte aligned
         else dp[0] = __float2bfloat16_rn(v0);
     }
+}
+
+// The element-wise epilogue of non-GLU outputs, in place on the fragments: bias -> act -> AdaLN gate (colscale) -> row mask -> +
+// residual read from global memory (a residual TMA-loaded into the staging slices is added by store_slices instead). Rows >= M and
+// columns >= N are left as they are: the stores skip or clip them.
+template <int ACT, int BN, int MH>
+__device__ __forceinline__ void epilogue_pass(const GemmParams& p, float (&acc)[MH][BN / 2], int tm, int tn, int cw, int wq, int lane) {
+    const bool resid_ldg = p.resid && !p.resid_tma;
+    if (!(ACT || p.bias || p.colscale || p.rowmask || resid_ldg)) return;   // plain outputs and split-K partials
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < MH; ++h) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int row = frag_row(tm, cw, wq, lane, MH, h, i);
+            if (row >= p.M) continue;
+            const bool masked = p.rowmask && p.rowmask[row] == 0;
+            const float* cs = p.colscale ? p.colscale + (long long)(row / p.rows_per_batch) * p.N : nullptr;
+            const __nv_bfloat16* rp = resid_ldg ? reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr : nullptr;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = tn * BN + 8 * j + cq;
+                if (col >= p.N) continue;
+                const bool two = col + 1 < p.N;
+                float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
+                if (p.bias) { v0 += __ldg(p.bias + col); if (two) v1 += __ldg(p.bias + col + 1); }
+                if constexpr (ACT == ACT_GELU) { const float2 g = gelu_erf2(make_float2(v0, v1)); v0 = g.x; v1 = g.y; }
+                if (cs) { v0 *= __ldg(cs + col); if (two) v1 *= __ldg(cs + col + 1); }
+                if (masked) { v0 = 0.f; v1 = 0.f; }
+                if (rp) {
+                    if (two) {
+                        const uint32_t u = *reinterpret_cast<const uint32_t*>(rp + col);
+                        v0 += bf16_lo(u); v1 += bf16_hi(u);
+                    } else {
+                        v0 += __bfloat162float(rp[col]);
+                    }
+                }
+                acc[h][4 * j + 2 * i] = v0;
+                acc[h][4 * j + 2 * i + 1] = v1;
+            }
+        }
+    }
+}
+
+// The finished fragments of a non-GLU output, pair by pair from registers: fp32 outputs, split-K partials, and bf16 outputs the TMA
+// cannot store (unaligned base or N % 8 != 0).
+template <int BN, int MH>
+__device__ __forceinline__ void store_frags(const GemmParams& p, float (&acc)[MH][BN / 2], int tm, int tn, int cw, int wq, int lane) {
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < MH; ++h) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int row = frag_row(tm, cw, wq, lane, MH, h, i);
+            if (row >= p.M) continue;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int col = tn * BN + 8 * j + cq;
+                if (col < p.N) store_pair(p, row, col, acc[h][4 * j + 2 * i], acc[h][4 * j + 2 * i + 1]);
+            }
+        }
+    }
+}
+
+// Work item w -> output tile (tm, tn) and its k-blocks [kb0, kb1) (split-K: the split's share of them); the producer thread and the
+// consumer warpgroups walk the same items.
+struct WorkItem { int tm, tn, kb0, kb1; };
+__device__ __forceinline__ WorkItem work_item(const GemmParams& p, int w) {
+    const int rest = w / p.tiles_m;
+    const int kb0 = rest / p.tiles_n * p.kb_per_split;
+    return WorkItem{w % p.tiles_m, rest % p.tiles_n, kb0, min(p.kb_total, kb0 + p.kb_per_split)};
 }
 
 // ACT = ACT_GELU: GELU(z + bias) ahead of the rest of the epilogue (b200_gemm_args.act; instantiated for K-major A and B only).
@@ -407,15 +494,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             uint32_t phase = 0;
             uint32_t ntile = 0;
             for (int w = blockIdx.x; w < p.num_work; w += gridDim.x, ++ntile) {
-                const int tm = w % p.tiles_m;
-                const int rest = w / p.tiles_m;
-                const int tn = rest % p.tiles_n;
-                const int sp = rest / p.tiles_n;
-                const int kb0 = sp * p.kb_per_split;
-                const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
-                const int arow = tm * BMT;
-                const int brow = tn * BN;
-                for (int kb = kb0; kb < kb1; ++kb) {
+                const WorkItem wi = work_item(p, w);
+                const int arow = wi.tm * BMT;
+                const int brow = wi.tn * BN;
+                for (int kb = wi.kb0; kb < wi.kb1; ++kb) {
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     mbar_arrive_expect_tx(&full_bar[stage], S::STAGE_BYTES);
                     uint8_t* a_dst = smA + stage * S::A_BYTES;
@@ -469,12 +551,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     uint32_t phase = 0;
     uint32_t ntile = 0;
     for (int w = blockIdx.x; w < p.num_work; w += gridDim.x, ++ntile) {
-        const int tm = w % p.tiles_m;
-        const int rest = w / p.tiles_m;
-        const int tn = rest % p.tiles_n;
-        const int sp = rest / p.tiles_n;
-        const int kb0 = sp * p.kb_per_split;
-        const int kb1 = min(p.kb_total, kb0 + p.kb_per_split);
+        const auto [tm, tn, kb0, kb1] = work_item(p, w);
         // resid_tma: each residual slice is TMA-loaded into the staging buffer its output slice will use and completes on that buffer's
         // barrier. The tile's first two go out two k-blocks before its mainloop ends, once the previous tile's stores have left both
         // buffers; the third and fourth as soon as the store of the first and second has left its buffer.
@@ -518,51 +595,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (prev >= 0 && t == 0) mbar_arrive(&empty_bar[prev]);
 
         // ---------------------------------------------------------------- epilogue from the accumulator fragments
-        // Fragment of an m64nBN accumulator: thread (wq, lane) holds rows 16 wq + lane / 4 (+ 8) and, for every 8-column group j,
-        // columns 8 j + 2 (lane % 4) + {0, 1}: acc[4 j + 2 i + c] = (row + 8 i, column + c).
-        const int cq = 2 * (lane & 3);
-        if (p.tma_store) {
-            // first the element-wise epilogue in place on the fragments (rows >= M and columns >= N are left as they are: the TMA
-            // store clips them), then the 64 x 64 slices; a TMA-loaded residual is added there, read from the address the output
-            // pair is written back to. The order stays bias -> AdaLN gate -> row mask -> + residual.
-            const bool resid_ldg = p.resid && !p.resid_tma;
-            if (ACT || p.bias || p.colscale || p.rowmask || resid_ldg) {
-#pragma unroll
-                for (int h = 0; h < MH; ++h) {
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
-                        if (row >= p.M) continue;
-                        const bool masked = p.rowmask && p.rowmask[row] == 0;
-                        const float* cs = p.colscale ? p.colscale + (long long)(row / p.rows_per_batch) * p.N : nullptr;
-                        const __nv_bfloat16* rp = resid_ldg ? reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr : nullptr;
-#pragma unroll
-                        for (int j = 0; j < BN / 8; ++j) {
-                            const int col = tn * BN + 8 * j + cq;
-                            if (col >= p.N) continue;
-                            const bool two = col + 1 < p.N;
-                            float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
-                            if (p.bias) { v0 += __ldg(p.bias + col); if (two) v1 += __ldg(p.bias + col + 1); }
-                            if constexpr (ACT == ACT_GELU) { const float2 g = gelu_erf2(make_float2(v0, v1)); v0 = g.x; v1 = g.y; }
-                            if (cs) { v0 *= __ldg(cs + col); if (two) v1 *= __ldg(cs + col + 1); }
-                            if (masked) { v0 = 0.f; v1 = 0.f; }
-                            if (rp) {
-                                if (two) {
-                                    const uint32_t u = *reinterpret_cast<const uint32_t*>(rp + col);
-                                    v0 += bf16_lo(u); v1 += bf16_hi(u);
-                                } else {
-                                    v0 += __bfloat162float(rp[col]);
-                                }
-                            }
-                            acc[h][4 * j + 2 * i] = v0;
-                            acc[h][4 * j + 2 * i + 1] = v1;
-                        }
-                    }
-                }
-            }
+        if (!p.geglu) {
+            epilogue_pass<ACT, BN, MH>(p, acc, tm, tn, cw, wq, lane);
             // a copy of the slice loop per case keeps the plain path free of per-element residual branches
             if (p.resid_tma) store_slices<true, BN, MH>(p, acc, &tmD, &tmR, my_stg, my_rbar, nslice, tm, tn, cw, wq, lane, t);
-            else store_slices<false, BN, MH>(p, acc, &tmD, &tmR, my_stg, my_rbar, nslice, tm, tn, cw, wq, lane, t);
+            else if (p.tma_store) store_slices<false, BN, MH>(p, acc, &tmD, &tmR, my_stg, my_rbar, nslice, tm, tn, cw, wq, lane, t);
+            else store_frags<BN, MH>(p, acc, tm, tn, cw, wq, lane);
         } else if (kGluTma && p.glu_tma) {
             if constexpr (kGluTma) {
                 if (glu_ops) mbar_wait(ops_full, ntile & 1);
@@ -571,38 +609,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 else glu_store_slices<GLU_RELU2, BN, MH>(p, acc, &tmD, &tmD2, my_stg, sops, sops + BN, nslice, tm, tn, cw, wq, lane, t);
                 // the last slice_store's barrier is behind every read of sops by this warpgroup
                 if (glu_ops && t == 0) mbar_arrive(ops_empty);
-            }
-        } else if (!p.geglu) {
-#pragma unroll
-            for (int h = 0; h < MH; ++h) {
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const int row = tm * BMT + (cw * MH + h) * 64 + wq * 16 + (lane >> 2) + 8 * i;
-                    if (row >= p.M) continue;
-                    const bool masked = p.rowmask && p.rowmask[row] == 0;
-                    const float* cs = p.colscale ? p.colscale + (long long)(row / p.rows_per_batch) * p.N : nullptr;
-                    const __nv_bfloat16* rp = p.resid ? reinterpret_cast<const __nv_bfloat16*>(p.resid) + (long long)row * p.ldr : nullptr;
-#pragma unroll
-                    for (int j = 0; j < BN / 8; ++j) {
-                        const int col = tn * BN + 8 * j + cq;
-                        if (col >= p.N) continue;
-                        const bool two = col + 1 < p.N;
-                        float v0 = acc[h][4 * j + 2 * i], v1 = acc[h][4 * j + 2 * i + 1];
-                        if (p.bias) { v0 += __ldg(p.bias + col); if (two) v1 += __ldg(p.bias + col + 1); }
-                        if constexpr (ACT == ACT_GELU) { const float2 g = gelu_erf2(make_float2(v0, v1)); v0 = g.x; v1 = g.y; }
-                        if (cs) { v0 *= __ldg(cs + col); if (two) v1 *= __ldg(cs + col + 1); }
-                        if (masked) { v0 = 0.f; v1 = 0.f; }
-                        if (rp) {
-                            if (two) {
-                                const uint32_t u = *reinterpret_cast<const uint32_t*>(rp + col);
-                                v0 += bf16_lo(u); v1 += bf16_hi(u);
-                            } else {
-                                v0 += __bfloat162float(rp[col]);
-                            }
-                        }
-                        store_pair(p, row, col, v0, v1);
-                    }
-                }
             }
         } else if (p.geglu == GLU_GELU) {   // one copy of the GLU epilogue per activation: no per-element branch on it
             glu_epilogue<GLU_GELU, BN, MH>(p, acc, tm, tn, cw, wq, lane);

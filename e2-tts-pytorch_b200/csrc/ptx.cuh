@@ -284,10 +284,18 @@ __device__ __forceinline__ DropWords drop_words(uint32_t seedmix, uint32_t pair)
     return w;
 }
 __device__ __forceinline__ uint32_t drop_thresh32(uint32_t thresh16) { return thresh16 << 16; }
-__device__ __forceinline__ uint32_t seed_mix32(uint64_t seed) { return (uint32_t)seed ^ ((uint32_t)(seed >> 32) * 0x85EBCA77u); }
-__device__ __forceinline__ bool dropout_keep16(uint64_t seed, uint64_t idx, uint32_t thresh) {
-    const DropWords w = drop_words(seed_mix32(seed), (uint32_t)(idx >> 1));
-    return ((idx & 1) ? w.b : w.a) >= drop_thresh32(thresh);
+// The 16-bit threshold of drop probability p, and the scale of the kept elements, 1 / P(keep) = 65536 / (65536 - thresh16).
+__host__ __device__ __forceinline__ uint32_t drop_thresh16(float p) { return (uint32_t)(p * 65536.f); }
+__host__ __device__ __forceinline__ float drop_keep_scale(uint32_t thresh16) { return 65536.f / (65536.f - (float)thresh16); }
+// The 32-bit seed word drop_words hashes with: seed plus the optional device addend (CUDA-graph replays), folded to 32 bits.
+__device__ __forceinline__ uint32_t drop_seed_word(uint64_t seed, const unsigned long long* seed_dev) {
+    const uint64_t s = seed + (seed_dev ? __ldg(seed_dev) : 0ull);
+    return (uint32_t)s ^ ((uint32_t)(s >> 32) * 0x85EBCA77u);
+}
+// Pair index of GLU hidden units (hcol, hcol + 1) of `row` in an [rows, inner] hidden tensor: the forward GEMM's GLU epilogue and
+// the GLU backward must agree on it. inner is even, so hidden units (2k, 2k+1) of one row share a pair.
+__device__ __forceinline__ uint32_t glu_drop_pair(long long row, int inner, int hcol) {
+    return (uint32_t)(((unsigned long long)row * (unsigned long long)inner + hcol) >> 1);
 }
 
 }  // namespace b200

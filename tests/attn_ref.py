@@ -50,7 +50,7 @@ def _mul32(x, c):
 
 
 def dropout_keep(seed, B, H, Np, p):
-    """The kernels' attention-dropout mask (ptx.cuh: seed_mix32, drop_words) for element ((b*H + h)*Np + i)*stride + j, as bool
+    """The kernels' attention-dropout mask (ptx.cuh: drop_seed_word, drop_words) for element ((b*H + h)*Np + i)*stride + j, as bool
     [B, H, Np, Np]: keep iff the 32-bit word of the element >= thresh16 << 16, thresh16 = int(p * 65536)."""
     stride = (Np + 1) & ~1
     seedmix = (seed & 0xFFFFFFFF) ^ (((seed >> 32) * 0x85EBCA77) & 0xFFFFFFFF)
