@@ -12,6 +12,7 @@ from .modules import (  # noqa: E402,F401
 from .vocos import Vocos  # noqa: E402,F401
 from . import lib, ops, optim  # noqa: E402,F401
 from .graphed import GraphedTrainStep, BucketedTrainStep  # noqa: E402,F401
+from .sampler import GraphedSampler  # noqa: E402,F401
 from .optim import GradSync, FusedAdoptEMA, broadcast_module  # noqa: E402,F401
 
-__all__ = ['E2TTS', 'DurationPredictor', 'Transformer', 'MelSpec', 'E2TTSReturn', 'LossBreakdown', 'inject_randomness', 'GraphedTrainStep', 'BucketedTrainStep', 'Vocos', 'GradSync', 'FusedAdoptEMA', 'broadcast_module']
+__all__ = ['E2TTS', 'DurationPredictor', 'Transformer', 'MelSpec', 'E2TTSReturn', 'LossBreakdown', 'inject_randomness', 'GraphedTrainStep', 'BucketedTrainStep', 'GraphedSampler', 'Vocos', 'GradSync', 'FusedAdoptEMA', 'broadcast_module']

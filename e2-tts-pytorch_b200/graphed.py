@@ -152,14 +152,15 @@ class BucketPlan:
     """The host side of BucketedTrainStep, no GPU needed: which bucket a batch of `n` frames goes to, how its text ids are padded,
     and every refusal that must come before a launch."""
 
-    def __init__(self, buckets, batch_size, max_seq_len, interpolated_text=False):
+    def __init__(self, buckets, batch_size, max_seq_len, interpolated_text=False, who='BucketedTrainStep'):
+        self.who = who
         b = sorted({int(x) for x in buckets})
         if not b or b[0] < 1:
-            raise ValueError(f'BucketedTrainStep: buckets must be positive frame counts, got {tuple(buckets)}')
+            raise ValueError(f'{who}: buckets must be positive frame counts, got {tuple(buckets)}')
         if b[-1] > max_seq_len:
-            raise ValueError(f'BucketedTrainStep: bucket {b[-1]} exceeds the transformer\'s max_seq_len ({max_seq_len})')
+            raise ValueError(f'{who}: bucket {b[-1]} exceeds the transformer\'s max_seq_len ({max_seq_len})')
         if not 1 <= int(batch_size) <= MAX_BATCH:
-            raise ValueError(f'BucketedTrainStep: batch_size {batch_size} is outside 1..{MAX_BATCH} (b200_small_linear takes at most '
+            raise ValueError(f'{who}: batch_size {batch_size} is outside 1..{MAX_BATCH} (b200_small_linear takes at most '
                              f'{MAX_BATCH} items per launch)')
         self.buckets, self.batch_size, self.interpolated_text = tuple(b), int(batch_size), bool(interpolated_text)
 
@@ -168,15 +169,15 @@ class BucketPlan:
         for nb in self.buckets:
             if n <= nb:
                 return nb
-        raise ValueError(f'BucketedTrainStep: a batch of {n} frames exceeds the largest bucket ({self.buckets[-1]})')
+        raise ValueError(f'{self.who}: a batch of {n} frames exceeds the largest bucket ({self.buckets[-1]})')
 
     def check(self, batch, n, text_width=None):
         """-> the bucket of a [batch, n, channels] mel with text ids `text_width` columns wide (None: no text); raises ValueError"""
         if batch != self.batch_size:
-            raise ValueError(f'BucketedTrainStep: batch of {batch} items, the graphs were captured for batch_size={self.batch_size}')
+            raise ValueError(f'{self.who}: batch of {batch} items, the graphs were captured for batch_size={self.batch_size}')
         nb = self.bucket(n)
         if self.interpolated_text and text_width is not None and text_width > nb:
-            raise ValueError(f'BucketedTrainStep: {text_width} text ids do not fit bucket {nb}: with interpolated_text the text is '
+            raise ValueError(f'{self.who}: {text_width} text ids do not fit bucket {nb}: with interpolated_text the text is '
                              'spread over the frames, so it cannot be cut')
         return nb
 

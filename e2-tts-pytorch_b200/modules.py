@@ -679,12 +679,22 @@ class Transformer(_PackOwner):
         return list(gains.unbind(0))
 
     # ------------------------------------------------------------------ the block stack
-    def _run_layers(self, P, xs, ts, gains, mask_u8, B, Np, seed):
-        """P: the per-layer packed operands; xs bf16 [T,S,d], ts bf16 [T,S,dt] | None -> final residual streams. Layer loop of e2_tts.py:825-939."""
+    def _run_layers(self, P, xs, ts, gains, mask_u8, B, Np, seed, Bt=None):
+        """P: the per-layer packed operands; xs bf16 [T,S,d], ts bf16 [Tt,S,dt] | None -> final residual streams. Layer loop of e2_tts.py:825-939.
+        Bt: the items that carry text, the first Bt of the B (Tt = Bt * Np; default all); the others pass the layers as without text."""
         # the audio and the text attention may differ in head count and width: each call takes both, and the rotary table, from its module
         rot = {dh: self._rotary(Np, dh, xs.device) for dh in {self.dim_head, self.text_dim_head}}
         p_drop = self.dropout if self.training else 0.0
         mbits = ops.attn_maskbits(mask_u8, B, Np, xs.device) if xs.is_cuda else None   # one key-mask bitmask for all 2 * depth attention calls
+        # Hyper-connection plumbing of one stream: a sub-block returns its depth connection PENDING — (residual', branch_out, beta) — and
+        # the next sub-block's width connection consumes it in one fused kernel (ops.HcDepthWidth) when the stream's rows allow it;
+        # `close` materialises the streams where something else reads them (cross-conditioning, skip path, final norm).
+        # (items, key mask, bitmask, fuse) of the audio and of the text stream: rows are item-major, so the text items' mask is a row
+        # prefix, and each stream decides the fusion on its own rows, as a pass over its items alone would
+        ageo = tgeo = (B, mask_u8, mbits, ops.hc_can_fuse(xs.shape[0], xs.shape[1]))
+        if Bt is not None and Bt != B:
+            tmask = mask_u8[:Bt] if mask_u8 is not None else None
+            tgeo = (Bt, tmask, ops.attn_maskbits(tmask, Bt, Np, xs.device) if xs.is_cuda else None, ops.hc_can_fuse(Bt * Np, xs.shape[1]))
         skips = []
         v_first, tv_first = None, None
         nseed = [seed]
@@ -693,16 +703,12 @@ class Transformer(_PackOwner):
             nseed[0] = (nseed[0] * 6364136223846793005 + 1442695040888963407) & 0x7FFFFFFFFFFFFFFF
             return nseed[0]
 
-        # Hyper-connection plumbing of one stream: a sub-block returns its depth connection PENDING — (residual', branch_out, beta) — and
-        # the next sub-block's width connection consumes it in one fused kernel (ops.HcDepthWidth); `close` materialises the streams
-        # where something else reads them (cross-conditioning, skip path, final norm).
-        fuse = ops.hc_can_fuse(xs.shape[0], xs.shape[1])
         # num_residual_streams=1 (e2_tts.py:607, disable=True): every sub-block is x + branch(norm(x)). The width connection is then
         # the branch norm alone (the conv sub-block has none) and hands x on as `rest`; the branch's last launch (the conv kernel, the
         # to_out / FF-out GEMM epilogue) adds it, so the depth connection is nothing but a view back to [T, 1, D].
         plain = self.num_streams == 1
 
-        def width(res, hcm, gain, mode):
+        def width(res, hcm, gain, mode, B):
             if plain:
                 x2 = res.view(res.shape[0], res.shape[-1])
                 if mode == 0:
@@ -713,7 +719,7 @@ class Transformer(_PackOwner):
                 return ops.HcDepthWidth.apply(*res, *hcm.params(), gain, mode, Np)
             return ops.HcWidth.apply(res, *hcm.params(), gain, mode, Np)
 
-        def depth(rest, y, beta):
+        def depth(rest, y, beta, fuse):
             if plain:
                 return y.view(y.shape[0], 1, y.shape[1])
             return (rest, y, beta) if fuse else ops.HcDepth.apply(rest, y, beta)
@@ -721,13 +727,15 @@ class Transformer(_PackOwner):
         def close(res):
             return ops.HcDepth.apply(*res) if isinstance(res, tuple) else res
 
-        def sub_conv(res, hcm, conv):
-            br, rest, beta = width(res, hcm, None, 0)
+        def sub_conv(res, hcm, conv, geo):
+            B, mask_u8, _, fuse = geo
+            br, rest, beta = width(res, hcm, None, 0, B)
             y = ops.DwConv.apply(br, conv.dw_conv1d[0].weight, conv.dw_conv1d[0].bias, mask_u8, B, Np, plain)
-            return depth(rest, y, beta)
+            return depth(rest, y, beta, fuse)
 
-        def sub_attn(res, hcm, gain, mode, attn, pk, vf, colscale, seed, lfe=None):
-            br, rest, beta = width(res, hcm, gain, mode)
+        def sub_attn(res, hcm, gain, mode, attn, pk, vf, colscale, seed, geo, lfe=None):
+            B, mask_u8, mbits, fuse = geo
+            br, rest, beta = width(res, hcm, gain, mode, B)
             if lfe is not None:   # attn_input_fourier_embed (:909): between the attention norm (fused into the width kernel) and the attention
                 br = ops.FourierLinear.apply(br, lfe.linear.weight, pk['lfe'], *lfe.split_dims)
             mix, gate = attn.to_value_residual_mix, attn.to_v_head_gate
@@ -738,29 +746,30 @@ class Transformer(_PackOwner):
                                         pk['qkv'], cs, sn, mask_u8, B, Np, attn.heads, p_drop, seed, self.softclamp, self._seed_dev, mbits,
                                         attn.dim_head)
             y = ops.OutProj.apply(og, attn.to_out.weight, pk['out'], colscale, mask_u8, B, Np, rest if plain else None)
-            return depth(rest, y, beta), (v if vf is None else vf)
+            return depth(rest, y, beta, fuse), (v if vf is None else vf)
 
-        def sub_ff(res, hcm, gain, mode, ff, pk, colscale, seed):
-            br, rest, beta = width(res, hcm, gain, mode)
+        def sub_ff(res, hcm, gain, mode, ff, pk, colscale, seed, geo):
+            B, fuse = geo[0], geo[3]
+            br, rest, beta = width(res, hcm, gain, mode, B)
             y = ops.FeedForward.apply(br, ff.ff[0].proj.weight, ff.ff[0].proj.bias, ff.ff[2].weight, ff.ff[2].bias,
                                       pk['w1'], pk['b1'], pk['w2'], colscale, B, Np, p_drop, seed, self._seed_dev,
                                       rest if plain else None, ff.act, ff.ff[0].mult_bias)
-            return close(depth(rest, y, beta))
+            return close(depth(rest, y, beta, fuse))
 
         def text_subblocks(i, ts, tvf, gains, seeds, pk):  # the three text sub-blocks of layer i (:853-882; no gains: plain RMSNorms)
             text, thc = self.layers[i][1], self.hyper_conns[i][1]
-            ts = sub_conv(ts, thc[0], text[0])
-            ts, tvf = sub_attn(ts, thc[1], text[1].g, 1, text[2], pk, tvf, None, seeds[0])
-            return sub_ff(ts, thc[2], text[3].g, 1, text[4], pk, None, seeds[1]), tvf
+            ts = sub_conv(ts, thc[0], text[0], tgeo)
+            ts, tvf = sub_attn(ts, thc[1], text[1].g, 1, text[2], pk, tvf, None, seeds[0], tgeo)
+            return sub_ff(ts, thc[2], text[3].g, 1, text[4], pk, None, seeds[1], tgeo), tvf
 
         def audio_subblocks(i, xs, vf, gains4, seeds, pk):  # the three audio sub-blocks of layer i (:900-939)
             speech, shc = self.layers[i][0], self.hyper_conns[i][0]
             g_an, g_az, g_fn, g_fz = gains4
             mode = 2 if self.cond_on_time else 1
-            xs = sub_conv(xs, shc[0], speech[1])  # :900-902
-            xs, vf = sub_attn(xs, shc[1], g_an, mode, speech[3], pk, vf, g_az, seeds[0],
+            xs = sub_conv(xs, shc[0], speech[1], ageo)  # :900-902
+            xs, vf = sub_attn(xs, shc[1], g_an, mode, speech[3], pk, vf, g_az, seeds[0], ageo,
                               speech[4] if isinstance(speech[4], LinearFourierEmbed) else None)  # :906-916
-            return sub_ff(xs, shc[2], g_fn, mode, speech[7], pk, g_fz, seeds[1]), vf  # :936-939
+            return sub_ff(xs, shc[2], g_fn, mode, speech[7], pk, g_fz, seeds[1], ageo), vf  # :936-939
 
         # Transformer(checkpoint_activations=True) under autograd: each layer's audio sub-blocks and each text block are one
         # ops.Segment, which keeps only its inputs and runs the sub-blocks again in the backward. The seeds are drawn here, in the
@@ -793,7 +802,7 @@ class Transformer(_PackOwner):
         two = TWO_STREAM and has_text(0) and xs.is_cuda
         if two:
             main, side = torch.cuda.current_stream(xs.device), _side_stream(xs.device)
-            for t in (mask_u8, mbits, *[x for pair in rot.values() for x in pair]):
+            for t in (*tgeo[1:3], *[x for pair in rot.values() for x in pair]):
                 if t is not None:
                     t.record_stream(side)
 
@@ -849,20 +858,25 @@ class Transformer(_PackOwner):
         y = self._forward_from_h(w, h, B, N, times, mask, te_bf16=te)
         return y.view(B, N, d).to(x.dtype)
 
-    def _forward_from_h(self, w, h, B, N, times, mask, text_ids=None, text_embed_module=None, te_bf16=None):
-        """w: the handles of `_add_weights`, already packed; h bf16 [B*N, d] (already projected) -> final-normed bf16 [B*N, d]."""
+    def _forward_from_h(self, w, h, B, N, times, mask, text_ids=None, text_embed_module=None, te_bf16=None, text_items=None):
+        """w: the handles of `_add_weights`, already packed; h bf16 [B*N, d] (already projected) -> final-normed bf16 [B*N, d].
+        text_items: how many of the B items the text ids / embeddings are for (the first ones; default all). The other items run as
+        without text — the text-dropped half of a batched classifier-free-guidance pass (E2TTS.cfg_pred_batched)."""
         S, R = self.num_streams, self.num_registers
+        Bt = default(text_items, B)
+        if Bt != B and torch.is_grad_enabled():
+            raise NotImplementedError('text on a prefix of the items (text_items) is inference only: CrossCondition has no backward for it')
         Np, mask_u8 = self._prepare(B, N, mask)
         abs_w = self.abs_pos_emb.weight if exists(self.abs_pos_emb) else None
         xs = ops.Assemble.apply(h, abs_w, self.registers, B, N, S)
         ts = None
         if exists(text_ids):
-            ts = ops.TextStem.apply(text_ids, text_embed_module.embed.weight, self.text_registers, B, N, S)
+            ts = ops.TextStem.apply(text_ids, text_embed_module.embed.weight, self.text_registers, Bt, N, S)
         elif exists(te_bf16):
-            ts = ops.Assemble.apply(te_bf16, None, self.text_registers, B, N, S)
+            ts = ops.Assemble.apply(te_bf16, None, self.text_registers, Bt, N, S)
         gains = self._cond_gains(times, B, w['cond']) if self.cond_on_time else None
         seed = int(torch.randint(0, 2 ** 62, (1,)).item()) if (self.training and self.dropout > 0) else 0
-        xs = self._run_layers(w['layers'], xs, ts, gains, mask_u8, B, Np, seed)
+        xs = self._run_layers(w['layers'], xs, ts, gains, mask_u8, B, Np, seed, Bt)
         return ops.FinalNorm.apply(xs, self.final_norm.g, B, N, R)
 
 
@@ -1303,20 +1317,52 @@ class E2TTS(_PackOwner):
         null_pred = cfg_null_model.transformer_with_pred_head(*args, drop_text_cond=null_drop, **kwargs)
         return ops.cfg_combine(pred, null_pred, float(cfg_strength), bool(remove_parallel_component), float(keep_parallel_frac))
 
-    @torch.no_grad()
     @_on_module_device
-    def sample(self, cond, *, text=None, lens=None, duration=None, steps=32, cfg_strength=1., cfg_null_model=None, max_duration=4096,
-               vocoder=None, return_raw_output=None, save_to_filename=None):
-        """e2_tts.py:1332-1466. The ODE on t = linspace(0, 1, steps) with the torchdiffeq method of `odeint_kwargs` (SURVEY A.7): the
-        fixed-grid midpoint / euler loop below, or rk4 and the adaptive Runge–Kutta methods of ode.py."""
-        ode_kw = _parse_odeint_kwargs(self.odeint_kwargs)   # odeint_kwargs is a plain attribute: checked again before any work
-        self.eval()
+    def cfg_pred_batched(self, x, cond, times, mask2, text, cfg_strength: float = 1., remove_parallel_component: bool = True,
+                         keep_parallel_frac: float = 0.):
+        """cfg_transformer_with_pred_head without a cfg_null_model, as ONE transformer pass over 2B items: items 0..B-1 are
+        (x, cond, text), items B..2B-1 the same x and cond with the text dropped. x, cond fp32 [B, N, C]; times a 0-dim tensor;
+        mask2 bool [2B, N] (the mask of the B items, twice) or None; text ids [B, nt] or None. Inference only."""
+        pred, null_pred = self._pred_pair(x, cond, times, mask2, text)
+        return ops.cfg_combine(pred, null_pred, float(cfg_strength), bool(remove_parallel_component), float(keep_parallel_frac))
+
+    def _pred_pair(self, x, cond, times, mask2, text):
+        """-> (the conditional, the text-dropped prediction), each fp32 [B, N, C]: the two halves of one [2B, N, C] prediction, which
+        cfg_combine reads in place. Rows are item-major, so the text stream covers a row prefix (Transformer._forward_from_h
+        text_items). With text None both halves would be the same pass, so one pass over the B items serves as both."""
+        B, N, C = x.shape
+        w = self._packed_weights()
+        A, _ = ops.stem_prepare(B, N, C, w['Cp'], x_in=x.to(F32).contiguous(), cond_in=cond.to(F32).contiguous(), concat=self.concat_cond)
+        mask = mask2[:B] if exists(mask2) else None
+        if not exists(text):
+            y = self._embed(w, A, B, N, times, mask, None, True)
+            pred = ops.PredHead.apply(y, self.to_pred.weight, self.to_pred.bias, w['pred']).view(B, N, C)
+            return pred, pred
+        bias = self.proj_in.bias if self.concat_cond else self.proj_in.bias + self.cond_proj_in.bias
+        h = ops.stem_linear_twice(A, w['stem'], bias)     # both halves start from the same x and cond
+        ids, te = None, None
+        if isinstance(self.embed_text, InterpolatedCharacterEmbed):
+            te = self.embed_text.embed_bf16(text, N, mask, w['interp'])
+        else:
+            ids = self.embed_text.ids(text, N)
+        y = self.transformer._forward_from_h(w['tr'], h, 2 * B, N, times, mask2, text_ids=ids, text_embed_module=self.embed_text,
+                                             te_bf16=te, text_items=B)
+        pred = ops.PredHead.apply(y, self.to_pred.weight, self.to_pred.bias, w['pred']).view(2 * B, N, C)
+        return pred[:B], pred[B:]
+
+    def _check_decoder(self, vocoder, return_raw_output, save_to_filename=None):
+        """sample()'s refusal to start an ODE solve whose output it could not decode"""
         no_vocos = self._use_vocos_requested and not exists(self.vocos)
         if not (exists(return_raw_output) and return_raw_output) and not exists(vocoder) and (no_vocos or exists(save_to_filename)):
             # fail BEFORE the ODE loop (124 transformer passes at the defaults), not after it
             raise NotImplementedError('Vocos decoding / audio saving needs the pretrained vocoder from the HF hub and is out of scope '
                                       '(SURVEY.md §2 row 10): call sample(..., return_raw_output=True), pass `vocoder=`, build '
                                       'E2TTS(use_vocos=False), or pass a local `pretrained_vocos_path`')
+
+    def _sample_inputs(self, cond, text, lens, duration, max_duration):
+        """sample()'s preparation ahead of the ODE (e2_tts.py:1356-1402): mel of a raw wave, tokens, lens = max(text lens, lens), the
+        duration (predicted when None), clamped to [lens + 1, max_duration]. -> (cond fp32 [B, md, C] zero-padded, cond_mask bool
+        [B, md, 1], text ids | None, duration [B]) with md = max(duration)."""
         if cond.ndim == 2:
             cond = self.mel_spec(cond).transpose(1, 2)
             assert cond.shape[-1] == self.num_channels
@@ -1340,6 +1386,32 @@ class E2TTS(_PackOwner):
         md = int(duration.amax())
         cond = F.pad(cond, (0, 0, 0, md - cond_seq_len), value=0.)
         cond_mask = F.pad(cond_mask, (0, md - cond_mask.shape[-1]), value=False)[..., None]
+        return cond, cond_mask, text, duration
+
+    def _sample_output(self, out, duration, vocoder, return_raw_output):
+        """sample()'s return value from the solved mel `out` [B, md, C] (e2_tts.py:1430-1466)"""
+        if exists(return_raw_output) and return_raw_output:
+            return out
+        if exists(vocoder):
+            assert not exists(self.vocos), '`use_vocos` should not be turned on if you are passing in a custom `vocoder` on sampling'
+            return vocoder(out.transpose(1, 2))
+        if exists(self.vocos):   # :1440-1451, the whole ragged batch in one decode: item b is out[b, :duration[b]]
+            audio = self.vocos.decode_padded(out, duration, db_to_amp=True)
+            hop = self.vocos.hop_length
+            return [audio[b, :int(n) * hop] for b, n in enumerate(duration.tolist())]
+        return out
+
+    @torch.no_grad()
+    @_on_module_device
+    def sample(self, cond, *, text=None, lens=None, duration=None, steps=32, cfg_strength=1., cfg_null_model=None, max_duration=4096,
+               vocoder=None, return_raw_output=None, save_to_filename=None):
+        """e2_tts.py:1332-1466. The ODE on t = linspace(0, 1, steps) with the torchdiffeq method of `odeint_kwargs` (SURVEY A.7): the
+        fixed-grid midpoint / euler loop below, or rk4 and the adaptive Runge–Kutta methods of ode.py."""
+        ode_kw = _parse_odeint_kwargs(self.odeint_kwargs)   # odeint_kwargs is a plain attribute: checked again before any work
+        self.eval()
+        self._check_decoder(vocoder, return_raw_output, save_to_filename)
+        cond, cond_mask, text, duration = self._sample_inputs(cond, text, lens, duration, max_duration)
+        dev = cond.device
         mask = lens_to_mask(duration)
         step_cond = torch.where(cond_mask, cond, torch.zeros_like(cond))  # step-invariant: hoisted out of fn (:1404)
 
@@ -1354,7 +1426,8 @@ class E2TTS(_PackOwner):
         # weights are fixed for the whole solve: pack each model's operands once (fresh), not once per function evaluation
         freeze_null = cfg_null_model._pack()[0].freeze() if exists(cfg_null_model) else contextlib.nullcontext()
         with self._pack()[0].freeze(), freeze_null:
-            fn_eval = fn   # (one function evaluation as a CUDA graph was measured: -1 % at cfg5, but re-capturing per call costs the e2e path 19 %)
+            fn_eval = fn   # (one function evaluation as a CUDA graph was measured: -1 % at cfg5, but re-capturing per call costs the e2e path 19 %;
+                           #  GraphedSampler captures the whole solve once instead)
             if method not in ('midpoint', 'euler'):   # rk4 and the adaptive Runge–Kutta methods
                 y = ode.odeint(fn_eval, y, steps, method, **ode_kw)
             else:
@@ -1366,17 +1439,7 @@ class E2TTS(_PackOwner):
                         half = 0.5 * dt
                         ymid = ops.axpy(y, fn_eval(t0, y), half)
                         y = ops.axpy(y, fn_eval(t0 + half, ymid), dt)
-        out = torch.where(cond_mask, cond, y)
-        if exists(return_raw_output) and return_raw_output:
-            return out
-        if exists(vocoder):
-            assert not exists(self.vocos), '`use_vocos` should not be turned on if you are passing in a custom `vocoder` on sampling'
-            return vocoder(out.transpose(1, 2))
-        if exists(self.vocos):   # :1440-1451, the whole ragged batch in one decode: item b is out[b, :duration[b]]
-            audio = self.vocos.decode_padded(out, duration, db_to_amp=True)
-            hop = self.vocos.hop_length
-            return [audio[b, :int(n) * hop] for b, n in enumerate(duration.tolist())]
-        return out
+        return self._sample_output(torch.where(cond_mask, cond, y), duration, vocoder, return_raw_output)
 
     @_on_module_device
     def forward(self, inp, *, text=None, times=None, lens=None, velocity_consistency_model=None, velocity_consistency_delta=1e-5):

@@ -105,17 +105,27 @@ def grid(steps):
     return torch.linspace(0, 1, steps).tolist()
 
 
-def rk4(fn, y0, steps, stats=None):
-    """Fixed-grid rk4 (torchdiffeq rk4_alt_step_func, the 3/8 rule) on t = linspace(0, 1, steps): per step
-    k1 = f(t0, y0), k2 = f(t0 + dt/3, y0 + dt k1/3), k3 = f(t0 + 2dt/3, y0 + dt (k2 - k1/3)), k4 = f(t1, y0 + dt (k1 - k2 + k3)),
-    y1 = y0 + (k1 + 3 (k2 + k3) + k4) dt/8; times and dt in fp32 as on torchdiffeq's fp32 grid."""
+def rk4_times(steps):
+    """the stage times of fixed-grid rk4 on t = linspace(0, 1, steps), four per step, fp32 as on torchdiffeq's fp32 grid"""
     ts = [F32(t) for t in grid(steps)]
     third, two_thirds = F32(1 / 3), F32(2 / 3)
     times = []
     for t0, t1 in zip(ts[:-1], ts[1:]):
         dt = F32(t1 - t0)
         times += [t0, F32(t0 + F32(dt * third)), F32(t0 + F32(dt * two_thirds)), t1]
-    tt = torch.tensor(times, dtype=torch.float32).to(y0.device)   # every stage time in one copy: no host synchronisation per step
+    return times
+
+
+def rk4(fn, y0, steps, stats=None, tt=None):
+    """Fixed-grid rk4 (torchdiffeq rk4_alt_step_func, the 3/8 rule) on t = linspace(0, 1, steps): per step
+    k1 = f(t0, y0), k2 = f(t0 + dt/3, y0 + dt k1/3), k3 = f(t0 + 2dt/3, y0 + dt (k2 - k1/3)), k4 = f(t1, y0 + dt (k1 - k2 + k3)),
+    y1 = y0 + (k1 + 3 (k2 + k3) + k4) dt/8; times and dt in fp32 as on torchdiffeq's fp32 grid. tt: rk4_times(steps) already on the
+    device (a CUDA-graph capture cannot copy them there)."""
+    ts = [F32(t) for t in grid(steps)]
+    third = F32(1 / 3)
+    times = rk4_times(steps)
+    if tt is None:
+        tt = torch.tensor(times, dtype=torch.float32).to(y0.device)   # every stage time in one copy: no host synchronisation per step
     y, stage, ring = y0, torch.empty_like(y0), [torch.empty_like(y0), torch.empty_like(y0)]
     for i, (t0, t1) in enumerate(zip(ts[:-1], ts[1:])):
         dt = F32(t1 - t0)

@@ -588,23 +588,28 @@ class FeedForward(Function):
 
 # ---------------------------------------------------------------------------------------------------- cross-stream GEMMs
 class CrossCondition(Function):
-    """TextAudioCrossCondition (e2_tts.py:486-513) on all S streams, concat never materialised (two-source K)."""
+    """TextAudioCrossCondition (e2_tts.py:486-513) on all S streams, concat never materialised (two-source K).
+    ts may hold fewer rows than xs (a batched CFG pass, where only the first items carry text): the GEMMs then run over those rows
+    and the other audio rows are carried over unchanged. That form is inference only."""
 
     @staticmethod
     def forward(ctx, xs, ts, w_ta, w_at, wstack):
         ctx.set_materialize_grads(False)   # the text stream's last output has no consumer: its gradient stays None instead of a zero fill
         T, S, D = xs.shape
         Dt = ts.shape[-1]
-        R = T * S
-        x2, t2 = xs.view(R, D), ts.view(R, Dt)
-        xo = gemm(x2, wstack, R, D, D + Dt, lda=D, A2=t2, lda2=Dt, K1=D, ldb=D + Dt, resid=x2, ldr=D)
+        R, Rt = T * S, ts.shape[0] * S
+        x2, t2 = xs.view(R, D), ts.view(Rt, Dt)
+        xo = torch.empty((R, D), device=xs.device, dtype=BF16) if Rt != R else None
+        xo = gemm(x2, wstack, Rt, D, D + Dt, lda=D, A2=t2, lda2=Dt, K1=D, ldb=D + Dt, resid=x2, ldr=D, out=xo)
+        if Rt != R:
+            xo[Rt:].copy_(x2[Rt:])    # the items without text: bit-for-bit the rows a pass without text hands on
         if w_at is not None:
-            to = gemm(x2, wstack[D:], R, Dt, D + Dt, lda=D, A2=t2, lda2=Dt, K1=D, ldb=D + Dt, resid=t2, ldr=Dt)
+            to = gemm(x2, wstack[D:], Rt, Dt, D + Dt, lda=D, A2=t2, lda2=Dt, K1=D, ldb=D + Dt, resid=t2, ldr=Dt)
         else:
-            to = ts.view(R, Dt)
+            to = t2
         ctx.save_for_backward(xs, ts, wstack)
         ctx.has_at = w_at is not None
-        return xo.view(T, S, D), to.view(T, S, Dt)
+        return xo.view(T, S, D), to.view(-1, S, Dt)
 
     @staticmethod
     @once_differentiable
@@ -722,6 +727,17 @@ class StemLinear(Function):
         db = colsum(d_h, T, D, D)
         half = Kp // 2
         return None, dWp[:, :C], db, (dWp[:, half:half + C] if has_cond else None), (db if has_cond else None), None
+
+
+def stem_linear_twice(A, wpack, bias):
+    """StemLinear's GEMM without autograd, written to both halves of one bf16 [2T, D] output: the stem of a batched CFG pass,
+    whose conditional and text-dropped items share x and cond (E2TTS.cfg_pred_batched)."""
+    T, Kp = A.shape
+    D = wpack.shape[0]
+    h = torch.empty((2 * T, D), device=A.device, dtype=BF16)
+    for half in (h[:T], h[T:]):
+        gemm(A, wpack, T, D, Kp, bias=bias, out=half)
+    return h
 
 
 class Assemble(Function):
