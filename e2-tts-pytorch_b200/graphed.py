@@ -12,7 +12,9 @@ the Python / driver side of that costs more than the GPU work. Capturing the ste
   * with more than one rank (torch.distributed initialised, or `process_group=` given) the graph ends with ONE gather of all
     parameter gradients into a flat fp32 buffer (x 1/world) and the replay is followed by ONE ncclAllReduce of that buffer
     (optim.GradSync): the data-parallel exchange of SURVEY §8e without DDP's bucket hooks, which cannot be captured cheaply and
-    whose NCCL kernels would compete with the persistent compute kernels for SMs all through backward.
+    whose NCCL kernels would compete with the persistent compute kernels for SMs all through backward;
+  * with a velocity-consistency teacher (the EMA model, e2_tts.py:1556-1589) the teacher's no-grad pass at t + delta is captured
+    ahead of the student's forward, through E2TTS.forward itself; its weights are packed from its parameters on every replay.
 Gradients are left in `param.grad` exactly as after `loss.backward()` (+ DDP's averaging when world > 1); run the optimiser after
 the call (optim.FusedAdoptEMA takes `step.grad_sync.flat` directly). Do not keep an output of an earlier EAGER forward of the same
 model alive while constructing this object: its autograd graph pins the parameters' AccumulateGrad nodes to the default (legacy)
@@ -55,10 +57,95 @@ def _new_seed_word(model, dev):
     return seed_dev
 
 
-def _train_pass(model, seed_dev, mel, text, lens):
-    """one forward + backward as captured: the seed word steps first, then the model's own training objective"""
-    lib.call('b200_seed_advance', seed_dev, torch.cuda.current_stream().cuda_stream)
-    out = model(mel, text=text, lens=lens)
+def _geometry(model):
+    """what a teacher must share with its student beyond the state_dict shapes: the stem layout and the attention geometry"""
+    t = model.transformer
+    return dict(concat_cond=model.concat_cond, num_channels=model.num_channels, heads=t.heads, dim_head=t.dim_head,
+                text_heads=t.text_heads, text_dim_head=t.text_dim_head, softclamp=t.softclamp, num_residual_streams=t.num_streams)
+
+
+class VelocityTeacher:
+    """The velocity-consistency teacher of a graphed step (e2_tts.py:1556-1589; the reference trainer passes its EMA model,
+    trainer.py:259-268): every refusal that must come before a launch, and the per-call check that the graph may still read it.
+
+    The graph runs E2TTS.forward(velocity_consistency_model=teacher) as the eager step does, so its teacher pass packs the teacher's
+    weights from the parameters' storage on every replay: an in-place update between replays (FusedAdoptEMA.copy_ema_to, ema-pytorch's
+    EMA.update) is picked up, a parameter with new storage is refused. A teacher in training mode gets a device seed word of its own,
+    stepped on every replay like the student's; its mode at construction is the one captured."""
+
+    def __init__(self, model, teacher, delta, frames, who):
+        from .modules import E2TTS
+        self.who = who
+        if not isinstance(model, E2TTS):
+            raise ValueError(f'{who}: velocity_consistency_model is given for a {type(model).__name__}; only an E2TTS has the '
+                             'velocity-consistency term')
+        if not float(model.velocity_consistency_weight) > 0.0:
+            raise ValueError(f'{who}: velocity_consistency_model is given but velocity_consistency_weight is '
+                             f'{model.velocity_consistency_weight}, so the teacher would never be used')
+        if not isinstance(teacher, E2TTS):
+            raise ValueError(f'{who}: velocity_consistency_model must be an E2TTS (the EMA copy of the model), got {type(teacher).__name__}')
+        if teacher is model:
+            raise ValueError(f'{who}: velocity_consistency_model is the model itself; pass a separate copy (the EMA model)')
+        mine, theirs = model.state_dict(), teacher.state_dict()
+        if list(mine) != list(theirs) or any(mine[k].shape != theirs[k].shape for k in mine):
+            diff = sorted(set(mine) ^ set(theirs)) or [k for k in mine if mine[k].shape != theirs[k].shape]
+            raise ValueError(f'{who}: velocity_consistency_model is not of the model\'s architecture (state_dict differs at {diff[0]!r})')
+        g_m, g_t = _geometry(model), _geometry(teacher)
+        for k in g_m:
+            if g_m[k] != g_t[k]:
+                raise ValueError(f'{who}: velocity_consistency_model is not of the model\'s architecture ({k} {g_t[k]} != {g_m[k]})')
+        dev_m, dev_t = next(model.parameters()).device, next(teacher.parameters()).device
+        if dev_m != dev_t:
+            raise ValueError(f'{who}: velocity_consistency_model lives on {dev_t}, the model on {dev_m}')
+        if frames > teacher.transformer.max_seq_len:
+            raise ValueError(f'{who}: {frames} frames exceed the velocity_consistency_model\'s max_seq_len ({teacher.transformer.max_seq_len})')
+        self.model, self.delta = teacher, float(delta)
+        self.seed_dev = None
+        self._ptrs, self._training, self._keep = None, None, None
+
+    def add_seed_word(self):
+        """a device seed word for a teacher in training mode (none in eval mode: it draws no dropout seed)"""
+        if self.model.training:
+            self.seed_dev = _new_seed_word(self.model, next(self.model.parameters()).device)
+
+    def seal(self):
+        """after capture: the storage and mode the graph was recorded against. The teacher's derived state (weight pack, rotary
+        tables) is held here too: the graph reads those buffers, and a `.to()` on the teacher would otherwise free them."""
+        self._ptrs = tuple(p.data_ptr() for p in self.model.parameters())
+        self._training = self.model.training
+        from .modules import _PackOwner
+        self._keep = [dict(m._derived) for m in self.model.modules() if isinstance(m, _PackOwner)]
+
+    def check(self):
+        if tuple(p.data_ptr() for p in self.model.parameters()) != self._ptrs:
+            raise ValueError(f'{self.who}: a velocity_consistency_model parameter has new storage since capture (the graph reads the '
+                             'old one); update the teacher in place (copy_ema_to, EMA.update) or build a new step')
+        if self.model.training != self._training:
+            raise ValueError(f'{self.who}: the velocity_consistency_model was captured in {"training" if self._training else "eval"} '
+                             'mode; switch it back or build a new step')
+
+
+def velocity_flag(teacher, velocity, who):
+    """the velocity switch of one call: default on when the step has a teacher; raises before any launch"""
+    v = (teacher is not None) if velocity is None else bool(velocity)
+    if v and teacher is None:
+        raise ValueError(f'{who}: velocity=True on a step built without velocity_consistency_model')
+    if v:
+        teacher.check()
+    return v
+
+
+def _train_pass(model, seed_dev, mel, text, lens, teacher=None):
+    """one forward + backward as captured: the seed words step first, then the model's own training objective (with the
+    velocity-consistency term of `teacher`, a VelocityTeacher, when given)"""
+    stream = torch.cuda.current_stream().cuda_stream
+    lib.call('b200_seed_advance', seed_dev, stream)
+    if teacher is None:
+        out = model(mel, text=text, lens=lens)
+    else:
+        if teacher.seed_dev is not None:
+            lib.call('b200_seed_advance', teacher.seed_dev, stream)
+        out = model(mel, text=text, lens=lens, velocity_consistency_model=teacher.model, velocity_consistency_delta=teacher.delta)
     if torch.is_tensor(out):       # DurationPredictor.forward returns the scalar loss itself (e2_tts.py:1113)
         out = _Loss(out)
     out.loss.backward()
@@ -71,10 +158,17 @@ def _clear_grads(model):
 
 
 class GraphedTrainStep:
-    def __init__(self, model, mel, *, text=None, lens=None, warmup=3, process_group=None, flat_grads=None):
+    def __init__(self, model, mel, *, text=None, lens=None, warmup=3, process_group=None, flat_grads=None,
+                 velocity_consistency_model=None, velocity_consistency_delta=1e-5):
         """model: an E2TTS or a DurationPredictor (NOT wrapped in DistributedDataParallel — the exchange is done here). flat_grads: True forces the flat
-        gradient buffer even on one rank (for the fused optimiser); default = only when world_size > 1."""
+        gradient buffer even on one rank (for the fused optimiser); default = only when world_size > 1.
+        velocity_consistency_model: the teacher of the velocity-consistency term (an E2TTS of the model's architecture, e.g. its EMA copy;
+        the model needs velocity_consistency_weight > 0). Then two graphs are captured into one pool, with and without the teacher
+        pass, and each call picks one with `velocity=` (default: with)."""
         _refuse_ddp_wrapper(model, 'GraphedTrainStep')
+        self.teacher = None
+        if velocity_consistency_model is not None:
+            self.teacher = VelocityTeacher(model, velocity_consistency_model, velocity_consistency_delta, int(mel.shape[1]), 'GraphedTrainStep')
         if model.training and 0.0 < float(getattr(model, 'cond_drop_prob', 0.0)) < 1.0:
             raise ValueError('GraphedTrainStep: cond_drop_prob must be 0 or 1 (the text-drop branch is decided on the host)')
         if not mel.is_cuda:
@@ -87,60 +181,86 @@ class GraphedTrainStep:
         world = _world(process_group)
         if world > 1:
             broadcast_module(model, 0, process_group)    # replicas must start identical (DDP does this when it wraps the module)
+            if self.teacher is not None:
+                broadcast_module(self.teacher.model, 0, process_group)
         use_flat = (world > 1) if flat_grads is None else bool(flat_grads) or world > 1
         self.grad_sync = GradSync(list(model.parameters()), process_group) if use_flat else None
         self._seed_dev = _new_seed_word(model, dev)
+        modes = (True, False) if self.teacher is not None else (False,)   # the teacher's graph first: it is the larger
+        if self.teacher is not None:
+            self.teacher.add_seed_word()
         cur = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(dev)
         side.wait_stream(cur)
         with torch.cuda.stream(side):          # warm-up off the capture stream: lazy initialisation, allocator pools, packed weights
-            for _ in range(max(1, warmup)):
-                self._eager()
-                self._clear_grads()
+            for v in modes:
+                for _ in range(max(1, warmup)):
+                    self._eager(v)
+                    self._clear_grads()
             if self.grad_sync is not None and world > 1:
                 self.grad_sync.all_reduce()    # NCCL communicator / channel setup outside the timed path
         cur.wait_stream(side)
         torch.cuda.synchronize(dev)
         torch.cuda.empty_cache()   # the warm-up's side-stream blocks would sit beside the graph's private pool (a full set of activations each)
-        self.graph = torch.cuda.CUDAGraph()
-        table = self.grad_sync.new_table() if self.grad_sync is not None else None
-        n0 = lib.launch_count()
-        with torch.cuda.graph(self.graph):
-            self.out = self._eager()
+        pool = torch.cuda.graph_pool_handle() if len(modes) > 1 else None
+        self.graphs, self.outs, self.launches, self._tables, self._grad_sets = {}, {}, {}, {}, {}
+        for v in modes:
+            self._clear_grads()      # each graph writes gradient tensors of its own (a backward into existing ones would add)
+            graph = torch.cuda.CUDAGraph()
+            table = self.grad_sync.new_table() if self.grad_sync is not None else None
+            n0 = lib.launch_count()
+            with torch.cuda.graph(graph, pool=pool):
+                out = self._eager(v)
+                if self.grad_sync is not None:
+                    static_grads = self.grad_sync.gather(table)   # recorded against the (still empty) chunk table
             if self.grad_sync is not None:
-                static_grads = self.grad_sync.gather(table)   # recorded against the (still empty) chunk table
+                self.grad_sync.fill_table(table, static_grads)    # the graph's static gradient tensors, known only now
+                self._tables[v] = table
+            self.launches[v] = lib.launch_count() - n0   # kernel nodes of ours in the graph (they all run on every replay)
+            # the gradient tensors the graph writes into: re-attached after every replay in case the training loop dropped them
+            # (optimizer.zero_grad(set_to_none=True)); each replay OVERWRITES them, exactly like backward() into empty .grad fields
+            self._grad_sets[v] = [(p, p.grad) for p in self.model.parameters() if p.grad is not None]
+            self.graphs[v], self.outs[v] = graph, out
+        if self.teacher is not None:
+            self.teacher.seal()
+        self.graph, self.out, self.launches_per_step = self.graphs[modes[0]], self.outs[modes[0]], self.launches[modes[0]]
+        self._grads = self._grad_sets[modes[0]]
         if self.grad_sync is not None:
-            self.grad_sync.fill_table(table, static_grads)    # the graph's static gradient tensors, known only now
-            self._table = table
-        self.launches_per_step = lib.launch_count() - n0   # kernel nodes of ours in the graph (they all run on every replay)
-        # the gradient tensors the graph writes into: re-attached after every replay in case the training loop dropped them
-        # (optimizer.zero_grad(set_to_none=True)); each replay OVERWRITES them, exactly like backward() into empty .grad fields
-        self._grads = [(p, p.grad) for p in self.model.parameters() if p.grad is not None]
-        if self.grad_sync is not None:
+            self._table = self._tables[modes[0]]
             self.grad_sync.attach()
+        else:
+            self._attach(self._grads)
 
-    def _eager(self):
-        return _train_pass(self.model, self._seed_dev, self.mel, self.text, self.lens)
+    def _eager(self, velocity=False):
+        return _train_pass(self.model, self._seed_dev, self.mel, self.text, self.lens, self.teacher if velocity else None)
 
     def _clear_grads(self):
         _clear_grads(self.model)
 
-    def __call__(self, mel=None, *, text=None, lens=None):
-        """Run one step on a new batch of the captured shapes; returns the (device) loss tensor of that step (this rank's)."""
+    @staticmethod
+    def _attach(grads):
+        for p, g in grads:
+            if p.grad is not g:
+                p.grad = g
+
+    def __call__(self, mel=None, *, text=None, lens=None, velocity=None):
+        """Run one step on a new batch of the captured shapes; returns the (device) loss tensor of that step (this rank's).
+        velocity: replay the graph with the velocity-consistency term (default: when the step has a teacher). `self.out` is then
+        that graph's output, with `out.loss_breakdown` (flow, velocity_consistency)."""
+        v = velocity_flag(self.teacher, velocity, 'GraphedTrainStep')
         if mel is not None:
             self.mel.copy_(mel, non_blocking=True)
         if text is not None:
             self.text.copy_(text, non_blocking=True)
         if lens is not None:
             self.lens.copy_(lens, non_blocking=True)
+        self.graph, self.out, self._grads = self.graphs[v], self.outs[v], self._grad_sets[v]
         self.graph.replay()
         if self.grad_sync is not None:
             self.grad_sync.all_reduce()
             self.grad_sync.attach()
         else:
-            for p, g in self._grads:
-                if p.grad is not g:
-                    p.grad = g
+            self._attach(self._grads)
         return self.out.loss
 
 
@@ -245,13 +365,21 @@ class BucketedTrainStep:
       previous window's views; feed the optimiser only when `sync_gradients` is set.
     * All graphs share one memory pool (captured largest bucket first) and one dropout seed word. Nothing a caller reads lives in
       the pool: the loss is copied into a buffer of its own and the gradients are consumed by the in-graph accumulate.
+    * With `velocity_consistency_model=` (the EMA teacher, VelocityTeacher) every (bucket, text mode) also gets a graph with the
+      teacher pass, in the same pool; `velocity=` picks one per call (the trainer's `ema_model.initted`), and the velocity part of
+      the loss is copied out to `velocity_loss`.
     FusedAdoptEMA runs one EMA update per optimiser step (ema-pytorch's EMA.update runs per micro-batch in trainer.py:279)."""
 
-    def __init__(self, model, batch_size, buckets, *, grad_accumulation_steps=1, process_group=None, warmup=3):
+    def __init__(self, model, batch_size, buckets, *, grad_accumulation_steps=1, process_group=None, warmup=3,
+                 velocity_consistency_model=None, velocity_consistency_delta=1e-5):
         _refuse_ddp_wrapper(model, 'BucketedTrainStep')
-        if float(getattr(model, 'velocity_consistency_weight', 0.0)) > 0.0:
-            raise ValueError('BucketedTrainStep: velocity consistency is not graphed (the reference trainer feeds it the EMA model '
-                             'each step, trainer.py:259-268); use the eager step')
+        self.teacher = None
+        if velocity_consistency_model is not None:
+            self.teacher = VelocityTeacher(model, velocity_consistency_model, velocity_consistency_delta, max(int(x) for x in buckets),
+                                           'BucketedTrainStep')
+        elif float(getattr(model, 'velocity_consistency_weight', 0.0)) > 0.0:
+            raise ValueError('BucketedTrainStep: velocity consistency needs its teacher (the reference trainer feeds it the EMA model '
+                             'each step, trainer.py:259-268); pass velocity_consistency_model=')
         k = int(grad_accumulation_steps)
         if k < 1:
             raise ValueError(f'BucketedTrainStep: grad_accumulation_steps must be >= 1, got {grad_accumulation_steps}')
@@ -263,12 +391,17 @@ class BucketedTrainStep:
             raise ValueError('BucketedTrainStep: the model must live on the GPU')
         self.model, self.grad_accumulation_steps = model, k
         self.modes = text_modes(model)
+        vmodes = (True, False) if self.teacher is not None else (False,)   # with the teacher first: the larger graph
         world = _world(process_group)
         if world > 1:
             broadcast_module(model, 0, process_group)    # replicas must start identical (DDP does this when it wraps the module)
+            if self.teacher is not None:
+                broadcast_module(self.teacher.model, 0, process_group)
         self.grad_sync = GradSync(list(model.parameters()), process_group)
         self._scale = 1.0 / (k * world)
         self._seed_dev = _new_seed_word(model, dev)
+        if self.teacher is not None:
+            self.teacher.add_seed_word()
         self._e2tts = hasattr(model, 'cond_drop_prob')
         B, C = self.plan.batch_size, model.num_channels
         order = sorted(self.plan.buckets, reverse=True)   # largest first: it sizes the zero pool and the caches before the small ones
@@ -280,8 +413,15 @@ class BucketedTrainStep:
             t = torch.full((B, nb), -1, device=dev, dtype=torch.int64)
             t[:, :max(1, nb // 4)] = ord('a')
             self._text[nb] = t
+        # per velocity mode: graphs, loss buffers and chunk tables keyed (bucket, text mode). The plain graphs keep the names they
+        # have without a teacher; the velocity graphs also copy out their velocity part.
         self._loss = {(nb, d): torch.zeros((), device=dev) for nb in order for d in self.modes}
         self.graphs, self._tables = {}, {}
+        self.velocity_graphs, self._vel_tables = {}, {}
+        self._vel_loss = {(nb, d): torch.zeros((), device=dev) for nb in order for d in self.modes} if self.teacher is not None else {}
+        self._vel_part = {(nb, d): torch.zeros((), device=dev) for nb in order for d in self.modes} if self.teacher is not None else {}
+        self._zero = torch.zeros((), device=dev)
+        self.launches = {}
         cdp = getattr(model, 'cond_drop_prob', None)
         t0 = time.perf_counter()
         with _KeepPythonRandom():
@@ -292,9 +432,10 @@ class BucketedTrainStep:
                 with torch.cuda.stream(side):   # warm-up off the capture stream: lazy initialisation, caches, packed weights, rotary tables
                     for nb in order:
                         for drop in self.modes:
-                            for _ in range(max(1, warmup)):
-                                self._pass(nb, drop)
-                                _clear_grads(model)
+                            for v in vmodes:
+                                for _ in range(max(1, warmup)):
+                                    self._pass(nb, drop, v)
+                                    _clear_grads(model)
                     if world > 1:
                         self.grad_sync.all_reduce()    # NCCL communicator / channel setup outside the timed path
                 cur.wait_stream(side)
@@ -304,36 +445,50 @@ class BucketedTrainStep:
                 n0 = lib.launch_count()
                 for nb in order:
                     for drop in self.modes:
-                        _clear_grads(model)      # no graph's backward may add into another graph's gradient tensors
-                        table = self.grad_sync.new_table()
-                        g = torch.cuda.CUDAGraph()
-                        with torch.cuda.graph(g, pool=self.pool):
-                            out = self._pass(nb, drop)
-                            self._loss[nb, drop].copy_(out.loss.reshape(()))
-                            grads = self.grad_sync.accumulate(table, self._scale)   # recorded against the (still empty) table
-                        self.grad_sync.fill_table(table, grads)
-                        del out, grads
-                        _clear_grads(model)
-                        self.graphs[nb, drop], self._tables[nb, drop] = g, table
-                self.launches_per_step = (lib.launch_count() - n0) // len(self.graphs)
+                        for v in vmodes:
+                            _clear_grads(model)      # no graph's backward may add into another graph's gradient tensors
+                            table = self.grad_sync.new_table()
+                            g = torch.cuda.CUDAGraph()
+                            n1 = lib.launch_count()
+                            with torch.cuda.graph(g, pool=self.pool):
+                                out = self._pass(nb, drop, v)
+                                (self._vel_loss if v else self._loss)[nb, drop].copy_(out.loss.reshape(()))
+                                if v:
+                                    self._vel_part[nb, drop].copy_(out.loss_breakdown.velocity_consistency.reshape(()))
+                                grads = self.grad_sync.accumulate(table, self._scale)   # recorded against the (still empty) table
+                            self.grad_sync.fill_table(table, grads)
+                            self.launches[nb, drop, v] = lib.launch_count() - n1
+                            del out, grads
+                            _clear_grads(model)
+                            if v:
+                                self.velocity_graphs[nb, drop], self._vel_tables[nb, drop] = g, table
+                            else:
+                                self.graphs[nb, drop], self._tables[nb, drop] = g, table
+                self.launches_per_step = (lib.launch_count() - n0) // (len(self.graphs) + len(self.velocity_graphs))
             finally:
                 if cdp is not None:
                     model.cond_drop_prob = cdp
+        if self.teacher is not None:
+            self.teacher.seal()
         torch.cuda.synchronize(dev)
         self.capture_seconds = time.perf_counter() - t0   # warm-ups + captures
         self.grad_sync.zero()
         self._micro = 0
         self.sync_gradients = False
+        self.velocity_loss = self._zero
 
-    def _pass(self, nb, drop):
+    def _pass(self, nb, drop, velocity=False):
         if self._e2tts:    # pin the coin inside the capture; python's random state is restored by the caller
             self.model.cond_drop_prob = 1.0 if drop else 0.0
         text = None if (drop and self._e2tts) else self._text[nb]
-        return _train_pass(self.model, self._seed_dev, self._mel[nb], text, self._lens[nb])
+        return _train_pass(self.model, self._seed_dev, self._mel[nb], text, self._lens[nb], self.teacher if velocity else None)
 
-    def __call__(self, mel, *, text=None, lens=None):
+    def __call__(self, mel, *, text=None, lens=None, velocity=None):
         """One micro-step on a [batch_size, n, channels] mel (n <= the largest bucket), text ids [batch_size, nt] or a list of
-        strings, optional lens [batch_size]. Returns this micro-batch's (unscaled) loss on the device."""
+        strings, optional lens [batch_size]. Returns this micro-batch's (unscaled) loss on the device. velocity: replay the graph
+        with the velocity-consistency term (default: when the step has a teacher); its velocity part is then in
+        `self.velocity_loss` (0 otherwise)."""
+        v = velocity_flag(self.teacher, velocity, 'BucketedTrainStep')
         if isinstance(text, list):
             from .modules import list_str_to_tensor
             text = (self.model.tokenizer(text) if self._e2tts else list_str_to_tensor(text)).to(mel.device)
@@ -355,11 +510,12 @@ class BucketedTrainStep:
             self._lens[nb].copy_(lens, non_blocking=True)
         if text is not None and not drop:
             self.plan.pad_text(text, nb, out=self._text[nb])
-        self.graphs[nb, drop].replay()
+        (self.velocity_graphs if v else self.graphs)[nb, drop].replay()
         self._micro += 1
         self.sync_gradients = self._micro == self.grad_accumulation_steps
         if self.sync_gradients:
             self._micro = 0
             self.grad_sync.all_reduce()
             self.grad_sync.attach()
-        return self._loss[nb, drop].clone()
+        self.velocity_loss = self._vel_part[nb, drop].clone() if v else self._zero
+        return (self._vel_loss if v else self._loss)[nb, drop].clone()
